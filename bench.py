@@ -47,7 +47,7 @@ def _baseline_metric():
         with open(os.path.join(ROOT, "BASELINE.json")) as f:
             return str(json.load(f)["metric"])
     except Exception:
-        return "MNIST-16x16 images/sec at batch 1M; achieved HBM GB/s vs B200 peak"
+        return "MNIST-16x16 images/sec at batch 1M; achieved HBM GB/s vs H100 peak"
 
 
 METRIC = _baseline_metric()
@@ -67,9 +67,9 @@ def measured_peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             d = json.load(f)
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", float(d.get("sm_max_mhz", 1965.0))
+        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", float(d.get("sm_max_mhz", 1980.0))
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)", 1965.0
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)", 1980.0
 
 
 def synth_images(n, img_bytes, seed, dist="uniform"):
@@ -98,7 +98,7 @@ def synth_images(n, img_bytes, seed, dist="uniform"):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING a timed region (B200_PROFILING.md recipe).  Auxiliary: whatever
+    """nvidia-smi clocks / throttle reasons sampled DURING a timed region .  Auxiliary: whatever
     goes wrong here (UUID-style CUDA_VISIBLE_DEVICES, no nvidia-smi) must never abort the measurement."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -341,7 +341,7 @@ class Ctx:
 
 
 class DeviceBatch:
-    """Two image buffers alternated per step (each n x 256 B = 268 MB at 1M: larger than the 126 MB L2) and double-buffered
+    """Two image buffers alternated per step (each n x 256 B = 268 MB at 1M: larger than the 50 MB L2) and double-buffered
     outputs: consecutive launches touch disjoint buffers."""
 
     def __init__(self, ctx, eng, host_imgs):
@@ -360,21 +360,33 @@ class DeviceBatch:
         return [(self.d_logits[k].cpu().numpy(), self.d_labels[k].cpu().numpy().view(np.uint32)) for k in range(2)]
 
 
+def dump_outputs(out_dir, logits, labels, budget=60_000_000):
+    """What the timed path returned in its last step: logits [n, C] and labels [n] as float64 (exact for int32).  When the full
+    arrays exceed the budget, a fixed seeded sample of rows is written, with the row indices as rows.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    n, per_row = logits.shape[0], 8 * (logits.shape[1] + 2)
+    if n * per_row > budget:
+        rows = np.sort(np.random.default_rng(0).choice(n, budget // per_row, replace=False))
+        logits, labels = logits[rows], labels[rows]
+        np.save(os.path.join(out_dir, "rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "logits.npy"), logits.astype(np.float64))
+    np.save(os.path.join(out_dir, "labels.npy"), labels.astype(np.float64))
+
+
 def int_alu_peak_ops(sm_max_mhz):
     """Integer-ALU roofline of the CNN front-end: the dot-product unit issues one IDP.4A warp instruction per 2 cycles per SM
-    sub-partition (tools/alu_rates.cu, profiles/r1_micro_alu_rates.txt: 2.00 cycles) = 64 lanes/clk/SM x 4 MAC x 2 ops, 148 SMs,
-    at the maximum SM clock.  (conv2/conv3 take int16/int32 activations and can only use IDP.2A / IMAD = 2 / 1 MAC per lane.)"""
-    return 148 * 64 * 8 * sm_max_mhz * 1e6
+    sub-partition = 64 lanes/clk/SM x 4 MAC x 2 ops, 132 SMs (H100 SXM), at the maximum SM clock.  (conv2/conv3 take int16/int32 activations and can only use IDP.2A / IMAD = 2 / 1 MAC per lane.)"""
+    return 132 * 64 * 8 * sm_max_mhz * 1e6
 
 
 def epilogue_alu_bound(model, sm_max_mhz):
-    """Second ceiling of the fused FC kernel: the integer ALU pipe of the in-TMEM ReLUNorm.  Every hidden-layer accumulator costs
+    """Second ceiling of the fused FC kernel: the integer ALU pipe of the in-register ReLUNorm.  Every hidden-layer accumulator costs
     2.33 ALU-pipe instructions (VIADDMNMX.RELU + 1/2 VIMNMX3 + 3/4 PRMT; the shift is an IMAD on the FMA pipe) at one warp
-    instruction per 2 cycles per SM sub-partition (tools/alu_rates.cu): images/s <= 148 SMs x 4 x 32 lanes / (accumulators x 2.33 x 2
+    instruction per 2 cycles per SM sub-partition (tools/alu_rates.cu): images/s <= 132 SMs x 4 x 32 lanes / (accumulators x 2.33 x 2
     cycles) x clock.  Wide models (Binary-160: 480 hidden accumulators per image) hit this ceiling far below the HBM roofline."""
     fc = model.fc_layers
     acc = sum(l.n_out for l in fc[:-1])
-    ips = 148 * 4 * 32 / (max(acc, 1) * 2.33 * 2) * sm_max_mhz * 1e6
+    ips = 132 * 4 * 32 / (max(acc, 1) * 2.33 * 2) * sm_max_mhz * 1e6
     return {"hidden_accumulators_per_image": acc, "images_per_s": ips, "alu_instructions_per_accumulator": 2.33}
 
 
@@ -399,7 +411,7 @@ def run_config(ctx, name, batch, steps, warmup, args, check_parity=True, host_im
         ops = 2.0 * model.macs_per_image * n / (ms * 1e-3)
         peak_ops = int_alu_peak_ops(sm_max)
         roof = {"bound": "int_alu", "achieved": ops / 1e12, "peak": peak_ops / 1e12, "unit": "Top/s", "frac": ops / peak_ops,
-                "peak_source": f"IDP.4A issue rate (1 warp instruction / 2 cycles / SM sub-partition, tools/alu_rates.cu) x 148 SMs x {sm_max:.0f} MHz",
+                "peak_source": f"IDP.4A issue rate (1 warp instruction / 2 cycles / SM sub-partition, tools/alu_rates.cu) x 132 SMs x {sm_max:.0f} MHz",
                 "macs_per_image": model.macs_per_image, "hbm_frac": hbm_ach / peak_gbs, "traffic": traffic_for(name, n)}
     else:
         roof = {"bound": "hbm", "achieved": hbm_ach, "peak": peak_gbs, "unit": "GB/s", "frac": hbm_ach / peak_gbs,
@@ -594,6 +606,8 @@ def main():
     ap.add_argument("--sustain-seconds", type=float, default=1.0)
     ap.add_argument("--path", default="auto", choices=["auto", "layers", "tcgen05"])
     ap.add_argument("--dist", default="uniform", choices=["uniform", "mnist"], help="synthetic image distribution (SURVEY.md 8d config 2)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the logits / labels of the last timed step as DIR/<name>.npy (float64; "
+                    "a fixed seeded sample of rows when the full arrays exceed 60 MB) so that two builds can be compared output for output")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -618,6 +632,8 @@ def main():
     value = world * n / (ms_per_step * 1e-3)
     snap_plain = db.snapshot()
     launches = args.steps * eng.launch_count(n)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *snap_plain[(args.steps - 1) & 1])
 
     # ---- the same steps, still plain launches, alternating between TWO streams: the ordinary CUDA way for a caller to say that
     # consecutive (double-buffered) batches are independent -- the tail of one launch then overlaps the head of the next

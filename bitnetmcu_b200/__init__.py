@@ -1,7 +1,7 @@
-"""bitnetmcu_b200 -- B200-native drop-in for the integer inference hot path of cpldcpu/BitNetMCU.
+"""bitnetmcu_b200 -- H100-native drop-in for the integer inference hot path of cpldcpu/BitNetMCU.
 
 Package contents (only what the path needs):
-  csrc/            hand-written sm_100a CUDA (fused tcgen05 FC chain, CUDA-core layer kernels, CNN front-end) + C ABI
+  csrc/            hand-written sm_90a CUDA (fused wgmma FC chain, CUDA-core layer kernels, CNN front-end) + C ABI
   model.py         BitNetMCU_model.h parser / runtime descriptor / BNM1 blob
   pack.py          exportquant-compatible weight packer
   engine.py        host-side mirror of the reference interface over the C ABI

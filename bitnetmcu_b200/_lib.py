@@ -52,7 +52,7 @@ def load() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise ImportError(f"{LIB_PATH} not built -- run `python -c 'import __graft_entry__ as g; g.build()'` "
-                          "(nvcc, sm_100a).  bitnetmcu_b200 has no CPU fallback.")
+                          "(nvcc, sm_90a).  bitnetmcu_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, u32, i32, sz, i64 = C.c_void_p, C.c_uint32, C.c_int32, C.c_size_t, C.c_int64
     sig = {

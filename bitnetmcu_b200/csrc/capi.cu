@@ -90,7 +90,7 @@ struct bnm_model {
     int32_t *small_h_out = nullptr, *small_d_out = nullptr;  // logits [n][n_classes] then labels [n]
     int8_t *d_f32_scratch = nullptr;   // bnm_infer_batch_device_f32 fallback: quantised images
     size_t f32_scratch_n = 0;
-    int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default, measured fastest: 14.3 vs 20.1 / 16.8 us per call): the kernel writes results
+    int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
                                // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
 };
 static const size_t kSmallBatch = 1024;
@@ -212,7 +212,7 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
     CU_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return fail(BNM_E_UNSUPPORTED, "device %s is sm_%d%d; this library is built for sm_100a only", prop.name, prop.major, prop.minor);
+    if (prop.major != 9) return fail(BNM_E_UNSUPPORTED, "device %s is sm_%d%d; this library is built for sm_90a (Hopper) only", prop.name, prop.major, prop.minor);
 
     bnm_model *m = new bnm_model();
     m->device = device;
@@ -344,7 +344,7 @@ extern "C" int bnm_model_set_option(bnm_model *m, int option, int64_t value) {
     switch (option) {
     case BNM_OPT_PATH:
         if (value < BNM_PATH_AUTO || value > BNM_PATH_TCGEN05) return fail(BNM_E_ARG, "bad path %lld", (long long)value);
-        if (value == BNM_PATH_TCGEN05 && !m->plan) return fail(BNM_E_UNSUPPORTED, "fused tcgen05 path unavailable for this model: %s", m->plan_err.c_str());
+        if (value == BNM_PATH_TCGEN05 && !m->plan) return fail(BNM_E_UNSUPPORTED, "fused tensor-core path unavailable for this model: %s", m->plan_err.c_str());
         m->opt_path = (int)value;
         return 0;
     case BNM_OPT_NF4_EXTENSION:
@@ -444,7 +444,7 @@ static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    if (gather && !fused) return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the tcgen05 path (model: %s)", m->plan_err.c_str());
+    if (gather && !fused) return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     if (fused && !cnn) {
         int rc = fc_chain_launch(m->plan, images, n, logits, labels, gather, st);
         return rc ? fail(BNM_E_CUDA, "fused FC kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;

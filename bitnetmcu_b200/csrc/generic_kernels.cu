@@ -5,7 +5,7 @@
 //   * processconv33ReLU / processmaxpool22 batched                                (inference.c:238-277, 300-322)
 //   * fused CNN front-end: conv,conv,pool,conv,pool per channel + ReLUNorm        (BitNetMCU_MNIST_dll.c:64-80)
 // These are the layer-by-layer path (BNM_PATH_LAYERS) and the front half of every CNN model; the fused
-// tcgen05 FC chain lives in fc_tcgen05.cu.
+// wgmma FC chain lives in fc_wgmma.cu.
 #include "kernels.h"
 
 namespace bnm {

@@ -23,8 +23,8 @@ struct GatherDst {
 struct FcLayerDev {
     int32_t enc = 0;
     uint32_t n_in = 0, n_out = 0;   // as in the model header (Lk_incoming_weights / Lk_outgoing_weights)
-    uint32_t k_pad = 0;             // n_in rounded up to 32 (one tcgen05 kind::i8 K-step), zero padded
-    uint32_t n_pad = 0;             // n_out rounded up to 16 (UMMA N granularity), zero padded
+    uint32_t k_pad = 0;             // n_in rounded up to 32 (one wgmma s8 K-step), zero padded
+    uint32_t n_pad = 0;             // n_out rounded up to 16 (wgmma N granularity), zero padded
     int8_t *dense_a = nullptr;      // [n_pad][k_pad] row-major int8: clamp(w, -128, 127)
     int8_t *dense_b = nullptr;      // [n_pad][k_pad] residual plane w - clamp(w) (only FP130's +128), or null
     int4 *quad_a = nullptr;         // dp4a layout [(n_pad/4)][k_pad/4] of int4 = 4 outputs x 4 k (layer kernels)
@@ -57,7 +57,7 @@ bool launch_cnn_frontend(const int8_t *images, const int8_t *w1, const int8_t *w
 bool cnn_conv3_fits_u16(const int8_t *w1, const int8_t *w2, uint32_t channels);
 bool cnn_frontend_tc_supported(uint32_t channels, uint32_t xy);
 
-// same front-end with conv1 on tcgen05 and the depthwise tail fed from TMEM (cnn_tcgen05.cu); false when the shape is not
+// same front-end with conv1 on wgmma and the depthwise tail fed from shared memory (cnn_wgmma.cu); false when the shape is not
 // covered (channels not a multiple of 16, > 128, or geometry other than 16x16)
 bool launch_cnn_frontend_tc(const int8_t *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
                             uint32_t xy, int8_t *features, uint32_t feat_stride, size_t n, int sm_count, int *d_err,
@@ -72,7 +72,7 @@ void launch_i32_to_i8(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t ou
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 
-// ---- fused tcgen05 FC chain (fc_tcgen05.cu)
+// ---- fused wgmma FC chain (fc_wgmma.cu)
 struct FcChainPlan;  // opaque, owned by the model
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
                                   char *err, size_t err_len);

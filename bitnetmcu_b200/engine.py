@@ -7,7 +7,7 @@ processfclayer / ReLUNorm / processconv33ReLU /        processfclayer / relunorm
 processmaxpool22 (BitNetMCU_inference.h:15-60)         (same argument meaning, batched over a leading axis)
 model = whichever header is named BitNetMCU_model.h    Engine(Model) from parse_header() / a .bnm blob
 
-Nothing here computes on the CPU: every call goes through libbitnetmcu_b200.so (hand-written sm_100a CUDA).
+Nothing here computes on the CPU: every call goes through libbitnetmcu_b200.so (hand-written sm_90a CUDA).
 torch is used only as plumbing for device memory / streams in ``infer_device``.
 """
 from __future__ import annotations

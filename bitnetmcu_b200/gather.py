@@ -10,7 +10,7 @@ that needs the results in one place has three ways to get them, all measured by 
 * ``none``      -- results stay sharded.
 
 An all-gathered logits tensor is NVLink-ingest bound whatever the kernels do: every GPU receives 40 B per image of the other
-ranks (<= ~900 GB/s in), so the box tops out near 22 G images/s per destination; labels (4 B/image) scale.
+ranks, so the box tops out at the NVLink ingest bandwidth / 40 B images/s per destination; labels (4 B/image) scale.
 """
 from __future__ import annotations
 

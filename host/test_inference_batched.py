@@ -5,7 +5,7 @@ The reference feeds the MNIST test set to `lib.Inference()` one image at a time:
 16x16 float image, scales it to int8 (test_inference.py:140-141) and calls the DLL.  Here the whole set takes three calls:
 
     q      = bnm_quantize_images(float images)          # same float32 arithmetic, on the GPU, bit-identical
-    logits, predicted = bnm_infer_batch(model, q)       # the fused sm_100a kernel
+    logits, predicted = bnm_infer_batch(model, q)       # the fused sm_90a kernel
     accuracy = mean(predicted == labels)
 
 and prints the reference's summary lines ("size of test data", "Mispredictions C", "Overall accuracy C").  The

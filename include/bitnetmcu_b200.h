@@ -1,9 +1,9 @@
 /*
- * bitnetmcu_b200.h -- C ABI of the B200-native BitNetMCU inference engine (libbitnetmcu_b200.so).
+ * bitnetmcu_b200.h -- C ABI of the H100-native BitNetMCU inference engine (libbitnetmcu_b200.so).
  *
  * Drop-in boundary for ONE path of cpldcpu/BitNetMCU: processfclayer + ReLUNorm + the per-channel
  * conv/maxpool loop of BitNetMCU_inference.c, chained as BitMnistInference does.  Host code stays
- * plain C; everything behind these entry points is hand-written sm_100a CUDA.  There is NO CPU
+ * plain C; everything behind these entry points is hand-written sm_90a CUDA.  There is NO CPU
  * fallback: every compute entry fails (negative return / aborts, see below) without a CUDA device.
  *
  * Section 1 keeps the reference's own symbols, signatures and semantics
@@ -79,23 +79,22 @@ typedef struct bnm_model bnm_model;   /* opaque; weights decoded and resident on
 
 /* execution path of the FC chain */
 enum {
-    BNM_PATH_AUTO = 0,     /* fused tcgen05 kernel when the model shape is supported, else BNM_PATH_LAYERS */
+    BNM_PATH_AUTO = 0,     /* fused wgmma kernel when the model shape is supported, else BNM_PATH_LAYERS   */
     BNM_PATH_LAYERS = 1,   /* one CUDA-core (dp4a) kernel per layer + ReLUNorm kernel; any shape          */
-    BNM_PATH_TCGEN05 = 2   /* fused persistent kernel: TMA -> tcgen05.mma kind::i8 -> in-TMEM ReLUNorm     */
+    BNM_PATH_TCGEN05 = 2   /* fused persistent kernel: TMA -> wgmma s8 -> in-register ReLUNorm             */
 };
 enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BNM_OPT_LAUNCH_OVERLAP = 4, BNM_OPT_CNN_FRONTEND = 5 };
 /* BNM_OPT_CNN_FRONTEND (CNN models, the conv/pool loop of BitNetMCU_MNIST_dll.c:64-80): 0 (default) conv1 on the tensor cores
- * (tcgen05, depthwise tail fed from TMEM) when the channel count is a multiple of 16 and <= 128, else the CUDA-core kernel;
+ * (wgmma, depthwise tail fed from shared memory) when the channel count is a multiple of 16 and <= 128, else the CUDA-core kernel;
  * 1 CUDA-core kernel; 2 tensor-core kernel or fail.  Results are identical. */
 /* BNM_OPT_LAUNCH_OVERLAP (fused kernel, consecutive bnm_infer_batch_device calls on one stream):
  *   0  (default) plain launches, ordinary stream semantics.
- *   1  programmatic dependent launch with a grid-dependency wait: the next launch's prologue (barriers, TMEM, weights) runs
+ *   1  programmatic dependent launch with a grid-dependency wait: the next launch's prologue (barriers, weights) runs
  *      under the tail of the previous one; inputs are read and outputs written only after the previous kernel has
- *      completed.  Ordinary stream semantics.  Measured erratic on B200 (-2 % ... +7 % against mode 0 for builds that
- *      differ in one instruction), hence not the default.
+ *      completed.  Ordinary stream semantics.
  *   2  the caller declares consecutive launches independent -- the images / logits / labels of one call are not the
  *      buffers of the call right before it (e.g. double-buffered batches), exactly what issuing them on two streams would
- *      promise.  The next launch's tiles then start on each SM as the previous launch leaves it (-6 ... -9 % per step).
+ *      promise.  The next launch's tiles then start on each SM as the previous launch leaves it.
  *      CONTRACT: an independent launch executes no grid-dependency wait, so it is ordered against NOTHING enqueued before it
  *      on the stream -- neither the previous bnm launch nor a producer kernel / copy that writes `images`.  The images of
  *      call k must therefore be complete before call k-1 was enqueued (resident inputs, or produced on another stream and
@@ -147,7 +146,7 @@ BNM_API int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n,
  * (bnm_ipc_export / bnm_ipc_open) or same-process P2P (bnm_enable_peer_access), so that the all-gather of the batch-sharded
  * results rides under the compute over NVLink instead of running as a collective after it.  Visibility at the destination
  * follows stream completion of this call on the source plus whatever cross-rank synchronisation the caller uses.
- * Only the fused tcgen05 path supports it. */
+ * Only the fused tensor-core path supports it. */
 #define BNM_MAX_GATHER_DST 8
 typedef struct bnm_gather {
     uint32_t n_labels_dst, n_logits_dst;

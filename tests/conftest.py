@@ -1,4 +1,4 @@
-"""Shared fixtures.  `-m "not gpu"` runs here on CPU; `-m gpu` needs a B200 (driver runs it at round end)."""
+"""Shared fixtures.  `-m "not gpu"` runs on any machine; `-m gpu` needs an H100 (sm_90)."""
 import os
 import sys
 
@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90); run with -m gpu")
 
 
 @pytest.fixture(scope="session")

@@ -1,4 +1,4 @@
-"""Discrete-event model of the fused FC kernel's per-CTA protocol (bitnetmcu_b200/csrc/fc_tcgen05.cu): the image-tile ring with
+"""Discrete-event model of a per-CTA image-tile ring protocol (the general form of bitnetmcu_b200/csrc/fc_wgmma.cu's ring): the ring with
 its "tile landed" mbarriers, the per-slot MMA / ready hand-off between a warpgroup's issuer warp and its epilogue warps, and the
 refill of a stage by the warp that sees the tile's layer-1 MMAs complete.
 

@@ -65,4 +65,4 @@ def test_epilogue_alu_bound_and_int_alu_peak():
     a, b = bench.epilogue_alu_bound(fc, 1965.0), bench.epilogue_alu_bound(b160, 1965.0)
     assert a["hidden_accumulators_per_image"] == 192 and b["hidden_accumulators_per_image"] == 480
     assert abs(a["images_per_s"] / b["images_per_s"] - 480 / 192) < 1e-9 and 3.5e10 < a["images_per_s"] < 4.5e10
-    assert abs(bench.int_alu_peak_ops(1965.0) - 148 * 64 * 8 * 1965e6) < 1
+    assert abs(bench.int_alu_peak_ops(1965.0) - 132 * 64 * 8 * 1965e6) < 1

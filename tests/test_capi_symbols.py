@@ -31,12 +31,12 @@ def test_library_exports_every_declared_symbol(built):
     assert lib.bnm_version() == 100
 
 
-def test_library_contains_blackwell_sass(built):
-    """tcgen05.mma / tcgen05.ld,st / TMA show up as UTC*MMA / LDTM,STTM / UTMALDG in the sm_100a SASS."""
+def test_library_contains_hopper_sass(built):
+    """wgmma s8 / TMA / bulk copies show up as IGMMA / UTMALDG / UBLKCP in the sm_90a SASS."""
     from bitnetmcu_b200 import _lib
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCIMMA", "LDTM", "STTM", "UTMALDG", "UBLKCP", "VIADDMNMX", "VIMNMX3", "IDP.4A"):
+    assert "sm_90a" in sass
+    for mnemonic in ("IGMMA", "WARPGROUP.ARRIVE", "UTMALDG", "UBLKCP", "VIADDMNMX", "VIMNMX3", "IDP.4A"):
         assert mnemonic in sass, mnemonic
 
 

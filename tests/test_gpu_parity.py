@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA paths, called through the C ABI, against the oracle and
+"""GPU parity tests (run with -m gpu on an H100): the CUDA paths, called through the C ABI, against the oracle and
 the committed golden vectors made by the unmodified reference.  Integer work: the bar is bit-exact."""
 import ctypes as C
 import json
@@ -31,7 +31,7 @@ def _engine(name, path, nf4=False, cnn_frontend=None):
 
 
 def _frontends(model):
-    """CNN models run once per front-end kernel (BNM_OPT_CNN_FRONTEND): CUDA cores and conv1-on-tcgen05; FC models once."""
+    """CNN models run once per front-end kernel (BNM_OPT_CNN_FRONTEND): CUDA cores and conv1-on-wgmma; FC models once."""
     from bitnetmcu_b200 import _lib
     if model.model_class != 1:
         return [None]
@@ -465,9 +465,9 @@ def test_processfclayer_on_tcgen05(lib, oracle, enc):
                                     (256, 64, 64, 64, 64, 64, 64, 64, 10), (256, 160, 144, 10), (256, 256, 10), (128, 176, 176, 176, 7),
                                     (256, 96, 96, 10)])
 def test_chains_on_tcgen05(lib, oracle, enc, widths):
-    """Random-code chains with odd shapes: A-from-TMEM (.ts) layers of every width class (16..224), the wide two-pass
-    ReLUNorm, FP130 with +128 (residual plane) in EVERY layer, > 16 classes, the 8-layer maximum; wide models with <= 16 classes
-    run the shared-memory-activation form (three / two accumulator-only slots, 16-column tails), 96-wide ones four warpgroups."""
+    """Random-code chains with odd shapes on the fused path: register-A layers of every width class (16..256, 64-wide pieces plus
+    16-wide tails), FP130 with +128 (residual plane) in EVERY layer, > 16 classes, the 8-layer maximum, all three accumulator
+    widths and both pipe counts."""
     from bitnetmcu_b200 import _lib, pack as P
     from bitnetmcu_b200.engine import Engine
     if enc == 1 and any(w % 32 for w in widths[:-1]):

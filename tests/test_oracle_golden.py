@@ -1,6 +1,6 @@
 """Pin the oracle (oracle/bitnet_oracle.c) against the reference: golden vectors made by the unmodified
-reference kernels (tests/golden/make_golden.py), the reference's own label KAT, and -- when oracle/_ref is
-present -- exhaustive decode sweeps and random function-level comparisons against the reference itself."""
+reference kernels (tests/golden/make_golden.py), the reference's own label KAT, and random function-level comparisons against
+outputs recorded from the reference itself (tests/golden/make_reference_vectors.py)."""
 import json
 import os
 import zlib
@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, load_model, model_names, xorshift_images
+from golden import reference_cases as RC
 from bitnetmcu_b200 import model as M
 from bitnetmcu_b200 import pack as P
 
@@ -98,57 +99,35 @@ def test_ternary_all_words(oracle):
     assert np.array_equal(oracle.decode_fc(packed, M.ENC_TERNARY, 10, 59049), trits)
 
 
-# ---- direct comparisons with the unmodified reference (skipped where oracle/_ref is absent) -------------
+# ---- comparisons with the unmodified reference: its outputs for these seeded inputs were recorded by
+# tests/golden/make_reference_vectors.py (tests/golden/reference_vectors.npz); the inputs are regenerated here
 
-@pytest.mark.parametrize("enc", [1, 2, 4, 12, 16, 20, 36, 64, 3])
-def test_fclayer_vs_reference(oracle, reference, enc):
-    rng = np.random.default_rng(enc)
-    for n_in, n_out in [(256, 64), (64, 10), (160, 160), (320, 7)]:
-        if enc == 64:
-            n_in = (n_in + 9) // 10 * 10
-            w = rng.integers(0, 65536, size=n_out * n_in // 10, dtype=np.uint32).astype(np.uint16)
-        else:
-            w = rng.integers(0, 2 ** 32, size=n_out * n_in // 4 + 4, dtype=np.uint64).astype(np.uint32)
-        act = rng.integers(-128, 128, size=n_in + 16).astype(np.int8)
-        assert np.array_equal(oracle.fclayer(act, w, enc, n_in, n_out), reference.fclayer(act, w, enc, n_in, n_out))
+@pytest.fixture(scope="module")
+def ref_vectors():
+    return np.load(os.path.join(GOLDEN, "reference_vectors.npz"))
 
 
-def test_relunorm_vs_reference(oracle, reference):
-    rng = np.random.default_rng(7)
-    for trial in range(300):
-        n = int(rng.integers(1, 300))
-        scale = int(rng.choice([1, 100, 20000, 500000, 4000000]))
-        x = rng.integers(-scale, scale + 1, size=n).astype(np.int32)
-        if trial % 7 == 0:
-            x = -np.abs(x) - 1
-        if trial % 11 == 0:
-            x[rng.integers(0, n)] = 2 ** (7 + trial % 20) - 1
+@pytest.mark.parametrize("enc", RC.FCLAYER_ENCS)
+def test_fclayer_vs_reference(oracle, ref_vectors, enc):
+    for key, (act, w, e, n_in, n_out) in RC.fclayer_cases([enc]):
+        assert np.array_equal(oracle.fclayer(act, w, e, n_in, n_out), ref_vectors["fclayer/" + key])
+
+
+def test_relunorm_vs_reference(oracle, ref_vectors):
+    for key, x in RC.relunorm_cases():
         a, pa = oracle.relunorm(x)
-        b, pb = reference.relunorm(x)
-        assert pa == pb and np.array_equal(a, b)
+        assert pa == int(ref_vectors["relunorm_pos/" + key]) and np.array_equal(a, ref_vectors["relunorm/" + key])
 
 
-def test_conv_pool_vs_reference(oracle, reference):
-    rng = np.random.default_rng(9)
-    for xy in (16, 14, 6, 4, 3):
-        for _ in range(20):
-            act = rng.integers(-20000, 20000, size=xy * xy).astype(np.int32)
-            w = rng.integers(-128, 128, size=9).astype(np.int8)
-            assert np.array_equal(oracle.conv33relu(act, w, xy, 4), reference.conv33relu(act, w, xy, 4))
-            if xy % 2 == 0:
-                assert np.array_equal(oracle.maxpool22(act, xy), reference.maxpool22(act, xy))
+def test_conv_pool_vs_reference(oracle, ref_vectors):
+    for key, (act, w, xy) in RC.conv_pool_cases():
+        assert np.array_equal(oracle.conv33relu(act, w, xy, 4), ref_vectors["conv/" + key])
+        if xy % 2 == 0:
+            assert np.array_equal(oracle.maxpool22(act, xy), ref_vectors["pool/" + key])
 
 
-@pytest.mark.parametrize("name", ["fc", "cnn", "cnn_48", "binary160", "ternary64", "rand_fp130_64", "rand_nf4_64", "1k"])
-def test_whole_model_vs_reference_random(oracle, reference, name):
+@pytest.mark.parametrize("name", RC.WHOLE_MODELS)
+def test_whole_model_vs_reference_random(oracle, ref_vectors, name):
     m = load_model(name)
-    rng = np.random.default_rng(11)
-    n = 3000 if m.model_class == M.MODEL_FCMNIST else 600
-    imgs = rng.integers(-128, 128, size=(n, 256)).astype(np.int8)
-    imgs[:50] = np.clip(imgs[:50], -20, 127)          # MNIST-like background
-    imgs[50:60] = -128
-    imgs[60:70] = 127
-    imgs[70:80] = 0
-    lo, la = oracle.infer(m, imgs)
-    lr, lar = reference.infer(m, imgs)
-    assert np.array_equal(lo, lr) and np.array_equal(la, lar)
+    lo, la = oracle.infer(m, RC.whole_model_images(m))
+    assert np.array_equal(lo, ref_vectors["model_logits/" + name]) and np.array_equal(la, ref_vectors["model_labels/" + name])

@@ -1,9 +1,12 @@
-"""The tile ring of the fused FC kernel (fc_tcgen05.cu: kFullBars "tile landed" barriers per stage) checked on a discrete-event
-model with arbitrary latencies: no parity wait may pass before its tile has landed, and every tile completes.  CPU only.
+"""The tile-ring rule behind the fused FC kernel's barriers, checked on a discrete-event model with arbitrary latencies: no parity
+wait may pass before its tile has landed, and every tile completes.  CPU only.
 
-The rule the kernel states: a shape with `slots` tile slots on `stages` ring stages needs at least slots / gcd(slots, stages)
-barriers per stage (the latest same-stage tile that is certain to have landed when the issuer reaches tile j is that many ring
-rounds back).  kFullBars = 8 covers every shape (slots <= 8)."""
+The rule: a shape with `slots` tile slots on `stages` ring stages needs at least slots / gcd(slots, stages) barriers per stage (the
+latest same-stage tile that is certain to have landed when the waiter reaches tile j is that many ring rounds back).  In fc_wgmma.cu
+every consumer warpgroup waits for every tile of its pipe in order -- in the model's terms one slot per pipe -- so one "full"
+barrier per stage suffices for any stage count.  The model covers this rule only: it does not replay the kernel's two consumer
+warpgroups per tile, its eight-arrival "empty" barrier or the producer's tile-order refill across two pipes.
+"""
 import re
 from math import gcd
 from pathlib import Path
@@ -12,18 +15,16 @@ import pytest
 
 from ring_protocol_sim import Violation, simulate
 
-# (warpgroups, slots per warpgroup, ring stages): the shapes the plans launch
-SHIPPED = [(3, 2, 6), (3, 2, 5),   # width-64 models; their gather launches (staging buffers cost a stage)
-           (4, 1, 5),              # four-warpgroup form (2bitsym-96)
-           (3, 1, 2), (2, 1, 2),   # shared-memory-activation form (Binary-160: three slots, two stages), 256-wide
-           (2, 1, 4), (3, 1, 4),   # wide models on TMEM activations
-           (2, 2, 4)]              # float-input launches
+# (waiters, slots per waiter, ring stages of a pipe): every stage count a ring can have (kMaxStages = 8); plans use two to six
+SHIPPED = [(1, 1, stages) for stages in range(1, 9)]
 FAST_CHAIN = dict(mma=(0.01, 0.05), epi=(0.01, 0.08), load_lat=(0.3, 4.0), slow_load=(0.05, 20.0))   # tiny model, slow loads
 
 
 def kernel_full_bars():
-    src = (Path(__file__).resolve().parents[1] / "bitnetmcu_b200" / "csrc" / "fc_tcgen05.cu").read_text()
-    return int(re.search(r"constexpr uint32_t kFullBars = (\d+);", src).group(1))
+    src = (Path(__file__).resolve().parents[1] / "bitnetmcu_b200" / "csrc" / "fc_wgmma.cu").read_text()
+    decl = re.search(r"uint64_t bar_full\[([^\]]+)\](\[[^\]]+\])?", src)
+    assert decl.group(1) == "kMaxStages" and decl.group(2) is None   # one barrier per stage
+    return 1
 
 
 @pytest.mark.parametrize("shape", SHIPPED)

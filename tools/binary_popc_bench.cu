@@ -6,9 +6,9 @@
 // This tool measures one Binary layer 256 -> 160 over a batch on CUDA cores both ways and checks that they agree:
 //   A. dp4a on weights pre-decoded to +-1 int8 (what BNM_PATH_LAYERS does)
 //   B. bit-plane AND/POPC (planes extracted with warp ballots, the cheapest extraction there is)
-// The fused tcgen05 path runs the whole 3-layer Binary-160 network faster than either runs this one layer (profiles/).
+// The fused tensor-core path decodes Binary weights once per model and runs them as int8 MMAs instead.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o binary_popc_bench binary_popc_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o binary_popc_bench binary_popc_bench.cu
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>

@@ -1,6 +1,7 @@
 """Fused float-input path vs the chain of the scaling kernel and the int8 kernel: us per step at batch 2^20."""
 import os, sys, numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from bench import measured_peaks
 from bitnetmcu_b200 import engine as E
 from bitnetmcu_b200.engine import Engine
 from bitnetmcu_b200.model import Model
@@ -24,4 +25,4 @@ def chained(i):
     E.quantize_images_device(x[i & 1], q); e.infer_device(q, lo2, la2)
 ch = t(chained)
 e.infer_device_f32(x[0], lo, la); chained(0); torch.cuda.synchronize()
-print(f"fused {fused:.1f} us = {n / fused / 1e3:.2f} G img/s ({1064 * n / fused / 1e3 / 6592.9:.3f} of HBM peak at 1064 B/img) | chained {ch:.1f} us = {n / ch / 1e3:.2f} G img/s | equal {bool(torch.equal(lo, lo2) and torch.equal(la, la2))}")
+print(f"fused {fused:.1f} us = {n / fused / 1e3:.2f} G img/s ({1064 * n / fused / 1e3 / measured_peaks()[0]:.3f} of HBM peak at 1064 B/img) | chained {ch:.1f} us = {n / ch / 1e3:.2f} G img/s | equal {bool(torch.equal(lo, lo2) and torch.equal(la, la2))}")

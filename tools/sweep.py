@@ -6,7 +6,7 @@
 
 Every point: 3 warm-up + 10 timed plain launches between two events, barrier + synchronise on both sides, max over ranks;
 parity of a 4096-image sample of every rank's result against the oracle (checker only).  Rank 0 prints a markdown table and
-writes gpurun_out/sweep_<N>gpu.json.
+writes sweep_out/sweep_<N>gpu.json.
 """
 import json, os, sys, statistics
 import numpy as np
@@ -26,10 +26,8 @@ if world > 1:
 torch.cuda.set_device(local_rank)
 dev = torch.device("cuda", local_rank)
 orc = Oracle()
-try:
-    PEAK = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
-except Exception:
-    PEAK = 6592.9
+from bench import measured_peaks  # noqa: E402
+PEAK = measured_peaks()[0]   # GB/s: MEASURED_PEAKS.json when present, else the H100 data-sheet figure
 
 
 def barrier():
@@ -94,7 +92,7 @@ for name in ("cnn", "cnn_48"):
     if rank == 0:
         print(f"| {r['model']} | 2^20 | {world} | {r['g_images_per_s']:.3f} | {r['hbm_frac_per_gpu']:.3f} | {r['ms_per_launch']:.4f} | {'bit-exact' if r['parity'] else 'MISMATCH'} |", flush=True)
 if rank == 0:
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(rows, open(os.path.join(ROOT, "gpurun_out", f"sweep_{world}gpu.json"), "w"), indent=0)
+    os.makedirs(os.path.join(ROOT, "sweep_out"), exist_ok=True)
+    json.dump(rows, open(os.path.join(ROOT, "sweep_out", f"sweep_{world}gpu.json"), "w"), indent=0)
 if world > 1:
     dist.destroy_process_group()
