@@ -77,6 +77,7 @@ struct FcChainPlan {
     uint32_t in_bytes = 0;
     uint32_t max_n = 0;               // accumulator width the kernel is instantiated for: 64, 128, 192 or 256 columns
     uint32_t pipes = 1;
+    uint32_t last_n = 0;              // wgmma width of the last layer in two-slot launches: 16 when it is at most 16 wide, else max_n
     int sm_count = 0;
     int device = 0;
     int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 plain launch, 1 dependent launch + wait, 2 independent launches
@@ -140,26 +141,81 @@ __device__ __forceinline__ uint32_t norm_pack4(uint32_t x0, uint32_t x1, uint32_
 }
 
 // ---------------------------------------------------------------------------------------------------
+// phase trace (diagnostics build only: make -C bitnetmcu_b200/csrc EXTRA=-DBNM_FC_TRACE; tools/fc_phase_trace.py reads it).
+// In the first kTraceCtas CTAs, lane 0 of warp 0 of every consumer warpgroup (writer cw) and the producer warp (writer
+// kTraceWriters - 1) record (clock64, event) pairs; thread 0 records %globaltimer and clock64 at kernel entry and exit so that
+// cycles convert to time.  The product build contains none of it.
+// ---------------------------------------------------------------------------------------------------
+#ifdef BNM_FC_TRACE
+constexpr uint32_t kTraceCtas = 4, kTraceWriters = 5, kTraceEvents = 2048;
+// event code: kind | slot << 8 | layer << 12
+enum : uint32_t { TR_FULL_BEGIN = 1, TR_FULL_END, TR_WAIT_BEGIN, TR_WAIT_END, TR_EPI_END, TR_EMPTY_BEGIN, TR_EMPTY_END, TR_ISSUE };
+struct FcTrace {
+    unsigned long long hdr[kTraceCtas][4];   // globaltimer / clock64 at entry, globaltimer / clock64 at exit
+    uint32_t count[kTraceCtas][kTraceWriters];
+    ulonglong2 ev[kTraceCtas][kTraceWriters][kTraceEvents];   // (clock64, event code)
+};
+__device__ FcTrace g_fc_trace;
+__device__ __forceinline__ unsigned long long globaltimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+#define BNM_TRACE_DECL(writer_, enabled_) const uint32_t tr_w = (writer_); const bool tr_on = (enabled_) && blockIdx.x < kTraceCtas; uint32_t tr_n = 0
+#define BNM_TRACE(kind_, slot_, layer_) do { if (tr_on && tr_n < kTraceEvents) g_fc_trace.ev[blockIdx.x][tr_w][tr_n++] = make_ulonglong2((unsigned long long)clock64(), (kind_) | (uint32_t)(slot_) << 8 | (uint32_t)(layer_) << 12); } while (0)
+#define BNM_TRACE_END() do { if (tr_on) g_fc_trace.count[blockIdx.x][tr_w] = tr_n; } while (0)
+#define BNM_TRACE_STAMP(k_) do { if (threadIdx.x == 0 && blockIdx.x < kTraceCtas) { g_fc_trace.hdr[blockIdx.x][2 * (k_)] = globaltimer(); g_fc_trace.hdr[blockIdx.x][2 * (k_) + 1] = clock64(); } } while (0)
+#else
+#define BNM_TRACE_DECL(writer_, enabled_) do {} while (0)
+#define BNM_TRACE(kind_, slot_, layer_) do {} while (0)
+#define BNM_TRACE_END() do {} while (0)
+#define BNM_TRACE_STAMP(k_) do {} while (0)
+#endif
+
+// ---------------------------------------------------------------------------------------------------
 // the kernel
 //
 // Roles (one CTA per SM, persistent over image tiles):
 //   * kPipes x 2 consumer warpgroups.  Warpgroup 2p + h takes rows 64h .. 64h+63 of every tile of pipe p (tiles i of this CTA with
-//     i % kPipes == p) and runs the whole layer chain on them in registers.
+//     i % kPipes == p) and runs the whole layer chain on them in registers.  With kSlots = 2 a warpgroup holds two consecutive tiles
+//     of its pipe at once (slots A and B, each with its own accumulators and fragments) and alternates between them, so that the
+//     MMAs of one slot are in flight while the warpgroup runs the ReLUNorm or the epilogue of the other.
 //   * one producer warp: barrier setup, the weight copy, and (int8 input) the TMA image loads of every pipe in tile order.
 //   * kFloatIn: eight quantiser warps in place of the TMA loads (see below).
 // Barriers: full[stage] (tile landed: TMA bytes, or the eight quantiser warps), empty[stage] (the eight consumer warps of the pipe
 // have finished reading the stage).  Every consumer and the producer visit the stages of their pipe in order, so every parity
-// wait starts after the barrier's previous phase has completed: one full and one empty barrier per stage suffice.
+// wait starts after the barrier's previous phase has completed: one full and one empty barrier per stage suffice.  Two slots keep
+// that order: slot A waits for tile j, slot B for tile j + 1, and A's next tile j + 2 is waited for after both.
 // ---------------------------------------------------------------------------------------------------
-// 256-wide models: 128 accumulator + 32 fragment registers per consumer thread do not fit the 168 registers a 288-thread CTA
-// gets, so the producer becomes a whole warpgroup that hands registers to the consumers (setmaxnreg: 2 x 128 x 224 + 128 x 56
-// <= 64 k)
-template <int kN, int kPipes, bool kFloatIn>
-constexpr int chain_threads() { return (kN == 256 ? 384 : kPipes * 256 + 32) + (kFloatIn ? 32 * kFloatQuantWarps : 0); }
+// The producer becomes a whole warpgroup that hands registers to the consumers (setmaxnreg) where the consumers need more than
+// an even share of the register file.  setmaxnreg moves registers inside the CTA's launch allocation (threads x the per-thread
+// count the launch bounds give), so the registers of all warps after it may not exceed that allocation:
+//   * 256-wide models: 128 accumulator + 32 fragment registers per consumer thread do not fit the 168 registers a 288-thread CTA
+//     gets; 384 threads x 168 = 2 x 128 x 224 + 128 x 56;
+//   * two slots: 2 x (32 + 8) registers of accumulators and fragments per consumer thread do not fit the 96 a 544-thread CTA gets
+//     (five warps on a sub-partition); 640 threads x 96 = 4 x 128 x 112 + 128 x 32.
+template <int kN, int kSlots>
+__host__ __device__ constexpr bool producer_warpgroup() { return kN == 256 || kSlots == 2; }
+template <int kN, int kPipes, bool kFloatIn, int kSlots>
+__host__ __device__ constexpr int chain_threads() {
+    return kPipes * 256 + (producer_warpgroup<kN, kSlots>() ? 128 : 32) + (kFloatIn ? 32 * kFloatQuantWarps : 0);
+}
+// registers per thread of a one-CTA-per-SM launch of `threads`: the warps share four sub-partitions of 16 k registers each,
+// allocated in steps of 8 per thread
+__host__ __device__ constexpr int launch_regs(int threads) { return 16384 / (32 * ((threads / 32 + 3) / 4)) / 8 * 8; }
 
-template <int kN, int kPipes, bool kFloatIn>
-__global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn>(), 1)
+// kSlots: tiles per consumer warpgroup in compute at once (1 or 2; 2 only for 64-wide int8 launches with two pipes).
+// kLastN: wgmma width of the last layer -- 16 when the plan's last layer is at most 16 wide (every classifier head), else kN.
+template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN>
+__global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn, kSlots>(), 1)
 fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
+    static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
+    constexpr bool kProducerWG = producer_warpgroup<kN, kSlots>();
+    constexpr uint32_t kProducerRegs = kN == 256 ? 56 : 32, kConsumerRegs = kN == 256 ? 224 : 112;
+    static_assert(!kProducerWG || 128 * kProducerRegs + 256 * kPipes * kConsumerRegs <=
+                  (uint32_t)(chain_threads<kN, kPipes, kFloatIn, kSlots>() * launch_regs(chain_threads<kN, kPipes, kFloatIn, kSlots>())),
+                  "setmaxnreg: the warps' registers must fit the CTA's launch allocation, or an increase never returns");
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t bar_full[kMaxStages], bar_empty[kMaxStages];
     __shared__ __align__(8) uint64_t bar_w;   // weight image landed (bulk async copies)
@@ -172,6 +228,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
     // the caller declares consecutive launches independent, its first tiles -- overlap the ragged end of this one.  Only when the
     // grid fills the GPU: a smaller grid leaves SMs free, where later launches could pile up next to earlier ones.
     if (P.early_trigger) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    BNM_TRACE_STAMP(0);
     const uint32_t n_st = P.n_stages;
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B tiles need 1024-byte alignment
     uint8_t *smem = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -180,7 +237,9 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
     const uint32_t my_tiles = tile0 < P.n_tiles ? (P.n_tiles - tile0 + tile_step - 1) / tile_step : 0;
     const uint32_t w_base = smem_base + P.off_w;
     const uint32_t prod_warp = kPipes * 8;
-    // tile i of this CTA: pipe i % kPipes, j-th tile of that pipe, stage (pipe, j % n_st), ring round j / n_st
+    // tile i of this CTA: pipe i % kPipes, j-th tile of that pipe, stage (pipe, j % n_st), ring round j / n_st.
+    // Two slots: a warpgroup waits for tile j + 1 of its pipe before it releases the stage of tile j (slot B's layer 1 is issued
+    // before slot A's completes), so a pipe needs at least two stages -- every two-pipe plan has them (fc_chain_plan_create).
     auto stage_of = [&](uint32_t i) { return (i % kPipes) * n_st + (i / kPipes) % n_st; };
     auto round_of = [&](uint32_t i) { return (i / kPipes) / n_st; };
 
@@ -196,9 +255,9 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
     }
     __syncthreads();
 
-    if (warp == prod_warp || (kN == 256 && warp > prod_warp)) {
-        // ======================= producer (256-wide: its whole warpgroup gives registers away, three warps of it idle) ============
-        if (kN == 256) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
+    if (warp == prod_warp || (kProducerWG && warp > prod_warp)) {
+        // ======================= producer (kProducerWG: its whole warpgroup gives registers away, three warps of it idle) ==========
+        if (kProducerWG) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs) : "memory");
         if (warp == prod_warp && lane == 0) {
             // weight image -> smem (same bytes for every CTA; L2-resident after the first wave).  The weights were written at model
             // build, long before any kernel that may still be running ahead of this one, so they are fetched before the grid
@@ -210,19 +269,23 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                 // everything else this kernel reads or writes may belong to the kernel launched before it
                 if (P.wait_prior_grid) asm volatile("griddepcontrol.wait;" ::: "memory");
                 const uint64_t l2_policy = policy_evict_first();   // images are read exactly once
+                BNM_TRACE_DECL(kTraceWriters - 1, true);
                 for (uint32_t i = 0; i < my_tiles; i++) {
                     const uint32_t s = stage_of(i), u = round_of(i);
+                    BNM_TRACE(TR_EMPTY_BEGIN, 0, 0);
                     if (u > 0) mbar_wait_relaxed(&bar_empty[s], (u - 1) & 1, P.err, 5);
+                    BNM_TRACE(TR_EMPTY_END, 0, 0);
                     mbar_arrive_expect_tx(&bar_full[s], P.stage_bytes);
                     const int32_t row = (int32_t)((tile0 + i * tile_step) * kTileM);
                     for (uint32_t a = 0; a < P.in_atoms; a++)
                         tma_load_2d_hint(smem + s * P.stage_bytes + a * 16384, &tmap_in, (int32_t)(a * 128), row, &bar_full[s], l2_policy);
                 }
+                BNM_TRACE_END();
             }
         }
     } else if (warp < prod_warp) {
         // ======================= consumer warpgroup cw = 2 pipe + half =======================
-        if (kN == 256) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;" ::: "memory");
+        if (kProducerWG) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs) : "memory");
         const uint32_t cw = warp >> 2, pipe = cw >> 1, half = cw & 1, wq = warp & 3;
         const uint32_t quad = lane & 3;
         const uint32_t row_in_tile = half * 64 + wq * 16 + (lane >> 2);   // this thread's first row; the second is 8 below
@@ -233,134 +296,224 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         // Every wgmma is issued at the kernel's full width kN, with no condition around it (a conditional wgmma cannot stay in
         // the asynchronous pipeline): columns past a layer's n_pad and K-steps past its k_steps read the zero tile at w_zero
         // instead (a piece that straddles n_pad reads up to 48 rows past its tile, which the zero tile behind the image also
-        // covers); the epilogue ignores those columns.
+        // covers); the epilogue ignores those columns.  With kLastN = 16 the last layer is issued 16 wide.
         const uint32_t w_zero = w_base + P.zero_off;
         auto b_desc = [](uint32_t t, int c0) { return make_smem_desc(t + (uint32_t)c0 / 8 * 256, 128, 256, GMMA_LAYOUT_NONE); };
-        uint32_t acc[kN / 2];
-        uint32_t afr[kN / 8];          // next layer's A fragments: 4 registers per K-step of 32
+        uint32_t acc[kSlots][kN / 2];
+        uint32_t afr[kSlots][kN / 8];          // next layer's A fragments: 4 registers per K-step of 32
+        BNM_TRACE_DECL(cw, wq == 0 && lane == 0);
+
+        // ---- layer 1 into a (A: the SW128 image in stage s, this warpgroup's 64 rows start 8 KB in for the lower half)
+        auto issue_layer1 = [&](uint32_t *a, uint32_t s) {
+            const uint64_t a0 = make_smem_desc(smem_base + s * P.stage_bytes + half * 8192, 16, 1024, GMMA_LAYOUT_SW128);
+            const uint32_t n_pad = P.n_pad[0], k_steps = P.k_steps[0];
+            BNM_TRACE(TR_ISSUE, 0, 0);
+            wgmma_fence();
 #pragma unroll 1
-        for (uint32_t i = pipe; i < my_tiles; i += kPipes) {
-            const uint32_t s = stage_of(i);
+            for (uint32_t pl = 0; pl < P.planes[0]; pl++)
+#pragma unroll 1
+                for (uint32_t k = 0; k < k_steps; k++) {
+                    // K advance inside a SW128 atom: +32 B (>>4 = 2); next atom: +16384 B (>>4 = 1024).  B: +n_pad x 32 B per K-step
+                    const uint64_t ad = a0 + (uint64_t)((k >> 2) * 1024 + (k & 3) * 2);
+                    const uint32_t bt = w_base + P.b_off[0] + (pl * k_steps + k) * n_pad * 32;
+#pragma unroll
+                    for (int c0 = 0; c0 < kN; c0 += 64)
+                        wgmma_ss_n64(a + c0 / 2, ad, b_desc((uint32_t)c0 < n_pad ? bt : w_zero, c0), (pl | k) != 0);
+                }
+        };
+        // ---- ReLUNorm of layer l's accumulators a into the A fragments f of layer l + 1
+        auto relunorm = [&](const uint32_t *a, uint32_t *f, int l) {
+            const uint32_t n_pad = P.n_pad[l];
+            int m0 = 0, m1 = 0;
+#pragma unroll
+            for (int j = 0; j < kN / 8; j += 2)
+                if ((uint32_t)j * 8 < n_pad) {
+                    m0 = __vimax3_s32(m0, (int)a[4 * j], (int)a[4 * j + 1]);
+                    m1 = __vimax3_s32(m1, (int)a[4 * j + 2], (int)a[4 * j + 3]);
+                    m0 = __vimax3_s32(m0, (int)a[4 * j + 4], (int)a[4 * j + 5]);
+                    m1 = __vimax3_s32(m1, (int)a[4 * j + 6], (int)a[4 * j + 7]);
+                }
+            m0 = max(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
+            m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+            m0 = max(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+            m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+            const NormCoef k0 = norm_coef(m0), k1 = norm_coef(m1);
+            // 16-column block b -> register 2b (upper row) / 2b + 1 (lower row) of the fragments, i.e. for K-step s = b / 2:
+            // f[4s] (upper row, block 2s), f[4s + 1] (lower, 2s), f[4s + 2] (upper, 2s + 1), f[4s + 3] (lower, 2s + 1)
+#pragma unroll
+            for (int b = 0; b < kN / 16; b++) {
+                const int fi = 4 * (b >> 1) + 2 * (b & 1);
+                if ((uint32_t)b * 16 < n_pad) {
+                    f[fi] = norm_pack4(a[8 * b], a[8 * b + 1], a[8 * b + 4], a[8 * b + 5], k0);
+                    f[fi + 1] = norm_pack4(a[8 * b + 2], a[8 * b + 3], a[8 * b + 6], a[8 * b + 7], k1);
+                } else {
+                    f[fi] = 0;
+                    f[fi + 1] = 0;
+                }
+            }
+        };
+        // ---- layer l >= 1 into a (A: the fragments f)
+        auto issue_layer = [&](uint32_t *a, const uint32_t *f, int l) {
+            const uint32_t n_pad = P.n_pad[l], k_steps = P.k_steps[l], b_l = w_base + P.b_off[l];
+            BNM_TRACE(TR_ISSUE, 0, l);
+            wgmma_fence();
+            if (kLastN < kN && l + 1 == n_layers) {
+#pragma unroll 1
+                for (uint32_t pl = 0; pl < P.planes[l]; pl++)
+#pragma unroll
+                    for (int k = 0; k < kN / 32; k++)
+                        wgmma_rs_n16(a, f + 4 * k, b_desc((uint32_t)k < k_steps ? b_l + (pl * k_steps + k) * n_pad * 32 : w_zero, 0), (pl | k) != 0);
+                return;
+            }
+#pragma unroll 1
+            for (uint32_t pl = 0; pl < P.planes[l]; pl++)
+#pragma unroll
+                for (int k = 0; k < kN / 32; k++) {   // unrolled: the fragment index stays a compile-time constant
+                    const uint32_t bt = (uint32_t)k < k_steps ? b_l + (pl * k_steps + k) * n_pad * 32 : w_zero;
+#pragma unroll
+                    for (int c0 = 0; c0 < kN; c0 += 64)
+                        wgmma_rs_n64(a + c0 / 2, f + 4 * k, b_desc((uint32_t)c0 < n_pad ? bt : w_zero, c0), (pl | k) != 0);
+                }
+        };
+        // ---- logits + label of tile i from the last layer's accumulators a (dll.c:115-116: the last ReLUNorm's argmax is what
+        // Inference() returns).  argmax = first maximum (strict '>' from -INT32_MAX, pos 255, inference.c:32-37): in column order
+        // per thread, then over the quad.  The last layer has at most kLastN columns.
+        auto epilogue = [&](const uint32_t *a, uint32_t i) {
+            const uint32_t tile = tile0 + i * tile_step;
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                const size_t img = (size_t)tile * kTileM + row_in_tile + 8 * r;
+                int best = -INT32_MAX;
+                uint32_t pos = 255;
+#pragma unroll
+                for (int j = 0; j < kLastN / 8; j++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const uint32_t col = 8 * j + 2 * quad + e;
+                        const int x = (int)a[4 * j + 2 * r + e];
+                        if (col < ncls && x > best) { best = x; pos = col; }
+                    }
+#pragma unroll
+                for (int sh = 1; sh <= 2; sh <<= 1) {
+                    const int ob = __shfl_xor_sync(0xffffffffu, best, sh);
+                    const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, sh);
+                    if (ob > best || (ob == best && op < pos)) { best = ob; pos = op; }
+                }
+                if (img < P.n) {
+                    auto store_row = [&](int32_t *d) {
+#pragma unroll
+                        for (int j = 0; j < kLastN / 8; j++) {
+                            const uint32_t col = 8 * j + 2 * quad;
+                            if ((ncls & 1) == 0) {   // rows are 8-byte aligned: 64-bit stores
+                                if (col < ncls) *reinterpret_cast<int2 *>(d + col) = make_int2((int)a[4 * j + 2 * r], (int)a[4 * j + 2 * r + 1]);
+                            } else {
+                                if (col < ncls) d[col] = (int)a[4 * j + 2 * r];
+                                if (col + 1 < ncls) d[col + 1] = (int)a[4 * j + 2 * r + 1];
+                            }
+                        }
+                    };
+                    store_row(P.logits + img * ncls);
+#pragma unroll 1
+                    for (uint32_t d = 0; d < P.n_log_dst; d++) store_row(P.log_dst[d] + (P.row0 + img) * ncls);   // peers, over NVLink
+                    if (quad == 0) {
+                        if (P.labels) P.labels[img] = pos;
+#pragma unroll 1
+                        for (uint32_t d = 0; d < P.n_lab_dst; d++) {
+                            if (P.lab_u8) reinterpret_cast<uint8_t *>(P.lab_dst[d])[P.row0 + img] = (uint8_t)pos;
+                            else P.lab_dst[d][P.row0 + img] = pos;
+                        }
+                    }
+                }
+            }
+        };
+        auto wait_full = [&](uint32_t s, uint32_t i, int slot) {   // tile i has landed in stage s
+            BNM_TRACE(TR_FULL_BEGIN, slot, 0);
             mbar_wait(&bar_full[s], round_of(i) & 1, P.err, 2);
-            // ---- layer 1 (A: the SW128 image stage, this warpgroup's 64 rows start 8 KB in for the lower half)
-            {
-                const uint64_t a0 = make_smem_desc(smem_base + s * P.stage_bytes + half * 8192, 16, 1024, GMMA_LAYOUT_SW128);
-                const uint32_t n_pad = P.n_pad[0], k_steps = P.k_steps[0];
-                wgmma_fence();
-#pragma unroll 1
-                for (uint32_t pl = 0; pl < P.planes[0]; pl++)
-#pragma unroll 1
-                    for (uint32_t k = 0; k < k_steps; k++) {
-                        // K advance inside a SW128 atom: +32 B (>>4 = 2); next atom: +16384 B (>>4 = 1024).  B: +n_pad x 32 B per K-step
-                        const uint64_t ad = a0 + (uint64_t)((k >> 2) * 1024 + (k & 3) * 2);
-                        const uint32_t bt = w_base + P.b_off[0] + (pl * k_steps + k) * n_pad * 32;
-#pragma unroll
-                        for (int c0 = 0; c0 < kN; c0 += 64)
-                            wgmma_ss_n64(acc + c0 / 2, ad, b_desc((uint32_t)c0 < n_pad ? bt : w_zero, c0), (pl | k) != 0);
-                    }
-                wgmma_commit();
-                wgmma_wait<0>();
-            }
+            BNM_TRACE(TR_FULL_END, slot, 0);
+        };
+        auto release_stage = [&](uint32_t s) {   // this warp's reads of stage s are complete
             __syncwarp();
-            if (lane == 0) mbar_arrive(&bar_empty[s]);   // this warp's reads of the stage are complete
-            for (int l = 0;; l++) {
-                const uint32_t n_pad = P.n_pad[l];
-                if (l + 1 < n_layers) {
-                    // ---- ReLUNorm of layer l into the A fragments of layer l + 1
-                    int m0 = 0, m1 = 0;
-#pragma unroll
-                    for (int j = 0; j < kN / 8; j += 2)
-                        if ((uint32_t)j * 8 < n_pad) {
-                            m0 = __vimax3_s32(m0, (int)acc[4 * j], (int)acc[4 * j + 1]);
-                            m1 = __vimax3_s32(m1, (int)acc[4 * j + 2], (int)acc[4 * j + 3]);
-                            m0 = __vimax3_s32(m0, (int)acc[4 * j + 4], (int)acc[4 * j + 5]);
-                            m1 = __vimax3_s32(m1, (int)acc[4 * j + 6], (int)acc[4 * j + 7]);
-                        }
-                    m0 = max(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
-                    m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
-                    m0 = max(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-                    m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-                    const NormCoef k0 = norm_coef(m0), k1 = norm_coef(m1);
-                    // 16-column block b -> register 2b (upper row) / 2b + 1 (lower row) of the fragments, i.e. for K-step s = b / 2:
-                    // a[4s] (upper row, block 2s), a[4s + 1] (lower, 2s), a[4s + 2] (upper, 2s + 1), a[4s + 3] (lower, 2s + 1)
-#pragma unroll
-                    for (int b = 0; b < kN / 16; b++) {
-                        const int f = 4 * (b >> 1) + 2 * (b & 1);
-                        if ((uint32_t)b * 16 < n_pad) {
-                            afr[f] = norm_pack4(acc[8 * b], acc[8 * b + 1], acc[8 * b + 4], acc[8 * b + 5], k0);
-                            afr[f + 1] = norm_pack4(acc[8 * b + 2], acc[8 * b + 3], acc[8 * b + 6], acc[8 * b + 7], k1);
-                        } else {
-                            afr[f] = 0;
-                            afr[f + 1] = 0;
-                        }
-                    }
-                    // ---- layer l + 1 (A: registers)
-                    const uint32_t n_next = P.n_pad[l + 1], k_steps = P.k_steps[l + 1], b_l = w_base + P.b_off[l + 1];
-                    wgmma_fence();
+            if (lane == 0) mbar_arrive(&bar_empty[s]);
+        };
+
+        if constexpr (kSlots == 1) {
+            // one tile at a time: every layer's MMAs complete before its ReLUNorm starts
 #pragma unroll 1
-                    for (uint32_t pl = 0; pl < P.planes[l + 1]; pl++)
-#pragma unroll
-                        for (int k = 0; k < kN / 32; k++) {   // unrolled: the fragment index stays a compile-time constant
-                            const uint32_t bt = (uint32_t)k < k_steps ? b_l + (pl * k_steps + k) * n_next * 32 : w_zero;
-#pragma unroll
-                            for (int c0 = 0; c0 < kN; c0 += 64)
-                                wgmma_rs_n64(acc + c0 / 2, afr + 4 * k, b_desc((uint32_t)c0 < n_next ? bt : w_zero, c0), (pl | k) != 0);
-                        }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    continue;
+            for (uint32_t i = pipe; i < my_tiles; i += kPipes) {
+                const uint32_t s = stage_of(i);
+                wait_full(s, i, 0);
+                issue_layer1(acc[0], s);
+                wgmma_commit();
+                BNM_TRACE(TR_WAIT_BEGIN, 0, 0);
+                wgmma_wait<0>();
+                BNM_TRACE(TR_WAIT_END, 0, 0);
+                release_stage(s);
+                for (int l = 0;; l++) {
+                    if (l + 1 < n_layers) {
+                        relunorm(acc[0], afr[0], l);
+                        issue_layer(acc[0], afr[0], l + 1);
+                        wgmma_commit();
+                        BNM_TRACE(TR_WAIT_BEGIN, 0, l + 1);
+                        wgmma_wait<0>();
+                        BNM_TRACE(TR_WAIT_END, 0, l + 1);
+                        continue;
+                    }
+                    epilogue(acc[0], i);
+                    BNM_TRACE(TR_EPI_END, 0, 0);
+                    break;
                 }
-                // ---- logits + label (dll.c:115-116: the last ReLUNorm's argmax is what Inference() returns).  argmax = first
-                // maximum (strict '>' from -INT32_MAX, pos 255, inference.c:32-37): in column order per thread, then over the quad
-                const uint32_t tile = tile0 + i * tile_step;
-#pragma unroll
-                for (int r = 0; r < 2; r++) {
-                    const size_t img = (size_t)tile * kTileM + row_in_tile + 8 * r;
-                    int best = -INT32_MAX;
-                    uint32_t pos = 255;
-#pragma unroll
-                    for (int j = 0; j < kN / 8; j++)
-#pragma unroll
-                        for (int e = 0; e < 2; e++) {
-                            const uint32_t col = 8 * j + 2 * quad + e;
-                            const int x = (int)acc[4 * j + 2 * r + e];
-                            if (col < ncls && x > best) { best = x; pos = col; }
-                        }
-#pragma unroll
-                    for (int sh = 1; sh <= 2; sh <<= 1) {
-                        const int ob = __shfl_xor_sync(0xffffffffu, best, sh);
-                        const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, sh);
-                        if (ob > best || (ob == best && op < pos)) { best = ob; pos = op; }
-                    }
-                    if (img < P.n) {
-                        auto store_row = [&](int32_t *d) {
-#pragma unroll
-                            for (int j = 0; j < kN / 8; j++) {
-                                const uint32_t col = 8 * j + 2 * quad;
-                                if ((ncls & 1) == 0) {   // rows are 8-byte aligned: 64-bit stores
-                                    if (col < ncls) *reinterpret_cast<int2 *>(d + col) = make_int2((int)acc[4 * j + 2 * r], (int)acc[4 * j + 2 * r + 1]);
-                                } else {
-                                    if (col < ncls) d[col] = (int)acc[4 * j + 2 * r];
-                                    if (col + 1 < ncls) d[col + 1] = (int)acc[4 * j + 2 * r + 1];
-                                }
-                            }
-                        };
-                        store_row(P.logits + img * ncls);
-#pragma unroll 1
-                        for (uint32_t d = 0; d < P.n_log_dst; d++) store_row(P.log_dst[d] + (P.row0 + img) * ncls);   // peers, over NVLink
-                        if (quad == 0) {
-                            if (P.labels) P.labels[img] = pos;
-#pragma unroll 1
-                            for (uint32_t d = 0; d < P.n_lab_dst; d++) {
-                                if (P.lab_u8) reinterpret_cast<uint8_t *>(P.lab_dst[d])[P.row0 + img] = (uint8_t)pos;
-                                else P.lab_dst[d][P.row0 + img] = pos;
-                            }
-                        }
-                    }
-                }
-                break;
             }
+        } else {
+            // two slots, stepped alternately.  Each step of slot x commits exactly one wgmma group (empty once x has no tile left),
+            // so the older of the two groups in flight is always x's and wait_group 1 means "x's MMAs are complete".  A step then
+            // runs x's ReLUNorm and issues its next layer, or, after the last layer, x's epilogue and the layer 1 of the pipe's
+            // next tile -- all while the other slot's group is in flight.
+            uint32_t ti[kSlots];   // tile of slot x (>= my_tiles: none left)
+            int ly[kSlots];        // its layer in flight
+            uint32_t next = pipe;  // next tile of this pipe to take
+#pragma unroll
+            for (int x = 0; x < kSlots; x++) {
+                ti[x] = next;
+                ly[x] = 0;
+                next += kPipes;
+                if (ti[x] < my_tiles) {
+                    wait_full(stage_of(ti[x]), ti[x], x);
+                    issue_layer1(acc[x], stage_of(ti[x]));
+                }
+                wgmma_commit();
+            }
+#pragma unroll 1
+            while (ti[0] < my_tiles || ti[1] < my_tiles) {
+#pragma unroll
+                for (int x = 0; x < kSlots; x++) {
+                    BNM_TRACE(TR_WAIT_BEGIN, x, ly[x]);
+                    wgmma_wait<kSlots - 1>();
+                    BNM_TRACE(TR_WAIT_END, x, ly[x]);
+                    if (ti[x] < my_tiles) {
+                        if (ly[x] == 0) release_stage(stage_of(ti[x]));
+                        if (ly[x] + 1 < n_layers) {
+                            relunorm(acc[x], afr[x], ly[x]);
+                            ly[x]++;
+                            issue_layer(acc[x], afr[x], ly[x]);
+                        } else {
+                            epilogue(acc[x], ti[x]);
+                            BNM_TRACE(TR_EPI_END, x, 0);
+                            ti[x] = next;
+                            ly[x] = 0;
+                            next += kPipes;
+                            if (ti[x] < my_tiles) {
+                                wait_full(stage_of(ti[x]), ti[x], x);
+                                issue_layer1(acc[x], stage_of(ti[x]));
+                            }
+                        }
+                    }
+                    wgmma_commit();
+                }
+            }
+            wgmma_wait<0>();
         }
+        BNM_TRACE_END();
+        BNM_TRACE_STAMP(1);
     } else if (kFloatIn) {
         // ======================= quantiser warps (float input): warp qw converts rows 16 qw .. 16 qw + 15 of every tile =======================
         // The input scaling of the reference's caller (test_inference.py:140-141: scale = 127 / max(max|x|, 1e-5), q = round-half-even
@@ -460,18 +613,47 @@ static EncodeTiledFn get_encode_fn() {
 
 static uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
-template <int kN, int kPipes, bool kFloatIn>
-static cudaError_t launch_chain(const cudaLaunchConfig_t &cfg, const CUtensorMap &tmap, const ChainParams &p) {
-    return cudaLaunchKernelEx(&cfg, fc_chain_kernel<kN, kPipes, kFloatIn>, tmap, p);
+#ifdef BNM_FC_TRACE
+// diagnostics build: with BNM_FC_TRACE_OUT set, every launch clears the trace buffer first and writes it to that file after the
+// kernel has completed (the layout of FcTrace, preceded by kTraceCtas, kTraceWriters, kTraceEvents as three uint32)
+static void trace_before(cudaStream_t st) {
+    void *d = nullptr;
+    if (getenv("BNM_FC_TRACE_OUT") && cudaGetSymbolAddress(&d, g_fc_trace) == cudaSuccess) cudaMemsetAsync(d, 0, sizeof(FcTrace), st);
 }
-template <int kN, int kPipes, bool kFloatIn>
+static void trace_after(cudaStream_t st) {
+    const char *path = getenv("BNM_FC_TRACE_OUT");
+    if (!path || cudaStreamSynchronize(st) != cudaSuccess) return;
+    std::vector<uint8_t> buf(sizeof(FcTrace));
+    if (cudaMemcpyFromSymbol(buf.data(), g_fc_trace, sizeof(FcTrace)) != cudaSuccess) return;
+    if (FILE *f = fopen(path, "wb")) {
+        const uint32_t dims[3] = {kTraceCtas, kTraceWriters, kTraceEvents};
+        fwrite(dims, sizeof(dims), 1, f);
+        fwrite(buf.data(), buf.size(), 1, f);
+        fclose(f);
+    }
+}
+#else
+static void trace_before(cudaStream_t) {}
+static void trace_after(cudaStream_t) {}
+#endif
+
+template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN>
+static cudaError_t launch_chain(cudaLaunchConfig_t cfg, const CUtensorMap &tmap, const ChainParams &p) {
+    cfg.blockDim = dim3(chain_threads<kN, kPipes, kFloatIn, kSlots>());
+    return cudaLaunchKernelEx(&cfg, fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN>, tmap, p);
+}
+template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN>
 static bool opt_in_smem(int bytes) {
-    return cudaFuncSetAttribute(fc_chain_kernel<kN, kPipes, kFloatIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess;
+    return cudaFuncSetAttribute(fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                bytes) == cudaSuccess;
 }
 
 static cudaError_t dispatch(const FcChainPlan *plan, bool float_in, const cudaLaunchConfig_t &cfg, const CUtensorMap &tmap, const ChainParams &p) {
     if (float_in) return launch_chain<64, 1, true>(cfg, tmap, p);   // plans of wider models have no float-input form
-    if (plan->max_n == 64) return plan->pipes == 2 ? launch_chain<64, 2, false>(cfg, tmap, p) : launch_chain<64, 1, false>(cfg, tmap, p);
+    if (plan->max_n == 64) {
+        if (plan->pipes == 1) return launch_chain<64, 1, false>(cfg, tmap, p);
+        return plan->last_n == 16 ? launch_chain<64, 2, false, 2, 16>(cfg, tmap, p) : launch_chain<64, 2, false, 2>(cfg, tmap, p);
+    }
     if (plan->max_n == 128) return launch_chain<128, 1, false>(cfg, tmap, p);
     if (plan->max_n == 192) return launch_chain<192, 1, false>(cfg, tmap, p);
     return launch_chain<256, 1, false>(cfg, tmap, p);
@@ -513,7 +695,8 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     if (w_fixed + 2 * p.stage_bytes > smem_limit) { delete plan; return fail("fused path: weights do not fit in shared memory"); }
     const uint32_t total_stages = std::min<uint32_t>(kMaxStages, (smem_limit - w_fixed) / p.stage_bytes);
     plan->pipes = (plan->max_n == 64 && total_stages >= 4) ? 2 : 1;
-    p.n_stages = std::min<uint32_t>(total_stages / plan->pipes, 6);
+    p.n_stages = std::min<uint32_t>(total_stages / plan->pipes, 6);   // >= 2 with two pipes: two tile slots need it
+    plan->last_n = layers[n_layers - 1].n_pad <= 16 ? 16 : plan->max_n;
     p.off_w = plan->pipes * p.n_stages * p.stage_bytes;
     // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared memory
     // enforces it once a CTA asks for more than half of the SM's 227 kB.
@@ -556,7 +739,8 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     p.w_image = plan->d_w_image;
     p.err = plan->d_err;
     const int smem_any = (int)std::max(plan->smem_bytes, plan->f_smem_bytes);
-    if (!opt_in_smem<64, 1, false>(smem_any) || !opt_in_smem<64, 2, false>(smem_any) || !opt_in_smem<128, 1, false>(smem_any) ||
+    if (!opt_in_smem<64, 1, false>(smem_any) || !opt_in_smem<64, 2, false, 2>(smem_any) || !opt_in_smem<64, 2, false, 2, 16>(smem_any) ||
+        !opt_in_smem<128, 1, false>(smem_any) ||
         !opt_in_smem<192, 1, false>(smem_any) || !opt_in_smem<256, 1, false>(smem_any) || !opt_in_smem<64, 1, true>(smem_any)) {
         fc_chain_plan_destroy(plan);
         return fail("cannot opt in to the required dynamic shared memory");
@@ -633,8 +817,7 @@ int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logi
     plan->prev_in = in; plan->prev_logits = logits; plan->prev_labels = labels; plan->prev_stream = st; plan->prev_valid = true;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(plan->max_n == 256 ? 384 : plan->pipes * 256 + 32);   // chain_threads()
+    cfg.gridDim = dim3(grid);   // blockDim: launch_chain (chain_threads of the instantiation)
     cfg.dynamicSmemBytes = plan->smem_bytes;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -642,7 +825,9 @@ int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logi
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = plan->overlap ? 1 : 0;
+    trace_before(st);
     if (dispatch(plan, false, cfg, *tmap_p, p) != cudaSuccess) return -4;
+    trace_after(st);
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 
@@ -675,7 +860,6 @@ int fc_chain_launch_f32(FcChainPlan *plan, const float *in, size_t n, int32_t *l
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)std::min<uint32_t>(p.n_tiles, (uint32_t)plan->sm_count));
-    cfg.blockDim = dim3(256 + 32 + 32 * kFloatQuantWarps);   // two consumer warpgroups + producer warp + the quantiser warps
     cfg.dynamicSmemBytes = plan->f_smem_bytes;
     cfg.stream = st;
     plan->prev_valid = false;
