@@ -78,6 +78,7 @@ struct FcChainPlan {
     uint32_t max_n = 0;               // accumulator width the kernel is instantiated for: 64, 128, 192 or 256 columns
     uint32_t pipes = 1;
     uint32_t last_n = 0;              // wgmma width of the last layer in two-slot launches: 16 when it is at most 16 wide, else max_n
+    bool fixed = false;               // the plan is of the fixed-shape kernel's class (kFixed)
     int sm_count = 0;
     int device = 0;
     int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 plain launch, 1 dependent launch + wait, 2 independent launches
@@ -204,13 +205,30 @@ __host__ __device__ constexpr int chain_threads() {
 // allocated in steps of 8 per thread
 __host__ __device__ constexpr int launch_regs(int threads) { return 16384 / (32 * ((threads / 32 + 3) / 4)) / 8 * 8; }
 
+// The shape class of the fixed-shape kernel (kFixed): 256-byte input rows (two SW128 atoms, eight layer-1 K-steps), three
+// 64-wide layers and a classes layer at most 16 wide, one weight plane each -- FC 4bitsym-64, Ternary-64 and the other 64-wide
+// models.  Every layer's shape and its place in the weight image are compile-time constants of that kernel.
+constexpr int kFixedLayers = 4;
+constexpr uint32_t kFixedInAtoms = 2;
+__host__ __device__ constexpr uint32_t fixed_n_pad(int l) { return l + 1 < kFixedLayers ? 64u : 16u; }
+__host__ __device__ constexpr uint32_t fixed_k_steps(int l) { return l == 0 ? kFixedInAtoms * 4 : 2u; }
+__host__ __device__ constexpr uint32_t fixed_b_off(int l) { return l == 0 ? 0u : fixed_b_off(l - 1) + fixed_k_steps(l - 1) * fixed_n_pad(l - 1) * 32; }
+// a shared-memory descriptor advanced by `units` x 16 bytes: the 14-bit start field of an address inside the CTA's shared memory
+// does not carry into the fields above it, so a 32-bit add of the low word is enough
+__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t units) {
+    return (d & 0xFFFFFFFF00000000ull) | (uint32_t)((uint32_t)d + units);
+}
+
 // kSlots: tiles per consumer warpgroup in compute at once (1 or 2; 2 only for 64-wide int8 launches with two pipes).
 // kLastN: wgmma width of the last layer -- 16 when the plan's last layer is at most 16 wide (every classifier head), else kN.
-template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN>
+// kFixed: the two-slot kernel specialised for the shape class above: no plane loop, no zero-tile selects, layer 1 issued as
+// one unrolled run of MMAs at compile-time descriptor offsets, ReLUNorm without predicates, ring position without divisions.
+template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
 __global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn, kSlots>(), 1)
 fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
     static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
+    static_assert(!kFixed || (kSlots == 2 && kLastN == fixed_n_pad(kFixedLayers - 1)), "fixed shape: two-slot launches of its class");
     constexpr bool kProducerWG = producer_warpgroup<kN, kSlots>();
     constexpr uint32_t kProducerRegs = kN == 256 ? 56 : 32, kConsumerRegs = kN == 256 ? 224 : 112;
     static_assert(!kProducerWG || 128 * kProducerRegs + 256 * kPipes * kConsumerRegs <=
@@ -289,7 +307,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         const uint32_t cw = warp >> 2, pipe = cw >> 1, half = cw & 1, wq = warp & 3;
         const uint32_t quad = lane & 3;
         const uint32_t row_in_tile = half * 64 + wq * 16 + (lane >> 2);   // this thread's first row; the second is 8 below
-        const int n_layers = P.n_layers;
+        const int n_layers = kFixed ? kFixedLayers : P.n_layers;
         const uint32_t ncls = P.n_classes;
         mbar_wait(&bar_w, 0, P.err, 6);   // weight tiles are in shared memory
         // B descriptor of the 64 columns from c0 of the K-step tile at smem address t (no-swizzle K-major: 8-row groups 256 B apart).
@@ -302,9 +320,22 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         uint32_t acc[kSlots][kN / 2];
         uint32_t afr[kSlots][kN / 8];          // next layer's A fragments: 4 registers per K-step of 32
         BNM_TRACE_DECL(cw, wq == 0 && lane == 0);
+        // kFixed: descriptors of stage 0 of this warpgroup's rows and of the weight image; every MMA adds a compile-time offset
+        // (and the stage's) to them.  No layer of the class has padded K-steps or columns, so the zero tile is never read.
+        const uint64_t a_base = make_smem_desc(smem_base + half * 8192, 16, 1024, GMMA_LAYOUT_SW128);
+        const uint64_t w_desc = b_desc(w_base, 0);
 
         // ---- layer 1 into a (A: the SW128 image in stage s, this warpgroup's 64 rows start 8 KB in for the lower half)
         auto issue_layer1 = [&](uint32_t *a, uint32_t s) {
+            if constexpr (kFixed) {
+                const uint32_t a_s = s * (kFixedInAtoms * 16384 / 16);
+                BNM_TRACE(TR_ISSUE, 0, 0);
+                wgmma_fence();
+#pragma unroll
+                for (uint32_t k = 0; k < fixed_k_steps(0); k++)
+                    wgmma_ss_n64(a, desc_add(a_base, a_s + (k >> 2) * 1024 + (k & 3) * 2), desc_add(w_desc, k * fixed_n_pad(0) * 32 / 16), k != 0);
+                return;
+            }
             const uint64_t a0 = make_smem_desc(smem_base + s * P.stage_bytes + half * 8192, 16, 1024, GMMA_LAYOUT_SW128);
             const uint32_t n_pad = P.n_pad[0], k_steps = P.k_steps[0];
             BNM_TRACE(TR_ISSUE, 0, 0);
@@ -323,7 +354,8 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         };
         // ---- ReLUNorm of layer l's accumulators a into the A fragments f of layer l + 1
         auto relunorm = [&](const uint32_t *a, uint32_t *f, int l) {
-            const uint32_t n_pad = P.n_pad[l];
+            // kFixed: every layer with a ReLUNorm (all but the last) is 64 wide, so every block is taken, with no predicates
+            const uint32_t n_pad = kFixed ? fixed_n_pad(0) : P.n_pad[l];
             int m0 = 0, m1 = 0;
 #pragma unroll
             for (int j = 0; j < kN / 8; j += 2)
@@ -354,6 +386,23 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         };
         // ---- layer l >= 1 into a (A: the fragments f)
         auto issue_layer = [&](uint32_t *a, const uint32_t *f, int l) {
+            if constexpr (kFixed) {
+                // layers 2 .. 4 take 2 K-steps each, and the 64-wide layers 2 and 3 are of equal size in the weight image
+                static_assert(fixed_b_off(3) == fixed_b_off(1) + 2 * fixed_k_steps(1) * fixed_n_pad(1) * 32, "kFixed weight image");
+                const uint32_t b_l = (fixed_b_off(1) + (uint32_t)(l - 1) * fixed_k_steps(1) * fixed_n_pad(1) * 32) / 16;
+                BNM_TRACE(TR_ISSUE, 0, l);
+                wgmma_fence();
+                if (l + 1 == kFixedLayers) {
+#pragma unroll
+                    for (uint32_t k = 0; k < fixed_k_steps(1); k++)
+                        wgmma_rs_n16(a, f + 4 * k, desc_add(w_desc, b_l + k * fixed_n_pad(kFixedLayers - 1) * 32 / 16), k != 0);
+                } else {
+#pragma unroll
+                    for (uint32_t k = 0; k < fixed_k_steps(1); k++)
+                        wgmma_rs_n64(a, f + 4 * k, desc_add(w_desc, b_l + k * fixed_n_pad(1) * 32 / 16), k != 0);
+                }
+                return;
+            }
             const uint32_t n_pad = P.n_pad[l], k_steps = P.k_steps[l], b_l = w_base + P.b_off[l];
             BNM_TRACE(TR_ISSUE, 0, l);
             wgmma_fence();
@@ -426,9 +475,9 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                 }
             }
         };
-        auto wait_full = [&](uint32_t s, uint32_t i, int slot) {   // tile i has landed in stage s
+        auto wait_full = [&](uint32_t s, uint32_t parity, int slot) {   // the tile of ring phase `parity` has landed in stage s
             BNM_TRACE(TR_FULL_BEGIN, slot, 0);
-            mbar_wait(&bar_full[s], round_of(i) & 1, P.err, 2);
+            mbar_wait(&bar_full[s], parity, P.err, 2);
             BNM_TRACE(TR_FULL_END, slot, 0);
         };
         auto release_stage = [&](uint32_t s) {   // this warp's reads of stage s are complete
@@ -441,7 +490,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
 #pragma unroll 1
             for (uint32_t i = pipe; i < my_tiles; i += kPipes) {
                 const uint32_t s = stage_of(i);
-                wait_full(s, i, 0);
+                wait_full(s, round_of(i) & 1, 0);
                 issue_layer1(acc[0], s);
                 wgmma_commit();
                 BNM_TRACE(TR_WAIT_BEGIN, 0, 0);
@@ -471,14 +520,28 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
             uint32_t ti[kSlots];   // tile of slot x (>= my_tiles: none left)
             int ly[kSlots];        // its layer in flight
             uint32_t next = pipe;  // next tile of this pipe to take
+            // kFixed: the ring position of the pipe's next tile as running counters (stage inside the pipe, phase parity), and
+            // the stage and phase of each slot's tile, instead of a division by the stage count per tile
+            uint32_t ring_s = 0, ring_ph = 0, st[kSlots], ph[kSlots];
+            auto take_ring = [&](int x) {
+                st[x] = pipe * n_st + ring_s;
+                ph[x] = ring_ph;
+                if (++ring_s == n_st) {
+                    ring_s = 0;
+                    ring_ph ^= 1;
+                }
+            };
+            auto stage_x = [&](int x) { return kFixed ? st[x] : stage_of(ti[x]); };
+            auto phase_x = [&](int x) { return kFixed ? ph[x] : round_of(ti[x]) & 1; };
 #pragma unroll
             for (int x = 0; x < kSlots; x++) {
                 ti[x] = next;
                 ly[x] = 0;
                 next += kPipes;
+                if constexpr (kFixed) take_ring(x);
                 if (ti[x] < my_tiles) {
-                    wait_full(stage_of(ti[x]), ti[x], x);
-                    issue_layer1(acc[x], stage_of(ti[x]));
+                    wait_full(stage_x(x), phase_x(x), x);
+                    issue_layer1(acc[x], stage_x(x));
                 }
                 wgmma_commit();
             }
@@ -490,7 +553,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                     wgmma_wait<kSlots - 1>();
                     BNM_TRACE(TR_WAIT_END, x, ly[x]);
                     if (ti[x] < my_tiles) {
-                        if (ly[x] == 0) release_stage(stage_of(ti[x]));
+                        if (ly[x] == 0) release_stage(stage_x(x));
                         if (ly[x] + 1 < n_layers) {
                             relunorm(acc[x], afr[x], ly[x]);
                             ly[x]++;
@@ -501,9 +564,10 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                             ti[x] = next;
                             ly[x] = 0;
                             next += kPipes;
+                            if constexpr (kFixed) take_ring(x);
                             if (ti[x] < my_tiles) {
-                                wait_full(stage_of(ti[x]), ti[x], x);
-                                issue_layer1(acc[x], stage_of(ti[x]));
+                                wait_full(stage_x(x), phase_x(x), x);
+                                issue_layer1(acc[x], stage_x(x));
                             }
                         }
                     }
@@ -637,19 +701,20 @@ static void trace_before(cudaStream_t) {}
 static void trace_after(cudaStream_t) {}
 #endif
 
-template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN>
+template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
 static cudaError_t launch_chain(cudaLaunchConfig_t cfg, const CUtensorMap &tmap, const ChainParams &p) {
     cfg.blockDim = dim3(chain_threads<kN, kPipes, kFloatIn, kSlots>());
-    return cudaLaunchKernelEx(&cfg, fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN>, tmap, p);
+    return cudaLaunchKernelEx(&cfg, fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed>, tmap, p);
 }
-template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN>
+template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
 static bool opt_in_smem(int bytes) {
-    return cudaFuncSetAttribute(fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    return cudaFuncSetAttribute(fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 bytes) == cudaSuccess;
 }
 
 static cudaError_t dispatch(const FcChainPlan *plan, bool float_in, const cudaLaunchConfig_t &cfg, const CUtensorMap &tmap, const ChainParams &p) {
     if (float_in) return launch_chain<64, 1, true>(cfg, tmap, p);   // plans of wider models have no float-input form
+    if (plan->fixed) return launch_chain<64, 2, false, 2, 16, true>(cfg, tmap, p);
     if (plan->max_n == 64) {
         if (plan->pipes == 1) return launch_chain<64, 1, false>(cfg, tmap, p);
         return plan->last_n == 16 ? launch_chain<64, 2, false, 2, 16>(cfg, tmap, p) : launch_chain<64, 2, false, 2>(cfg, tmap, p);
@@ -697,6 +762,10 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     plan->pipes = (plan->max_n == 64 && total_stages >= 4) ? 2 : 1;
     p.n_stages = std::min<uint32_t>(total_stages / plan->pipes, 6);   // >= 2 with two pipes: two tile slots need it
     plan->last_n = layers[n_layers - 1].n_pad <= 16 ? 16 : plan->max_n;
+    // the fixed-shape kernel for plans of exactly its class (kFixedLayers and the fixed_* shapes)
+    plan->fixed = plan->pipes == 2 && plan->last_n == 16 && n_layers == kFixedLayers && p.in_atoms == kFixedInAtoms;
+    for (int l = 0; l < n_layers && plan->fixed; l++)
+        plan->fixed = p.planes[l] == 1 && p.n_pad[l] == fixed_n_pad(l) && p.k_steps[l] == fixed_k_steps(l) && p.b_off[l] == fixed_b_off(l);
     p.off_w = plan->pipes * p.n_stages * p.stage_bytes;
     // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared memory
     // enforces it once a CTA asks for more than half of the SM's 227 kB.
@@ -713,8 +782,9 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
         }
     }
     if (getenv("BNM_VERBOSE"))   // diagnostics: the shapes this plan launches
-        fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem\n",
-                plan->max_n, plan->pipes, p.n_stages, p.w_bytes, plan->smem_bytes);
+        fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, %s\n",
+                plan->max_n, plan->pipes, p.n_stages, p.w_bytes, plan->smem_bytes,
+                plan->fixed ? "two slots, fixed shape" : plan->pipes == 2 ? "two slots" : "one slot");
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
     plan->device = device;
@@ -740,7 +810,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     p.err = plan->d_err;
     const int smem_any = (int)std::max(plan->smem_bytes, plan->f_smem_bytes);
     if (!opt_in_smem<64, 1, false>(smem_any) || !opt_in_smem<64, 2, false, 2>(smem_any) || !opt_in_smem<64, 2, false, 2, 16>(smem_any) ||
-        !opt_in_smem<128, 1, false>(smem_any) ||
+        !opt_in_smem<64, 2, false, 2, 16, true>(smem_any) || !opt_in_smem<128, 1, false>(smem_any) ||
         !opt_in_smem<192, 1, false>(smem_any) || !opt_in_smem<256, 1, false>(smem_any) || !opt_in_smem<64, 1, true>(smem_any)) {
         fc_chain_plan_destroy(plan);
         return fail("cannot opt in to the required dynamic shared memory");
