@@ -372,20 +372,12 @@ bool launch_cnn_frontend_tc(const int8_t *images, const int8_t *w1, const int8_t
     if (!smem) return false;
     p.images = images; p.w1 = w1; p.w2 = w2; p.w3 = w3; p.feats = features; p.feat_stride = feat_stride; p.n = n;
     p.n_groups = (n + p.G - 1) / p.G;
-    static size_t granted = 0;
-    if (smem > granted) {
-        if (cudaFuncSetAttribute(k_cnn_frontend16_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-            cudaFuncSetAttribute(k_cnn_frontend16_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-            cudaGetLastError();   // not sticky: leave no stale error behind for the caller's launch check
-            return false;
-        }
-        granted = smem;
-    }
+    auto *kernel = conv3_fits_u16 ? k_cnn_frontend16_tc<true> : k_cnn_frontend16_tc<false>;
+    if (!raise_smem_limit((const void *)kernel, smem)) return false;
     // as many resident CTAs as shared memory allows, persistent over the groups
     const size_t per_sm = std::max<size_t>(1, (227 * 1024) / (smem + 1024));
     const unsigned grid = (unsigned)std::min<size_t>(p.n_groups, (size_t)sm_count * per_sm);
-    if (conv3_fits_u16) k_cnn_frontend16_tc<true><<<grid, 128, smem, st>>>(p);
-    else k_cnn_frontend16_tc<false><<<grid, 128, smem, st>>>(p);
+    kernel<<<grid, 128, smem, st>>>(p);
     return true;
 }
 

@@ -18,6 +18,7 @@
 // work of ReLUNorm, which bounds this kernel.  Weights of every encoding are pre-decoded once per model into int8 planes
 // (kernels.h FcLayerDev); FP130's +128 does not fit s8 and is carried by a second residual plane accumulated into the same D.
 // All arithmetic is integer: results are bit-exact with the reference.
+#include <array>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -68,6 +69,8 @@ struct ChainParams {
     uint32_t off_fring;               // float-input launches: smem offset of the quantiser warps' float rings (8 warps x 2 slots x 4 kB)
 };
 
+struct ChainKernel;
+
 struct FcChainPlan {
     ChainParams p{};
     uint8_t *d_w_image = nullptr;
@@ -75,10 +78,8 @@ struct FcChainPlan {
     int *h_err = nullptr;
     size_t smem_bytes = 0;
     uint32_t in_bytes = 0;
-    uint32_t max_n = 0;               // accumulator width the kernel is instantiated for: 64, 128, 192 or 256 columns
-    uint32_t pipes = 1;
-    uint32_t last_n = 0;              // wgmma width of the last layer in two-slot launches: 16 when it is at most 16 wide, else max_n
-    bool fixed = false;               // the plan is of the fixed-shape kernel's class (kFixed)
+    const ChainKernel *kernel = nullptr;       // the instantiation of int8 launches
+    const ChainKernel *kernel_f32 = nullptr;   // and of float-input launches (null: not supported)
     int sm_count = 0;
     int device = 0;
     int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 plain launch, 1 dependent launch + wait, 2 independent launches
@@ -219,14 +220,27 @@ __device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t units) {
     return (d & 0xFFFFFFFF00000000ull) | (uint32_t)((uint32_t)d + units);
 }
 
+// Ring position of a pipe's next tile: its stage inside the pipe and the parity of its ring round.  Every role visits the tiles
+// of a pipe in order and advances the position once per tile, so no role divides by the stage count.  Both live in one word:
+// with two, the one-slot kernels need up to two more registers.
+struct RingPos {
+    uint32_t word = 0;   // stage | phase << 31
+    __device__ __forceinline__ uint32_t stage() const { return word & 0x7fffffffu; }
+    __device__ __forceinline__ uint32_t phase() const { return word >> 31; }
+    __device__ __forceinline__ void advance(uint32_t n_st) {
+        if ((++word & 0x7fffffffu) == n_st) word = (word & 0x80000000u) ^ 0x80000000u;
+    }
+};
+
 // kSlots: tiles per consumer warpgroup in compute at once (1 or 2; 2 only for 64-wide int8 launches with two pipes).
 // kLastN: wgmma width of the last layer -- 16 when the plan's last layer is at most 16 wide (every classifier head), else kN.
 // kFixed: the two-slot kernel specialised for the shape class above: no plane loop, no zero-tile selects, layer 1 issued as
-// one unrolled run of MMAs at compile-time descriptor offsets, ReLUNorm without predicates, ring position without divisions.
+// one unrolled run of MMAs at compile-time descriptor offsets, ReLUNorm without predicates.
 template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
 __global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn, kSlots>(), 1)
 fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
+    static_assert(!kFloatIn || kPipes == 1, "float input: one pipe, whose stages the quantiser warps fill");
     static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
     static_assert(!kFixed || (kSlots == 2 && kLastN == fixed_n_pad(kFixedLayers - 1)), "fixed shape: two-slot launches of its class");
     constexpr bool kProducerWG = producer_warpgroup<kN, kSlots>();
@@ -258,8 +272,6 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
     // tile i of this CTA: pipe i % kPipes, j-th tile of that pipe, stage (pipe, j % n_st), ring round j / n_st.
     // Two slots: a warpgroup waits for tile j + 1 of its pipe before it releases the stage of tile j (slot B's layer 1 is issued
     // before slot A's completes), so a pipe needs at least two stages -- every two-pipe plan has them (fc_chain_plan_create).
-    auto stage_of = [&](uint32_t i) { return (i % kPipes) * n_st + (i / kPipes) % n_st; };
-    auto round_of = [&](uint32_t i) { return (i / kPipes) / n_st; };
 
     if (warp == prod_warp) {
         if (lane < kPipes * n_st) {
@@ -288,15 +300,25 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                 if (P.wait_prior_grid) asm volatile("griddepcontrol.wait;" ::: "memory");
                 const uint64_t l2_policy = policy_evict_first();   // images are read exactly once
                 BNM_TRACE_DECL(kTraceWriters - 1, true);
+                // the pipes take turns, so each pipe's tile is at the same ring position: one position serves them all
+                RingPos ring;
+                uint32_t pipe = 0;
                 for (uint32_t i = 0; i < my_tiles; i++) {
-                    const uint32_t s = stage_of(i), u = round_of(i);
+                    // Only lane 0 runs this loop, so the shuffle names lane 0 alone and returns its own value.  It is kept for
+                    // ptxas: with the stage computed from the counters alone, ptxas (CUDA 12.9) serialises the wgmma pipeline of
+                    // the fixed-shape kernel (remark C7511).
+                    const uint32_t s = __shfl_sync(1u, pipe * n_st + ring.stage(), 0);
                     BNM_TRACE(TR_EMPTY_BEGIN, 0, 0);
-                    if (u > 0) mbar_wait_relaxed(&bar_empty[s], (u - 1) & 1, P.err, 5);
+                    if (i >= kPipes * n_st) mbar_wait_relaxed(&bar_empty[s], ring.phase() ^ 1, P.err, 5);   // past the first round
                     BNM_TRACE(TR_EMPTY_END, 0, 0);
                     mbar_arrive_expect_tx(&bar_full[s], P.stage_bytes);
                     const int32_t row = (int32_t)((tile0 + i * tile_step) * kTileM);
                     for (uint32_t a = 0; a < P.in_atoms; a++)
                         tma_load_2d_hint(smem + s * P.stage_bytes + a * 16384, &tmap_in, (int32_t)(a * 128), row, &bar_full[s], l2_policy);
+                    if (++pipe == kPipes) {
+                        pipe = 0;
+                        ring.advance(n_st);
+                    }
                 }
                 BNM_TRACE_END();
             }
@@ -485,12 +507,15 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
             if (lane == 0) mbar_arrive(&bar_empty[s]);
         };
 
+        RingPos ring;   // ring position of the pipe's next tile
         if constexpr (kSlots == 1) {
-            // one tile at a time: every layer's MMAs complete before its ReLUNorm starts
+            // one tile at a time: every layer's MMAs complete before its ReLUNorm starts.  (The slot loop below would serve one
+            // slot as well, but ptxas gives it about 10 to 20 more registers per one-slot instantiation and spills at kN = 256.)
 #pragma unroll 1
             for (uint32_t i = pipe; i < my_tiles; i += kPipes) {
-                const uint32_t s = stage_of(i);
-                wait_full(s, round_of(i) & 1, 0);
+                const uint32_t s = pipe * n_st + ring.stage();
+                wait_full(s, ring.phase(), 0);
+                ring.advance(n_st);
                 issue_layer1(acc[0], s);
                 wgmma_commit();
                 BNM_TRACE(TR_WAIT_BEGIN, 0, 0);
@@ -519,30 +544,23 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
             // next tile -- all while the other slot's group is in flight.
             uint32_t ti[kSlots];   // tile of slot x (>= my_tiles: none left)
             int ly[kSlots];        // its layer in flight
+            uint32_t st[kSlots], ph[kSlots];   // its stage and ring phase
             uint32_t next = pipe;  // next tile of this pipe to take
-            // kFixed: the ring position of the pipe's next tile as running counters (stage inside the pipe, phase parity), and
-            // the stage and phase of each slot's tile, instead of a division by the stage count per tile
-            uint32_t ring_s = 0, ring_ph = 0, st[kSlots], ph[kSlots];
-            auto take_ring = [&](int x) {
-                st[x] = pipe * n_st + ring_s;
-                ph[x] = ring_ph;
-                if (++ring_s == n_st) {
-                    ring_s = 0;
-                    ring_ph ^= 1;
-                }
-            };
-            auto stage_x = [&](int x) { return kFixed ? st[x] : stage_of(ti[x]); };
-            auto phase_x = [&](int x) { return kFixed ? ph[x] : round_of(ti[x]) & 1; };
-#pragma unroll
-            for (int x = 0; x < kSlots; x++) {
+            auto take_tile = [&](int x) {   // slot x takes the pipe's next tile and, if there is one, issues its layer 1
                 ti[x] = next;
                 ly[x] = 0;
                 next += kPipes;
-                if constexpr (kFixed) take_ring(x);
+                st[x] = pipe * n_st + ring.stage();
+                ph[x] = ring.phase();
+                ring.advance(n_st);
                 if (ti[x] < my_tiles) {
-                    wait_full(stage_x(x), phase_x(x), x);
-                    issue_layer1(acc[x], stage_x(x));
+                    wait_full(st[x], ph[x], x);
+                    issue_layer1(acc[x], st[x]);
                 }
+            };
+#pragma unroll
+            for (int x = 0; x < kSlots; x++) {
+                take_tile(x);
                 wgmma_commit();
             }
 #pragma unroll 1
@@ -553,7 +571,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                     wgmma_wait<kSlots - 1>();
                     BNM_TRACE(TR_WAIT_END, x, ly[x]);
                     if (ti[x] < my_tiles) {
-                        if (ly[x] == 0) release_stage(stage_x(x));
+                        if (ly[x] == 0) release_stage(st[x]);
                         if (ly[x] + 1 < n_layers) {
                             relunorm(acc[x], afr[x], ly[x]);
                             ly[x]++;
@@ -561,14 +579,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                         } else {
                             epilogue(acc[x], ti[x]);
                             BNM_TRACE(TR_EPI_END, x, 0);
-                            ti[x] = next;
-                            ly[x] = 0;
-                            next += kPipes;
-                            if constexpr (kFixed) take_ring(x);
-                            if (ti[x] < my_tiles) {
-                                wait_full(stage_x(x), phase_x(x), x);
-                                issue_layer1(acc[x], stage_x(x));
-                            }
+                            take_tile(x);
                         }
                     }
                     wgmma_commit();
@@ -610,11 +621,13 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         };
         const uint32_t u = lane >> 3, sub = lane & 7;   // row of the pass, position inside the row's eight-lane team
         uint32_t fphase = 0;   // one phase bit per ring slot
+        RingPos pos;           // ring position of the current tile (one pipe)
         if (n_groups > 0) issue_group(0);
         if (n_groups > 1) issue_group(1);
         for (uint32_t gi = 0; gi < n_groups; gi++) {
-            const uint32_t i = gi / kGroupsPerTile, k = gi % kGroupsPerTile, s = stage_of(i), rnd = round_of(i);
-            if (k == 0 && rnd > 0) mbar_wait(&bar_empty[s], (rnd - 1) & 1, P.err, 8);   // the tile that used this stage is through layer 1
+            const uint32_t i = gi / kGroupsPerTile, k = gi % kGroupsPerTile;
+            const uint32_t s = pos.stage();
+            if (k == 0 && i >= n_st) mbar_wait(&bar_empty[s], pos.phase() ^ 1, P.err, 8);   // the tile that used this stage is through layer 1
             uint8_t *stage = smem + s * P.stage_bytes;
             size_t row;
             const uint32_t valid = group_rows(gi, row);
@@ -653,6 +666,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                 fence_proxy_async_smem();   // the layer-1 MMAs (async proxy) read what these generic-proxy stores wrote
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&bar_full[s]);
+                pos.advance(n_st);
             }
         }
     }
@@ -701,28 +715,29 @@ static void trace_before(cudaStream_t) {}
 static void trace_after(cudaStream_t) {}
 #endif
 
+// the instantiations of fc_chain_kernel, one row each, named by their template arguments <kN, kPipes, kSlots, kLastN>
+struct ChainKernel {
+    const char *name;
+    void (*fn)(CUtensorMap, ChainParams);
+    int threads;
+};
 template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
-static cudaError_t launch_chain(cudaLaunchConfig_t cfg, const CUtensorMap &tmap, const ChainParams &p) {
-    cfg.blockDim = dim3(chain_threads<kN, kPipes, kFloatIn, kSlots>());
-    return cudaLaunchKernelEx(&cfg, fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed>, tmap, p);
+static ChainKernel chain_kernel(const char *name) {
+    return {name, fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed>, chain_threads<kN, kPipes, kFloatIn, kSlots>()};
 }
-template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
-static bool opt_in_smem(int bytes) {
-    return cudaFuncSetAttribute(fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                bytes) == cudaSuccess;
-}
-
-static cudaError_t dispatch(const FcChainPlan *plan, bool float_in, const cudaLaunchConfig_t &cfg, const CUtensorMap &tmap, const ChainParams &p) {
-    if (float_in) return launch_chain<64, 1, true>(cfg, tmap, p);   // plans of wider models have no float-input form
-    if (plan->fixed) return launch_chain<64, 2, false, 2, 16, true>(cfg, tmap, p);
-    if (plan->max_n == 64) {
-        if (plan->pipes == 1) return launch_chain<64, 1, false>(cfg, tmap, p);
-        return plan->last_n == 16 ? launch_chain<64, 2, false, 2, 16>(cfg, tmap, p) : launch_chain<64, 2, false, 2>(cfg, tmap, p);
-    }
-    if (plan->max_n == 128) return launch_chain<128, 1, false>(cfg, tmap, p);
-    if (plan->max_n == 192) return launch_chain<192, 1, false>(cfg, tmap, p);
-    return launch_chain<256, 1, false>(cfg, tmap, p);
-}
+enum ChainRow { kRow64, kRow64x2, kRow64x2Last16, kRowFixed, kRow128, kRow192, kRow256, kRowFloat, kChainRows };
+static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
+    std::array<ChainKernel, kChainRows> t{};
+    t[kRow64] = chain_kernel<64, 1, false>("<64,1>");
+    t[kRow64x2] = chain_kernel<64, 2, false, 2>("<64,2,2,64>");
+    t[kRow64x2Last16] = chain_kernel<64, 2, false, 2, 16>("<64,2,2,16>");
+    t[kRowFixed] = chain_kernel<64, 2, false, 2, 16, true>("<64,2,2,16,fixed>");
+    t[kRow128] = chain_kernel<128, 1, false>("<128,1>");
+    t[kRow192] = chain_kernel<192, 1, false>("<192,1>");
+    t[kRow256] = chain_kernel<256, 1, false>("<256,1>");
+    t[kRowFloat] = chain_kernel<64, 1, true>("<64,1,float>");
+    return t;
+}();
 
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
                                   char *err, size_t err_len) {
@@ -751,27 +766,31 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     // the kernel's accumulator width: the widest layer rounded up to the 64-column wgmma pieces.  Accumulator registers per thread
     // = max_n / 2.  Two pipes (four consumer warpgroups, 544 threads: up to five warps share an SM sub-partition, <= 96 registers
     // each) only for models up to 64 wide; wider ones run one pipe (288 threads, <= 168 registers)
-    plan->max_n = round_up(max_n, 64);
+    max_n = round_up(max_n, 64);
     p.zero_off = w_off;                    // [max_n x 32 B] of zeros behind the layers (cudaMemset below)
-    p.w_bytes = w_off + plan->max_n * 32;
+    p.w_bytes = w_off + max_n * 32;
     p.n_classes = layers[n_layers - 1].n_out;
     const uint32_t smem_limit = 227 * 1024 - 1024 /*alignment slack*/ - 1024 /*static: barriers*/;
     const uint32_t w_fixed = round_up(p.w_bytes, 128);
     if (w_fixed + 2 * p.stage_bytes > smem_limit) { delete plan; return fail("fused path: weights do not fit in shared memory"); }
     const uint32_t total_stages = std::min<uint32_t>(kMaxStages, (smem_limit - w_fixed) / p.stage_bytes);
-    plan->pipes = (plan->max_n == 64 && total_stages >= 4) ? 2 : 1;
-    p.n_stages = std::min<uint32_t>(total_stages / plan->pipes, 6);   // >= 2 with two pipes: two tile slots need it
-    plan->last_n = layers[n_layers - 1].n_pad <= 16 ? 16 : plan->max_n;
-    // the fixed-shape kernel for plans of exactly its class (kFixedLayers and the fixed_* shapes)
-    plan->fixed = plan->pipes == 2 && plan->last_n == 16 && n_layers == kFixedLayers && p.in_atoms == kFixedInAtoms;
-    for (int l = 0; l < n_layers && plan->fixed; l++)
-        plan->fixed = p.planes[l] == 1 && p.n_pad[l] == fixed_n_pad(l) && p.k_steps[l] == fixed_k_steps(l) && p.b_off[l] == fixed_b_off(l);
-    p.off_w = plan->pipes * p.n_stages * p.stage_bytes;
+    const uint32_t pipes = (max_n == 64 && total_stages >= 4) ? 2 : 1;
+    p.n_stages = std::min<uint32_t>(total_stages / pipes, 6);   // >= 2 with two pipes: two tile slots need it
+    // two pipes run two slots, which issue a last layer of at most 16 columns 16 wide (kLastN); plans of exactly the fixed
+    // shape class (kFixedLayers and the fixed_* shapes) run the fixed-shape kernel
+    const bool last16 = layers[n_layers - 1].n_pad <= 16;
+    bool fixed = pipes == 2 && last16 && n_layers == kFixedLayers && p.in_atoms == kFixedInAtoms;
+    for (int l = 0; l < n_layers && fixed; l++)
+        fixed = p.planes[l] == 1 && p.n_pad[l] == fixed_n_pad(l) && p.k_steps[l] == fixed_k_steps(l) && p.b_off[l] == fixed_b_off(l);
+    int row = max_n == 64 ? kRow64 : max_n == 128 ? kRow128 : max_n == 192 ? kRow192 : kRow256;
+    if (pipes == 2) row = fixed ? kRowFixed : last16 ? kRow64x2Last16 : kRow64x2;
+    plan->kernel = &kChainKernels[row];
+    p.off_w = pipes * p.n_stages * p.stage_bytes;
     // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared memory
     // enforces it once a CTA asks for more than half of the SM's 227 kB.
     plan->smem_bytes = std::max<size_t>((size_t)p.off_w + w_fixed + 1024, 116 * 1024);
     // float-input path: the eight quantiser warps make 17 warps, so at most 96 registers per thread -- models up to 64 wide
-    if (in_bytes <= 256 && p.n_classes <= 16 && plan->max_n == 64) {
+    if (in_bytes <= 256 && p.n_classes <= 16 && max_n == 64) {
         const uint32_t fring = kFloatQuantWarps * 2 * kFloatGroupRows * 1024;
         const uint32_t fixed_f = w_fixed + fring;
         if (fixed_f + 2 * p.stage_bytes <= smem_limit) {
@@ -779,12 +798,13 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
             plan->f_off_w = plan->f_n_stages * p.stage_bytes;
             plan->f_off_fring = plan->f_off_w + w_fixed;
             plan->f_smem_bytes = std::max<size_t>((size_t)plan->f_off_fring + fring + 1024, 116 * 1024);
+            plan->kernel_f32 = &kChainKernels[kRowFloat];
         }
     }
     if (getenv("BNM_VERBOSE"))   // diagnostics: the shapes this plan launches
-        fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, %s\n",
-                plan->max_n, plan->pipes, p.n_stages, p.w_bytes, plan->smem_bytes,
-                plan->fixed ? "two slots, fixed shape" : plan->pipes == 2 ? "two slots" : "one slot");
+        fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, "
+                "fc_chain_kernel%s%s%s\n", max_n, pipes, p.n_stages, p.w_bytes, plan->smem_bytes, plan->kernel->name,
+                plan->kernel_f32 ? ", float input " : "", plan->kernel_f32 ? plan->kernel_f32->name : "");
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
     plan->device = device;
@@ -808,10 +828,8 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     if (cudaDeviceSynchronize() != cudaSuccess) { fc_chain_plan_destroy(plan); return fail("weight image kernel failed"); }
     p.w_image = plan->d_w_image;
     p.err = plan->d_err;
-    const int smem_any = (int)std::max(plan->smem_bytes, plan->f_smem_bytes);
-    if (!opt_in_smem<64, 1, false>(smem_any) || !opt_in_smem<64, 2, false, 2>(smem_any) || !opt_in_smem<64, 2, false, 2, 16>(smem_any) ||
-        !opt_in_smem<64, 2, false, 2, 16, true>(smem_any) || !opt_in_smem<128, 1, false>(smem_any) ||
-        !opt_in_smem<192, 1, false>(smem_any) || !opt_in_smem<256, 1, false>(smem_any) || !opt_in_smem<64, 1, true>(smem_any)) {
+    if (!raise_smem_limit((const void *)plan->kernel->fn, plan->smem_bytes) ||
+        (plan->kernel_f32 && !raise_smem_limit((const void *)plan->kernel_f32->fn, plan->f_smem_bytes))) {
         fc_chain_plan_destroy(plan);
         return fail("cannot opt in to the required dynamic shared memory");
     }
@@ -852,17 +870,32 @@ static const CUtensorMap *plan_tensor_map(FcChainPlan *plan, const int8_t *in, s
     return &t.map;
 }
 
-int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather,
-                    cudaStream_t st) {
-    if (n == 0) return 0;
-    if (n > 0x7fffff00ull) return -2;
-    ChainParams p = plan->p;
+// the per-launch part of the parameters (outputs, no gather destinations) and the configuration of a launch of kernel k with
+// `smem` bytes of dynamic shared memory: a CTA per tile, at most one per SM
+static cudaLaunchConfig_t launch_setup(const FcChainPlan *plan, const ChainKernel *k, size_t smem, size_t n, int32_t *logits,
+                                       uint32_t *labels, cudaStream_t st, ChainParams &p) {
     p.logits = logits;
     p.labels = labels;
     p.n = n;
     p.n_lab_dst = p.n_log_dst = 0;
     p.row0 = 0;
     p.lab_u8 = 0;
+    p.n_tiles = (uint32_t)((n + kTileM - 1) / kTileM);
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)std::min<uint32_t>(p.n_tiles, (uint32_t)plan->sm_count));
+    cfg.blockDim = dim3(k->threads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    return cfg;
+}
+
+int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather,
+                    cudaStream_t st) {
+    if (n == 0) return 0;
+    if (n > 0x7fffff00ull) return -2;
+    ChainParams p = plan->p;
+    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel, plan->smem_bytes, n, logits, labels, st, p);
     if (gather) {
         if (gather->n_labels_dst > (uint32_t)kMaxGatherDst || gather->n_logits_dst > (uint32_t)kMaxGatherDst) return -5;
         p.n_lab_dst = gather->n_labels_dst;
@@ -873,36 +906,29 @@ int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logi
         for (uint32_t d = 0; d < p.n_lab_dst; d++) p.lab_dst[d] = gather->labels_dst[d];
         for (uint32_t d = 0; d < p.n_log_dst; d++) p.log_dst[d] = gather->logits_dst[d];
     }
-    p.n_tiles = (uint32_t)((n + kTileM - 1) / kTileM);
     const CUtensorMap *tmap_p = plan_tensor_map(plan, in, n);
     if (!tmap_p) return -3;
-    const unsigned grid = (unsigned)std::min<uint32_t>(p.n_tiles, (uint32_t)plan->sm_count);
     // Mode 2 drops the grid-dependency wait, i.e. EVERY ordering against the work enqueued before this launch on the stream
     // (the previous bnm launch and any producer kernel of `images` alike).  The library keeps the wait whenever it can see the
     // promise being broken: first launch on this plan / another stream / a buffer of the previous launch reused.
     bool independent = plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && in != plan->prev_in &&
                        logits != plan->prev_logits && (labels == nullptr || labels != plan->prev_labels);
     p.wait_prior_grid = !independent;
-    p.early_trigger = plan->overlap != 0 && grid == (unsigned)plan->sm_count;
+    p.early_trigger = plan->overlap != 0 && cfg.gridDim.x == (unsigned)plan->sm_count;
     plan->prev_in = in; plan->prev_logits = logits; plan->prev_labels = labels; plan->prev_stream = st; plan->prev_valid = true;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);   // blockDim: launch_chain (chain_threads of the instantiation)
-    cfg.dynamicSmemBytes = plan->smem_bytes;
-    cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = plan->overlap ? 1 : 0;
     trace_before(st);
-    if (dispatch(plan, false, cfg, *tmap_p, p) != cudaSuccess) return -4;
+    if (cudaLaunchKernelEx(&cfg, plan->kernel->fn, *tmap_p, p) != cudaSuccess) return -4;
     trace_after(st);
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 
 bool fc_chain_float_input_supported(const FcChainPlan *plan) {
-    return plan && plan->f_smem_bytes != 0 && plan->in_bytes % 16 == 0;
+    return plan && plan->kernel_f32 && plan->in_bytes % 16 == 0;
 }
 
 // float32 images [n][in_bytes elements] -> logits / labels, the input scaling fused into the load stage (kFloatIn)
@@ -911,29 +937,18 @@ int fc_chain_launch_f32(FcChainPlan *plan, const float *in, size_t n, int32_t *l
     if (n > 0x7fffff00ull) return -2;
     if (!fc_chain_float_input_supported(plan)) return -6;
     ChainParams p = plan->p;
-    p.logits = logits;
-    p.labels = labels;
-    p.n = n;
-    p.n_lab_dst = p.n_log_dst = 0;
-    p.row0 = 0;
-    p.lab_u8 = 0;
+    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_f32, plan->f_smem_bytes, n, logits, labels, st, p);
     p.fimages = in;
     p.in_elems = plan->in_bytes;
     p.n_stages = plan->f_n_stages;
     p.off_w = plan->f_off_w;
     p.off_fring = plan->f_off_fring;
-    p.n_tiles = (uint32_t)((n + kTileM - 1) / kTileM);
     p.wait_prior_grid = 1;
     p.early_trigger = 0;
     CUtensorMap tmap;   // not used by the float-input kernel (no TMA image loads)
     memset(&tmap, 0, sizeof(tmap));
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)std::min<uint32_t>(p.n_tiles, (uint32_t)plan->sm_count));
-    cfg.dynamicSmemBytes = plan->f_smem_bytes;
-    cfg.stream = st;
     plan->prev_valid = false;
-    if (dispatch(plan, true, cfg, tmap, p) != cudaSuccess) return -4;
+    if (cudaLaunchKernelEx(&cfg, plan->kernel_f32->fn, tmap, p) != cudaSuccess) return -4;
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 

@@ -6,6 +6,11 @@
 //   * fused CNN front-end: conv,conv,pool,conv,pool per channel + ReLUNorm        (BitNetMCU_MNIST_dll.c:64-80)
 // These are the layer-by-layer path (BNM_PATH_LAYERS) and the front half of every CNN model; the fused
 // wgmma FC chain lives in fc_wgmma.cu.
+#include <algorithm>
+#include <map>
+#include <mutex>
+#include <utility>
+
 #include "kernels.h"
 
 namespace bnm {
@@ -150,16 +155,29 @@ bool launch_fc_dp4a(const int8_t *act, uint32_t act_stride, const FcLayerDev &L,
     if (smem > 227 * 1024) return false;   // 128 staged rows of more than ~1.8k inputs do not fit an SM
     unsigned grid = (unsigned)((n + 127) / 128);
     uint32_t valid = act_stride < L.k_pad ? act_stride : L.k_pad;
-    static size_t granted[2] = {48 * 1024, 48 * 1024};   // opt-in dynamic shared memory granted so far, per instantiation
-    const int vi = L.dense_b ? 1 : 0;
-    if (smem > granted[vi]) {
-        const cudaError_t e = vi ? cudaFuncSetAttribute(k_fc_dp4a<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                 : cudaFuncSetAttribute(k_fc_dp4a<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { cudaGetLastError(); return false; }
-        granted[vi] = smem;
+    auto *kernel = L.dense_b ? k_fc_dp4a<true> : k_fc_dp4a<false>;
+    if (!raise_smem_limit((const void *)kernel, smem)) return false;
+    kernel<<<grid, 128, smem, st>>>(act, act_stride, valid, L.quad_a, L.dense_b ? L.quad_b : L.quad_a, k4n, L.n_out, L.n_pad, out, n);
+    return true;
+}
+
+bool raise_smem_limit(const void *kernel, size_t bytes) {
+    static std::mutex mu;   // a concurrent raise to fewer bytes must not undo one to more
+    static std::map<std::pair<int, const void *>, size_t> known;   // (device, kernel) -> a limit it is known to have
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return false; }
+    std::lock_guard<std::mutex> lock(mu);
+    size_t &limit = known[{dev, kernel}];
+    if (bytes <= limit) return true;
+    cudaFuncAttributes a;
+    cudaError_t e = cudaFuncGetAttributes(&a, kernel);
+    if (e == cudaSuccess && bytes > (size_t)a.maxDynamicSharedSizeBytes)
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();   // not sticky: leave no stale error behind for the caller's launch check
+        return false;
     }
-    if (vi) k_fc_dp4a<true><<<grid, 128, smem, st>>>(act, act_stride, valid, L.quad_a, L.quad_b, k4n, L.n_out, L.n_pad, out, n);
-    else k_fc_dp4a<false><<<grid, 128, smem, st>>>(act, act_stride, valid, L.quad_a, L.quad_a, k4n, L.n_out, L.n_pad, out, n);
+    limit = std::max(bytes, (size_t)a.maxDynamicSharedSizeBytes);
     return true;
 }
 

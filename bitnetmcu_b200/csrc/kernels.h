@@ -31,6 +31,10 @@ struct FcLayerDev {
     int4 *quad_b = nullptr;
 };
 
+// Lets `kernel` launch with `bytes` of dynamic shared memory on the current device: raises its
+// cudaFuncAttributeMaxDynamicSharedMemorySize there when it is lower, never lowers it.  false (no error left pending) on failure.
+bool raise_smem_limit(const void *kernel, size_t bytes);
+
 // ---- weight decode (packed exportquant words -> dense planes); returns whether plane B is needed via *d_flag
 void launch_decode_fc(const void *d_packed, int32_t enc, uint32_t n_in, uint32_t n_out, uint32_t k_pad, uint32_t n_pad,
                       int8_t *dense_a, int8_t *dense_b, int4 *quad_a, int4 *quad_b, int nf4_extension, int *d_flag,

@@ -54,3 +54,15 @@ def test_relunorm_unpredicated(fixed_sass):
 def test_consumer_has_no_division(fixed_sass):
     """the ring position advances by counters, not by a division by the stage count per tile"""
     assert not [i for i in _consumer(fixed_sass) if "MUFU.RCP" in i]
+
+
+def test_every_instantiation_divides_once(built):
+    """every role of every fc_chain_kernel instantiation advances its ring position by counters: the one unsigned integer
+    division left (I2F.U32.RP starts its sequence) is the entry code's count of the CTA's tiles"""
+    from bitnetmcu_b200 import _lib
+    out = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    kernels = re.split(r"\n\s*Function : ", out)[1:]
+    chain = {k.split()[0]: k for k in kernels if k.startswith("_ZN3bnm15fc_chain_kernel")}
+    assert FIXED in chain and len(chain) == 8, sorted(chain)
+    for name, sass in chain.items():
+        assert sass.count("I2F.U32.RP") == 1, name

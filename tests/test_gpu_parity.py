@@ -488,6 +488,20 @@ def test_chains_on_tcgen05(lib, oracle, enc, widths):
     e.close()
 
 
+def test_later_model_keeps_earlier_models_shared_memory(lib, oracle):
+    """Creating a model must not lower the dynamic shared memory limit of a kernel another live model launches: FC 4bitsym-64's
+    fused launch asks for more shared memory than Binary-160's."""
+    from bitnetmcu_b200 import _lib
+    fc = _engine("fc", _lib.PATH_TCGEN05)
+    b160 = _engine("binary160", _lib.PATH_TCGEN05)
+    imgs = _rand_images(5000 + 37, seed=3)
+    lo, la = fc.infer(imgs)
+    oo, ol = oracle.infer(load_model("fc"), imgs)
+    assert np.array_equal(lo, oo) and np.array_equal(la, ol)
+    b160.close()
+    fc.close()
+
+
 def test_launch_overlap_mode2_reused_buffers_keep_stream_order(lib, oracle):
     """ADVICE r1: mode 2 drops the grid-dependency wait only for launches whose buffers differ from the previous call's.
     Reusing the SAME buffers with a producer copy in front of every launch (the pattern mode 2 does not promise) must still
