@@ -389,14 +389,15 @@ extern "C" int64_t bnm_model_get_option(const bnm_model *m, int option) {
 static const size_t kLayeredChunk = 1 << 17;   // images per pass of the layer-by-layer path (bounds its scratch)
 static const size_t kFusedCnnChunk = 1 << 20;  // fused path, CNN models: images per front-end + FC launch pair (256 B of features each)
 
-// FC chain, one CUDA-core kernel per layer: input int8 [n][in_stride]
+// FC chain, one CUDA-core kernel per layer: input int8 [n][in_stride].  Without logits the last layer's accumulators go to the
+// scratch (n x max_nout) like every other layer's, and only its ReLUNorm's argmax leaves it.
 static int run_fc_layers(bnm_model *m, const int8_t *in, uint32_t in_stride, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st) {
     const int8_t *act = in;
     uint32_t stride = in_stride;
     const size_t nl = m->fc.size();
     for (size_t l = 0; l < nl; l++) {
         const bool last = l + 1 == nl;
-        int32_t *acc = last ? logits : m->d_acc;
+        int32_t *acc = last && logits ? logits : m->d_acc;
         if (!launch_fc_dp4a(act, stride, m->fc[l], acc, n, st))
             return fail(BNM_E_UNSUPPORTED, "FC layer %zu: %u inputs need more shared memory than an SM has (layer kernel stages 128 rows)", l, m->fc[l].n_in);
         if (last) {
@@ -433,13 +434,20 @@ extern "C" int bnm_infer_launch_count(const bnm_model *m, size_t n) {
     return (int)(chunks * per);
 }
 
-// slot_feat: a caller-owned feature buffer for n images (the host pipeline's per-slot buffers); null = the model's own scratch
+// a call must produce something: logits, labels or (gather) a destination in another buffer
+static bool has_output(const int32_t *logits, const uint32_t *labels, const GatherDst *gather) {
+    return logits || labels || (gather && (gather->n_labels_dst || gather->n_logits_dst));
+}
+
+// slot_feat: a caller-owned feature buffer for n images (the host pipeline's per-slot buffers); null = the model's own scratch.
+// logits and labels may each be null.
 static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather, void *stream,
                              int8_t *slot_feat = nullptr) {
-    if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_infer_batch_device: null argument");
+    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch_device: null argument");
+    if (n && !has_output(logits, labels, gather)) return fail(BNM_E_ARG, "bnm_infer_batch_device: no output (logits, labels and gather destinations all absent)");
     if (n == 0) return 0;
     if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned (TMA)");
-    if ((uintptr_t)logits & 7) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
+    if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
     CU_TRY(cudaSetDevice(m->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
@@ -456,7 +464,7 @@ static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         const int8_t *img = images + b * m->img_bytes;
-        int32_t *lg = logits + b * m->n_classes;
+        int32_t *lg = logits ? logits + b * m->n_classes : nullptr;
         uint32_t *lb = labels ? labels + b : nullptr;
         const int8_t *fc_in = img;
         uint32_t fc_stride = m->img_bytes;
@@ -565,19 +573,20 @@ static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *lo
     if (m->small_zero_copy >= 2) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(const_cast<int8_t **>(&d_in)), m->small_h_in, 0));
     else CU_TRY(cudaMemcpyAsync(m->small_d_in, m->small_h_in, n * (size_t)m->img_bytes, cudaMemcpyHostToDevice, st));
     if (m->small_zero_copy >= 1) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), m->small_h_out, 0));
-    const size_t n_log = n * (size_t)m->n_classes;
+    const size_t n_log = logits ? n * (size_t)m->n_classes : 0;   // labels-only calls: the labels start the staging buffer
     uint32_t *d_lab = reinterpret_cast<uint32_t *>(d_out + n_log);
-    int rc = bnm_infer_batch_device(m, d_in, n, d_out, labels ? d_lab : nullptr, st);
+    int rc = bnm_infer_batch_device(m, d_in, n, logits ? d_out : nullptr, labels ? d_lab : nullptr, st);
     if (rc) return rc;
     if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(m->small_h_out, m->small_d_out, (n_log + (labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
-    memcpy(logits, m->small_h_out, n_log * 4);
+    if (logits) memcpy(logits, m->small_h_out, n_log * 4);
     if (labels) memcpy(labels, m->small_h_out + n_log, n * 4);
     return 0;
 }
 
 extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
-    if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_infer_batch: null argument");
+    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch: null argument");
+    if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_infer_batch: no output (logits and labels both NULL)");
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);
@@ -605,9 +614,10 @@ extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int
         const size_t nb = std::min(chunk, n - b);
         PipeSlot &s = m->slots[shared_scratch ? 0 : k % 3];
         CU_TRY(cudaMemcpyAsync(s.d_images, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
-        int rc = infer_device_impl(m, s.d_images, nb, s.d_logits, labels ? s.d_labels : nullptr, nullptr, s.stream, shared_scratch ? nullptr : s.d_feat);
+        int rc = infer_device_impl(m, s.d_images, nb, logits ? s.d_logits : nullptr, labels ? s.d_labels : nullptr, nullptr, s.stream,
+                                   shared_scratch ? nullptr : s.d_feat);
         if (rc) return rc;
-        CU_TRY(cudaMemcpyAsync(logits + b * m->n_classes, s.d_logits, nb * (size_t)m->n_classes * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
+        if (logits) CU_TRY(cudaMemcpyAsync(logits + b * m->n_classes, s.d_logits, nb * (size_t)m->n_classes * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
         if (labels) CU_TRY(cudaMemcpyAsync(labels + b, s.d_labels, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
     }
     for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
@@ -763,10 +773,11 @@ extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_
 // float images -> logits / labels on the device.  FC models on the fused path (rows of <= 256 elements, <= 16 classes): ONE kernel, the
 // input scaling fused into its load stage.  Everything else: the scaling kernel into a scratch buffer, then the ordinary path.
 extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
-    if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_infer_batch_device_f32: null argument");
+    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch_device_f32: null argument");
+    if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_infer_batch_device_f32: no output (logits and labels both NULL)");
     if (n == 0) return 0;
     if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
-    if ((uintptr_t)logits & 7) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
+    if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
     CU_TRY(cudaSetDevice(m->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool fused_fc = bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST;

@@ -331,6 +331,9 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         const uint32_t row_in_tile = half * 64 + wq * 16 + (lane >> 2);   // this thread's first row; the second is 8 below
         const int n_layers = kFixed ? kFixedLayers : P.n_layers;
         const uint32_t ncls = P.n_classes;
+        // labels-only launches pass no logits buffer.  The shuffle is a value no-op (a uniform flag), kept for ptxas: testing
+        // P.logits at the store instead serialises the fixed-shape kernel's wgmma pipeline (C7511, CUDA 12.9).
+        const bool has_logits = __shfl_sync(0xffffffffu, (uint32_t)(P.logits != nullptr), 0);
         mbar_wait(&bar_w, 0, P.err, 6);   // weight tiles are in shared memory
         // B descriptor of the 64 columns from c0 of the K-step tile at smem address t (no-swizzle K-major: 8-row groups 256 B apart).
         // Every wgmma is issued at the kernel's full width kN, with no condition around it (a conditional wgmma cannot stay in
@@ -483,7 +486,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                             }
                         }
                     };
-                    store_row(P.logits + img * ncls);
+                    if (has_logits) store_row(P.logits + img * ncls);
 #pragma unroll 1
                     for (uint32_t d = 0; d < P.n_log_dst; d++) store_row(P.log_dst[d] + (P.row0 + img) * ncls);   // peers, over NVLink
                     if (quad == 0) {
@@ -910,9 +913,10 @@ int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logi
     if (!tmap_p) return -3;
     // Mode 2 drops the grid-dependency wait, i.e. EVERY ordering against the work enqueued before this launch on the stream
     // (the previous bnm launch and any producer kernel of `images` alike).  The library keeps the wait whenever it can see the
-    // promise being broken: first launch on this plan / another stream / a buffer of the previous launch reused.
+    // promise being broken: first launch on this plan / another stream / a buffer of the previous launch reused.  A null output
+    // is no buffer: it neither reuses nor differs from one.
     bool independent = plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && in != plan->prev_in &&
-                       logits != plan->prev_logits && (labels == nullptr || labels != plan->prev_labels);
+                       (logits == nullptr || logits != plan->prev_logits) && (labels == nullptr || labels != plan->prev_labels);
     p.wait_prior_grid = !independent;
     p.early_trigger = plan->overlap != 0 && cfg.gridDim.x == (unsigned)plan->sm_count;
     plan->prev_in = in; plan->prev_logits = logits; plan->prev_labels = labels; plan->prev_stream = st; plan->prev_valid = true;
@@ -931,7 +935,7 @@ bool fc_chain_float_input_supported(const FcChainPlan *plan) {
     return plan && plan->kernel_f32 && plan->in_bytes % 16 == 0;
 }
 
-// float32 images [n][in_bytes elements] -> logits / labels, the input scaling fused into the load stage (kFloatIn)
+// float32 images [n][in_bytes elements] -> logits / labels (either may be null), the input scaling fused into the load stage (kFloatIn)
 int fc_chain_launch_f32(FcChainPlan *plan, const float *in, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;

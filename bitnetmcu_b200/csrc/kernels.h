@@ -83,7 +83,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
 void fc_chain_plan_destroy(FcChainPlan *p);
 // 0 plain launches, 1 programmatic dependent launch (inputs read after the previous kernel completed), 2 launches declared independent
 void fc_chain_plan_set_overlap(FcChainPlan *p, int mode);
-// images int8 [n][in_bytes] (device, 16B aligned) -> logits int32 [n][n_classes], labels uint32 [n] (may be null)
+// images int8 [n][in_bytes] (device, 16B aligned) -> logits int32 [n][n_classes], labels uint32 [n] (each may be null)
 // gather (may be null): extra destination buffers every row is also stored to (peer memory), fused into the epilogue
 int fc_chain_launch(FcChainPlan *p, const int8_t *in, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather,
                     cudaStream_t st);

@@ -68,24 +68,30 @@ class Engine:
         return int(self.lib.bnm_infer_launch_count(self.handle, n))
 
     # ---- batched inference over host arrays (H2D / kernels / D2H pipelined inside the library) -----------
-    def infer(self, images: np.ndarray, want_labels: bool = True, out_logits: Optional[np.ndarray] = None,
-              out_labels: Optional[np.ndarray] = None) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+    def infer(self, images: np.ndarray, want_labels: bool = True, want_logits: bool = True, out_logits: Optional[np.ndarray] = None,
+              out_labels: Optional[np.ndarray] = None) -> Tuple[Optional[np.ndarray], Optional[np.ndarray]]:
+        """images int8 [n, img_bytes] -> (logits int32 [n, n_classes], labels uint32 [n]).  ``want_logits=False`` returns
+        ``(None, labels)``: the logits are neither copied back nor, on the fused path, written to GPU memory."""
+        if not (want_labels or want_logits):
+            raise ValueError("Engine.infer: ask for logits, labels or both")
         imgs = np.ascontiguousarray(images, dtype=np.int8).reshape(-1, self.img_bytes)
         n = imgs.shape[0]
-        logits = out_logits if out_logits is not None else np.empty((n, self.n_classes), dtype=np.int32)
+        logits = None
+        if want_logits:
+            logits = out_logits if out_logits is not None else np.empty((n, self.n_classes), dtype=np.int32)
         labels = out_labels if out_labels is not None else (np.empty(n, dtype=np.uint32) if want_labels else None)
         _lib.check(self.lib.bnm_infer_batch(self.handle, _ptr(imgs), n, _ptr(logits), _ptr(labels)), "bnm_infer_batch")
         return logits, labels
 
     def inference(self, image: np.ndarray) -> int:
         """``uint32_t Inference(int8_t *input)`` (BitNetMCU_MNIST_dll.c:24): predicted class of one image."""
-        _, labels = self.infer(np.asarray(image, dtype=np.int8).reshape(1, self.img_bytes))
+        _, labels = self.infer(np.asarray(image, dtype=np.int8).reshape(1, self.img_bytes), want_logits=False)
         return int(labels[0])
 
     # ---- device pointers (torch tensors as plumbing) ---------------------------------------------------
     def infer_device(self, images, logits, labels=None, stream: Optional[int] = None) -> None:
-        """images: torch.int8 [n, img_bytes] on this GPU; logits: torch.int32 [n, n_classes]; labels: torch.int32/uint32 [n]
-        or None.  Asynchronous on ``stream`` (a cudaStream_t as int; default: torch's current stream).
+        """images: torch.int8 [n, img_bytes] on this GPU; logits: torch.int32 [n, n_classes] or None; labels: torch.int32/uint32
+        [n] or None (not both None).  Asynchronous on ``stream`` (a cudaStream_t as int; default: torch's current stream).
 
         With ``OPT_LAUNCH_OVERLAP`` = 2 a launch whose buffers differ from the previous call's is NOT ordered against earlier
         work on the stream (include/bitnetmcu_b200.h): its images must already be complete when the previous call was
@@ -94,14 +100,25 @@ class Engine:
         n = images.shape[0]
         if stream is None:
             stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.is_contiguous() and logits.is_contiguous() and images.dtype == torch.int8 and logits.dtype == torch.int32
-        assert images.shape[1] == self.img_bytes and tuple(logits.shape) == (n, self.n_classes)
-        lab_ptr = None
-        if labels is not None:
-            assert labels.is_contiguous() and labels.element_size() == 4 and labels.numel() == n
-            lab_ptr = C.c_void_p(labels.data_ptr())
-        _lib.check(self.lib.bnm_infer_batch_device(self.handle, C.c_void_p(images.data_ptr()), n, C.c_void_p(logits.data_ptr()),
-                                                   lab_ptr, C.c_void_p(stream)), "bnm_infer_batch_device")
+        assert images.is_contiguous() and images.dtype == torch.int8 and images.shape[1] == self.img_bytes
+        _lib.check(self.lib.bnm_infer_batch_device(self.handle, C.c_void_p(images.data_ptr()), n, self._logits_ptr(logits, n),
+                                                   self._labels_ptr(labels, n), C.c_void_p(stream)), "bnm_infer_batch_device")
+
+    def _logits_ptr(self, logits, n: int):
+        """a torch.int32 [n, n_classes] device tensor as a pointer argument, None as NULL"""
+        import torch
+        if logits is None:
+            return None
+        assert logits.is_contiguous() and logits.dtype == torch.int32 and tuple(logits.shape) == (n, self.n_classes)
+        return C.c_void_p(logits.data_ptr())
+
+    @staticmethod
+    def _labels_ptr(labels, n: int):
+        """a 4-byte [n] device tensor as a pointer argument, None as NULL"""
+        if labels is None:
+            return None
+        assert labels.is_contiguous() and labels.element_size() == 4 and labels.numel() == n
+        return C.c_void_p(labels.data_ptr())
 
 
     def inference_quantized(self, input_data: np.ndarray) -> np.ndarray:
@@ -115,23 +132,23 @@ class Engine:
 
     def infer_device_f32(self, images, logits, labels=None, stream: Optional[int] = None) -> None:
         """images: torch.float32 [n, img_bytes] on this GPU (un-normalised pixels, as test_inference.py:140 sees them) -> logits
-        torch.int32 [n, n_classes], labels [n].  FC models: one kernel with the input scaling fused into its load stage."""
+        torch.int32 [n, n_classes] or None, labels [n] or None (not both None).  FC models: one kernel with the input scaling fused
+        into its load stage."""
         import torch
         n = images.shape[0]
         if stream is None:
             stream = torch.cuda.current_stream(images.device).cuda_stream
         assert images.is_contiguous() and images.dtype == torch.float32 and images.shape[1] == self.img_bytes
-        assert logits.is_contiguous() and logits.dtype == torch.int32 and tuple(logits.shape) == (n, self.n_classes)
-        lab_ptr = C.c_void_p(labels.data_ptr()) if labels is not None else None
-        _lib.check(self.lib.bnm_infer_batch_device_f32(self.handle, C.c_void_p(images.data_ptr()), n, C.c_void_p(logits.data_ptr()), lab_ptr,
-                                                       C.c_void_p(stream)), "bnm_infer_batch_device_f32")
+        _lib.check(self.lib.bnm_infer_batch_device_f32(self.handle, C.c_void_p(images.data_ptr()), n, self._logits_ptr(logits, n),
+                                                       self._labels_ptr(labels, n), C.c_void_p(stream)), "bnm_infer_batch_device_f32")
 
-    def infer_tensor(self, images):
+    def infer_tensor(self, images, want_logits: bool = True):
         """images: torch.int8 [n, img_bytes] on this engine's GPU -> (logits torch.int32 [n, n_classes], labels torch.int32 [n]) on
-        the same GPU, asynchronous on torch's current stream (device memory end to end; plumbing for ``dist.sharded_infer``)."""
+        the same GPU, asynchronous on torch's current stream (device memory end to end; plumbing for ``dist.sharded_infer``).
+        ``want_logits=False`` returns ``(None, labels)``."""
         import torch
         n = images.shape[0]
-        logits = torch.empty((n, self.n_classes), dtype=torch.int32, device=images.device)
+        logits = torch.empty((n, self.n_classes), dtype=torch.int32, device=images.device) if want_logits else None
         labels = torch.empty(n, dtype=torch.int32, device=images.device)
         if n:
             self.infer_device(images.contiguous(), logits, labels)

@@ -115,11 +115,12 @@ class PeerGatherBuffers:
 
 def infer_gather(eng, images, logits, labels, buffers: PeerGatherBuffers, labels_to, logits_to, stream: int, labels_u8: bool = False) -> None:
     """``Engine.infer_device`` whose epilogue also stores this rank's rows into the gather buffers of the ranks listed in
-    ``labels_to`` / ``logits_to`` (pass this rank's own slice of its buffer as ``logits`` / ``labels`` and leave it out of the lists)."""
+    ``labels_to`` / ``logits_to`` (pass this rank's own slice of its buffer as ``logits`` / ``labels`` and leave it out of the lists).
+    ``logits`` / ``labels`` may be None: no local copy of that output (the call still needs one output or destination)."""
     g = buffers.spec(labels_to, logits_to, labels_u8)
-    lab_ptr = C.c_void_p(labels.data_ptr()) if labels is not None else None
-    _lib.check(eng.lib.bnm_infer_batch_device_gather(eng.handle, C.c_void_p(images.data_ptr()), images.shape[0], C.c_void_p(logits.data_ptr()),
-                                                     lab_ptr, C.byref(g), C.c_void_p(stream)), "bnm_infer_batch_device_gather")
+    n = images.shape[0]
+    _lib.check(eng.lib.bnm_infer_batch_device_gather(eng.handle, C.c_void_p(images.data_ptr()), n, eng._logits_ptr(logits, n),
+                                                     eng._labels_ptr(labels, n), C.byref(g), C.c_void_p(stream)), "bnm_infer_batch_device_gather")
 
 
 def bench_gathers(ctx, eng, db, ms_compute: float) -> dict:

@@ -42,9 +42,8 @@ static bnm_model *model(void)
 /* BitMnistInference, dll.c:48-121: one 16x16 int8 image in, predicted class out */
 uint32_t BitMnistInference(int8_t *input)
 {
-    int32_t logits[BNM_MODEL_N_CLASSES];
     uint32_t label = 255;
-    if (bnm_infer_batch(model(), input, 1, logits, &label) != 0) {
+    if (bnm_infer_batch(model(), input, 1, NULL, &label) != 0) {   /* the class only: no logits */
         fprintf(stderr, "bitnetmcu_b200: inference failed: %s\n", bnm_last_error());
         abort();
     }
@@ -53,7 +52,8 @@ uint32_t BitMnistInference(int8_t *input)
 
 EXPORT uint32_t Inference(int8_t *input) { return BitMnistInference(input); }
 
-/* n images int8 [n][256] -> int32 logits [n][n_classes] + uint32 labels [n] (NULL allowed); 0 on success */
+/* n images int8 [n][256] -> int32 logits [n][n_classes] + uint32 labels [n]; 0 on success.  Either output may be NULL, not
+ * both: InferenceBatch(images, n, NULL, labels) returns the classes alone and copies no logits back from the GPU. */
 EXPORT int InferenceBatch(const int8_t *images, size_t n, int32_t *logits, uint32_t *labels)
 {
     return bnm_infer_batch(model(), images, n, logits, labels);

@@ -100,7 +100,8 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      call k must therefore be complete before call k-1 was enqueued (resident inputs, or produced on another stream and
  *      joined by an event before call k-1).  The library keeps ordinary stream semantics (the wait) for every launch where it
  *      can see the promise broken: the first launch after the option is set, a launch on another stream than the one before,
- *      and a launch that reuses the images, logits or labels pointer of the one before.  Producer -> inference chains on one
+ *      and a launch that reuses the images, logits or labels pointer of the one before.  A NULL logits or labels pointer is
+ *      no buffer: two labels-only launches in a row do not share their (absent) logits.  Producer -> inference chains on one
  *      stream (bnm_quantize_images_device then bnm_infer_batch_device) belong to mode 0 or 1.
  *      Only launches that fill the GPU (>= one 128-image tile per SM) trigger early, and every launch occupies its SM
  *      exclusively (more than half of the shared memory): at most two consecutive launches are ever in flight together.
@@ -129,8 +130,11 @@ BNM_API int bnm_model_active_path(const bnm_model *m);
  * ------------------------------------------------------------------------------------------- */
 
 /* images: int8 [n][img_bytes] row-major (what Inference() takes, n times).  logits: int32 [n][n_classes]
- * = layer_out after the last processfclayer (dll.c:89,115; the reference computes but never returns them).
+ * = layer_out after the last processfclayer (dll.c:89,115; the reference computes but never returns them), may be NULL.
  * labels: uint32 [n] = the value Inference() returns (argmax of the last ReLUNorm), may be NULL.
+ * Every call with n > 0 needs at least one output: non-NULL logits, non-NULL labels or (bnm_infer_batch_device_gather) a
+ * destination buffer; otherwise it returns BNM_E_ARG (-1).  A labels-only call (logits NULL) writes and copies no logits at
+ * all: 40 B per image less GPU memory traffic for 10 classes on the fused path, no logits copy over PCIe on the host path.
  * Host version: buffers are ordinary (ideally pinned, see bnm_host_alloc) host memory; the call streams them
  * through the GPU in chunks with copies overlapped and returns when the results are in `logits`/`labels`. */
 BNM_API int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels);
@@ -195,7 +199,8 @@ BNM_API int bnm_maxpool22_batch(const int32_t *activations, uint32_t xy_input, i
 /* Float images straight to logits / labels (device buffers, asynchronous on `stream`): for FC models on the fused path (image rows of
  * <= 256 elements, <= 16 classes) this is ONE kernel -- four extra warps read the float rows, reduce the row maximum, quantise and write
  * the int8 rows into the shared-memory stage the tensor core reads, so a float image costs 1 024 B of HBM traffic once.  Other models:
- * the scaling kernel into a scratch buffer, then bnm_infer_batch_device.  Results are those of bnm_quantize_images + bnm_infer_batch. */
+ * the scaling kernel into a scratch buffer, then bnm_infer_batch_device.  Results are those of bnm_quantize_images + bnm_infer_batch.
+ * logits or labels may be NULL, not both (section 3). */
 BNM_API int bnm_infer_batch_device_f32(bnm_model *m, const float *images, size_t n, int32_t *logits, uint32_t *labels, void *stream);
 BNM_API int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out);                       /* host buffers */
 BNM_API int bnm_quantize_images_device(const float *images, size_t n, uint32_t elems, int8_t *out, void *stream);  /* device buffers */
@@ -209,6 +214,7 @@ BNM_API int bnm_quantize_images_device(const float *images, size_t n, uint32_t e
  *    "4bit" levels carry a +0.01 offset (BitNetMCU.py:159) and NF4 levels are non-dyadic: those two are approximated by the
  *    engine's integer weights (statistical parity only).
  * ------------------------------------------------------------------------------------------- */
+/* logits are this entry's only output and may not be NULL (BNM_E_ARG) */
 BNM_API int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits);
 
 #ifdef __cplusplus

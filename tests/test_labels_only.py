@@ -1,0 +1,290 @@
+"""Labels-only inference (GPU, H100): every batched entry takes a NULL logits buffer and then produces the labels alone.
+The labels must equal the oracle's on every path, every CNN front-end and every instantiation of the fused FC kernel."""
+import ctypes as C
+import re
+
+import numpy as np
+import pytest
+
+from conftest import load_model, model_names
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope="module")
+def lib(built):
+    from bitnetmcu_b200 import _lib
+    l = _lib.load()
+    assert l.bnm_device_count() > 0, "no CUDA device"
+    return l
+
+
+def _images(n, img_bytes=256, seed=0):
+    rng = np.random.default_rng(seed)
+    imgs = rng.integers(-128, 128, size=(n, img_bytes)).astype(np.int8)
+    imgs[: min(n, 64)] = np.clip(imgs[: min(n, 64)], -20, 127)   # MNIST-like rows: background ~ -20, strokes to 127
+    return imgs
+
+
+def _frontends(model):
+    from bitnetmcu_b200 import _lib
+    if model.model_class != 1:
+        return [None]
+    return [_lib.CNN_CUDA_CORES, _lib.CNN_TENSOR_CORES] if model.channels % 16 == 0 else [_lib.CNN_CUDA_CORES]
+
+
+def _engine(model, path=0, cnn_frontend=None):
+    from bitnetmcu_b200 import _lib
+    from bitnetmcu_b200.engine import Engine
+    e = Engine(model, device=0, path=path)
+    if cnn_frontend is not None:
+        e.set_option(_lib.OPT_CNN_FRONTEND, cnn_frontend)
+    return e
+
+
+@pytest.mark.parametrize("path", ["layers", "tcgen05"])
+@pytest.mark.parametrize("name", model_names())
+def test_golden_models_labels_only(lib, oracle, name, path):
+    """Every fixture model, both paths, every CNN front-end: a ragged batch (not a multiple of the 128-image tile)."""
+    from bitnetmcu_b200 import _lib
+    m = load_model(name)
+    imgs = _images(5037, seed=len(name))
+    _, want = oracle.infer(m, imgs)
+    p = _lib.PATH_LAYERS if path == "layers" else _lib.PATH_TCGEN05
+    for fe in _frontends(m):
+        e = _engine(m, p, fe)
+        assert e.active_path == p
+        lo, la = e.infer(imgs, want_logits=False)
+        assert lo is None and np.array_equal(la, want), (name, path, fe)
+        e.close()
+
+
+@pytest.mark.parametrize("n", [0, 1, 127, 128, 129, 1000])
+def test_edge_batch_sizes_labels_only(lib, oracle, n):
+    from bitnetmcu_b200 import _lib
+    imgs = _images(n, seed=n)
+    for name in ("fc", "cnn_48"):
+        m = load_model(name)
+        want = oracle.infer(m, imgs)[1] if n else np.empty(0, dtype=np.uint32)
+        for path in (_lib.PATH_LAYERS, _lib.PATH_TCGEN05):
+            for fe in _frontends(m):
+                e = _engine(m, path, fe)
+                lo, la = e.infer(imgs, want_logits=False)
+                assert lo is None and la.shape == (n,) and np.array_equal(la, want), (name, path, fe)
+                e.close()
+
+
+def _random(enc, widths, seed):
+    from bitnetmcu_b200 import pack as P
+    m = P.random_fc_model(enc, widths, seed=seed)
+    m.img_bytes = widths[0]
+    return m
+
+
+# every row of kChainKernels (fc_wgmma.cu), with a model that selects it (checked against the plan's BNM_VERBOSE line)
+_ROWS = [
+    ("<64,1>", lambda: _random(4, (512, 64, 64, 10), 1)),           # 512-byte rows: room for three 64 kB stages, one pipe
+    ("<64,2,2,64>", lambda: _random(4, (256, 64, 64, 37), 2)),      # 37 classes: the last layer is wider than 16
+    ("<64,2,2,16>", lambda: load_model("1k")),                      # 16-wide layers, three of them: not the fixed class
+    ("<64,2,2,16,fixed>", lambda: load_model("fc")),
+    ("<128,1>", lambda: load_model("2bitsym96")),
+    ("<192,1>", lambda: load_model("binary160")),
+    ("<256,1>", lambda: _random(4, (256, 256, 10), 3)),
+]
+
+
+@pytest.mark.parametrize("row", [r for r, _ in _ROWS])
+def test_every_chain_kernel_row_labels_only(lib, oracle, capfd, monkeypatch, row):
+    from bitnetmcu_b200 import _lib
+    monkeypatch.setenv("BNM_VERBOSE", "1")
+    m = dict(_ROWS)[row]()
+    capfd.readouterr()
+    e = _engine(m, _lib.PATH_TCGEN05)
+    plan = [l for l in capfd.readouterr().err.splitlines() if "fused FC plan" in l]
+    assert plan and re.search(r"fc_chain_kernel(<[^>]*>)", plan[-1]).group(1) == row, plan
+    n = 148 * 128 * 2 + 77                 # several tiles per CTA and a ragged last tile
+    imgs = _images(n, m.img_bytes, seed=len(row))
+    _, want = oracle.infer(m, imgs)
+    lo, la = e.infer(imgs, want_logits=False)
+    assert lo is None and np.array_equal(la, want), row
+    e.close()
+
+
+def test_float_input_row_labels_only(lib, oracle, capfd, monkeypatch):
+    """the fused float-input row (<64,1,float>) through bnm_infer_batch_device_f32 with NULL logits"""
+    import torch
+    from bitnetmcu_b200 import _lib
+    monkeypatch.setenv("BNM_VERBOSE", "1")
+    m = load_model("fc")
+    capfd.readouterr()
+    e = _engine(m, _lib.PATH_TCGEN05)
+    assert "float input <64,1,float>" in capfd.readouterr().err
+    _float_case(e, m, oracle, 148 * 128 * 2 + 77)
+    e.close()
+
+
+def _float_case(e, m, oracle, n):
+    import torch
+    rng = np.random.default_rng(n)
+    x = rng.normal(size=(n, m.img_bytes)).astype(np.float32)
+    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
+    q = np.round(x * scale).clip(-128, 127).astype(np.int8)
+    _, want = oracle.infer(m, q)
+    d_x = torch.from_numpy(x).cuda()
+    d_lab = torch.full((n,), -1, dtype=torch.int32, device="cuda")
+    for _ in range(2):                      # twice: the stage ring wraps and the launch is repeatable
+        e.infer_device_f32(d_x, None, d_lab)
+    torch.cuda.synchronize()
+    assert np.array_equal(d_lab.cpu().numpy().astype(np.uint32), want)
+
+
+@pytest.mark.parametrize("name", ["fc", "binary160"])
+def test_float_input_labels_only(lib, oracle, name):
+    """fc: the fused float kernel; binary160 (192 columns): the scaling kernel into scratch, then the int8 entry"""
+    m = load_model(name)
+    e = _engine(m)
+    _float_case(e, m, oracle, 3001)
+    e.close()
+
+
+@pytest.mark.parametrize("name", ["fc", "cnn_48"])
+def test_device_labels_only_on_torch_stream(lib, oracle, name):
+    import torch
+    m = load_model(name)
+    imgs = _images(3000, seed=4)
+    _, want = oracle.infer(m, imgs)
+    e = _engine(m)
+    d_img = torch.from_numpy(imgs).cuda()
+    d_lab = torch.full((3000,), -1, dtype=torch.int32, device="cuda")
+    s = torch.cuda.Stream()
+    with torch.cuda.stream(s):
+        e.infer_device(d_img, None, d_lab)
+    s.synchronize()
+    assert np.array_equal(d_lab.cpu().numpy().astype(np.uint32), want)
+    e.close()
+
+
+@pytest.mark.parametrize("name", ["fc", "cnn"])
+def test_host_pipeline_labels_only(lib, oracle, name):
+    """bnm_infer_batch with NULL logits: the chunked three-stream pipeline at several chunk sizes and the small-batch path"""
+    from bitnetmcu_b200 import _lib
+    m = load_model(name)
+    imgs = _images(10000, seed=3)
+    _, want = oracle.infer(m, imgs)
+    for chunk in (128, 1024, 4096):
+        e = _engine(m)
+        e.set_option(_lib.OPT_CHUNK_IMAGES, chunk)
+        lo, la = e.infer(imgs, want_logits=False)
+        assert lo is None and np.array_equal(la, want), chunk
+        e.close()
+    e = _engine(m)
+    for n in (1, 777, 1024):               # n <= 1024: staged through the small-batch buffers
+        lo, la = e.infer(imgs[:n], want_logits=False)
+        assert lo is None and np.array_equal(la, want[:n]), n
+    lo, la = e.infer(imgs[:777])           # and a call with logits after labels-only ones
+    assert np.array_equal(la, want[:777]) and np.array_equal(lo, oracle.infer(m, imgs[:777])[0])
+    e.close()
+
+
+@pytest.mark.parametrize("mode", [1, 2])
+def test_launch_overlap_labels_only(lib, oracle, mode):
+    """BNM_OPT_LAUNCH_OVERLAP with NULL logits: back-to-back launches on one stream, images and labels double-buffered, stay
+    bit-exact.  Then one labels buffer reused by every launch (resident images, a consumer copy after each): the library must see
+    the reuse and keep the launches ordered, whatever the absent logits."""
+    import torch
+    from bitnetmcu_b200 import _lib
+    m = load_model("fc")
+    n = 148 * 128 * 7 + 77                  # fills the GPU: launches trigger early
+    batches = [_images(n, seed=60 + k) for k in range(4)]
+    want = [oracle.infer(m, b)[1] for b in batches]
+    e = _engine(m)
+    e.set_option(_lib.OPT_LAUNCH_OVERLAP, mode)
+    src = [torch.from_numpy(b).cuda() for b in batches]     # resident inputs: consecutive launches never share a buffer
+    d_lab = [torch.full((n,), -1, dtype=torch.int32, device="cuda") for _ in range(2)]
+    s = torch.cuda.Stream()
+    torch.cuda.synchronize()
+    with torch.cuda.stream(s):
+        for rep in range(6):
+            for k in range(4):
+                e.infer_device(src[k], None, d_lab[k & 1])
+        s.synchronize()
+        # the last two launches wrote batches 2 and 3 into label buffers 0 and 1
+        got = [d_lab[0].cpu().numpy(), d_lab[1].cpu().numpy()]
+        assert np.array_equal(got[0].astype(np.uint32), want[2]) and np.array_equal(got[1].astype(np.uint32), want[3])
+        one = torch.full((n,), -1, dtype=torch.int32, device="cuda")
+        seen = []
+        for rep in range(3):
+            for k in range(4):
+                e.infer_device(src[k], None, one)
+                seen.append(one.clone())
+        s.synchronize()
+    for i, t in enumerate(seen):
+        assert np.array_equal(t.cpu().numpy().astype(np.uint32), want[i % 4]), i
+    e.close()
+
+
+def test_gather_labels_only(lib, oracle):
+    """single-GPU result exchange with NULL logits: local labels plus a labels destination, then the destination alone"""
+    import torch
+    from bitnetmcu_b200 import _lib
+    m = load_model("fc")
+    n, rows, off = 148 * 128 * 2 + 77, 148 * 128 * 2 + 77 + 640, 512
+    imgs = _images(n, seed=77)
+    _, want = oracle.infer(m, imgs)
+    e = _engine(m, _lib.PATH_TCGEN05)
+    d_img = torch.from_numpy(imgs).cuda()
+    d_lab = torch.full((n,), -1, dtype=torch.int32, device="cuda")
+    dst = [torch.full((rows,), -7, dtype=torch.int32, device="cuda") for _ in range(2)]
+    s = torch.cuda.current_stream()
+    for k, local in enumerate((d_lab, None)):
+        g = _lib.BnmGather()
+        g.n_labels_dst, g.n_logits_dst, g.row_offset = 1, 0, off
+        g.labels_dst[0] = dst[k].data_ptr()
+        lab_ptr = C.c_void_p(local.data_ptr()) if local is not None else None
+        _lib.check(lib.bnm_infer_batch_device_gather(e.handle, C.c_void_p(d_img.data_ptr()), n, None, lab_ptr, C.byref(g),
+                                                     C.c_void_p(s.cuda_stream)), "gather")
+    s.synchronize()
+    assert np.array_equal(d_lab.cpu().numpy().astype(np.uint32), want)
+    for k in range(2):
+        h = dst[k].cpu().numpy()
+        assert np.array_equal(h[off:off + n].astype(np.uint32), want) and (h[:off] == -7).all() and (h[off + n:] == -7).all(), k
+    e.close()
+
+
+def test_no_output_is_an_error(lib):
+    """every entry needs at least one output; the emulation entry keeps its logits mandatory"""
+    import torch
+    from bitnetmcu_b200 import _lib
+    e = _engine(load_model("fc"))
+    imgs = _images(300)
+    d_img = torch.from_numpy(imgs).cuda()
+    d_x = torch.zeros((300, 256), dtype=torch.float32, device="cuda")
+    h = e.handle
+    assert lib.bnm_infer_batch(h, C.c_void_p(imgs.ctypes.data), 300, None, None) == -1
+    assert b"no output" in lib.bnm_last_error()
+    assert lib.bnm_infer_batch_device(h, C.c_void_p(d_img.data_ptr()), 300, None, None, None) == -1
+    assert lib.bnm_infer_batch_device_f32(h, C.c_void_p(d_x.data_ptr()), 300, None, None, None) == -1
+    g = _lib.BnmGather()                    # a gather with no destinations is no output either
+    assert lib.bnm_infer_batch_device_gather(h, C.c_void_p(d_img.data_ptr()), 300, None, None, C.byref(g), None) == -1
+    x = np.zeros((300, 256), dtype=np.float32)
+    assert lib.bnm_emulate_inference_quantized(h, C.c_void_p(x.ctypes.data), 300, None) == -1
+    with pytest.raises(ValueError):
+        e.infer(imgs, want_labels=False, want_logits=False)
+    torch.cuda.synchronize()
+    e.close()
+
+
+@pytest.mark.parametrize("name", ["fc", "cnn"])
+def test_c_shim_inference_batch_labels_only(built, oracle, tmp_path, name):
+    """InferenceBatch(images, n, NULL, labels) through the gcc-built plain-C shim"""
+    from test_host_c_shim import _build
+    dll, _, d = _build(str(tmp_path), name)
+    lib = C.CDLL(dll)
+    lib.InferenceBatch.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    lib.InferenceBatch.restype = C.c_int
+    imgs = np.ascontiguousarray(np.concatenate([d["images"], _images(2000, seed=5)]))
+    _, want = oracle.infer(load_model(name), imgs)
+    labels = np.full(len(imgs), 255, dtype=np.uint32)
+    assert lib.InferenceBatch(imgs.ctypes.data, len(imgs), None, labels.ctypes.data) == 0
+    assert np.array_equal(labels, want) and np.array_equal(labels[:10], d["labels"])
+    assert lib.InferenceBatch(imgs.ctypes.data, 1, None, None) != 0
