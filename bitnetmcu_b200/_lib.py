@@ -20,7 +20,7 @@ EXPORTED = [
     "bnm_processfclayer_batch", "bnm_relunorm_batch", "bnm_conv33relu_batch", "bnm_maxpool22_batch",
     "bnm_quantize_images", "bnm_quantize_images_device",
     "bnm_infer_batch_device_gather", "bnm_device_alloc", "bnm_device_free", "bnm_ipc_export", "bnm_ipc_open", "bnm_ipc_close",
-    "bnm_enable_peer_access", "bnm_emulate_inference_quantized", "bnm_infer_batch_device_f32",
+    "bnm_enable_peer_access", "bnm_emulate_inference_quantized", "bnm_infer_batch_device_f32", "bnm_emulate_batch_device",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
@@ -78,6 +78,7 @@ def load() -> C.CDLL:
         "bnm_ipc_export": (C.c_int, [vp, vp]), "bnm_ipc_open": (C.c_int, [C.c_int, vp, C.POINTER(vp)]), "bnm_ipc_close": (C.c_int, [vp]),
         "bnm_enable_peer_access": (C.c_int, [C.c_int, C.c_int]),
         "bnm_emulate_inference_quantized": (C.c_int, [vp, vp, sz, vp]),
+        "bnm_emulate_batch_device": (C.c_int, [vp, vp, sz, vp, vp, vp]),
         "bnm_infer_batch_device_f32": (C.c_int, [vp, vp, sz, vp, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),

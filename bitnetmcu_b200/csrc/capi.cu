@@ -90,6 +90,14 @@ struct bnm_model {
     int32_t *small_h_out = nullptr, *small_d_out = nullptr;  // logits [n][n_classes] then labels [n]
     int8_t *d_f32_scratch = nullptr;   // bnm_infer_batch_device_f32 fallback: quantised images
     size_t f32_scratch_n = 0;
+    // emulation mode (grow-only): the fallback's quantised images and CNN int32 planes, next to the layered path's scratch;
+    // the host entry's device copies of its images and logits
+    int8_t *d_emul_q = nullptr;
+    int32_t *d_emul_planes[2] = {nullptr, nullptr};
+    size_t emul_n = 0;
+    float *d_emul_in = nullptr;
+    double *d_emul_out = nullptr;
+    size_t emul_host_n = 0;
     int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
                                // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
 };
@@ -317,6 +325,11 @@ extern "C" void bnm_model_destroy(bnm_model *m) {
     cudaFree(m->small_d_in);
     cudaFree(m->small_d_out);
     cudaFree(m->d_f32_scratch);
+    cudaFree(m->d_emul_q);
+    cudaFree(m->d_emul_planes[0]);
+    cudaFree(m->d_emul_planes[1]);
+    cudaFree(m->d_emul_in);
+    cudaFree(m->d_emul_out);
     if (m->small_h_in) cudaFreeHost(m->small_h_in);
     if (m->small_h_out) cudaFreeHost(m->small_h_out);
     for (auto &s : m->slots) {
@@ -814,37 +827,44 @@ extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems
 // round-half-even for BitLinear, per-image renormalisation of every conv output) instead of the C engine's.  It reuses the
 // engine's integer kernels (decoded weights, dp4a layers, conv / pool); weight levels are the engine's integers divided by
 // level_scale (2 for 2bitsym / 4bitsym), so every intermediate is an exact dyadic rational and the result equals NumPy's.
+// FC models on the fused path (rows of <= 256 elements, <= 16 classes) run it as one kernel, fc_emul_kernel (fc_wgmma.cu).
 // -----------------------------------------------------------------------------------------------
 static int level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
+static const size_t kEmulChunkFc = 65536, kEmulChunkCnn = 2048;   // images per pass of the layer kernels (CNN: 2 x C kB of planes each)
 
-extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits) {
-    if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_emulate_inference_quantized: null argument");
-    if (n == 0) return 0;
-    CU_TRY(cudaSetDevice(m->device));
+// The emulator on device buffers, asynchronous on st: images float32 [n][img_bytes] -> logits float64 [n][n_classes] and / or labels
+// (first maximum).  Path selection follows bnm_infer_batch_device_f32.  The fallback runs in chunks through the model's scratch
+// arena, which the layer-by-layer path shares: like that path, one stream at a time per model.
+static int emulate_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, cudaStream_t st) {
+    const size_t nl = m->fc.size();
+    const int out_shift = level_shift_of(m->fc[nl - 1].enc);   // logits = last layer's accumulators / its level scale
+    const bool fused_fc = bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST;
+    if (fused_fc && fc_chain_float_input_supported(m->plan)) {
+        int rc = fc_chain_launch_emul(m->plan, images, n, out_shift, logits, labels, st);
+        return rc ? fail(BNM_E_CUDA, "fused emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
+    }
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
     const uint32_t C = m->channels, elems = m->img_bytes;
-    const size_t chunk = std::min<size_t>(n, cnn ? 2048 : 65536);
-    const size_t nl = m->fc.size();
-    uint32_t max_nout = 1, max_kpad = round_up(std::max(m->img_bytes, m->feat_stride), 32);
-    for (auto &L : m->fc) { max_nout = std::max(max_nout, L.n_out); max_kpad = std::max(max_kpad, L.k_pad); }
-    DevBuf d_f, d_q, d_acc, d_a0, d_a1, d_p0, d_p1;
-    if (d_f.alloc(chunk * elems * 4) || d_q.alloc(chunk * elems) || d_acc.alloc(chunk * (size_t)max_nout * 4) || d_a0.alloc(chunk * (size_t)max_kpad) ||
-        d_a1.alloc(chunk * (size_t)max_kpad) || (cnn && (d_p0.alloc(chunk * C * 256 * 4) || d_p1.alloc(chunk * C * 256 * 4))))
-        return fail(BNM_E_CUDA, "cudaMalloc failed (emulation scratch)");
-    CU_TRY(cudaMemset(d_a0.p, 0, chunk * (size_t)max_kpad));
-    CU_TRY(cudaMemset(d_a1.p, 0, chunk * (size_t)max_kpad));
-    std::vector<int32_t> h_acc(chunk * (size_t)m->n_classes);
-    cudaStream_t st = 0;
+    const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
+    if (int rc = ensure_scratch(m, chunk, true)) return rc;   // accumulators and the two int8 activation buffers
+    if (m->emul_n < chunk) {
+        cudaFree(m->d_emul_q); cudaFree(m->d_emul_planes[0]); cudaFree(m->d_emul_planes[1]);
+        m->d_emul_q = nullptr; m->d_emul_planes[0] = m->d_emul_planes[1] = nullptr; m->emul_n = 0;
+        CU_TRY(cudaMalloc(&m->d_emul_q, chunk * elems));
+        if (cnn)
+            for (auto &p : m->d_emul_planes) CU_TRY(cudaMalloc(&p, chunk * C * 256 * 4));
+        m->emul_n = chunk;
+    }
+    int8_t *q = m->d_emul_q, *a0 = m->d_act[0], *a1 = m->d_act[1];
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
-        CU_TRY(cudaMemcpy(d_f.p, images + b * elems, nb * elems * 4, cudaMemcpyHostToDevice));
-        launch_quantize_images(d_f.as<float>(), elems, d_q.as<int8_t>(), nb, st);   // BitNetMCU.py:435-436
-        const int8_t *act = d_q.as<int8_t>();
+        launch_quantize_images(images + b * elems, elems, q, nb, st);   // BitNetMCU.py:435-436
+        const int8_t *act = q;
         uint32_t stride = elems;
         if (cnn) {
             // conv (ReLU, no shift) -> per-image renormalisation, pools in between (BitNetMCU.py:459-526), planes [(image, channel)][xy*xy]
-            int32_t *p0 = d_p0.as<int32_t>(), *p1 = d_p1.as<int32_t>();
-            launch_expand_image(d_q.as<int8_t>(), p0, C, 256, nb, st);
+            int32_t *p0 = m->d_emul_planes[0], *p1 = m->d_emul_planes[1];
+            launch_expand_image(q, p0, C, 256, nb, st);
             launch_conv33relu(p0, m->d_conv[0], C, 16, 0, p1, nb * C, st);
             launch_conv_renorm(p1, C * 196, nb, st);
             launch_conv33relu(p1, m->d_conv[1], C, 14, 0, p0, nb * C, st);
@@ -853,23 +873,56 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
             launch_conv33relu(p1, m->d_conv[2], C, 6, 0, p0, nb * C, st);
             launch_conv_renorm(p0, C * 16, nb, st);
             launch_maxpool22(p0, 4, p1, nb * C, st);
-            launch_i32_to_i8(p1, C * 4, d_a1.as<int8_t>(), m->feat_stride, nb, st);   // flatten (C, 2, 2) -> features (BitNetMCU.py:443-445)
-            act = d_a1.as<int8_t>();
+            launch_i32_to_i8(p1, C * 4, a1, m->feat_stride, nb, st);   // flatten (C, 2, 2) -> features (BitNetMCU.py:443-445)
+            act = a1;
             stride = m->feat_stride;
         }
         for (size_t l = 0; l < nl; l++) {
-            if (!launch_fc_dp4a(act, stride, m->fc[l], d_acc.as<int32_t>(), nb, st)) return fail(BNM_E_UNSUPPORTED, "FC layer %zu too wide for the layer kernel", l);
+            if (!launch_fc_dp4a(act, stride, m->fc[l], m->d_acc, nb, st)) return fail(BNM_E_UNSUPPORTED, "FC layer %zu too wide for the layer kernel", l);
             if (l + 1 == nl) break;   // no renormalisation for the last layer (BitNetMCU.py:528-530)
-            int8_t *next = (l & 1) ? d_a1.as<int8_t>() : d_a0.as<int8_t>();   // CNN features sit in d_a1 and are dead once layer 0 has run
+            int8_t *next = (l & 1) ? a1 : a0;   // CNN features sit in a1 and are dead once layer 0 has run
             const uint32_t next_stride = m->fc[l + 1].k_pad;
-            launch_relunorm_emul(d_acc.as<int32_t>(), m->fc[l].n_out, level_shift_of(m->fc[l].enc), next, next_stride, nb, st);
+            launch_relunorm_emul(m->d_acc, m->fc[l].n_out, level_shift_of(m->fc[l].enc), next, next_stride, nb, st);
             act = next;
             stride = next_stride;
         }
-        CU_TRY(cudaGetLastError());
-        CU_TRY(cudaMemcpy(h_acc.data(), d_acc.p, nb * (size_t)m->n_classes * 4, cudaMemcpyDeviceToHost));
-        const double inv = 1.0 / (double)(1 << level_shift_of(m->fc[nl - 1].enc));
-        for (size_t i = 0; i < nb * (size_t)m->n_classes; i++) logits[b * m->n_classes + i] = (double)h_acc[i] * inv;
+        launch_emul_logits(m->d_acc, m->n_classes, out_shift, logits ? logits + b * m->n_classes : nullptr, labels ? labels + b : nullptr, nb, st);
+    }
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+}
+
+extern "C" int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream) {
+    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_emulate_batch_device: null argument");
+    if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_emulate_batch_device: no output (logits and labels both NULL)");
+    if (n == 0) return 0;
+    if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
+    if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned");
+    CU_TRY(cudaSetDevice(m->device));
+    return emulate_device(m, images, n, logits, labels, static_cast<cudaStream_t>(stream));
+}
+
+// host buffers: per chunk, images in -> emulate_device -> logits out, synchronously
+extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits) {
+    if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_emulate_inference_quantized: null argument");
+    if (n == 0) return 0;
+    CU_TRY(cudaSetDevice(m->device));
+    const size_t elems = m->img_bytes, ncls = m->n_classes;
+    const size_t chunk = std::min(n, m->model_class == BNM_MODEL_CNNMNIST ? kEmulChunkCnn : kEmulChunkFc);
+    if (m->emul_host_n < chunk) {
+        cudaFree(m->d_emul_in); cudaFree(m->d_emul_out);
+        m->d_emul_in = nullptr; m->d_emul_out = nullptr; m->emul_host_n = 0;
+        CU_TRY(cudaMalloc(&m->d_emul_in, chunk * elems * sizeof(float)));
+        CU_TRY(cudaMalloc(&m->d_emul_out, chunk * ncls * sizeof(double)));
+        m->emul_host_n = chunk;
+    }
+    cudaStream_t st = m->slots[0].stream;
+    for (size_t b = 0; b < n; b += chunk) {
+        const size_t nb = std::min(chunk, n - b);
+        CU_TRY(cudaMemcpyAsync(m->d_emul_in, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
+        if (int rc = emulate_device(m, m->d_emul_in, nb, m->d_emul_out, nullptr, st)) return rc;
+        CU_TRY(cudaMemcpyAsync(logits + b * ncls, m->d_emul_out, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
     }
     return 0;
 }

@@ -67,6 +67,10 @@ struct ChainParams {
     const float *fimages;             // float-input launches: float32 [n][in_elems] instead of the int8 tensor map
     uint32_t in_elems;                // real elements per image row (<= 256 for the float path)
     uint32_t off_fring;               // float-input launches: smem offset of the quantiser warps' float rings (8 warps x 2 slots x 4 kB)
+    // emulator launches (fc_emul_kernel): float64 logits [n][n_classes] (or null) = last layer's accumulators x logit_scale, the
+    // emulator's 2^-level_shift of that layer's encoding (0.5 for 2bitsym / 4bitsym, else 1)
+    double *emul_logits;
+    double emul_logit_scale;
 };
 
 struct ChainKernel;
@@ -80,6 +84,7 @@ struct FcChainPlan {
     uint32_t in_bytes = 0;
     const ChainKernel *kernel = nullptr;       // the instantiation of int8 launches
     const ChainKernel *kernel_f32 = nullptr;   // and of float-input launches (null: not supported)
+    const ChainKernel *kernel_emul = nullptr;  // fc_emul_kernel: with kernel_f32, on its shared-memory layout (f_* below)
     int sm_count = 0;
     int device = 0;
     int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 plain launch, 1 dependent launch + wait, 2 independent launches
@@ -140,6 +145,38 @@ __device__ __forceinline__ uint32_t norm_pack4(uint32_t x0, uint32_t x1, uint32_
     asm("mul.lo.u32 %0, %1, %2;" : "=r"(z3) : "r"((uint32_t)__viaddmin_s32_relu((int)x3, c.rounding, c.cap)), "r"(c.mult));
     uint32_t lo = __byte_perm(z0, z1, 0x0073), hi = __byte_perm(z2, z3, 0x0073);
     return __byte_perm(lo, hi, 0x5410);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// The hidden-layer rule of the reference's Python emulator (BitNetMCU.py:452-457, restated in k_relunorm_emul) in registers:
+//   out = round_half_even(relu(acc) * 2^e),  e = floor(log2(127 / m)),  m = row maximum;  m <= 0: the whole row is zero.
+// The emulator divides acc by the level scale 2^ls before it takes the maximum and multiplies by 2^floor(log2(127 * 2^ls / m))
+// after: the 2^ls cancels exactly, so e does not depend on the encoding.  With z = clz(m) (bit length 32 - z), m << z lies in
+// [2^31, 2^32): e = z - 25, minus 1 when m << z exceeds 127 << 25.  m * 2^e <= 127, so the clip to 127 never triggers.
+// Per element, with t = relu(v) * 2^max(e, 0) and s = max(-e, 0):  q = (t + 2^(s-1) - 1 + ((t >> s) & 1)) >> s  (round half to
+// even; for s = 0 both addends are zero).  t < 2^31 and 2^(s-1) <= 2^24, so the unsigned sum does not wrap.
+// ---------------------------------------------------------------------------------------------------
+struct EmulCoef { uint32_t mult, s, bias, odd; };
+
+__device__ __forceinline__ EmulCoef emul_coef(int row_max_relu) {
+    const uint32_t m = (uint32_t)max(row_max_relu, 1);   // m = 0: every v <= 0, any e gives zeros -- take m = 1 (no shift by 32)
+    const uint32_t z = __clz(m);
+    const int e = (int)z - 25 - ((m << z) > (127u << 25) ? 1 : 0);
+    EmulCoef c;
+    c.mult = e > 0 ? 1u << e : 1u;
+    c.s = e < 0 ? (uint32_t)-e : 0u;
+    c.bias = c.s ? (1u << (c.s - 1)) - 1u : 0u;
+    c.odd = c.s ? 1u : 0u;
+    return c;
+}
+__device__ __forceinline__ uint32_t emul_q(uint32_t x, const EmulCoef &c) {
+    uint32_t t;
+    asm("mul.lo.u32 %0, %1, %2;" : "=r"(t) : "r"((uint32_t)max((int)x, 0)), "r"(c.mult));   // an IMAD, as in norm_pack4
+    return (t + c.bias + ((t >> c.s) & c.odd)) >> c.s;
+}
+// four int32 accumulators -> four int8 (0..127) packed little-endian, emulator rule
+__device__ __forceinline__ uint32_t norm_pack4(uint32_t x0, uint32_t x1, uint32_t x2, uint32_t x3, const EmulCoef &c) {
+    return __byte_perm(__byte_perm(emul_q(x0, c), emul_q(x1, c), 0x0040), __byte_perm(emul_q(x2, c), emul_q(x3, c), 0x0040), 0x5410);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -236,10 +273,13 @@ struct RingPos {
 // kLastN: wgmma width of the last layer -- 16 when the plan's last layer is at most 16 wide (every classifier head), else kN.
 // kFixed: the two-slot kernel specialised for the shape class above: no plane loop, no zero-tile selects, layer 1 issued as
 // one unrolled run of MMAs at compile-time descriptor offsets, ReLUNorm without predicates.
-template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
-__global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn, kSlots>(), 1)
-fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+// kEmul: the reference's Python emulator instead of the C engine (fc_emul_kernel): its hidden-layer rule (emul_coef) and float64
+// logits (P.emul_logits); no result exchange.
+// The body of both kernels below; tmap_in and P are their __grid_constant__ parameters (TMA reads the tensor map by address).
+template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, bool kEmul>
+__device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const ChainParams &P) {
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
+    static_assert(!kEmul || (kFloatIn && kN == 64), "emulator: the 64-wide float-input launch");
     static_assert(!kFloatIn || kPipes == 1, "float input: one pipe, whose stages the quantiser warps fill");
     static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
     static_assert(!kFixed || (kSlots == 2 && kLastN == fixed_n_pad(kFixedLayers - 1)), "fixed shape: two-slot launches of its class");
@@ -333,7 +373,7 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
         const uint32_t ncls = P.n_classes;
         // labels-only launches pass no logits buffer.  The shuffle is a value no-op (a uniform flag), kept for ptxas: testing
         // P.logits at the store instead serialises the fixed-shape kernel's wgmma pipeline (C7511, CUDA 12.9).
-        const bool has_logits = __shfl_sync(0xffffffffu, (uint32_t)(P.logits != nullptr), 0);
+        const bool has_logits = __shfl_sync(0xffffffffu, (uint32_t)(kEmul ? P.emul_logits != nullptr : P.logits != nullptr), 0);
         mbar_wait(&bar_w, 0, P.err, 6);   // weight tiles are in shared memory
         // B descriptor of the 64 columns from c0 of the K-step tile at smem address t (no-swizzle K-major: 8-row groups 256 B apart).
         // Every wgmma is issued at the kernel's full width kN, with no condition around it (a conditional wgmma cannot stay in
@@ -394,7 +434,8 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
             m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
             m0 = max(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
             m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-            const NormCoef k0 = norm_coef(m0), k1 = norm_coef(m1);
+            auto coef = [](int m) { if constexpr (kEmul) return emul_coef(m); else return norm_coef(m); };
+            const auto k0 = coef(m0), k1 = coef(m1);
             // 16-column block b -> register 2b (upper row) / 2b + 1 (lower row) of the fragments, i.e. for K-step s = b / 2:
             // f[4s] (upper row, block 2s), f[4s + 1] (lower, 2s), f[4s + 2] (upper, 2s + 1), f[4s + 3] (lower, 2s + 1)
 #pragma unroll
@@ -473,7 +514,20 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
                     const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, sh);
                     if (ob > best || (ob == best && op < pos)) { best = ob; pos = op; }
                 }
-                if (img < P.n) {
+                if (kEmul && img < P.n) {
+                    // float64 logits: (double)acc x 2^-level_shift is exact, and argmax of the int32 accumulators is that of them
+                    if (has_logits) {
+                        double *d = P.emul_logits + img * ncls;
+                        const double sc = P.emul_logit_scale;
+#pragma unroll
+                        for (int j = 0; j < kLastN / 8; j++) {
+                            const uint32_t col = 8 * j + 2 * quad;
+                            if (col < ncls) d[col] = (double)(int)a[4 * j + 2 * r] * sc;
+                            if (col + 1 < ncls) d[col + 1] = (double)(int)a[4 * j + 2 * r + 1] * sc;
+                        }
+                    }
+                    if (quad == 0 && P.labels) P.labels[img] = pos;
+                } else if (img < P.n) {
                     auto store_row = [&](int32_t *d) {
 #pragma unroll
                         for (int j = 0; j < kLastN / 8; j++) {
@@ -675,6 +729,19 @@ fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_consta
     }
 }
 
+template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
+__global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn, kSlots>(), 1)
+fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed, false>(tmap_in, P);
+}
+
+// QuantizedModel.inference_quantized (BitNetMCU.py:420-535) of FC models: the float-input launch <64,1,float> with the emulator's
+// hidden-layer rule and float64 logits.  The input scaling of BitNetMCU.py:435-436 is the quantiser warps' (test_inference.py:140-141).
+__global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
+fc_emul_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<64, 1, true, 1, 64, false, true>(tmap_in, P);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -741,6 +808,7 @@ static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
     t[kRowFloat] = chain_kernel<64, 1, true>("<64,1,float>");
     return t;
 }();
+static const ChainKernel kEmulKernel = {"<64,1,float,emul>", fc_emul_kernel, chain_threads<64, 1, true, 1>()};
 
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
                                   char *err, size_t err_len) {
@@ -802,12 +870,14 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
             plan->f_off_fring = plan->f_off_w + w_fixed;
             plan->f_smem_bytes = std::max<size_t>((size_t)plan->f_off_fring + fring + 1024, 116 * 1024);
             plan->kernel_f32 = &kChainKernels[kRowFloat];
+            plan->kernel_emul = &kEmulKernel;
         }
     }
     if (getenv("BNM_VERBOSE"))   // diagnostics: the shapes this plan launches
         fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, "
-                "fc_chain_kernel%s%s%s\n", max_n, pipes, p.n_stages, p.w_bytes, plan->smem_bytes, plan->kernel->name,
-                plan->kernel_f32 ? ", float input " : "", plan->kernel_f32 ? plan->kernel_f32->name : "");
+                "fc_chain_kernel%s%s%s%s%s\n", max_n, pipes, p.n_stages, p.w_bytes, plan->smem_bytes, plan->kernel->name,
+                plan->kernel_f32 ? ", float input " : "", plan->kernel_f32 ? plan->kernel_f32->name : "",
+                plan->kernel_emul ? ", emulator " : "", plan->kernel_emul ? plan->kernel_emul->name : "");
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
     plan->device = device;
@@ -832,7 +902,8 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     p.w_image = plan->d_w_image;
     p.err = plan->d_err;
     if (!raise_smem_limit((const void *)plan->kernel->fn, plan->smem_bytes) ||
-        (plan->kernel_f32 && !raise_smem_limit((const void *)plan->kernel_f32->fn, plan->f_smem_bytes))) {
+        (plan->kernel_f32 && !raise_smem_limit((const void *)plan->kernel_f32->fn, plan->f_smem_bytes)) ||
+        (plan->kernel_emul && !raise_smem_limit((const void *)plan->kernel_emul->fn, plan->f_smem_bytes))) {
         fc_chain_plan_destroy(plan);
         return fail("cannot opt in to the required dynamic shared memory");
     }
@@ -935,13 +1006,9 @@ bool fc_chain_float_input_supported(const FcChainPlan *plan) {
     return plan && plan->kernel_f32 && plan->in_bytes % 16 == 0;
 }
 
-// float32 images [n][in_bytes elements] -> logits / labels (either may be null), the input scaling fused into the load stage (kFloatIn)
-int fc_chain_launch_f32(FcChainPlan *plan, const float *in, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st) {
-    if (n == 0) return 0;
-    if (n > 0x7fffff00ull) return -2;
-    if (!fc_chain_float_input_supported(plan)) return -6;
-    ChainParams p = plan->p;
-    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_f32, plan->f_smem_bytes, n, logits, labels, st, p);
+// a launch of kernel k (kernel_f32 or kernel_emul) on float32 images [n][in_bytes elements], the input scaling fused into the load
+// stage (kFloatIn); p holds the outputs
+static int launch_float_input(FcChainPlan *plan, const ChainKernel *k, cudaLaunchConfig_t &cfg, ChainParams &p, const float *in) {
     p.fimages = in;
     p.in_elems = plan->in_bytes;
     p.n_stages = plan->f_n_stages;
@@ -952,8 +1019,29 @@ int fc_chain_launch_f32(FcChainPlan *plan, const float *in, size_t n, int32_t *l
     CUtensorMap tmap;   // not used by the float-input kernel (no TMA image loads)
     memset(&tmap, 0, sizeof(tmap));
     plan->prev_valid = false;
-    if (cudaLaunchKernelEx(&cfg, plan->kernel_f32->fn, tmap, p) != cudaSuccess) return -4;
+    if (cudaLaunchKernelEx(&cfg, k->fn, tmap, p) != cudaSuccess) return -4;
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
+}
+
+// float32 images [n][in_bytes elements] -> logits / labels (either may be null)
+int fc_chain_launch_f32(FcChainPlan *plan, const float *in, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st) {
+    if (n == 0) return 0;
+    if (n > 0x7fffff00ull) return -2;
+    if (!fc_chain_float_input_supported(plan)) return -6;
+    ChainParams p = plan->p;
+    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_f32, plan->f_smem_bytes, n, logits, labels, st, p);
+    return launch_float_input(plan, plan->kernel_f32, cfg, p, in);
+}
+
+int fc_chain_launch_emul(FcChainPlan *plan, const float *in, size_t n, int level_shift, double *logits, uint32_t *labels, cudaStream_t st) {
+    if (n == 0) return 0;
+    if (n > 0x7fffff00ull) return -2;
+    if (!fc_chain_float_input_supported(plan) || !plan->kernel_emul) return -6;
+    ChainParams p = plan->p;
+    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_emul, plan->f_smem_bytes, n, nullptr, labels, st, p);
+    p.emul_logits = logits;
+    p.emul_logit_scale = level_shift ? 0.5 : 1.0;
+    return launch_float_input(plan, plan->kernel_emul, cfg, p, in);
 }
 
 }  // namespace bnm

@@ -345,6 +345,26 @@ __global__ void k_i32_to_i8(const int32_t *__restrict__ in, uint32_t n_in, int8_
     out[idx] = c < n_in ? (int8_t)in[row * n_in + c] : (int8_t)0;
 }
 
+// one thread per image: logits = acc x 2^-level_shift (exact in float64), label = first maximum
+__global__ void k_emul_logits(const int32_t *__restrict__ acc, uint32_t n_cls, double scale, double *__restrict__ logits,
+                              uint32_t *__restrict__ labels, size_t n) {
+    const size_t row = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= n) return;
+    const int32_t *x = acc + row * n_cls;
+    int32_t best = x[0];
+    uint32_t pos = 0;
+    for (uint32_t c = 0; c < n_cls; c++) {
+        const int32_t v = x[c];
+        if (logits) logits[row * n_cls + c] = (double)v * scale;
+        if (v > best) { best = v; pos = c; }
+    }
+    if (labels) labels[row] = pos;
+}
+
+void launch_emul_logits(const int32_t *acc, uint32_t n_cls, int level_shift, double *logits, uint32_t *labels, size_t n, cudaStream_t st) {
+    if (n && n_cls) k_emul_logits<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(acc, n_cls, level_shift ? 0.5 : 1.0, logits, labels, n);
+}
+
 void launch_relunorm_emul(const int32_t *in, uint32_t n_in, int level_shift, int8_t *out, uint32_t out_stride, size_t n, cudaStream_t st) {
     if (n) k_relunorm_emul<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(in, n_in, level_shift, out, out_stride, n);
 }

@@ -72,6 +72,9 @@ void launch_relunorm_emul(const int32_t *in, uint32_t n_in, int level_shift, int
 void launch_expand_image(const int8_t *img, int32_t *planes, uint32_t C, uint32_t elems, size_t n, cudaStream_t st);
 void launch_conv_renorm(int32_t *planes, uint32_t elems_per_image, size_t n, cudaStream_t st);
 void launch_i32_to_i8(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t out_stride, size_t n, cudaStream_t st);
+// the last layer's int32 accumulators [n][n_cls] -> float64 logits x 2^-level_shift and first-maximum labels (np.argmax); either
+// output may be null
+void launch_emul_logits(const int32_t *acc, uint32_t n_cls, int level_shift, double *logits, uint32_t *labels, size_t n, cudaStream_t st);
 
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
@@ -92,5 +95,9 @@ int fc_chain_launch(FcChainPlan *p, const int8_t *in, size_t n, int32_t *logits,
 // kernel's load stage; supported for image rows of up to 256 elements and up to 16 classes
 bool fc_chain_float_input_supported(const FcChainPlan *p);
 int fc_chain_launch_f32(FcChainPlan *p, const float *in, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st);
+// the same launch with the reference's Python emulator in place of the C engine (fc_emul_kernel): its hidden-layer rule and float64
+// logits = last layer's accumulators x 2^-level_shift (level_shift 0 or 1); logits / labels may each be null.  Where
+// fc_chain_float_input_supported holds.
+int fc_chain_launch_emul(FcChainPlan *p, const float *in, size_t n, int level_shift, double *logits, uint32_t *labels, cudaStream_t st);
 
 }  // namespace bnm

@@ -130,6 +130,22 @@ class Engine:
         _lib.check(self.lib.bnm_emulate_inference_quantized(self.handle, _ptr(x), x.shape[0], _ptr(out)), "bnm_emulate_inference_quantized")
         return out
 
+    def inference_quantized_device(self, images, logits=None, labels=None, stream: Optional[int] = None) -> None:
+        """``inference_quantized`` on device buffers: images torch.float32 [n, img_bytes] on this GPU -> logits torch.float64
+        [n, n_classes] or None, labels [n] (4-byte elements: ``np.argmax`` of the logits) or None (not both None).  Asynchronous on
+        ``stream`` (a cudaStream_t as int; default: torch's current stream).  FC models up to 64 wide: one kernel."""
+        import torch
+        n = images.shape[0]
+        if stream is None:
+            stream = torch.cuda.current_stream(images.device).cuda_stream
+        assert images.is_contiguous() and images.dtype == torch.float32 and images.shape[1] == self.img_bytes
+        lp = None
+        if logits is not None:
+            assert logits.is_contiguous() and logits.dtype == torch.float64 and tuple(logits.shape) == (n, self.n_classes)
+            lp = C.c_void_p(logits.data_ptr())
+        _lib.check(self.lib.bnm_emulate_batch_device(self.handle, C.c_void_p(images.data_ptr()), n, lp, self._labels_ptr(labels, n),
+                                                     C.c_void_p(stream)), "bnm_emulate_batch_device")
+
     def infer_device_f32(self, images, logits, labels=None, stream: Optional[int] = None) -> None:
         """images: torch.float32 [n, img_bytes] on this GPU (un-normalised pixels, as test_inference.py:140 sees them) -> logits
         torch.int32 [n, n_classes] or None, labels [n] or None (not both None).  FC models: one kernel with the input scaling fused

@@ -208,7 +208,7 @@ BNM_API int bnm_quantize_images_device(const float *images, size_t n, uint32_t e
 /* ---------------------------------------------------------------------------------------------
  * 6. Emulation mode: QuantizedModel.inference_quantized of the reference on the GPU
  *    (/root/reference/BitNetMCU.py:420-535; what exportquant.py:537-559 and test_inference.py:153-154 call per image).
- *    images float32 [n][img_bytes] (host) -> float64 [n][n_classes] (host): the emulator's logits, i.e. WITH its normalisation
+ *    images float32 [n][img_bytes] -> float64 [n][n_classes] (host or device buffers): the emulator's logits, i.e. WITH its normalisation
  *    rules (rescale = 2^floor(log2(127/max)), np.round; per-image conv renormalisation), which differ from the C engine's by
  *    design (SURVEY.md section 4).  Exact for Binary / Ternary / 2bitsym / 4bitsym / 8bit / FP130 weights; the reference's
  *    "4bit" levels carry a +0.01 offset (BitNetMCU.py:159) and NF4 levels are non-dyadic: those two are approximated by the
@@ -216,6 +216,15 @@ BNM_API int bnm_quantize_images_device(const float *images, size_t n, uint32_t e
  * ------------------------------------------------------------------------------------------- */
 /* logits are this entry's only output and may not be NULL (BNM_E_ARG) */
 BNM_API int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits);
+/* QuantizedModel.inference_quantized on device buffers, asynchronous on `stream`.  images float32 [n][img_bytes] (16-byte
+ * aligned) -> logits float64 [n][n_classes] (8-byte aligned), the emulator's logits bit for bit, and / or labels uint32 [n] =
+ * np.argmax of them (first maximum).  logits or labels may be NULL, not both (BNM_E_ARG).  Results equal those of
+ * bnm_emulate_inference_quantized.  FC models on the fused path (image rows of <= 256 elements, <= 16 classes, <= 64 wide, the
+ * models of bnm_infer_batch_device_f32's one-kernel path) run ONE kernel: the float-input kernel with the emulator's hidden-layer
+ * rule and float64 logits.  Every other model runs the emulation kernels layer by layer through scratch the model owns (grown on
+ * the first large call, then reused): calls on one model must then not overlap in time on different streams.  Either way the
+ * call makes no host synchronisation once its scratch has grown. */
+BNM_API int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream);
 
 #ifdef __cplusplus
 }
