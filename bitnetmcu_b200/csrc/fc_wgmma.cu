@@ -873,11 +873,14 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
             plan->kernel_emul = &kEmulKernel;
         }
     }
-    if (getenv("BNM_VERBOSE"))   // diagnostics: the shapes this plan launches
+    if (getenv("BNM_VERBOSE")) {   // diagnostics: the shapes this plan launches
+        char f_stages[32] = "";
+        if (plan->kernel_f32) snprintf(f_stages, sizeof(f_stages), ", float input stages %u", plan->f_n_stages);
         fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, "
-                "fc_chain_kernel%s%s%s%s%s\n", max_n, pipes, p.n_stages, p.w_bytes, plan->smem_bytes, plan->kernel->name,
+                "fc_chain_kernel%s%s%s%s%s%s\n", max_n, pipes, p.n_stages, p.w_bytes, plan->smem_bytes, plan->kernel->name,
                 plan->kernel_f32 ? ", float input " : "", plan->kernel_f32 ? plan->kernel_f32->name : "",
-                plan->kernel_emul ? ", emulator " : "", plan->kernel_emul ? plan->kernel_emul->name : "");
+                plan->kernel_emul ? ", emulator " : "", plan->kernel_emul ? plan->kernel_emul->name : "", f_stages);
+    }
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
     plan->device = device;

@@ -224,7 +224,8 @@ def test_fused_equals_layered_and_restatement(lib, capfd, monkeypatch, idx):
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", [1, 127, 128, 129, 148 * 128 * 2 + 77])
 def test_batch_sizes(lib, n):
-    """ragged tiles, one tile, several tiles per CTA; twice in a row (the stage ring wraps, the launch is repeatable)"""
+    """ragged tiles, one tile, several tiles per CTA; twice in a row (the launch is repeatable: each one starts its ring at stage
+    0, phase 0; tests/test_fc_ring_rounds.py runs the ring past its first rounds)"""
     m = load_model("fc")
     x = _float_images(n, 256, seed=n)
     want = emulate_fc(m, x)

@@ -683,7 +683,7 @@ def test_float_input_fused_into_the_fc_kernel(lib, oracle, name, n):
     d_x = torch.from_numpy(x).cuda()
     d_log = torch.empty((n, m.n_classes), dtype=torch.int32, device="cuda")
     d_lab = torch.empty(n, dtype=torch.int32, device="cuda")
-    for _ in range(2):                      # twice: the stage ring wraps and the launch is repeatable
+    for _ in range(2):                      # twice: the launch is repeatable (each one starts its ring at stage 0, phase 0)
         e.infer_device_f32(d_x, d_log, d_lab)
     torch.cuda.synchronize()
     got = d_log.cpu().numpy()

@@ -132,7 +132,7 @@ def _float_case(e, m, oracle, n):
     _, want = oracle.infer(m, q)
     d_x = torch.from_numpy(x).cuda()
     d_lab = torch.full((n,), -1, dtype=torch.int32, device="cuda")
-    for _ in range(2):                      # twice: the stage ring wraps and the launch is repeatable
+    for _ in range(2):                      # twice: the launch is repeatable (each one starts its ring at stage 0, phase 0)
         e.infer_device_f32(d_x, None, d_lab)
     torch.cuda.synchronize()
     assert np.array_equal(d_lab.cpu().numpy().astype(np.uint32), want)
