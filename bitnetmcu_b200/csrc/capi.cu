@@ -98,6 +98,8 @@ struct bnm_model {
     float *d_emul_in = nullptr;
     double *d_emul_out = nullptr;
     size_t emul_host_n = 0;
+    int8_t *d_emul_rows = nullptr;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
+    size_t emul_rows_n = 0;
     int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
                                // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
 };
@@ -200,6 +202,16 @@ static int ensure_scratch(bnm_model *m, size_t n, bool layered) {
 }
 
 static int require_device_index(int device);
+
+// the kernels of the emulator (emulate_device): fc_emul_kernel on float images; fc_emul_i8_kernel after the scaling kernel (FC)
+// or k_cnn_emul_frontend (CNN); or the emulation kernels layer by layer
+enum EmulRoute { kEmulFloatRow, kEmulInt8Row, kEmulLayers };
+static EmulRoute emul_route(const bnm_model *m) {
+    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
+    if (bnm_model_active_path(m) != BNM_PATH_TCGEN05 || (cnn && m->channels > kCnnEmulMaxChannels)) return kEmulLayers;
+    return !cnn && fc_chain_float_input_supported(m->plan) ? kEmulFloatRow : kEmulInt8Row;
+}
+
 extern "C" int bnm_version(void) { return BNM_VERSION; }
 extern "C" const char *bnm_last_error(void) { return g_err.c_str(); }
 extern "C" int bnm_device_count(void) {
@@ -288,6 +300,13 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
             if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaStreamCreate failed"); break; }
     }
     if (rc != 0) { std::string keep = g_err; bnm_model_destroy(m); g_err = keep; return rc; }
+    if (getenv("BNM_VERBOSE")) {   // diagnostics: the kernels bnm_emulate_batch_device runs on the default path
+        const EmulRoute r = emul_route(m);
+        fprintf(stderr, "bitnetmcu_b200: emulator route: %s%s\n",
+                r == kEmulLayers ? "layer by layer" : r == kEmulFloatRow ? "fc_emul_kernel" :
+                m->model_class == BNM_MODEL_CNNMNIST ? "k_cnn_emul_frontend + fc_emul_i8_kernel" : "k_quantize_images + fc_emul_i8_kernel",
+                r == kEmulLayers ? "" : fc_chain_emul_name(m->plan, r == kEmulFloatRow));
+    }
     *out = m;
     return 0;
 }
@@ -330,6 +349,7 @@ extern "C" void bnm_model_destroy(bnm_model *m) {
     cudaFree(m->d_emul_planes[1]);
     cudaFree(m->d_emul_in);
     cudaFree(m->d_emul_out);
+    cudaFree(m->d_emul_rows);
     if (m->small_h_in) cudaFreeHost(m->small_h_in);
     if (m->small_h_out) cudaFreeHost(m->small_h_out);
     for (auto &s : m->slots) {
@@ -827,24 +847,49 @@ extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems
 // round-half-even for BitLinear, per-image renormalisation of every conv output) instead of the C engine's.  It reuses the
 // engine's integer kernels (decoded weights, dp4a layers, conv / pool); weight levels are the engine's integers divided by
 // level_scale (2 for 2bitsym / 4bitsym), so every intermediate is an exact dyadic rational and the result equals NumPy's.
-// FC models on the fused path (rows of <= 256 elements, <= 16 classes) run it as one kernel, fc_emul_kernel (fc_wgmma.cu).
+// On the fused path (fc_wgmma.cu):
+//   * FC models whose rows have <= 256 elements, up to 64 wide with <= 16 classes: one kernel, fc_emul_kernel;
+//   * other FC models: the scaling kernel (k_quantize_images), then fc_emul_i8_kernel at the plan's width;
+//   * CNN models up to kCnnEmulMaxChannels channels: the front-end kernel k_cnn_emul_frontend, then fc_emul_i8_kernel on its features.
+// BNM_PATH_LAYERS, models without a fused plan and wider CNN models run the emulation kernels layer by layer.
 // -----------------------------------------------------------------------------------------------
 static int level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
 static const size_t kEmulChunkFc = 65536, kEmulChunkCnn = 2048;   // images per pass of the layer kernels (CNN: 2 x C kB of planes each)
 
 // The emulator on device buffers, asynchronous on st: images float32 [n][img_bytes] -> logits float64 [n][n_classes] and / or labels
-// (first maximum).  Path selection follows bnm_infer_batch_device_f32.  The fallback runs in chunks through the model's scratch
-// arena, which the layer-by-layer path shares: like that path, one stream at a time per model.
+// (first maximum).  The routes other than fc_emul_kernel run in chunks through scratch the model owns (grow-only), which the
+// layer-by-layer path shares: like that path, one stream at a time per model.
 static int emulate_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, cudaStream_t st) {
     const size_t nl = m->fc.size();
     const int out_shift = level_shift_of(m->fc[nl - 1].enc);   // logits = last layer's accumulators / its level scale
-    const bool fused_fc = bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST;
-    if (fused_fc && fc_chain_float_input_supported(m->plan)) {
+    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
+    const uint32_t C = m->channels, elems = m->img_bytes;
+    const EmulRoute route = emul_route(m);
+    if (route == kEmulFloatRow) {
         int rc = fc_chain_launch_emul(m->plan, images, n, out_shift, logits, labels, st);
         return rc ? fail(BNM_E_CUDA, "fused emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    const uint32_t C = m->channels, elems = m->img_bytes;
+    if (route == kEmulInt8Row) {
+        const size_t chunk = std::min(n, kFusedCnnChunk);
+        const size_t row_bytes = cnn ? m->feat_stride : elems;
+        if (m->emul_rows_n < chunk) {
+            cudaFree(m->d_emul_rows);
+            m->d_emul_rows = nullptr; m->emul_rows_n = 0;
+            CU_TRY(cudaMalloc(&m->d_emul_rows, chunk * row_bytes));
+            m->emul_rows_n = chunk;
+        }
+        for (size_t b = 0; b < n; b += chunk) {
+            const size_t nb = std::min(chunk, n - b);
+            if (!cnn) launch_quantize_images(images + b * elems, elems, m->d_emul_rows, nb, st);   // BitNetMCU.py:435-436
+            else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0], m->d_conv[1], m->d_conv[2], C, m->d_emul_rows, m->feat_stride, nb, st))
+                return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
+            int rc = fc_chain_launch_emul_i8(m->plan, m->d_emul_rows, nb, out_shift, logits ? logits + b * m->n_classes : nullptr,
+                                             labels ? labels + b : nullptr, st);
+            if (rc) return fail(BNM_E_CUDA, "fused int8 emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+        }
+        cudaError_t e = cudaGetLastError();
+        return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+    }
     const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
     if (int rc = ensure_scratch(m, chunk, true)) return rc;   // accumulators and the two int8 activation buffers
     if (m->emul_n < chunk) {

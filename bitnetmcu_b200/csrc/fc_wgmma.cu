@@ -91,6 +91,11 @@ struct FcChainPlan {
     // float-input launches: one pipe, fewer int8 stages, the freed shared memory holds the quantiser warps' float rings
     uint32_t f_n_stages = 0, f_off_w = 0, f_off_fring = 0;
     size_t f_smem_bytes = 0;
+    // emulator launches on int8 rows (fc_emul_i8_kernel at the plan's width): one pipe, so a 64-wide plan, whose int8 launches run
+    // two, needs its own stage count and shared-memory layout
+    const ChainKernel *kernel_emul_i8 = nullptr;
+    uint32_t e_n_stages = 0, e_off_w = 0;
+    size_t e_smem_bytes = 0;
     struct TmapSlot { const void *ptr = nullptr; size_t n = 0; CUtensorMap map; };
     TmapSlot tmaps[4];                // tensor maps of the most recent (pointer, n) pairs: double/triple-buffered callers hit every time
     unsigned tmap_next = 0;
@@ -279,7 +284,8 @@ struct RingPos {
 template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, bool kEmul>
 __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const ChainParams &P) {
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
-    static_assert(!kEmul || (kFloatIn && kN == 64), "emulator: the 64-wide float-input launch");
+    static_assert(!kEmul || (kPipes == 1 && kSlots == 1 && kLastN == kN && !kFixed && (kN == 64 || !kFloatIn)),
+                  "emulator: the 64-wide float-input launch, or one-pipe one-slot int8 launches at full width");
     static_assert(!kFloatIn || kPipes == 1, "float input: one pipe, whose stages the quantiser warps fill");
     static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
     static_assert(!kFixed || (kSlots == 2 && kLastN == fixed_n_pad(kFixedLayers - 1)), "fixed shape: two-slot launches of its class");
@@ -742,6 +748,14 @@ fc_emul_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
     fc_chain_body<64, 1, true, 1, 64, false, true>(tmap_in, P);
 }
 
+// The same emulator on int8 rows that are already scaled (k_quantize_images, or the features of k_cnn_emul_frontend): TMA
+// loads, one pipe, one slot, the last layer at the full width kN -- every width, and up to kN classes.
+template <int kN>
+__global__ void __launch_bounds__(chain_threads<kN, 1, false, 1>(), 1)
+fc_emul_i8_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<kN, 1, false, 1, kN, false, true>(tmap_in, P);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -809,6 +823,12 @@ static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
     return t;
 }();
 static const ChainKernel kEmulKernel = {"<64,1,float,emul>", fc_emul_kernel, chain_threads<64, 1, true, 1>()};
+// the instantiations of fc_emul_i8_kernel, row max_n / 64 - 1
+template <int kN>
+static ChainKernel emul_i8_kernel(const char *name) { return {name, fc_emul_i8_kernel<kN>, chain_threads<kN, 1, false, 1>()}; }
+static const std::array<ChainKernel, 4> kEmulI8Kernels = {
+    emul_i8_kernel<64>("<64,1,emul>"), emul_i8_kernel<128>("<128,1,emul>"), emul_i8_kernel<192>("<192,1,emul>"),
+    emul_i8_kernel<256>("<256,1,emul>")};
 
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
                                   char *err, size_t err_len) {
@@ -873,13 +893,19 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
             plan->kernel_emul = &kEmulKernel;
         }
     }
+    // emulator on int8 rows: the one-pipe layout (for max_n > 64 the same as the int8 launches')
+    plan->kernel_emul_i8 = &kEmulI8Kernels[max_n / 64 - 1];
+    plan->e_n_stages = std::min<uint32_t>(total_stages, 6);
+    plan->e_off_w = plan->e_n_stages * p.stage_bytes;
+    plan->e_smem_bytes = std::max<size_t>((size_t)plan->e_off_w + w_fixed + 1024, 116 * 1024);
     if (getenv("BNM_VERBOSE")) {   // diagnostics: the shapes this plan launches
         char f_stages[32] = "";
         if (plan->kernel_f32) snprintf(f_stages, sizeof(f_stages), ", float input stages %u", plan->f_n_stages);
         fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, "
-                "fc_chain_kernel%s%s%s%s%s%s\n", max_n, pipes, p.n_stages, p.w_bytes, plan->smem_bytes, plan->kernel->name,
-                plan->kernel_f32 ? ", float input " : "", plan->kernel_f32 ? plan->kernel_f32->name : "",
-                plan->kernel_emul ? ", emulator " : "", plan->kernel_emul ? plan->kernel_emul->name : "", f_stages);
+                "fc_chain_kernel%s%s%s%s%s%s, int8 emulator fc_emul_i8_kernel%s x %u stages\n", max_n, pipes, p.n_stages, p.w_bytes,
+                plan->smem_bytes, plan->kernel->name, plan->kernel_f32 ? ", float input " : "", plan->kernel_f32 ? plan->kernel_f32->name : "",
+                plan->kernel_emul ? ", emulator " : "", plan->kernel_emul ? plan->kernel_emul->name : "", f_stages,
+                plan->kernel_emul_i8->name, plan->e_n_stages);
     }
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
@@ -906,7 +932,8 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     p.err = plan->d_err;
     if (!raise_smem_limit((const void *)plan->kernel->fn, plan->smem_bytes) ||
         (plan->kernel_f32 && !raise_smem_limit((const void *)plan->kernel_f32->fn, plan->f_smem_bytes)) ||
-        (plan->kernel_emul && !raise_smem_limit((const void *)plan->kernel_emul->fn, plan->f_smem_bytes))) {
+        (plan->kernel_emul && !raise_smem_limit((const void *)plan->kernel_emul->fn, plan->f_smem_bytes)) ||
+        !raise_smem_limit((const void *)plan->kernel_emul_i8->fn, plan->e_smem_bytes)) {
         fc_chain_plan_destroy(plan);
         return fail("cannot opt in to the required dynamic shared memory");
     }
@@ -1045,6 +1072,29 @@ int fc_chain_launch_emul(FcChainPlan *plan, const float *in, size_t n, int level
     p.emul_logits = logits;
     p.emul_logit_scale = level_shift ? 0.5 : 1.0;
     return launch_float_input(plan, plan->kernel_emul, cfg, p, in);
+}
+
+const char *fc_chain_emul_name(const FcChainPlan *plan, bool float_row) {
+    return float_row ? plan->kernel_emul->name : plan->kernel_emul_i8->name;
+}
+
+int fc_chain_launch_emul_i8(FcChainPlan *plan, const int8_t *in, size_t n, int level_shift, double *logits, uint32_t *labels,
+                            cudaStream_t st) {
+    if (n == 0) return 0;
+    if (n > 0x7fffff00ull) return -2;
+    ChainParams p = plan->p;
+    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_emul_i8, plan->e_smem_bytes, n, nullptr, labels, st, p);
+    p.emul_logits = logits;
+    p.emul_logit_scale = level_shift ? 0.5 : 1.0;
+    p.n_stages = plan->e_n_stages;
+    p.off_w = plan->e_off_w;
+    p.wait_prior_grid = 0;   // a plain launch: stream order alone
+    p.early_trigger = 0;
+    const CUtensorMap *tmap_p = plan_tensor_map(plan, in, n);
+    if (!tmap_p) return -3;
+    plan->prev_valid = false;   // the next C-engine launch keeps its grid-dependency wait
+    if (cudaLaunchKernelEx(&cfg, plan->kernel_emul_i8->fn, *tmap_p, p) != cudaSuccess) return -4;
+    return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 
 }  // namespace bnm

@@ -236,6 +236,13 @@ void launch_relunorm(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t out
 // One warp per image; every operation is a single correctly rounded IEEE float32 op (no FMA contraction), so the result
 // is bit-identical to the NumPy expression.
 // ------------------------------------------------------------------------------------------------
+// scale of an image whose largest |x| is absmax, and one pixel scaled with it (k_quantize_images, k_cnn_emul_frontend)
+__device__ __forceinline__ float quant_scale(float absmax) { return __fdiv_rn(127.0f, fmaxf(absmax, 1e-5f)); }
+__device__ __forceinline__ int quant_pixel(float x, float scale) {
+    const float y = rintf(__fmul_rn(x, scale));            // np.round: round half to even
+    return (int)fminf(fmaxf(y, -128.0f), 127.0f);          // .clip(-128, 127)
+}
+
 __global__ void __launch_bounds__(256) k_quantize_images(const float *__restrict__ in, uint32_t elems, int8_t *__restrict__ out, size_t n) {
     const uint32_t lane = threadIdx.x & 31;
     const size_t img = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -245,13 +252,9 @@ __global__ void __launch_bounds__(256) k_quantize_images(const float *__restrict
     for (uint32_t i = lane; i < elems; i += 32) m = fmaxf(m, fabsf(x[i]));
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
-    const float scale = __fdiv_rn(127.0f, fmaxf(m, 1e-5f));
+    const float scale = quant_scale(m);
     int8_t *q = out + img * elems;
-    for (uint32_t i = lane; i < elems; i += 32) {
-        float y = rintf(__fmul_rn(x[i], scale));            // np.round: round half to even
-        y = fminf(fmaxf(y, -128.0f), 127.0f);               // .clip(-128, 127)
-        q[i] = (int8_t)(int)y;
-    }
+    for (uint32_t i = lane; i < elems; i += 32) q[i] = (int8_t)quant_pixel(x[i], scale);
 }
 
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st) {
@@ -316,6 +319,14 @@ __global__ void k_expand_image(const int8_t *__restrict__ img, int32_t *__restri
     planes[idx] = img[(item / C) * elems + idx % elems];
 }
 
+// BitConv2d's renormalisation of one ReLU'd conv output v >= 0 of an image whose conv outputs have the maximum m:
+// round_half_even(v * (127.0 / m)).clip(0, 127), float64 like NumPy (k_conv_renorm, k_cnn_emul_frontend).  m <= 0 (every output
+// is zero): NumPy divides by zero there (nan); the scale 0 defines the result as zeros.
+__device__ __forceinline__ double conv_renorm_scale(int m) { return m > 0 ? 127.0 / (double)m : 0.0; }
+__device__ __forceinline__ int conv_renorm(int v, double scale) {
+    return (int)fmin(fmax(rint(__dmul_rn((double)v, scale)), 0.0), 127.0);
+}
+
 // per image: v = round_half_even(v * (127.0 / max)).clip(0, 127) over its C * H * W conv outputs (already >= 0), float64 like NumPy
 __global__ void __launch_bounds__(256) k_conv_renorm(int32_t *__restrict__ planes, uint32_t elems, size_t n) {
     __shared__ int s_max[8];
@@ -329,12 +340,9 @@ __global__ void __launch_bounds__(256) k_conv_renorm(int32_t *__restrict__ plane
     m = s_max[0];
 #pragma unroll
     for (int w = 1; w < 8; w++) m = max(m, s_max[w]);
-    if (m <= 0) return;   // all-zero conv output: NumPy divides by zero here (nan); defined as zeros
-    const double scale = 127.0 / (double)m;
-    for (uint32_t i = threadIdx.x; i < elems; i += 256) {
-        const double y = rint(__dmul_rn((double)p[i], scale));
-        p[i] = (int)fmin(fmax(y, 0.0), 127.0);
-    }
+    if (m <= 0) return;   // all-zero conv output: already the result (conv_renorm_scale)
+    const double scale = conv_renorm_scale(m);
+    for (uint32_t i = threadIdx.x; i < elems; i += 256) p[i] = conv_renorm(p[i], scale);
 }
 
 __global__ void k_i32_to_i8(const int32_t *__restrict__ in, uint32_t n_in, int8_t *__restrict__ out, uint32_t out_stride, size_t n) {
@@ -378,6 +386,190 @@ void launch_conv_renorm(int32_t *planes, uint32_t elems_per_image, size_t n, cud
 void launch_i32_to_i8(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t out_stride, size_t n, cudaStream_t st) {
     const size_t total = n * out_stride;
     if (total) k_i32_to_i8<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, n_in, out, out_stride, n);
+}
+
+// ------------------------------------------------------------------------------------------------
+// The emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) as one kernel, step for step the layered route of emulate_device
+// (capi.cu): input scaling; conv1 (1 -> C), ReLU, renormalisation over the image's C*196 outputs; depthwise conv2, ReLU,
+// renormalisation over C*144, 2x2 max-pool; depthwise conv3, ReLU, renormalisation over C*16, 2x2 max-pool; the (C, 2, 2)
+// flatten.  Convolutions follow k_conv33relu: output (y, x) = sum of w[3 dr + dc] * in[y + dr][x + dc], no shift.
+// Thread = (image, channel), ipb images per CTA.  Each renormalisation needs the maximum over all channels of the image (a
+// shared-memory atomicMax, then a barrier), so conv1 and conv2 run twice: once for the maximum, once to renormalise what they
+// recompute.  The one intermediate in shared memory is a channel's renormalised conv1 plane (14 rows of 16 bytes, 57 words apart:
+// no bank conflicts); conv2's pooled outputs and conv3's outputs stay in registers.  conv1 and conv2 take three dp4a per output
+// over 4-byte sliding windows of their input rows (the fourth weight byte is zero); conv3 is 9 IMAD per output.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kCnnEmulThreads = 256, kCnnEmulMaxImages = 16;
+constexpr uint32_t kEmulImgStride = 260;     // bytes per scaled 16x16 image in shared memory (65 words)
+constexpr uint32_t kEmulC1Words = 57;        // words per renormalised conv1 plane
+
+// the 4-byte windows starting at bytes 0 .. kW-1 of a 16-byte row (four words; bytes past the row read as zero)
+template <int kW>
+__device__ __forceinline__ void row_windows(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t (&win)[kW]) {
+    const uint32_t w[5] = {w0, w1, w2, w3, 0u};
+#pragma unroll
+    for (int x = 0; x < kW; x++) win[x] = __funnelshift_r(w[x >> 2], w[(x >> 2) + 1], 8 * (x & 3));
+}
+__device__ __forceinline__ int pack_taps(const int8_t *k) {   // one kernel row (k[0], k[1], k[2], 0) as int8x4
+    return (int)((uint32_t)(uint8_t)k[0] | (uint32_t)(uint8_t)k[1] << 8 | (uint32_t)(uint8_t)k[2] << 16);
+}
+
+// conv1 + ReLU of one channel over the scaled image im (16 rows of 16 bytes).  kRenorm false: returns the maximum.  kRenorm true:
+// stores the renormalised rows into the plane c1 (14 rows x 4 words) and returns 0.
+template <bool kRenorm>
+__device__ __forceinline__ int emul_conv1(const uint32_t *im, const int (&k)[3], double scale, uint32_t *c1) {
+    uint32_t win[3][14];
+    int m = 0;
+#pragma unroll
+    for (int y = 0; y < 16; y++) {
+        row_windows<14>(im[4 * y], im[4 * y + 1], im[4 * y + 2], im[4 * y + 3], win[y % 3]);
+        if (y < 2) continue;
+        const int r = y - 2;
+        uint32_t out[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int x = 0; x < 14; x++) {
+            int s = __dp4a((int)win[r % 3][x], k[0], 0);
+            s = __dp4a((int)win[(r + 1) % 3][x], k[1], s);
+            s = __dp4a((int)win[(r + 2) % 3][x], k[2], s);
+            s = max(s, 0);
+            if (kRenorm) out[x >> 2] |= (uint32_t)conv_renorm(s, scale) << (8 * (x & 3));
+            else m = max(m, s);
+        }
+        if (kRenorm)
+#pragma unroll
+            for (int j = 0; j < 4; j++) c1[4 * r + j] = out[j];
+    }
+    return m;
+}
+
+// conv2 + ReLU of one channel over its renormalised conv1 plane c1.  kRenorm false: returns the maximum.  kRenorm true:
+// renormalises, max-pools 2x2, runs conv3 (taps w3) + ReLU on the pooled rows as they complete into u and returns u's maximum.
+template <bool kRenorm>
+__device__ __forceinline__ int emul_conv2(const uint32_t *c1, const int (&k)[3], double scale, const int8_t *w3, int (&u)[4][4]) {
+    uint32_t win[3][12];
+    int even[12];   // the renormalised even row awaiting its odd partner
+    int pl[3][6];   // the last three pooled rows
+    int m = 0;
+#pragma unroll
+    for (int y = 0; y < 14; y++) {
+        row_windows<12>(c1[4 * y], c1[4 * y + 1], c1[4 * y + 2], c1[4 * y + 3], win[y % 3]);
+        if (y < 2) continue;
+        const int r = y - 2;
+#pragma unroll
+        for (int x = 0; x < 12; x++) {
+            int s = __dp4a((int)win[r % 3][x], k[0], 0);
+            s = __dp4a((int)win[(r + 1) % 3][x], k[1], s);
+            s = __dp4a((int)win[(r + 2) % 3][x], k[2], s);
+            s = max(s, 0);
+            if (!kRenorm) {
+                m = max(m, s);
+            } else if ((r & 1) == 0) {
+                even[x] = conv_renorm(s, scale);
+            } else {
+                const int v = max(even[x], conv_renorm(s, scale));
+                pl[(r >> 1) % 3][x >> 1] = (x & 1) ? max(pl[(r >> 1) % 3][x >> 1], v) : v;
+            }
+        }
+        if (kRenorm && (r & 1) && (r >> 1) >= 2) {
+            const int q = (r >> 1) - 2;   // conv3 output row
+#pragma unroll
+            for (int x = 0; x < 4; x++) {
+                int s = 0;
+#pragma unroll
+                for (int dr = 0; dr < 3; dr++)
+#pragma unroll
+                    for (int dc = 0; dc < 3; dc++) s += (int)w3[3 * dr + dc] * pl[(q + dr) % 3][x + dc];
+                u[q][x] = max(s, 0);
+                m = max(m, u[q][x]);
+            }
+        }
+    }
+    return m;
+}
+
+__global__ void __launch_bounds__(kCnnEmulThreads, 2)
+k_cnn_emul_frontend(const float *__restrict__ images, const int8_t *__restrict__ w1, const int8_t *__restrict__ w2,
+                    const int8_t *__restrict__ w3, uint32_t C, uint32_t ipb, int8_t *__restrict__ feats, uint32_t feat_stride, size_t n) {
+    extern __shared__ __align__(16) uint32_t s_emul[];
+    int *s_max = reinterpret_cast<int *>(s_emul);                  // [3][ipb]: the image maxima of conv1, conv2, conv3
+    uint32_t *s_img = s_emul + 3 * ipb;                             // [ipb][kEmulImgStride / 4]
+    uint32_t *s_c1 = s_img + ipb * (kEmulImgStride / 4);            // [ipb * C][kEmulC1Words]
+    const uint32_t t = threadIdx.x, lane = t & 31;
+    const size_t img0 = (size_t)blockIdx.x * ipb;
+
+    // input scaling (BitNetMCU.py:435-436): warp w scales images w, w + 8, ...; lane l holds elements 4l .. 4l+3 and 128 + 4l ..
+    for (uint32_t il = t >> 5; il < ipb; il += kCnnEmulThreads / 32) {
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+        if (img0 + il < n) {
+            const float4 *x = reinterpret_cast<const float4 *>(images + (img0 + il) * 256);
+            a = x[lane];
+            b = x[lane + 32];
+        }
+        float m = fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))),
+                        fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w))));
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+        const float sc = quant_scale(m);
+        auto pack = [&](float4 v) {
+            return (uint32_t)(quant_pixel(v.x, sc) & 255) | (uint32_t)(quant_pixel(v.y, sc) & 255) << 8 |
+                   (uint32_t)(quant_pixel(v.z, sc) & 255) << 16 | (uint32_t)(quant_pixel(v.w, sc) & 255) << 24;
+        };
+        s_img[il * (kEmulImgStride / 4) + lane] = pack(a);
+        s_img[il * (kEmulImgStride / 4) + 32 + lane] = pack(b);
+    }
+    if (t < 3 * ipb) s_max[t] = 0;
+    __syncthreads();
+
+    const bool active = t < ipb * C;
+    const uint32_t il = active ? t / C : 0, ch = active ? t % C : 0;
+    int k1[3], k2[3];
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+        k1[r] = pack_taps(w1 + ch * 9 + 3 * r);
+        k2[r] = pack_taps(w2 + ch * 9 + 3 * r);
+    }
+    const uint32_t *im = s_img + il * (kEmulImgStride / 4);
+    uint32_t *c1 = s_c1 + t * kEmulC1Words;
+    int u[4][4];   // conv3 + ReLU
+
+    if (active) atomicMax(&s_max[il], emul_conv1<false>(im, k1, 0.0, c1));
+    __syncthreads();
+    if (active) {
+        emul_conv1<true>(im, k1, conv_renorm_scale(s_max[il]), c1);
+        atomicMax(&s_max[ipb + il], emul_conv2<false>(c1, k2, 0.0, w3 + ch * 9, u));
+    }
+    __syncthreads();
+    if (active) atomicMax(&s_max[2 * ipb + il], emul_conv2<true>(c1, k2, conv_renorm_scale(s_max[ipb + il]), w3 + ch * 9, u));
+    __syncthreads();
+    if (active && img0 + il < n) {
+        const double sc = conv_renorm_scale(s_max[2 * ipb + il]);
+        uint32_t f = 0;
+#pragma unroll
+        for (int py = 0; py < 2; py++)
+#pragma unroll
+            for (int px = 0; px < 2; px++) {
+                const int v = max(max(conv_renorm(u[2 * py][2 * px], sc), conv_renorm(u[2 * py][2 * px + 1], sc)),
+                                  max(conv_renorm(u[2 * py + 1][2 * px], sc), conv_renorm(u[2 * py + 1][2 * px + 1], sc)));
+                f |= (uint32_t)v << (8 * (2 * py + px));   // flatten (C, 2, 2): feature 4 ch + 2 py + px
+            }
+        uint32_t *row = reinterpret_cast<uint32_t *>(feats + (img0 + il) * feat_stride);
+        row[ch] = f;
+        for (uint32_t w = C + ch; w < feat_stride / 4; w += C) row[w] = 0u;   // the row's zero padding
+    }
+}
+
+static uint32_t cnn_emul_ipb(uint32_t C) { return std::min(kCnnEmulMaxImages, kCnnEmulThreads / C); }
+
+bool launch_cnn_emul_frontend(const float *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
+                              int8_t *features, uint32_t feat_stride, size_t n, cudaStream_t st) {
+    if (channels == 0 || channels > kCnnEmulMaxChannels) return false;
+    if (n == 0) return true;
+    const uint32_t ipb = cnn_emul_ipb(channels);
+    const size_t smem = 4 * ((size_t)3 * ipb + ipb * (kEmulImgStride / 4) + (size_t)ipb * channels * kEmulC1Words);
+    if (!raise_smem_limit((const void *)k_cnn_emul_frontend, smem)) return false;
+    k_cnn_emul_frontend<<<(unsigned)((n + ipb - 1) / ipb), kCnnEmulThreads, smem, st>>>(images, w1, w2, w3, channels, ipb, features,
+                                                                                       feat_stride, n);
+    return true;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -99,5 +99,15 @@ int fc_chain_launch_f32(FcChainPlan *p, const float *in, size_t n, int32_t *logi
 // logits = last layer's accumulators x 2^-level_shift (level_shift 0 or 1); logits / labels may each be null.  Where
 // fc_chain_float_input_supported holds.
 int fc_chain_launch_emul(FcChainPlan *p, const float *in, size_t n, int level_shift, double *logits, uint32_t *labels, cudaStream_t st);
+// the emulator on int8 rows [n][in_bytes] (device, 16B aligned) that are already scaled (fc_emul_i8_kernel, every plan)
+int fc_chain_launch_emul_i8(FcChainPlan *p, const int8_t *in, size_t n, int level_shift, double *logits, uint32_t *labels,
+                            cudaStream_t st);
+// the template arguments of the emulator row a launch takes: fc_emul_kernel (float_row) or fc_emul_i8_kernel, e.g. "<192,1,emul>"
+const char *fc_chain_emul_name(const FcChainPlan *p, bool float_row);
+// the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
+// [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
+constexpr uint32_t kCnnEmulMaxChannels = 128;
+bool launch_cnn_emul_frontend(const float *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
+                              int8_t *features, uint32_t feat_stride, size_t n, cudaStream_t st);
 
 }  // namespace bnm

@@ -219,9 +219,12 @@ BNM_API int bnm_emulate_inference_quantized(bnm_model *m, const float *images, s
 /* QuantizedModel.inference_quantized on device buffers, asynchronous on `stream`.  images float32 [n][img_bytes] (16-byte
  * aligned) -> logits float64 [n][n_classes] (8-byte aligned), the emulator's logits bit for bit, and / or labels uint32 [n] =
  * np.argmax of them (first maximum).  logits or labels may be NULL, not both (BNM_E_ARG).  Results equal those of
- * bnm_emulate_inference_quantized.  FC models on the fused path (image rows of <= 256 elements, <= 16 classes, <= 64 wide, the
- * models of bnm_infer_batch_device_f32's one-kernel path) run ONE kernel: the float-input kernel with the emulator's hidden-layer
- * rule and float64 logits.  Every other model runs the emulation kernels layer by layer through scratch the model owns (grown on
+ * bnm_emulate_inference_quantized.  On the fused path, FC models with image rows of <= 256 elements, <= 16 classes and <= 64
+ * wide (the models of bnm_infer_batch_device_f32's one-kernel path) run ONE kernel: the float-input kernel with the emulator's
+ * hidden-layer rule and float64 logits.  Other FC models run the input scaling kernel, then the int8-input FC kernel with the
+ * emulator's rule at the model's width (up to 256); CNN models of up to 128 channels run the emulator's CNN front-end as one
+ * kernel, then that FC kernel on its features; both in chunks of 2^20 images.  BNM_PATH_LAYERS, models without a fused plan and
+ * wider CNN models run the emulation kernels layer by layer.  Every route but the first uses scratch the model owns (grown on
  * the first large call, then reused): calls on one model must then not overlap in time on different streams.  Either way the
  * call makes no host synchronisation once its scratch has grown. */
 BNM_API int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream);
