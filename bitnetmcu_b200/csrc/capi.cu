@@ -36,6 +36,37 @@ enum { BNM_E_ARG = -1, BNM_E_NODEV = -2, BNM_E_UNSUPPORTED = -3, BNM_E_CUDA = -4
 
 static uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
+// One allocation of T and its only owner, which frees it: device memory, or mapped pinned host memory (kPinned).  grow(need) makes
+// it at least `need` bytes large: a larger request discards the contents and allocates anew (zeroed on request); one it already
+// meets makes no CUDA call.
+template <class T, bool kPinned>
+struct Buffer {
+    T *p = nullptr;
+    size_t bytes = 0;
+    Buffer() = default;
+    Buffer(const Buffer &) = delete;
+    Buffer &operator=(const Buffer &) = delete;
+    ~Buffer() { release(); }
+    void release() {
+        if (p) kPinned ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr;
+        bytes = 0;
+    }
+    cudaError_t grow(size_t need, bool zero = false) {
+        if (need <= bytes) return cudaSuccess;
+        release();
+        void *q = nullptr;
+        cudaError_t e = kPinned ? cudaHostAlloc(&q, need, cudaHostAllocMapped) : cudaMalloc(&q, need);
+        if (e != cudaSuccess) return e;
+        p = static_cast<T *>(q);
+        if (zero && (e = cudaMemset(p, 0, need)) != cudaSuccess) { release(); return e; }
+        bytes = need;
+        return cudaSuccess;
+    }
+};
+template <class T> using DevBuf = Buffer<T, false>;
+template <class T> using PinnedBuf = Buffer<T, true>;
+
 // -----------------------------------------------------------------------------------------------
 // model
 // -----------------------------------------------------------------------------------------------
@@ -48,10 +79,10 @@ struct FcLayerHost {
 
 struct PipeSlot {
     cudaStream_t stream = nullptr;
-    int8_t *d_images = nullptr;
-    int32_t *d_logits = nullptr;
-    uint32_t *d_labels = nullptr;
-    int8_t *d_feat = nullptr;    // CNN models: this slot's own feature buffer, so that the slots' chunks may overlap in time
+    DevBuf<int8_t> d_images;
+    DevBuf<int32_t> d_logits;
+    DevBuf<uint32_t> d_labels;
+    DevBuf<int8_t> d_feat;   // CNN models: this slot's own feature buffer, so that the slots' chunks may overlap in time
 };
 
 struct bnm_model {
@@ -62,7 +93,7 @@ struct bnm_model {
     std::vector<FcLayerDev> fc;
     // CNN front-end
     uint32_t channels = 0, xy0 = 0, feat_stride = 0;
-    int8_t *d_conv[3] = {nullptr, nullptr, nullptr};
+    DevBuf<int8_t> d_conv[3];
     // options
     int opt_path = BNM_PATH_AUTO;
     int nf4_ext = 0;
@@ -71,35 +102,30 @@ struct bnm_model {
     int cnn_frontend = 0;            // BNM_OPT_CNN_FRONTEND
     bool conv3_fits_u16 = false;     // static range of conv3's inputs for this model's weights (cnn_conv3_fits_u16)
     std::vector<int8_t> h_conv[3];   // host copies of the conv weights (range analysis)
-    int *d_err = nullptr;            // error word of the bounded device-side waits
+    DevBuf<int> d_err;               // error word of the bounded device-side waits
     // fused plan
     FcChainPlan *plan = nullptr;
     std::string plan_err;
     // device scratch (grow-only): layered path accumulators / activations, CNN features
-    size_t scratch_n = 0;
-    int32_t *d_acc = nullptr;
-    int8_t *d_act[2] = {nullptr, nullptr};
-    int8_t *d_feat = nullptr;
+    DevBuf<int32_t> d_acc;
+    DevBuf<int8_t> d_act[2], d_feat;
     uint32_t max_kpad = 0, max_nout = 0;
     // host pipeline
     PipeSlot slots[3];
-    size_t slot_n = 0;
     // small-batch path of bnm_infer_batch (the reference's own calling pattern: one image per Inference() call,
     // test_inference.py:146-150): pinned staging buffers, one stream, one synchronisation
-    int8_t *small_h_in = nullptr, *small_d_in = nullptr;     // [kSmallBatch][img_bytes]
-    int32_t *small_h_out = nullptr, *small_d_out = nullptr;  // logits [n][n_classes] then labels [n]
-    int8_t *d_f32_scratch = nullptr;   // bnm_infer_batch_device_f32 fallback: quantised images
-    size_t f32_scratch_n = 0;
+    PinnedBuf<int8_t> small_h_in;    // [kSmallBatch][img_bytes]
+    PinnedBuf<int32_t> small_h_out;  // logits [n][n_classes] then labels [n]
+    DevBuf<int8_t> small_d_in;       // their device counterparts
+    DevBuf<int32_t> small_d_out;
+    DevBuf<int8_t> d_f32_scratch;   // bnm_infer_batch_device_f32 fallback: quantised images
     // emulation mode (grow-only): the fallback's quantised images and CNN int32 planes, next to the layered path's scratch;
     // the host entry's device copies of its images and logits
-    int8_t *d_emul_q = nullptr;
-    int32_t *d_emul_planes[2] = {nullptr, nullptr};
-    size_t emul_n = 0;
-    float *d_emul_in = nullptr;
-    double *d_emul_out = nullptr;
-    size_t emul_host_n = 0;
-    int8_t *d_emul_rows = nullptr;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
-    size_t emul_rows_n = 0;
+    DevBuf<int8_t> d_emul_q;
+    DevBuf<int32_t> d_emul_planes[2];
+    DevBuf<float> d_emul_in;
+    DevBuf<double> d_emul_out;
+    DevBuf<int8_t> d_emul_rows;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
     int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
                                // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
 };
@@ -172,32 +198,17 @@ static int build_fc_dev(bnm_model *m) {
     m->plan = fc_chain_plan_create(m->fc.data(), (int)m->fc.size(), in_bytes, m->device, m->sm_count, err, sizeof(err));
     m->plan_err = err;
     fc_chain_plan_set_overlap(m->plan, effective_overlap(m));
-    // scratch must be re-sized for the new widths
-    m->scratch_n = 0;
     return 0;
 }
 
+// scratch for n images: CNN features, and with `layered` the layer-by-layer path's int32 accumulators and ping-pong int8
+// activations, which the fused path needs neither of
 static int ensure_scratch(bnm_model *m, size_t n, bool layered) {
-    if (n <= m->scratch_n && (!layered || m->d_acc)) return 0;
-    n = std::max(n, m->scratch_n);
-    cudaFree(m->d_acc);
-    cudaFree(m->d_act[0]);
-    cudaFree(m->d_act[1]);
-    cudaFree(m->d_feat);
-    m->d_acc = nullptr; m->d_act[0] = m->d_act[1] = nullptr; m->d_feat = nullptr;
-    m->scratch_n = 0;
-    if (layered) {   // int32 accumulators + ping-pong int8 activations of the layer-by-layer path; the fused path needs neither
-        CU_TRY(cudaMalloc(&m->d_acc, n * (size_t)std::max(m->max_nout, 1u) * sizeof(int32_t)));
-        for (int i = 0; i < 2; i++) {
-            CU_TRY(cudaMalloc(&m->d_act[i], n * (size_t)m->max_kpad));
-            CU_TRY(cudaMemset(m->d_act[i], 0, n * (size_t)m->max_kpad));
-        }
+    if (layered) {
+        CU_TRY(m->d_acc.grow(n * (size_t)std::max(m->max_nout, 1u) * sizeof(int32_t)));
+        for (auto &a : m->d_act) CU_TRY(a.grow(n * (size_t)m->max_kpad, true));
     }
-    if (m->model_class == BNM_MODEL_CNNMNIST) {
-        CU_TRY(cudaMalloc(&m->d_feat, n * (size_t)m->feat_stride));
-        CU_TRY(cudaMemset(m->d_feat, 0, n * (size_t)m->feat_stride));
-    }
-    m->scratch_n = n;
+    if (m->model_class == BNM_MODEL_CNNMNIST) CU_TRY(m->d_feat.grow(n * (size_t)m->feat_stride, true));
     return 0;
 }
 
@@ -209,7 +220,7 @@ enum EmulRoute { kEmulFloatRow, kEmulInt8Row, kEmulLayers };
 static EmulRoute emul_route(const bnm_model *m) {
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
     if (bnm_model_active_path(m) != BNM_PATH_TCGEN05 || (cnn && m->channels > kCnnEmulMaxChannels)) return kEmulLayers;
-    return !cnn && fc_chain_float_input_supported(m->plan) ? kEmulFloatRow : kEmulInt8Row;
+    return !cnn && fc_chain_has_form(m->plan, kFormEmulFloat) ? kEmulFloatRow : kEmulInt8Row;
 }
 
 extern "C" int bnm_version(void) { return BNM_VERSION; }
@@ -268,8 +279,8 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
             if (!L.weights || L.weight_bytes < (size_t)L.n_out * 9) { rc = fail(BNM_E_ARG, "conv layer %u: needs %u int8 weights", i, L.n_out * 9); break; }
             if (n_conv == 0) { m->channels = L.n_out; m->xy0 = L.n_in; }
             else if (L.n_out != m->channels) { rc = fail(BNM_E_UNSUPPORTED, "conv layers must share the channel count (dll.c:66)"); break; }
-            if (cudaMalloc(&m->d_conv[n_conv], (size_t)L.n_out * 9) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaMalloc failed"); break; }
-            cudaMemcpy(m->d_conv[n_conv], L.weights, (size_t)L.n_out * 9, cudaMemcpyHostToDevice);
+            if (m->d_conv[n_conv].grow((size_t)L.n_out * 9) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaMalloc failed"); break; }
+            cudaMemcpy(m->d_conv[n_conv].p, L.weights, (size_t)L.n_out * 9, cudaMemcpyHostToDevice);
             m->h_conv[n_conv].assign(static_cast<const int8_t *>(L.weights), static_cast<const int8_t *>(L.weights) + (size_t)L.n_out * 9);
             n_conv++;
         } else if (L.kind == BNM_LAYER_MAXPOOL22) {
@@ -293,9 +304,10 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
     }
     if (rc == 0 && model_class == BNM_MODEL_FCMNIST && !front.empty()) rc = fail(BNM_E_ARG, "MODEL_FCMNIST with conv/pool layers");
     if (rc == 0) rc = build_fc_dev(m);
-    if (rc == 0 && (cudaMalloc(&m->d_err, sizeof(int)) != cudaSuccess || cudaMemset(m->d_err, 0, sizeof(int)) != cudaSuccess)) rc = fail(BNM_E_CUDA, "cudaMalloc failed");
+    if (rc == 0 && m->d_err.grow(sizeof(int), true) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaMalloc failed");
     if (rc == 0) {
         if (const char *e = getenv("BNM_CNN_FRONTEND")) m->cnn_frontend = std::max(0, std::min(2, atoi(e)));   // development override, read once per model
+        if (const char *e = getenv("BNM_SMALL_ZC")) m->small_zero_copy = std::max(0, std::min(2, atoi(e)));     // development knob, likewise
         for (auto &s : m->slots)
             if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaStreamCreate failed"); break; }
     }
@@ -305,7 +317,7 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         fprintf(stderr, "bitnetmcu_b200: emulator route: %s%s\n",
                 r == kEmulLayers ? "layer by layer" : r == kEmulFloatRow ? "fc_emul_kernel" :
                 m->model_class == BNM_MODEL_CNNMNIST ? "k_cnn_emul_frontend + fc_emul_i8_kernel" : "k_quantize_images + fc_emul_i8_kernel",
-                r == kEmulLayers ? "" : fc_chain_emul_name(m->plan, r == kEmulFloatRow));
+                r == kEmulLayers ? "" : fc_chain_form_name(m->plan, r == kEmulFloatRow ? kFormEmulFloat : kFormEmulInt8));
     }
     *out = m;
     return 0;
@@ -335,31 +347,9 @@ extern "C" void bnm_model_destroy(bnm_model *m) {
     cudaDeviceSynchronize();
     free_fc_dev(m);
     for (auto &H : m->fc_host) cudaFree(H.d_packed);
-    for (auto &p : m->d_conv) cudaFree(p);
-    cudaFree(m->d_acc);
-    cudaFree(m->d_act[0]);
-    cudaFree(m->d_act[1]);
-    cudaFree(m->d_feat);
-    cudaFree(m->d_err);
-    cudaFree(m->small_d_in);
-    cudaFree(m->small_d_out);
-    cudaFree(m->d_f32_scratch);
-    cudaFree(m->d_emul_q);
-    cudaFree(m->d_emul_planes[0]);
-    cudaFree(m->d_emul_planes[1]);
-    cudaFree(m->d_emul_in);
-    cudaFree(m->d_emul_out);
-    cudaFree(m->d_emul_rows);
-    if (m->small_h_in) cudaFreeHost(m->small_h_in);
-    if (m->small_h_out) cudaFreeHost(m->small_h_out);
-    for (auto &s : m->slots) {
-        cudaFree(s.d_images);
-        cudaFree(s.d_logits);
-        cudaFree(s.d_labels);
-        cudaFree(s.d_feat);
+    for (auto &s : m->slots)
         if (s.stream) cudaStreamDestroy(s.stream);
-    }
-    delete m;
+    delete m;   // and with it the buffers it owns as members
 }
 
 extern "C" uint32_t bnm_model_n_classes(const bnm_model *m) { return m ? m->n_classes : 0; }
@@ -430,13 +420,13 @@ static int run_fc_layers(bnm_model *m, const int8_t *in, uint32_t in_stride, siz
     const size_t nl = m->fc.size();
     for (size_t l = 0; l < nl; l++) {
         const bool last = l + 1 == nl;
-        int32_t *acc = last && logits ? logits : m->d_acc;
+        int32_t *acc = last && logits ? logits : m->d_acc.p;
         if (!launch_fc_dp4a(act, stride, m->fc[l], acc, n, st))
             return fail(BNM_E_UNSUPPORTED, "FC layer %zu: %u inputs need more shared memory than an SM has (layer kernel stages 128 rows)", l, m->fc[l].n_in);
         if (last) {
             if (labels) launch_relunorm(acc, m->fc[l].n_out, nullptr, 0, labels, n, st);
         } else {
-            int8_t *next = m->d_act[l & 1];
+            int8_t *next = m->d_act[l & 1].p;
             uint32_t next_stride = m->fc[l + 1].k_pad;
             launch_relunorm(acc, m->fc[l].n_out, next, next_stride, nullptr, n, st);
             act = next;
@@ -448,8 +438,8 @@ static int run_fc_layers(bnm_model *m, const int8_t *in, uint32_t in_stride, siz
 
 // CNN front-end into feat (int8 [n][feat_stride])
 static int run_cnn_front(bnm_model *m, const int8_t *images, size_t n, int8_t *feat, cudaStream_t st) {
-    if (launch_cnn_frontend(images, m->d_conv[0], m->d_conv[1], m->d_conv[2], m->channels, m->xy0, feat, m->feat_stride, n,
-                            m->sm_count, m->cnn_frontend, m->d_err, m->conv3_fits_u16, st))
+    if (launch_cnn_frontend(images, m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, m->channels, m->xy0, feat, m->feat_stride, n,
+                            m->sm_count, m->cnn_frontend, m->d_err.p, m->conv3_fits_u16, st))
         return 0;
     return fail(BNM_E_UNSUPPORTED, "CNN front-end: %u channels at %ux%u not supported by the selected kernel (the reference hard-codes 16x16, dll.c:68)",
                 m->channels, m->xy0, m->xy0);
@@ -487,13 +477,13 @@ static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
     if (gather && !fused) return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     if (fused && !cnn) {
-        int rc = fc_chain_launch(m->plan, images, n, logits, labels, gather, st);
+        int rc = fc_chain_launch(m->plan, kFormInt8, images, n, logits, labels, 0, gather, st);
         return rc ? fail(BNM_E_CUDA, "fused FC kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
     const size_t chunk = slot_feat ? n : std::min(n, fused ? kFusedCnnChunk : kLayeredChunk);
     int rc = (slot_feat && fused) ? 0 : ensure_scratch(m, chunk, !fused);
     if (rc) return rc;
-    int8_t *feat = slot_feat ? slot_feat : m->d_feat;
+    int8_t *feat = slot_feat ? slot_feat : m->d_feat.p;
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         const int8_t *img = images + b * m->img_bytes;
@@ -510,7 +500,7 @@ static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32
         if (fused) {
             GatherDst gchunk;
             if (gather) { gchunk = *gather; gchunk.row_offset += b; }
-            rc = fc_chain_launch(m->plan, fc_in, nb, lg, lb, gather ? &gchunk : nullptr, st);
+            rc = fc_chain_launch(m->plan, kFormInt8, fc_in, nb, lg, lb, 0, gather ? &gchunk : nullptr, st);
             if (rc) return fail(BNM_E_CUDA, "fused FC kernel launch failed (%d)", rc);
         } else {
             rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, lb, st);
@@ -591,29 +581,30 @@ extern "C" int bnm_enable_peer_access(int device, int peer) {
 // -----------------------------------------------------------------------------------------------
 // n <= kSmallBatch images: staging buffers allocated once, one stream, one synchronisation per call
 static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
-    const size_t in_bytes = kSmallBatch * (size_t)m->img_bytes, out_ints = kSmallBatch * ((size_t)m->n_classes + 1);
-    if (!m->small_h_in) {
-        if (const char *e = getenv("BNM_SMALL_ZC")) m->small_zero_copy = std::max(0, std::min(2, atoi(e)));   // development knob, read once per model
-        CU_TRY(cudaHostAlloc(reinterpret_cast<void **>(&m->small_h_in), in_bytes, cudaHostAllocMapped));
-        CU_TRY(cudaHostAlloc(reinterpret_cast<void **>(&m->small_h_out), out_ints * 4, cudaHostAllocMapped));
-        CU_TRY(cudaMalloc(&m->small_d_in, in_bytes));
-        CU_TRY(cudaMalloc(&m->small_d_out, out_ints * 4));
+    const size_t in_bytes = kSmallBatch * (size_t)m->img_bytes, out_bytes = kSmallBatch * ((size_t)m->n_classes + 1) * 4;
+    cudaError_t e = m->small_h_in.grow(in_bytes);
+    if (e == cudaSuccess) e = m->small_h_out.grow(out_bytes);
+    if (e == cudaSuccess) e = m->small_d_in.grow(in_bytes);
+    if (e == cudaSuccess) e = m->small_d_out.grow(out_bytes);
+    if (e != cudaSuccess) {   // all four buffers or none
+        m->small_h_in.release(); m->small_h_out.release(); m->small_d_in.release(); m->small_d_out.release();
+        return fail(-100 - (int)e, "small-batch staging buffers: %s", cudaGetErrorString(e));
     }
     cudaStream_t st = m->slots[0].stream;
-    memcpy(m->small_h_in, images, n * (size_t)m->img_bytes);
-    const int8_t *d_in = m->small_d_in;
-    int32_t *d_out = m->small_d_out;
-    if (m->small_zero_copy >= 2) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(const_cast<int8_t **>(&d_in)), m->small_h_in, 0));
-    else CU_TRY(cudaMemcpyAsync(m->small_d_in, m->small_h_in, n * (size_t)m->img_bytes, cudaMemcpyHostToDevice, st));
-    if (m->small_zero_copy >= 1) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), m->small_h_out, 0));
+    memcpy(m->small_h_in.p, images, n * (size_t)m->img_bytes);
+    const int8_t *d_in = m->small_d_in.p;
+    int32_t *d_out = m->small_d_out.p;
+    if (m->small_zero_copy >= 2) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(const_cast<int8_t **>(&d_in)), m->small_h_in.p, 0));
+    else CU_TRY(cudaMemcpyAsync(m->small_d_in.p, m->small_h_in.p, n * (size_t)m->img_bytes, cudaMemcpyHostToDevice, st));
+    if (m->small_zero_copy >= 1) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), m->small_h_out.p, 0));
     const size_t n_log = logits ? n * (size_t)m->n_classes : 0;   // labels-only calls: the labels start the staging buffer
     uint32_t *d_lab = reinterpret_cast<uint32_t *>(d_out + n_log);
     int rc = bnm_infer_batch_device(m, d_in, n, logits ? d_out : nullptr, labels ? d_lab : nullptr, st);
     if (rc) return rc;
-    if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(m->small_h_out, m->small_d_out, (n_log + (labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
+    if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(m->small_h_out.p, m->small_d_out.p, (n_log + (labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
-    if (logits) memcpy(logits, m->small_h_out, n_log * 4);
-    if (labels) memcpy(labels, m->small_h_out + n_log, n * 4);
+    if (logits) memcpy(logits, m->small_h_out.p, n_log * 4);
+    if (labels) memcpy(labels, m->small_h_out.p + n_log, n * 4);
     return 0;
 }
 
@@ -624,20 +615,15 @@ extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int
     CU_TRY(cudaSetDevice(m->device));
     if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);
     const size_t chunk = std::min(n, m->chunk_images);
-    if (m->slot_n < chunk) {
-        CU_TRY(cudaDeviceSynchronize());
+    // the last slot's labels are the last buffer grown: smaller than a chunk's until every slot has all of its buffers
+    if (m->slots[2].d_labels.bytes < chunk * sizeof(uint32_t)) {
+        CU_TRY(cudaDeviceSynchronize());   // no chunk of an earlier call may still use a buffer that is reallocated
         for (auto &s : m->slots) {
-            cudaFree(s.d_images); cudaFree(s.d_logits); cudaFree(s.d_labels); cudaFree(s.d_feat);
-            s.d_images = nullptr; s.d_logits = nullptr; s.d_labels = nullptr; s.d_feat = nullptr;
-            if (m->model_class == BNM_MODEL_CNNMNIST) {
-                CU_TRY(cudaMalloc(&s.d_feat, chunk * (size_t)m->feat_stride));
-                CU_TRY(cudaMemset(s.d_feat, 0, chunk * (size_t)m->feat_stride));
-            }
-            CU_TRY(cudaMalloc(&s.d_images, chunk * (size_t)m->img_bytes));
-            CU_TRY(cudaMalloc(&s.d_logits, chunk * (size_t)m->n_classes * sizeof(int32_t)));
-            CU_TRY(cudaMalloc(&s.d_labels, chunk * sizeof(uint32_t)));
+            if (m->model_class == BNM_MODEL_CNNMNIST) CU_TRY(s.d_feat.grow(chunk * (size_t)m->feat_stride, true));
+            CU_TRY(s.d_images.grow(chunk * (size_t)m->img_bytes));
+            CU_TRY(s.d_logits.grow(chunk * (size_t)m->n_classes * sizeof(int32_t)));
+            CU_TRY(s.d_labels.grow(chunk * sizeof(uint32_t)));
         }
-        m->slot_n = chunk;
     }
     // the layer-by-layer path shares one scratch arena (accumulators / activations): its chunks must not overlap in time -> one
     // stream.  The fused path has no shared state (CNN models: one feature buffer per slot) and uses all three.
@@ -646,12 +632,12 @@ extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int
     for (size_t b = 0; b < n; b += chunk, k++) {
         const size_t nb = std::min(chunk, n - b);
         PipeSlot &s = m->slots[shared_scratch ? 0 : k % 3];
-        CU_TRY(cudaMemcpyAsync(s.d_images, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
-        int rc = infer_device_impl(m, s.d_images, nb, logits ? s.d_logits : nullptr, labels ? s.d_labels : nullptr, nullptr, s.stream,
-                                   shared_scratch ? nullptr : s.d_feat);
+        CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
+        int rc = infer_device_impl(m, s.d_images.p, nb, logits ? s.d_logits.p : nullptr, labels ? s.d_labels.p : nullptr, nullptr, s.stream,
+                                   shared_scratch ? nullptr : s.d_feat.p);
         if (rc) return rc;
-        if (logits) CU_TRY(cudaMemcpyAsync(logits + b * m->n_classes, s.d_logits, nb * (size_t)m->n_classes * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
-        if (labels) CU_TRY(cudaMemcpyAsync(labels + b, s.d_labels, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+        if (logits) CU_TRY(cudaMemcpyAsync(logits + b * m->n_classes, s.d_logits.p, nb * (size_t)m->n_classes * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
+        if (labels) CU_TRY(cudaMemcpyAsync(labels + b, s.d_labels.p, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
     }
     for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
     return 0;
@@ -667,13 +653,6 @@ extern "C" void bnm_host_free(void *p) { if (p) cudaFreeHost(p); }
 // -----------------------------------------------------------------------------------------------
 // the four kernels, batched over host buffers
 // -----------------------------------------------------------------------------------------------
-struct DevBuf {
-    void *p = nullptr;
-    ~DevBuf() { if (p) cudaFree(p); }
-    int alloc(size_t bytes) { return cudaMalloc(&p, bytes ? bytes : 16) == cudaSuccess ? 0 : -1; }
-    template <class T> T *as() { return static_cast<T *>(p); }
-};
-
 static int require_device() {
     if (bnm_device_count() == 0) return fail(BNM_E_NODEV, "no CUDA device: this engine has no CPU fallback");
     return 0;
@@ -704,19 +683,22 @@ extern "C" int bnm_processfclayer_batch(const int8_t *activations, const uint32_
     L.k_pad = round_up(std::max(n_input, 1u), 32);
     L.n_pad = round_up(n_output, 16);
     const size_t plane = (size_t)L.k_pad * L.n_pad;
-    DevBuf packed, da, db, qa, qb, flag, act, out;
-    if (packed.alloc(need + 16) || da.alloc(plane) || db.alloc(plane) || qa.alloc(plane) || qb.alloc(plane) || flag.alloc(4) ||
-        act.alloc(n * (size_t)L.k_pad) || out.alloc(n * (size_t)n_output * 4))
+    DevBuf<uint8_t> packed;
+    DevBuf<int8_t> da, db, act;
+    DevBuf<int4> qa, qb;
+    DevBuf<int> flag;
+    DevBuf<int32_t> out;
+    if (packed.grow(need + 16) || da.grow(plane) || db.grow(plane) || qa.grow(plane) || qb.grow(plane) || flag.grow(4) ||
+        act.grow(n * (size_t)L.k_pad) || out.grow(n * (size_t)n_output * 4))
         return fail(BNM_E_CUDA, "cudaMalloc failed");
     CU_TRY(cudaMemset(packed.p, 0, need + 16));
     if (need) CU_TRY(cudaMemcpy(packed.p, weights, need, cudaMemcpyHostToDevice));
     CU_TRY(cudaMemset(flag.p, 0, 4));
-    L.dense_a = da.as<int8_t>(); L.quad_a = qa.as<int4>();
-    launch_decode_fc(packed.p, enc, n_input, n_output, L.k_pad, L.n_pad, L.dense_a, db.as<int8_t>(), L.quad_a, qb.as<int4>(), nf4_extension,
-                     flag.as<int>(), 0);
+    L.dense_a = da.p; L.quad_a = qa.p;
+    launch_decode_fc(packed.p, enc, n_input, n_output, L.k_pad, L.n_pad, L.dense_a, db.p, L.quad_a, qb.p, nf4_extension, flag.p, 0);
     int f = 0;
     CU_TRY(cudaMemcpy(&f, flag.p, 4, cudaMemcpyDeviceToHost));
-    if (f) { L.dense_b = db.as<int8_t>(); L.quad_b = qb.as<int4>(); }
+    if (f) { L.dense_b = db.p; L.quad_b = qb.p; }
     CU_TRY(cudaMemset(act.p, 0, n * (size_t)L.k_pad));
     // Ternary layers declare n_input padded to a multiple of 10 with zero trits (exportquant.py:132-137,166) and the
     // reference never reads the activations under a zero trit (inference.c:128): a caller may hand in a 256-byte row for
@@ -738,7 +720,7 @@ extern "C" int bnm_processfclayer_batch(const int8_t *activations, const uint32_
             }
     }
     if (valid_in) CU_TRY(cudaMemcpy2D(act.p, L.k_pad, activations, n_input, valid_in, n, cudaMemcpyHostToDevice));
-    if (!launch_fc_dp4a(act.as<int8_t>(), L.k_pad, L, out.as<int32_t>(), n, 0))
+    if (!launch_fc_dp4a(act.p, L.k_pad, L, out.p, n, 0))
         return fail(BNM_E_UNSUPPORTED, "processfclayer: n_input %u needs more shared memory than an SM has (layer kernel stages 128 rows)", n_input);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpy(output, out.p, n * (size_t)n_output * 4, cudaMemcpyDeviceToHost));
@@ -753,10 +735,12 @@ extern "C" int bnm_relunorm_batch(const int32_t *input, int8_t *output, uint32_t
         return 0;
     }
     if (!input) return fail(BNM_E_ARG, "bnm_relunorm_batch: null input");
-    DevBuf in, out, am;
-    if (in.alloc(n * (size_t)n_input * 4) || out.alloc(n * (size_t)n_input) || am.alloc(n * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
+    DevBuf<int32_t> in;
+    DevBuf<int8_t> out;
+    DevBuf<uint32_t> am;
+    if (in.grow(n * (size_t)n_input * 4) || out.grow(n * (size_t)n_input) || am.grow(n * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
     CU_TRY(cudaMemcpy(in.p, input, n * (size_t)n_input * 4, cudaMemcpyHostToDevice));   // copied first: output may alias input
-    launch_relunorm(in.as<int32_t>(), n_input, output ? out.as<int8_t>() : nullptr, n_input, am.as<uint32_t>(), n, 0);
+    launch_relunorm(in.p, n_input, output ? out.p : nullptr, n_input, am.p, n, 0);
     CU_TRY(cudaGetLastError());
     if (argmax) CU_TRY(cudaMemcpy(argmax, am.p, n * 4, cudaMemcpyDeviceToHost));
     else CU_TRY(cudaDeviceSynchronize());
@@ -770,11 +754,12 @@ extern "C" int bnm_conv33relu_batch(const int32_t *activations, const int8_t *we
     if (n == 0 || xy < 3) return 0;
     if (!activations || !weights || !output || n_w == 0) return fail(BNM_E_ARG, "bnm_conv33relu_batch: null argument");
     const size_t in_el = n * (size_t)xy * xy, out_el = n * (size_t)(xy - 2) * (xy - 2);
-    DevBuf in, w, out;
-    if (in.alloc(in_el * 4) || w.alloc((size_t)n_w * 9) || out.alloc(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
+    DevBuf<int32_t> in, out;
+    DevBuf<int8_t> w;
+    if (in.grow(in_el * 4) || w.grow((size_t)n_w * 9) || out.grow(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
     CU_TRY(cudaMemcpy(in.p, activations, in_el * 4, cudaMemcpyHostToDevice));
     CU_TRY(cudaMemcpy(w.p, weights, (size_t)n_w * 9, cudaMemcpyHostToDevice));
-    launch_conv33relu(in.as<int32_t>(), w.as<int8_t>(), n_w, xy, n_shift, out.as<int32_t>(), n, 0);
+    launch_conv33relu(in.p, w.p, n_w, xy, n_shift, out.p, n, 0);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpy(output, out.p, out_el * 4, cudaMemcpyDeviceToHost));
     return 0;
@@ -785,10 +770,10 @@ extern "C" int bnm_maxpool22_batch(const int32_t *activations, uint32_t xy, int3
     if (n == 0 || xy < 2) return 0;
     if (!activations || !output) return fail(BNM_E_ARG, "bnm_maxpool22_batch: null argument");
     const size_t in_el = n * (size_t)xy * xy, out_el = n * (size_t)(xy / 2) * (xy / 2);
-    DevBuf in, out;
-    if (in.alloc(in_el * 4) || out.alloc(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
+    DevBuf<int32_t> in, out;
+    if (in.grow(in_el * 4) || out.grow(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
     CU_TRY(cudaMemcpy(in.p, activations, in_el * 4, cudaMemcpyHostToDevice));
-    launch_maxpool22(in.as<int32_t>(), xy, out.as<int32_t>(), n, 0);
+    launch_maxpool22(in.p, xy, out.p, n, 0);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpy(output, out.p, out_el * 4, cudaMemcpyDeviceToHost));
     return 0;
@@ -814,28 +799,24 @@ extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, siz
     CU_TRY(cudaSetDevice(m->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool fused_fc = bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST;
-    if (fused_fc && fc_chain_float_input_supported(m->plan)) {
-        int rc = fc_chain_launch_f32(m->plan, images, n, logits, labels, st);
+    if (fused_fc && fc_chain_has_form(m->plan, kFormFloat)) {
+        int rc = fc_chain_launch(m->plan, kFormFloat, images, n, logits, labels, 0, nullptr, st);
         return rc ? fail(BNM_E_CUDA, "fused float-input kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
-    if (m->f32_scratch_n < n) {
-        cudaFree(m->d_f32_scratch);
-        m->d_f32_scratch = nullptr; m->f32_scratch_n = 0;
-        CU_TRY(cudaMalloc(&m->d_f32_scratch, n * (size_t)m->img_bytes));
-        m->f32_scratch_n = n;
-    }
-    launch_quantize_images(images, m->img_bytes, m->d_f32_scratch, n, st);
-    return bnm_infer_batch_device(m, m->d_f32_scratch, n, logits, labels, stream);
+    CU_TRY(m->d_f32_scratch.grow(n * (size_t)m->img_bytes));
+    launch_quantize_images(images, m->img_bytes, m->d_f32_scratch.p, n, st);
+    return bnm_infer_batch_device(m, m->d_f32_scratch.p, n, logits, labels, stream);
 }
 
 extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out) {
     if (int rc = require_device()) return rc;
     if (n == 0 || elems == 0) return 0;
     if (!images || !out) return fail(BNM_E_ARG, "bnm_quantize_images: null argument");
-    DevBuf in, q;
-    if (in.alloc(n * (size_t)elems * 4) || q.alloc(n * (size_t)elems)) return fail(BNM_E_CUDA, "cudaMalloc failed");
+    DevBuf<float> in;
+    DevBuf<int8_t> q;
+    if (in.grow(n * (size_t)elems * 4) || q.grow(n * (size_t)elems)) return fail(BNM_E_CUDA, "cudaMalloc failed");
     CU_TRY(cudaMemcpy(in.p, images, n * (size_t)elems * 4, cudaMemcpyHostToDevice));
-    launch_quantize_images(in.as<float>(), elems, q.as<int8_t>(), n, 0);
+    launch_quantize_images(in.p, elems, q.p, n, 0);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpy(out, q.p, n * (size_t)elems, cudaMemcpyDeviceToHost));
     return 0;
@@ -866,25 +847,21 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
     const uint32_t C = m->channels, elems = m->img_bytes;
     const EmulRoute route = emul_route(m);
     if (route == kEmulFloatRow) {
-        int rc = fc_chain_launch_emul(m->plan, images, n, out_shift, logits, labels, st);
+        int rc = fc_chain_launch(m->plan, kFormEmulFloat, images, n, logits, labels, out_shift, nullptr, st);
         return rc ? fail(BNM_E_CUDA, "fused emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
     if (route == kEmulInt8Row) {
         const size_t chunk = std::min(n, kFusedCnnChunk);
         const size_t row_bytes = cnn ? m->feat_stride : elems;
-        if (m->emul_rows_n < chunk) {
-            cudaFree(m->d_emul_rows);
-            m->d_emul_rows = nullptr; m->emul_rows_n = 0;
-            CU_TRY(cudaMalloc(&m->d_emul_rows, chunk * row_bytes));
-            m->emul_rows_n = chunk;
-        }
+        CU_TRY(m->d_emul_rows.grow(chunk * row_bytes));
+        int8_t *rows = m->d_emul_rows.p;
         for (size_t b = 0; b < n; b += chunk) {
             const size_t nb = std::min(chunk, n - b);
-            if (!cnn) launch_quantize_images(images + b * elems, elems, m->d_emul_rows, nb, st);   // BitNetMCU.py:435-436
-            else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0], m->d_conv[1], m->d_conv[2], C, m->d_emul_rows, m->feat_stride, nb, st))
+            if (!cnn) launch_quantize_images(images + b * elems, elems, rows, nb, st);   // BitNetMCU.py:435-436
+            else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, rows, m->feat_stride, nb, st))
                 return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
-            int rc = fc_chain_launch_emul_i8(m->plan, m->d_emul_rows, nb, out_shift, logits ? logits + b * m->n_classes : nullptr,
-                                             labels ? labels + b : nullptr, st);
+            int rc = fc_chain_launch(m->plan, kFormEmulInt8, rows, nb, logits ? logits + b * m->n_classes : nullptr,
+                                     labels ? labels + b : nullptr, out_shift, nullptr, st);
             if (rc) return fail(BNM_E_CUDA, "fused int8 emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
         }
         cudaError_t e = cudaGetLastError();
@@ -892,15 +869,10 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
     }
     const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
     if (int rc = ensure_scratch(m, chunk, true)) return rc;   // accumulators and the two int8 activation buffers
-    if (m->emul_n < chunk) {
-        cudaFree(m->d_emul_q); cudaFree(m->d_emul_planes[0]); cudaFree(m->d_emul_planes[1]);
-        m->d_emul_q = nullptr; m->d_emul_planes[0] = m->d_emul_planes[1] = nullptr; m->emul_n = 0;
-        CU_TRY(cudaMalloc(&m->d_emul_q, chunk * elems));
-        if (cnn)
-            for (auto &p : m->d_emul_planes) CU_TRY(cudaMalloc(&p, chunk * C * 256 * 4));
-        m->emul_n = chunk;
-    }
-    int8_t *q = m->d_emul_q, *a0 = m->d_act[0], *a1 = m->d_act[1];
+    CU_TRY(m->d_emul_q.grow(chunk * elems));
+    if (cnn)
+        for (auto &p : m->d_emul_planes) CU_TRY(p.grow(chunk * C * 256 * 4));
+    int8_t *q = m->d_emul_q.p, *a0 = m->d_act[0].p, *a1 = m->d_act[1].p;
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         launch_quantize_images(images + b * elems, elems, q, nb, st);   // BitNetMCU.py:435-436
@@ -908,14 +880,14 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
         uint32_t stride = elems;
         if (cnn) {
             // conv (ReLU, no shift) -> per-image renormalisation, pools in between (BitNetMCU.py:459-526), planes [(image, channel)][xy*xy]
-            int32_t *p0 = m->d_emul_planes[0], *p1 = m->d_emul_planes[1];
+            int32_t *p0 = m->d_emul_planes[0].p, *p1 = m->d_emul_planes[1].p;
             launch_expand_image(q, p0, C, 256, nb, st);
-            launch_conv33relu(p0, m->d_conv[0], C, 16, 0, p1, nb * C, st);
+            launch_conv33relu(p0, m->d_conv[0].p, C, 16, 0, p1, nb * C, st);
             launch_conv_renorm(p1, C * 196, nb, st);
-            launch_conv33relu(p1, m->d_conv[1], C, 14, 0, p0, nb * C, st);
+            launch_conv33relu(p1, m->d_conv[1].p, C, 14, 0, p0, nb * C, st);
             launch_conv_renorm(p0, C * 144, nb, st);
             launch_maxpool22(p0, 12, p1, nb * C, st);
-            launch_conv33relu(p1, m->d_conv[2], C, 6, 0, p0, nb * C, st);
+            launch_conv33relu(p1, m->d_conv[2].p, C, 6, 0, p0, nb * C, st);
             launch_conv_renorm(p0, C * 16, nb, st);
             launch_maxpool22(p0, 4, p1, nb * C, st);
             launch_i32_to_i8(p1, C * 4, a1, m->feat_stride, nb, st);   // flatten (C, 2, 2) -> features (BitNetMCU.py:443-445)
@@ -923,15 +895,15 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
             stride = m->feat_stride;
         }
         for (size_t l = 0; l < nl; l++) {
-            if (!launch_fc_dp4a(act, stride, m->fc[l], m->d_acc, nb, st)) return fail(BNM_E_UNSUPPORTED, "FC layer %zu too wide for the layer kernel", l);
+            if (!launch_fc_dp4a(act, stride, m->fc[l], m->d_acc.p, nb, st)) return fail(BNM_E_UNSUPPORTED, "FC layer %zu too wide for the layer kernel", l);
             if (l + 1 == nl) break;   // no renormalisation for the last layer (BitNetMCU.py:528-530)
             int8_t *next = (l & 1) ? a1 : a0;   // CNN features sit in a1 and are dead once layer 0 has run
             const uint32_t next_stride = m->fc[l + 1].k_pad;
-            launch_relunorm_emul(m->d_acc, m->fc[l].n_out, level_shift_of(m->fc[l].enc), next, next_stride, nb, st);
+            launch_relunorm_emul(m->d_acc.p, m->fc[l].n_out, level_shift_of(m->fc[l].enc), next, next_stride, nb, st);
             act = next;
             stride = next_stride;
         }
-        launch_emul_logits(m->d_acc, m->n_classes, out_shift, logits ? logits + b * m->n_classes : nullptr, labels ? labels + b : nullptr, nb, st);
+        launch_emul_logits(m->d_acc.p, m->n_classes, out_shift, logits ? logits + b * m->n_classes : nullptr, labels ? labels + b : nullptr, nb, st);
     }
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
@@ -954,19 +926,14 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
     CU_TRY(cudaSetDevice(m->device));
     const size_t elems = m->img_bytes, ncls = m->n_classes;
     const size_t chunk = std::min(n, m->model_class == BNM_MODEL_CNNMNIST ? kEmulChunkCnn : kEmulChunkFc);
-    if (m->emul_host_n < chunk) {
-        cudaFree(m->d_emul_in); cudaFree(m->d_emul_out);
-        m->d_emul_in = nullptr; m->d_emul_out = nullptr; m->emul_host_n = 0;
-        CU_TRY(cudaMalloc(&m->d_emul_in, chunk * elems * sizeof(float)));
-        CU_TRY(cudaMalloc(&m->d_emul_out, chunk * ncls * sizeof(double)));
-        m->emul_host_n = chunk;
-    }
+    CU_TRY(m->d_emul_in.grow(chunk * elems * sizeof(float)));
+    CU_TRY(m->d_emul_out.grow(chunk * ncls * sizeof(double)));
     cudaStream_t st = m->slots[0].stream;
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
-        CU_TRY(cudaMemcpyAsync(m->d_emul_in, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
-        if (int rc = emulate_device(m, m->d_emul_in, nb, m->d_emul_out, nullptr, st)) return rc;
-        CU_TRY(cudaMemcpyAsync(logits + b * ncls, m->d_emul_out, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(m->d_emul_in.p, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
+        if (int rc = emulate_device(m, m->d_emul_in.p, nb, m->d_emul_out.p, nullptr, st)) return rc;
+        CU_TRY(cudaMemcpyAsync(logits + b * ncls, m->d_emul_out.p, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
     }
     return 0;

@@ -75,27 +75,24 @@ struct ChainParams {
 
 struct ChainKernel;
 
+// a launch form of a plan: its kernel row and its shared-memory layout, which every launch of the form copies into ChainParams
+struct FormLayout {
+    const ChainKernel *kernel = nullptr;   // null: the plan has no such form
+    uint32_t n_stages = 0;                 // stages per pipe
+    uint32_t off_w = 0, off_fring = 0;     // as in ChainParams; off_fring only for the float-input forms
+    size_t smem_bytes = 0;                 // dynamic shared memory
+};
+
 struct FcChainPlan {
     ChainParams p{};
     uint8_t *d_w_image = nullptr;
     int *d_err = nullptr;             // error word of the bounded device-side waits: mapped pinned host memory, readable after a trap
     int *h_err = nullptr;
-    size_t smem_bytes = 0;
     uint32_t in_bytes = 0;
-    const ChainKernel *kernel = nullptr;       // the instantiation of int8 launches
-    const ChainKernel *kernel_f32 = nullptr;   // and of float-input launches (null: not supported)
-    const ChainKernel *kernel_emul = nullptr;  // fc_emul_kernel: with kernel_f32, on its shared-memory layout (f_* below)
+    FormLayout forms[kFcForms];
     int sm_count = 0;
     int device = 0;
     int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 plain launch, 1 dependent launch + wait, 2 independent launches
-    // float-input launches: one pipe, fewer int8 stages, the freed shared memory holds the quantiser warps' float rings
-    uint32_t f_n_stages = 0, f_off_w = 0, f_off_fring = 0;
-    size_t f_smem_bytes = 0;
-    // emulator launches on int8 rows (fc_emul_i8_kernel at the plan's width): one pipe, so a 64-wide plan, whose int8 launches run
-    // two, needs its own stage count and shared-memory layout
-    const ChainKernel *kernel_emul_i8 = nullptr;
-    uint32_t e_n_stages = 0, e_off_w = 0;
-    size_t e_smem_bytes = 0;
     struct TmapSlot { const void *ptr = nullptr; size_t n = 0; CUtensorMap map; };
     TmapSlot tmaps[4];                // tensor maps of the most recent (pointer, n) pairs: double/triple-buffered callers hit every time
     unsigned tmap_next = 0;
@@ -799,7 +796,8 @@ static void trace_before(cudaStream_t) {}
 static void trace_after(cudaStream_t) {}
 #endif
 
-// the instantiations of fc_chain_kernel, one row each, named by their template arguments <kN, kPipes, kSlots, kLastN>
+// the instantiations of fc_chain_kernel, fc_emul_kernel and fc_emul_i8_kernel, one row each, named by their template arguments
+// <kN, kPipes, kSlots, kLastN>
 struct ChainKernel {
     const char *name;
     void (*fn)(CUtensorMap, ChainParams);
@@ -809,7 +807,14 @@ template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bo
 static ChainKernel chain_kernel(const char *name) {
     return {name, fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed>, chain_threads<kN, kPipes, kFloatIn, kSlots>()};
 }
-enum ChainRow { kRow64, kRow64x2, kRow64x2Last16, kRowFixed, kRow128, kRow192, kRow256, kRowFloat, kChainRows };
+template <int kN>
+static ChainKernel emul_i8_kernel(const char *name) { return {name, fc_emul_i8_kernel<kN>, chain_threads<kN, 1, false, 1>()}; }
+enum ChainRow {
+    kRow64, kRow64x2, kRow64x2Last16, kRowFixed, kRow128, kRow192, kRow256, kRowFloat,
+    kRowEmulFloat,
+    kRowEmul64, kRowEmul128, kRowEmul192, kRowEmul256,   // row kRowEmul64 + max_n / 64 - 1
+    kChainRows
+};
 static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
     std::array<ChainKernel, kChainRows> t{};
     t[kRow64] = chain_kernel<64, 1, false>("<64,1>");
@@ -820,15 +825,13 @@ static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
     t[kRow192] = chain_kernel<192, 1, false>("<192,1>");
     t[kRow256] = chain_kernel<256, 1, false>("<256,1>");
     t[kRowFloat] = chain_kernel<64, 1, true>("<64,1,float>");
+    t[kRowEmulFloat] = {"<64,1,float,emul>", fc_emul_kernel, chain_threads<64, 1, true, 1>()};
+    t[kRowEmul64] = emul_i8_kernel<64>("<64,1,emul>");
+    t[kRowEmul128] = emul_i8_kernel<128>("<128,1,emul>");
+    t[kRowEmul192] = emul_i8_kernel<192>("<192,1,emul>");
+    t[kRowEmul256] = emul_i8_kernel<256>("<256,1,emul>");
     return t;
 }();
-static const ChainKernel kEmulKernel = {"<64,1,float,emul>", fc_emul_kernel, chain_threads<64, 1, true, 1>()};
-// the instantiations of fc_emul_i8_kernel, row max_n / 64 - 1
-template <int kN>
-static ChainKernel emul_i8_kernel(const char *name) { return {name, fc_emul_i8_kernel<kN>, chain_threads<kN, 1, false, 1>()}; }
-static const std::array<ChainKernel, 4> kEmulI8Kernels = {
-    emul_i8_kernel<64>("<64,1,emul>"), emul_i8_kernel<128>("<128,1,emul>"), emul_i8_kernel<192>("<192,1,emul>"),
-    emul_i8_kernel<256>("<256,1,emul>")};
 
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
                                   char *err, size_t err_len) {
@@ -864,9 +867,20 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     const uint32_t smem_limit = 227 * 1024 - 1024 /*alignment slack*/ - 1024 /*static: barriers*/;
     const uint32_t w_fixed = round_up(p.w_bytes, 128);
     if (w_fixed + 2 * p.stage_bytes > smem_limit) { delete plan; return fail("fused path: weights do not fit in shared memory"); }
-    const uint32_t total_stages = std::min<uint32_t>(kMaxStages, (smem_limit - w_fixed) / p.stage_bytes);
-    const uint32_t pipes = (max_n == 64 && total_stages >= 4) ? 2 : 1;
-    p.n_stages = std::min<uint32_t>(total_stages / pipes, 6);   // >= 2 with two pipes: two tile slots need it
+    // the layout of a form: `pipes` rings of at most `cap` stages each in what the weight image and `extra` bytes (the float-input
+    // forms' quantiser rings) leave, then the weights, then the extra bytes
+    auto layout = [&](int row, uint32_t pipes, uint32_t cap, uint32_t extra) {
+        FormLayout f;
+        f.kernel = &kChainKernels[row];
+        f.n_stages = std::min<uint32_t>(cap, (smem_limit - w_fixed - extra) / p.stage_bytes / pipes);
+        f.off_w = pipes * f.n_stages * p.stage_bytes;
+        f.off_fring = extra ? f.off_w + w_fixed : 0;
+        // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared
+        // memory enforces it once a CTA asks for more than half of the SM's 227 kB.
+        f.smem_bytes = std::max<size_t>((size_t)f.off_w + w_fixed + extra + 1024, 116 * 1024);
+        return f;
+    };
+    const uint32_t pipes = (max_n == 64 && (smem_limit - w_fixed) / p.stage_bytes >= 4) ? 2 : 1;
     // two pipes run two slots, which issue a last layer of at most 16 columns 16 wide (kLastN); plans of exactly the fixed
     // shape class (kFixedLayers and the fixed_* shapes) run the fixed-shape kernel
     const bool last16 = layers[n_layers - 1].n_pad <= 16;
@@ -875,37 +889,28 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
         fixed = p.planes[l] == 1 && p.n_pad[l] == fixed_n_pad(l) && p.k_steps[l] == fixed_k_steps(l) && p.b_off[l] == fixed_b_off(l);
     int row = max_n == 64 ? kRow64 : max_n == 128 ? kRow128 : max_n == 192 ? kRow192 : kRow256;
     if (pipes == 2) row = fixed ? kRowFixed : last16 ? kRow64x2Last16 : kRow64x2;
-    plan->kernel = &kChainKernels[row];
-    p.off_w = pipes * p.n_stages * p.stage_bytes;
-    // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared memory
-    // enforces it once a CTA asks for more than half of the SM's 227 kB.
-    plan->smem_bytes = std::max<size_t>((size_t)p.off_w + w_fixed + 1024, 116 * 1024);
-    // float-input path: the eight quantiser warps make 17 warps, so at most 96 registers per thread -- models up to 64 wide
-    if (in_bytes <= 256 && p.n_classes <= 16 && max_n == 64) {
-        const uint32_t fring = kFloatQuantWarps * 2 * kFloatGroupRows * 1024;
-        const uint32_t fixed_f = w_fixed + fring;
-        if (fixed_f + 2 * p.stage_bytes <= smem_limit) {
-            plan->f_n_stages = std::min<uint32_t>(4, (smem_limit - fixed_f) / p.stage_bytes);
-            plan->f_off_w = plan->f_n_stages * p.stage_bytes;
-            plan->f_off_fring = plan->f_off_w + w_fixed;
-            plan->f_smem_bytes = std::max<size_t>((size_t)plan->f_off_fring + fring + 1024, 116 * 1024);
-            plan->kernel_f32 = &kChainKernels[kRowFloat];
-            plan->kernel_emul = &kEmulKernel;
-        }
+    FormLayout *forms = plan->forms;
+    // at most kMaxStages over the pipes and 6 per pipe; >= 2 with two pipes: two tile slots need it
+    forms[kFormInt8] = layout(row, pipes, std::min<uint32_t>(kMaxStages / pipes, 6), 0);
+    // float-input forms: the eight quantiser warps make 17 warps, so at most 96 registers per thread -- models up to 64 wide.
+    // One pipe, fewer int8 stages, the freed shared memory holds the quantiser warps' float rings
+    const uint32_t fring = kFloatQuantWarps * 2 * kFloatGroupRows * 1024;
+    if (in_bytes <= 256 && p.n_classes <= 16 && max_n == 64 && w_fixed + fring + 2 * p.stage_bytes <= smem_limit) {
+        forms[kFormFloat] = layout(kRowFloat, 1, 4, fring);
+        forms[kFormEmulFloat] = layout(kRowEmulFloat, 1, 4, fring);
     }
-    // emulator on int8 rows: the one-pipe layout (for max_n > 64 the same as the int8 launches')
-    plan->kernel_emul_i8 = &kEmulI8Kernels[max_n / 64 - 1];
-    plan->e_n_stages = std::min<uint32_t>(total_stages, 6);
-    plan->e_off_w = plan->e_n_stages * p.stage_bytes;
-    plan->e_smem_bytes = std::max<size_t>((size_t)plan->e_off_w + w_fixed + 1024, 116 * 1024);
+    // the emulator on int8 rows runs one pipe at every width, so a 64-wide plan, whose int8 form runs two, has its own layout
+    forms[kFormEmulInt8] = layout(kRowEmul64 + max_n / 64 - 1, 1, 6, 0);
     if (getenv("BNM_VERBOSE")) {   // diagnostics: the shapes this plan launches
+        const bool has_float = forms[kFormFloat].kernel;
         char f_stages[32] = "";
-        if (plan->kernel_f32) snprintf(f_stages, sizeof(f_stages), ", float input stages %u", plan->f_n_stages);
+        if (has_float) snprintf(f_stages, sizeof(f_stages), ", float input stages %u", forms[kFormFloat].n_stages);
         fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, "
-                "fc_chain_kernel%s%s%s%s%s%s, int8 emulator fc_emul_i8_kernel%s x %u stages\n", max_n, pipes, p.n_stages, p.w_bytes,
-                plan->smem_bytes, plan->kernel->name, plan->kernel_f32 ? ", float input " : "", plan->kernel_f32 ? plan->kernel_f32->name : "",
-                plan->kernel_emul ? ", emulator " : "", plan->kernel_emul ? plan->kernel_emul->name : "", f_stages,
-                plan->kernel_emul_i8->name, plan->e_n_stages);
+                "fc_chain_kernel%s%s%s%s%s%s, int8 emulator fc_emul_i8_kernel%s x %u stages\n", max_n, pipes, forms[kFormInt8].n_stages,
+                p.w_bytes, forms[kFormInt8].smem_bytes, forms[kFormInt8].kernel->name, has_float ? ", float input " : "",
+                has_float ? forms[kFormFloat].kernel->name : "", has_float ? ", emulator " : "",
+                has_float ? forms[kFormEmulFloat].kernel->name : "", f_stages, forms[kFormEmulInt8].kernel->name,
+                forms[kFormEmulInt8].n_stages);
     }
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
@@ -930,13 +935,11 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     if (cudaDeviceSynchronize() != cudaSuccess) { fc_chain_plan_destroy(plan); return fail("weight image kernel failed"); }
     p.w_image = plan->d_w_image;
     p.err = plan->d_err;
-    if (!raise_smem_limit((const void *)plan->kernel->fn, plan->smem_bytes) ||
-        (plan->kernel_f32 && !raise_smem_limit((const void *)plan->kernel_f32->fn, plan->f_smem_bytes)) ||
-        (plan->kernel_emul && !raise_smem_limit((const void *)plan->kernel_emul->fn, plan->f_smem_bytes)) ||
-        !raise_smem_limit((const void *)plan->kernel_emul_i8->fn, plan->e_smem_bytes)) {
-        fc_chain_plan_destroy(plan);
-        return fail("cannot opt in to the required dynamic shared memory");
-    }
+    for (const FormLayout &f : plan->forms)
+        if (f.kernel && !raise_smem_limit((const void *)f.kernel->fn, f.smem_bytes)) {
+            fc_chain_plan_destroy(plan);
+            return fail("cannot opt in to the required dynamic shared memory");
+        }
     return plan;
 }
 
@@ -974,34 +977,34 @@ static const CUtensorMap *plan_tensor_map(FcChainPlan *plan, const int8_t *in, s
     return &t.map;
 }
 
-// the per-launch part of the parameters (outputs, no gather destinations) and the configuration of a launch of kernel k with
-// `smem` bytes of dynamic shared memory: a CTA per tile, at most one per SM
-static cudaLaunchConfig_t launch_setup(const FcChainPlan *plan, const ChainKernel *k, size_t smem, size_t n, int32_t *logits,
-                                       uint32_t *labels, cudaStream_t st, ChainParams &p) {
-    p.logits = logits;
-    p.labels = labels;
-    p.n = n;
-    p.n_lab_dst = p.n_log_dst = 0;
-    p.row0 = 0;
-    p.lab_u8 = 0;
-    p.n_tiles = (uint32_t)((n + kTileM - 1) / kTileM);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)std::min<uint32_t>(p.n_tiles, (uint32_t)plan->sm_count));
-    cfg.blockDim = dim3(k->threads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    return cfg;
-}
+bool fc_chain_has_form(const FcChainPlan *plan, FcForm f) { return plan && plan->forms[f].kernel; }
 
-int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather,
-                    cudaStream_t st) {
+const char *fc_chain_form_name(const FcChainPlan *plan, FcForm f) { return plan->forms[f].kernel->name; }
+
+static const CUtensorMap kNoTensorMap{};   // the float-input forms' tensor map: not used (no TMA image loads)
+
+int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
+                    const GatherDst *gather, cudaStream_t st) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
-    ChainParams p = plan->p;
-    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel, plan->smem_bytes, n, logits, labels, st, p);
+    const FormLayout &form = plan->forms[f];
+    if (!form.kernel) return -6;
+    const bool engine_i8 = f == kFormInt8, float_in = f == kFormFloat || f == kFormEmulFloat;
+    ChainParams p = plan->p;   // the model's shapes; null outputs, no result exchange
+    p.n_stages = form.n_stages;
+    p.off_w = form.off_w;
+    p.off_fring = form.off_fring;
+    if (f == kFormEmulFloat || f == kFormEmulInt8) {
+        p.emul_logits = static_cast<double *>(logits);
+        p.emul_logit_scale = level_shift ? 0.5 : 1.0;
+    } else {
+        p.logits = static_cast<int32_t *>(logits);
+    }
+    p.labels = labels;
+    p.n = n;
+    p.n_tiles = (uint32_t)((n + kTileM - 1) / kTileM);
     if (gather) {
-        if (gather->n_labels_dst > (uint32_t)kMaxGatherDst || gather->n_logits_dst > (uint32_t)kMaxGatherDst) return -5;
+        if (!engine_i8 || gather->n_labels_dst > (uint32_t)kMaxGatherDst || gather->n_logits_dst > (uint32_t)kMaxGatherDst) return -5;
         p.n_lab_dst = gather->n_labels_dst;
         p.n_log_dst = gather->n_logits_dst;
         p.row0 = gather->row_offset;
@@ -1010,90 +1013,38 @@ int fc_chain_launch(FcChainPlan *plan, const int8_t *in, size_t n, int32_t *logi
         for (uint32_t d = 0; d < p.n_lab_dst; d++) p.lab_dst[d] = gather->labels_dst[d];
         for (uint32_t d = 0; d < p.n_log_dst; d++) p.log_dst[d] = gather->logits_dst[d];
     }
-    const CUtensorMap *tmap_p = plan_tensor_map(plan, in, n);
-    if (!tmap_p) return -3;
-    // Mode 2 drops the grid-dependency wait, i.e. EVERY ordering against the work enqueued before this launch on the stream
-    // (the previous bnm launch and any producer kernel of `images` alike).  The library keeps the wait whenever it can see the
-    // promise being broken: first launch on this plan / another stream / a buffer of the previous launch reused.  A null output
-    // is no buffer: it neither reuses nor differs from one.
-    bool independent = plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && in != plan->prev_in &&
-                       (logits == nullptr || logits != plan->prev_logits) && (labels == nullptr || labels != plan->prev_labels);
+    const CUtensorMap *tmap_p = &kNoTensorMap;
+    if (float_in) {
+        p.fimages = static_cast<const float *>(in);
+        p.in_elems = plan->in_bytes;
+    } else if (!(tmap_p = plan_tensor_map(plan, static_cast<const int8_t *>(in), n))) {
+        return -3;
+    }
+    // a CTA per tile, at most one per SM
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)std::min<uint32_t>(p.n_tiles, (uint32_t)plan->sm_count));
+    cfg.blockDim = dim3(form.kernel->threads);
+    cfg.dynamicSmemBytes = form.smem_bytes;
+    cfg.stream = st;
+    // Only the C engine's int8 form overlaps launches; every other form is a plain launch, ordered by the stream alone, whose
+    // grid-dependency wait returns at once.  Mode 2 drops the wait, i.e. EVERY ordering against the work enqueued before this
+    // launch on the stream (the previous bnm launch and any producer kernel of `images` alike).  The library keeps the wait
+    // whenever it can see the promise being broken: first launch on this plan / another stream / a buffer of the previous launch
+    // reused / a launch of another form in between.  A null output is no buffer: it neither reuses nor differs from one.
+    const bool independent = engine_i8 && plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && in != plan->prev_in &&
+                             (logits == nullptr || logits != plan->prev_logits) && (labels == nullptr || labels != plan->prev_labels);
     p.wait_prior_grid = !independent;
-    p.early_trigger = plan->overlap != 0 && cfg.gridDim.x == (unsigned)plan->sm_count;
-    plan->prev_in = in; plan->prev_logits = logits; plan->prev_labels = labels; plan->prev_stream = st; plan->prev_valid = true;
+    p.early_trigger = engine_i8 && plan->overlap != 0 && cfg.gridDim.x == (unsigned)plan->sm_count;
+    plan->prev_in = in; plan->prev_logits = logits; plan->prev_labels = labels; plan->prev_stream = st; plan->prev_valid = engine_i8;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = plan->overlap ? 1 : 0;
+    cfg.numAttrs = engine_i8 && plan->overlap ? 1 : 0;
     trace_before(st);
-    if (cudaLaunchKernelEx(&cfg, plan->kernel->fn, *tmap_p, p) != cudaSuccess) return -4;
+    if (cudaLaunchKernelEx(&cfg, form.kernel->fn, *tmap_p, p) != cudaSuccess) return -4;
     trace_after(st);
-    return cudaGetLastError() == cudaSuccess ? 0 : -4;
-}
-
-bool fc_chain_float_input_supported(const FcChainPlan *plan) {
-    return plan && plan->kernel_f32 && plan->in_bytes % 16 == 0;
-}
-
-// a launch of kernel k (kernel_f32 or kernel_emul) on float32 images [n][in_bytes elements], the input scaling fused into the load
-// stage (kFloatIn); p holds the outputs
-static int launch_float_input(FcChainPlan *plan, const ChainKernel *k, cudaLaunchConfig_t &cfg, ChainParams &p, const float *in) {
-    p.fimages = in;
-    p.in_elems = plan->in_bytes;
-    p.n_stages = plan->f_n_stages;
-    p.off_w = plan->f_off_w;
-    p.off_fring = plan->f_off_fring;
-    p.wait_prior_grid = 1;
-    p.early_trigger = 0;
-    CUtensorMap tmap;   // not used by the float-input kernel (no TMA image loads)
-    memset(&tmap, 0, sizeof(tmap));
-    plan->prev_valid = false;
-    if (cudaLaunchKernelEx(&cfg, k->fn, tmap, p) != cudaSuccess) return -4;
-    return cudaGetLastError() == cudaSuccess ? 0 : -4;
-}
-
-// float32 images [n][in_bytes elements] -> logits / labels (either may be null)
-int fc_chain_launch_f32(FcChainPlan *plan, const float *in, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st) {
-    if (n == 0) return 0;
-    if (n > 0x7fffff00ull) return -2;
-    if (!fc_chain_float_input_supported(plan)) return -6;
-    ChainParams p = plan->p;
-    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_f32, plan->f_smem_bytes, n, logits, labels, st, p);
-    return launch_float_input(plan, plan->kernel_f32, cfg, p, in);
-}
-
-int fc_chain_launch_emul(FcChainPlan *plan, const float *in, size_t n, int level_shift, double *logits, uint32_t *labels, cudaStream_t st) {
-    if (n == 0) return 0;
-    if (n > 0x7fffff00ull) return -2;
-    if (!fc_chain_float_input_supported(plan) || !plan->kernel_emul) return -6;
-    ChainParams p = plan->p;
-    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_emul, plan->f_smem_bytes, n, nullptr, labels, st, p);
-    p.emul_logits = logits;
-    p.emul_logit_scale = level_shift ? 0.5 : 1.0;
-    return launch_float_input(plan, plan->kernel_emul, cfg, p, in);
-}
-
-const char *fc_chain_emul_name(const FcChainPlan *plan, bool float_row) {
-    return float_row ? plan->kernel_emul->name : plan->kernel_emul_i8->name;
-}
-
-int fc_chain_launch_emul_i8(FcChainPlan *plan, const int8_t *in, size_t n, int level_shift, double *logits, uint32_t *labels,
-                            cudaStream_t st) {
-    if (n == 0) return 0;
-    if (n > 0x7fffff00ull) return -2;
-    ChainParams p = plan->p;
-    cudaLaunchConfig_t cfg = launch_setup(plan, plan->kernel_emul_i8, plan->e_smem_bytes, n, nullptr, labels, st, p);
-    p.emul_logits = logits;
-    p.emul_logit_scale = level_shift ? 0.5 : 1.0;
-    p.n_stages = plan->e_n_stages;
-    p.off_w = plan->e_off_w;
-    p.wait_prior_grid = 0;   // a plain launch: stream order alone
-    p.early_trigger = 0;
-    const CUtensorMap *tmap_p = plan_tensor_map(plan, in, n);
-    if (!tmap_p) return -3;
-    plan->prev_valid = false;   // the next C-engine launch keeps its grid-dependency wait
-    if (cudaLaunchKernelEx(&cfg, plan->kernel_emul_i8->fn, *tmap_p, p) != cudaSuccess) return -4;
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 

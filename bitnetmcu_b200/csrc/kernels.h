@@ -84,26 +84,25 @@ struct FcChainPlan;  // opaque, owned by the model
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
                                   char *err, size_t err_len);
 void fc_chain_plan_destroy(FcChainPlan *p);
-// 0 plain launches, 1 programmatic dependent launch (inputs read after the previous kernel completed), 2 launches declared independent
+// kFormInt8 launches: 0 plain launches, 1 programmatic dependent launch (inputs read after the previous kernel completed), 2 launches
+// declared independent
 void fc_chain_plan_set_overlap(FcChainPlan *p, int mode);
-// images int8 [n][in_bytes] (device, 16B aligned) -> logits int32 [n][n_classes], labels uint32 [n] (each may be null)
-// gather (may be null): extra destination buffers every row is also stored to (peer memory), fused into the epilogue
-int fc_chain_launch(FcChainPlan *p, const int8_t *in, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather,
-                    cudaStream_t st);
-
-// float32 images [n][in_bytes] (elements) -> logits / labels with the input scaling of test_inference.py:140-141 fused into the
-// kernel's load stage; supported for image rows of up to 256 elements and up to 16 classes
-bool fc_chain_float_input_supported(const FcChainPlan *p);
-int fc_chain_launch_f32(FcChainPlan *p, const float *in, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st);
-// the same launch with the reference's Python emulator in place of the C engine (fc_emul_kernel): its hidden-layer rule and float64
-// logits = last layer's accumulators x 2^-level_shift (level_shift 0 or 1); logits / labels may each be null.  Where
-// fc_chain_float_input_supported holds.
-int fc_chain_launch_emul(FcChainPlan *p, const float *in, size_t n, int level_shift, double *logits, uint32_t *labels, cudaStream_t st);
-// the emulator on int8 rows [n][in_bytes] (device, 16B aligned) that are already scaled (fc_emul_i8_kernel, every plan)
-int fc_chain_launch_emul_i8(FcChainPlan *p, const int8_t *in, size_t n, int level_shift, double *logits, uint32_t *labels,
-                            cudaStream_t st);
-// the template arguments of the emulator row a launch takes: fc_emul_kernel (float_row) or fc_emul_i8_kernel, e.g. "<192,1,emul>"
-const char *fc_chain_emul_name(const FcChainPlan *p, bool float_row);
+// The launch forms of a plan, by input and by rule:
+//   kFormInt8       the C engine on int8 images [n][in_bytes] (device, 16B aligned): fc_chain_kernel, every plan
+//   kFormFloat      the C engine on float32 images [n][in_bytes elements], the input scaling of test_inference.py:140-141 fused
+//                   into the kernel's load stage: FC rows of up to 256 elements, models up to 64 wide with up to 16 classes
+//   kFormEmulFloat  the reference's Python emulator in place of the C engine (fc_emul_kernel): the plans with kFormFloat
+//   kFormEmulInt8   the emulator on int8 rows [n][in_bytes] that are already scaled (fc_emul_i8_kernel), every plan
+// The emulator forms have the emulator's hidden-layer rule and float64 logits = last layer's accumulators x 2^-level_shift (0 or 1).
+enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFcForms };
+bool fc_chain_has_form(const FcChainPlan *p, FcForm f);
+// the template arguments of the kernel of a form the plan has, e.g. "<192,1,emul>"
+const char *fc_chain_form_name(const FcChainPlan *p, FcForm f);
+// one launch of form f on n images `in` -> logits (int32 [n][n_classes], float64 for the emulator forms) and labels uint32 [n];
+// each may be null.  gather (kFormInt8 only, may be null): extra destination buffers every row is also stored to (peer memory),
+// fused into the epilogue.  0, or a negative code (-6: the plan has no form f)
+int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
+                    const GatherDst *gather, cudaStream_t st);
 // the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
 // [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
 constexpr uint32_t kCnnEmulMaxChannels = 128;

@@ -342,7 +342,7 @@ def test_ring_rounds(lib, capfd, monkeypatch, width):
     m = P.random_fc_model(M.ENC_8BIT, (256, width, width, 17), seed=width)
     e, route = _route(m, capfd, monkeypatch)
     assert route == f"k_quantize_images + fc_emul_i8_kernel<{width},1,emul>", route
-    max_stages = 6   # fc_chain_plan_create: e_n_stages <= 6
+    max_stages = 6   # fc_chain_plan_create: the int8 emulator form has at most 6 stages
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     n = sms * 128 * (3 * max_stages + 1) + 77
     d_x = _device_images(n, seed=width)
