@@ -21,6 +21,7 @@ EXPORTED = [
     "bnm_quantize_images", "bnm_quantize_images_device",
     "bnm_infer_batch_device_gather", "bnm_device_alloc", "bnm_device_free", "bnm_ipc_export", "bnm_ipc_open", "bnm_ipc_close",
     "bnm_enable_peer_access", "bnm_emulate_inference_quantized", "bnm_infer_batch_device_f32", "bnm_emulate_batch_device",
+    "bnm_compare_engines_device",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
@@ -80,6 +81,7 @@ def load() -> C.CDLL:
         "bnm_emulate_inference_quantized": (C.c_int, [vp, vp, sz, vp]),
         "bnm_emulate_batch_device": (C.c_int, [vp, vp, sz, vp, vp, vp]),
         "bnm_infer_batch_device_f32": (C.c_int, [vp, vp, sz, vp, vp, vp]),
+        "bnm_compare_engines_device": (C.c_int, [vp, vp, sz, vp, vp, vp, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

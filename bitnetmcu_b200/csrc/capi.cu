@@ -126,6 +126,7 @@ struct bnm_model {
     DevBuf<float> d_emul_in;
     DevBuf<double> d_emul_out;
     DevBuf<int8_t> d_emul_rows;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
+    DevBuf<uint32_t> d_engine_labels[2];   // bnm_compare_engines_device's two routes: C / emulator labels the caller does not take
     int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
                                // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
 };
@@ -223,6 +224,12 @@ static EmulRoute emul_route(const bnm_model *m) {
     return !cnn && fc_chain_has_form(m->plan, kFormEmulFloat) ? kEmulFloatRow : kEmulInt8Row;
 }
 
+// bnm_compare_engines_device: fc_engines_kernel for the models both float-input rows serve, else the two entries' routes and
+// k_engine_counts
+static bool engines_fused(const bnm_model *m) {
+    return bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST && fc_chain_has_form(m->plan, kFormEngines);
+}
+
 extern "C" int bnm_version(void) { return BNM_VERSION; }
 extern "C" const char *bnm_last_error(void) { return g_err.c_str(); }
 extern "C" int bnm_device_count(void) {
@@ -318,6 +325,9 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
                 r == kEmulLayers ? "layer by layer" : r == kEmulFloatRow ? "fc_emul_kernel" :
                 m->model_class == BNM_MODEL_CNNMNIST ? "k_cnn_emul_frontend + fc_emul_i8_kernel" : "k_quantize_images + fc_emul_i8_kernel",
                 r == kEmulLayers ? "" : fc_chain_form_name(m->plan, r == kEmulFloatRow ? kFormEmulFloat : kFormEmulInt8));
+        // and the kernels of bnm_compare_engines_device
+        if (engines_fused(m)) fprintf(stderr, "bitnetmcu_b200: engines route: fc_engines_kernel%s\n", fc_chain_form_name(m->plan, kFormEngines));
+        else fprintf(stderr, "bitnetmcu_b200: engines route: bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts\n");
     }
     *out = m;
     return 0;
@@ -937,6 +947,49 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
         CU_TRY(cudaStreamSynchronize(st));
     }
     return 0;
+}
+
+// -----------------------------------------------------------------------------------------------
+// Both engines in one call (test_inference.py:130-175): the C engine's and the emulator's labels of the same float images, and
+// counts of their agreement and of their accuracy against truth.  The one-pass kernel where both float-input rows exist; every
+// other model runs bnm_infer_batch_device_f32's and emulate_device's routes per chunk, into the caller's label buffers or the
+// model's scratch, then k_engine_counts.
+// -----------------------------------------------------------------------------------------------
+static const size_t kEnginesChunk = 1 << 20;   // images per pass of the two routes (bounds the label scratch)
+
+extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth, uint32_t *labels_c,
+                                          uint32_t *labels_py, bnm_engine_counts *counts, void *stream) {
+    static_assert(sizeof(bnm_engine_counts) == 4 * sizeof(unsigned long long), "bnm_engine_counts: four 64-bit counters");
+    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_compare_engines_device: null argument");
+    if (!labels_c && !labels_py && !counts) return fail(BNM_E_ARG, "bnm_compare_engines_device: no output (labels_c, labels_py and counts all NULL)");
+    if (truth && !counts) return fail(BNM_E_ARG, "bnm_compare_engines_device: truth without counts");
+    if (n == 0) return 0;
+    if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
+    if ((uintptr_t)counts & 7) return fail(BNM_E_ARG, "the device counts must be 8-byte aligned");
+    CU_TRY(cudaSetDevice(m->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    auto *cnt = reinterpret_cast<unsigned long long *>(counts);
+    if (engines_fused(m)) {
+        const EngineOutputs out{labels_py, truth, cnt};
+        int rc = fc_chain_launch(m->plan, kFormEngines, images, n, nullptr, labels_c, 0, nullptr, st, &out);
+        return rc ? fail(BNM_E_CUDA, "fused two-engine kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
+    }
+    const size_t chunk = std::min(n, kEnginesChunk), elems = m->img_bytes;
+    if (counts && !labels_c) CU_TRY(m->d_engine_labels[0].grow(chunk * sizeof(uint32_t)));
+    if (counts && !labels_py) CU_TRY(m->d_engine_labels[1].grow(chunk * sizeof(uint32_t)));
+    for (size_t b = 0; b < n; b += chunk) {
+        const size_t nb = std::min(chunk, n - b);
+        const float *img = images + b * elems;
+        uint32_t *lc = labels_c ? labels_c + b : counts ? m->d_engine_labels[0].p : nullptr;
+        uint32_t *lp = labels_py ? labels_py + b : counts ? m->d_engine_labels[1].p : nullptr;
+        if (lc)
+            if (int rc = bnm_infer_batch_device_f32(m, img, nb, nullptr, lc, st)) return rc;
+        if (lp)
+            if (int rc = emulate_device(m, img, nb, nullptr, lp, st)) return rc;
+        if (counts) launch_engine_counts(lc, lp, truth ? truth + b : nullptr, nb, m->n_classes, cnt, st);
+    }
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
 }
 
 // -----------------------------------------------------------------------------------------------

@@ -23,6 +23,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "kernels.h"
@@ -71,6 +72,11 @@ struct ChainParams {
     // emulator's 2^-level_shift of that layer's encoding (0.5 for 2bitsym / 4bitsym, else 1)
     double *emul_logits;
     double emul_logit_scale;
+    // both-engine launches (fc_engines_kernel): `labels` are the C engine's, labels_py the emulator's; truth [n] and counts
+    // (EngineTally's {images, correct_c, correct_py, mismatches}) may be null
+    uint32_t *labels_py;
+    const uint32_t *truth;
+    unsigned long long *counts;
 };
 
 struct ChainKernel;
@@ -277,12 +283,16 @@ struct RingPos {
 // one unrolled run of MMAs at compile-time descriptor offsets, ReLUNorm without predicates.
 // kEmul: the reference's Python emulator instead of the C engine (fc_emul_kernel): its hidden-layer rule (emul_coef) and float64
 // logits (P.emul_logits); no result exchange.
-// The body of both kernels below; tmap_in and P are their __grid_constant__ parameters (TMA reads the tensor map by address).
-template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, bool kEmul>
+// kEngines: both engines on one tile (fc_engines_kernel): layer 1 once, its accumulators through both hidden-layer rules, the C
+// chain and then the emulator's chain, both labels and their EngineTally counts; no logits, no result exchange.
+// The body of the kernels below; tmap_in and P are their __grid_constant__ parameters (TMA reads the tensor map by address).
+template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, bool kEmul, bool kEngines = false>
 __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const ChainParams &P) {
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
     static_assert(!kEmul || (kPipes == 1 && kSlots == 1 && kLastN == kN && !kFixed && (kN == 64 || !kFloatIn)),
                   "emulator: the 64-wide float-input launch, or one-pipe one-slot int8 launches at full width");
+    static_assert(!kEngines || (kN == 64 && kPipes == 1 && kFloatIn && kSlots == 1 && kLastN == kN && !kFixed && !kEmul),
+                  "both engines: the 64-wide float-input launch");
     static_assert(!kFloatIn || kPipes == 1, "float input: one pipe, whose stages the quantiser warps fill");
     static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
     static_assert(!kFixed || (kSlots == 2 && kLastN == fixed_n_pad(kFixedLayers - 1)), "fixed shape: two-slot launches of its class");
@@ -420,8 +430,9 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                         wgmma_ss_n64(a + c0 / 2, ad, b_desc((uint32_t)c0 < n_pad ? bt : w_zero, c0), (pl | k) != 0);
                 }
         };
-        // ---- ReLUNorm of layer l's accumulators a into the A fragments f of layer l + 1
-        auto relunorm = [&](const uint32_t *a, uint32_t *f, int l) {
+        // ---- ReLUNorm of layer l's accumulators a into the A fragments f of layer l + 1, by the emulator's rule when emul is
+        // std::true_type, else by the C engine's
+        auto relunorm_rule = [&](const uint32_t *a, uint32_t *f, int l, auto emul) {
             // kFixed: every layer with a ReLUNorm (all but the last) is 64 wide, so every block is taken, with no predicates
             const uint32_t n_pad = kFixed ? fixed_n_pad(0) : P.n_pad[l];
             int m0 = 0, m1 = 0;
@@ -437,7 +448,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
             m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
             m0 = max(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
             m1 = max(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-            auto coef = [](int m) { if constexpr (kEmul) return emul_coef(m); else return norm_coef(m); };
+            auto coef = [](int m) { if constexpr (decltype(emul)::value) return emul_coef(m); else return norm_coef(m); };
             const auto k0 = coef(m0), k1 = coef(m1);
             // 16-column block b -> register 2b (upper row) / 2b + 1 (lower row) of the fragments, i.e. for K-step s = b / 2:
             // f[4s] (upper row, block 2s), f[4s + 1] (lower, 2s), f[4s + 2] (upper, 2s + 1), f[4s + 3] (lower, 2s + 1)
@@ -453,6 +464,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                 }
             }
         };
+        auto relunorm = [&](const uint32_t *a, uint32_t *f, int l) { relunorm_rule(a, f, l, std::bool_constant<kEmul>{}); };
         // ---- layer l >= 1 into a (A: the fragments f)
         auto issue_layer = [&](uint32_t *a, const uint32_t *f, int l) {
             if constexpr (kFixed) {
@@ -496,6 +508,8 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
         // ---- logits + label of tile i from the last layer's accumulators a (dll.c:115-116: the last ReLUNorm's argmax is what
         // Inference() returns).  argmax = first maximum (strict '>' from -INT32_MAX, pos 255, inference.c:32-37): in column order
         // per thread, then over the quad.  The last layer has at most kLastN columns.
+        // (row_label below is the same argmax for the two-engine kernel; the epilogue keeps its own copy, whose instruction
+        // schedule in the other kernels a shared lambda would change.)
         auto epilogue = [&](const uint32_t *a, uint32_t i) {
             const uint32_t tile = tile0 + i * tile_step;
 #pragma unroll
@@ -568,7 +582,87 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
         };
 
         RingPos ring;   // ring position of the pipe's next tile
-        if constexpr (kSlots == 1) {
+        if constexpr (kEngines) {
+            // Both engines scale the image alike and multiply it by the same weights (the emulator's level scale cancels, see
+            // emul_coef), so their layer-1 accumulators are the same: layer 1 runs once and feeds both hidden-layer rules, the
+            // emulator's fragments in afr_py.  Then the C chain and the emulator's chain run one after the other from their own
+            // fragments.  A one-layer model has no hidden layer: both labels are the argmax of layer 1.
+            uint32_t afr_py[kN / 8];
+            EngineTally tally;
+            auto row_label = [&](const uint32_t *a, int r) {   // the epilogue's argmax of row r (0: this thread's first row, 1: 8 below)
+                int best = -INT32_MAX;
+                uint32_t pos = 255;
+#pragma unroll
+                for (int j = 0; j < kLastN / 8; j++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const uint32_t col = 8 * j + 2 * quad + e;
+                        const int x = (int)a[4 * j + 2 * r + e];
+                        if (col < ncls && x > best) { best = x; pos = col; }
+                    }
+#pragma unroll
+                for (int sh = 1; sh <= 2; sh <<= 1) {
+                    const int ob = __shfl_xor_sync(0xffffffffu, best, sh);
+                    const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, sh);
+                    if (ob > best || (ob == best && op < pos)) { best = ob; pos = op; }
+                }
+                return pos;
+            };
+#pragma unroll 1
+            for (uint32_t i = 0; i < my_tiles; i++) {
+                const uint32_t s = ring.stage();
+                wait_full(s, ring.phase(), 0);
+                ring.advance(n_st);
+                issue_layer1(acc[0], s);
+                wgmma_commit();
+                wgmma_wait<0>();
+                release_stage(s);
+                uint32_t lab_c[2], lab_py[2];
+                if (n_layers > 1) relunorm_rule(acc[0], afr_py, 0, std::true_type{});
+                for (int l = 0;; l++) {   // the C engine
+                    if (l + 1 < n_layers) {
+                        relunorm_rule(acc[0], afr[0], l, std::false_type{});
+                        issue_layer(acc[0], afr[0], l + 1);
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        continue;
+                    }
+                    lab_c[0] = row_label(acc[0], 0);
+                    lab_c[1] = row_label(acc[0], 1);
+                    break;
+                }
+                lab_py[0] = lab_c[0];
+                lab_py[1] = lab_c[1];
+                for (int l = 1; l < n_layers; l++) {   // the emulator
+                    issue_layer(acc[0], afr_py, l);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    if (l + 1 < n_layers) {
+                        relunorm_rule(acc[0], afr_py, l, std::true_type{});
+                    } else {
+                        lab_py[0] = row_label(acc[0], 0);
+                        lab_py[1] = row_label(acc[0], 1);
+                    }
+                }
+                const size_t img0 = (size_t)(tile0 + i * tile_step) * kTileM + row_in_tile;
+#pragma unroll
+                for (int r = 0; r < 2; r++) {
+                    const size_t img = img0 + 8 * r;
+                    const bool row = quad == 0 && img < P.n;
+                    uint32_t truth = ~0u;
+                    if (row) {
+                        if (P.labels) P.labels[img] = lab_c[r];
+                        if (P.labels_py) P.labels_py[img] = lab_py[r];
+                        if (P.truth) truth = P.truth[img];
+                    }
+                    tally.add(row, lab_c[r], lab_py[r], truth, ncls);
+                }
+            }
+            if (P.counts) {
+                tally.flush(P.counts);
+                if (blockIdx.x == 0 && tid == 0) atomicAdd(&P.counts[0], (unsigned long long)P.n);
+            }
+        } else if constexpr (kSlots == 1) {
             // one tile at a time: every layer's MMAs complete before its ReLUNorm starts.  (The slot loop below would serve one
             // slot as well, but ptxas gives it about 10 to 20 more registers per one-slot instantiation and spills at kN = 256.)
 #pragma unroll 1
@@ -753,6 +847,13 @@ fc_emul_i8_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
     fc_chain_body<kN, 1, false, 1, kN, false, true>(tmap_in, P);
 }
 
+// The reference's check of its two engines (test_inference.py:130-175) in one pass: the float-input launch <64,1,float> that
+// runs the C engine's chain and the emulator's after one shared layer 1, and writes both labels and their counts.
+__global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
+fc_engines_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<64, 1, true, 1, 64, false, false, true>(tmap_in, P);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -796,8 +897,8 @@ static void trace_before(cudaStream_t) {}
 static void trace_after(cudaStream_t) {}
 #endif
 
-// the instantiations of fc_chain_kernel, fc_emul_kernel and fc_emul_i8_kernel, one row each, named by their template arguments
-// <kN, kPipes, kSlots, kLastN>
+// the instantiations of fc_chain_kernel, fc_emul_kernel, fc_emul_i8_kernel and fc_engines_kernel, one row each, named by their
+// template arguments <kN, kPipes, kSlots, kLastN>
 struct ChainKernel {
     const char *name;
     void (*fn)(CUtensorMap, ChainParams);
@@ -813,6 +914,7 @@ enum ChainRow {
     kRow64, kRow64x2, kRow64x2Last16, kRowFixed, kRow128, kRow192, kRow256, kRowFloat,
     kRowEmulFloat,
     kRowEmul64, kRowEmul128, kRowEmul192, kRowEmul256,   // row kRowEmul64 + max_n / 64 - 1
+    kRowEngines,
     kChainRows
 };
 static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
@@ -830,6 +932,7 @@ static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
     t[kRowEmul128] = emul_i8_kernel<128>("<128,1,emul>");
     t[kRowEmul192] = emul_i8_kernel<192>("<192,1,emul>");
     t[kRowEmul256] = emul_i8_kernel<256>("<256,1,emul>");
+    t[kRowEngines] = {"<64,1,float,engines>", fc_engines_kernel, chain_threads<64, 1, true, 1>()};
     return t;
 }();
 
@@ -898,6 +1001,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     if (in_bytes <= 256 && p.n_classes <= 16 && max_n == 64 && w_fixed + fring + 2 * p.stage_bytes <= smem_limit) {
         forms[kFormFloat] = layout(kRowFloat, 1, 4, fring);
         forms[kFormEmulFloat] = layout(kRowEmulFloat, 1, 4, fring);
+        forms[kFormEngines] = layout(kRowEngines, 1, 4, fring);
     }
     // the emulator on int8 rows runs one pipe at every width, so a 64-wide plan, whose int8 form runs two, has its own layout
     forms[kFormEmulInt8] = layout(kRowEmul64 + max_n / 64 - 1, 1, 6, 0);
@@ -984,12 +1088,13 @@ const char *fc_chain_form_name(const FcChainPlan *plan, FcForm f) { return plan-
 static const CUtensorMap kNoTensorMap{};   // the float-input forms' tensor map: not used (no TMA image loads)
 
 int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
-                    const GatherDst *gather, cudaStream_t st) {
+                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
     const FormLayout &form = plan->forms[f];
     if (!form.kernel) return -6;
-    const bool engine_i8 = f == kFormInt8, float_in = f == kFormFloat || f == kFormEmulFloat;
+    if ((f == kFormEngines) != (engines != nullptr) || (engines && logits)) return -5;
+    const bool engine_i8 = f == kFormInt8, float_in = f == kFormFloat || f == kFormEmulFloat || f == kFormEngines;
     ChainParams p = plan->p;   // the model's shapes; null outputs, no result exchange
     p.n_stages = form.n_stages;
     p.off_w = form.off_w;
@@ -1001,6 +1106,11 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void 
         p.logits = static_cast<int32_t *>(logits);
     }
     p.labels = labels;
+    if (engines) {
+        p.labels_py = engines->labels_py;
+        p.truth = engines->truth;
+        p.counts = engines->counts;
+    }
     p.n = n;
     p.n_tiles = (uint32_t)((n + kTileM - 1) / kTileM);
     if (gather) {

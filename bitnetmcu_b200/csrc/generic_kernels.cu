@@ -388,6 +388,27 @@ void launch_i32_to_i8(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t ou
     if (total) k_i32_to_i8<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, n_in, out, out_stride, n);
 }
 
+// bnm_compare_engines_device off the one-pass kernel: the two engines' labels, compared and scored by a grid-stride loop whose
+// warps count with EngineTally, as fc_engines_kernel's epilogue does.  The loop bound is uniform per block: every warp runs
+// every ballot.
+__global__ void __launch_bounds__(256) k_engine_counts(const uint32_t *__restrict__ labels_c, const uint32_t *__restrict__ labels_py,
+                                                        const uint32_t *__restrict__ truth, size_t n, uint32_t n_classes,
+                                                        unsigned long long *counts) {
+    EngineTally tally;
+    for (size_t base = (size_t)blockIdx.x * blockDim.x; base < n; base += (size_t)gridDim.x * blockDim.x) {
+        const size_t i = base + threadIdx.x;
+        const bool row = i < n;
+        tally.add(row, row ? labels_c[i] : 0u, row ? labels_py[i] : 0u, row && truth ? truth[i] : ~0u, n_classes);
+    }
+    tally.flush(counts);
+    if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counts[0], (unsigned long long)n);
+}
+
+void launch_engine_counts(const uint32_t *labels_c, const uint32_t *labels_py, const uint32_t *truth, size_t n, uint32_t n_classes,
+                          unsigned long long *counts, cudaStream_t st) {
+    if (n) k_engine_counts<<<(unsigned)std::min<size_t>((n + 255) / 256, 1024), 256, 0, st>>>(labels_c, labels_py, truth, n, n_classes, counts);
+}
+
 // ------------------------------------------------------------------------------------------------
 // The emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) as one kernel, step for step the layered route of emulate_device
 // (capi.cu): input scaling; conv1 (1 -> C), ReLU, renormalisation over the image's C*196 outputs; depthwise conv2, ReLU,

@@ -79,6 +79,29 @@ void launch_emul_logits(const int32_t *acc, uint32_t n_cls, int level_shift, dou
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 
+// ---- scoring both engines (bnm_compare_engines_device): counts = uint64 {images, correct_c, correct_py, mismatches}, the layout of
+// bnm_engine_counts.  A warp's counters: every lane of the warp calls add() with the row it holds (row = false: none); the flags
+// are counted by ballot, kept in registers across the warp's rows, and flush() adds them with one 64-bit atomic per non-zero
+// counter.  A truth value of n_classes or more never matches (no truth: pass ~0u).
+struct EngineTally {
+    uint32_t correct_c = 0, correct_py = 0, mismatches = 0;
+    __device__ __forceinline__ void add(bool row, uint32_t label_c, uint32_t label_py, uint32_t truth, uint32_t n_classes) {
+        const bool known = row && truth < n_classes;
+        correct_c += __popc(__ballot_sync(0xffffffffu, known && label_c == truth));
+        correct_py += __popc(__ballot_sync(0xffffffffu, known && label_py == truth));
+        mismatches += __popc(__ballot_sync(0xffffffffu, row && label_c != label_py));
+    }
+    __device__ __forceinline__ void flush(unsigned long long *counts) const {
+        if ((threadIdx.x & 31) != 0) return;
+        if (correct_c) atomicAdd(&counts[1], (unsigned long long)correct_c);
+        if (correct_py) atomicAdd(&counts[2], (unsigned long long)correct_py);
+        if (mismatches) atomicAdd(&counts[3], (unsigned long long)mismatches);
+    }
+};
+// the two engines' labels [n] (and truth [n] or null) -> counts += their tallies and images += n
+void launch_engine_counts(const uint32_t *labels_c, const uint32_t *labels_py, const uint32_t *truth, size_t n, uint32_t n_classes,
+                          unsigned long long *counts, cudaStream_t st);
+
 // ---- fused wgmma FC chain (fc_wgmma.cu)
 struct FcChainPlan;  // opaque, owned by the model
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
@@ -93,16 +116,26 @@ void fc_chain_plan_set_overlap(FcChainPlan *p, int mode);
 //                   into the kernel's load stage: FC rows of up to 256 elements, models up to 64 wide with up to 16 classes
 //   kFormEmulFloat  the reference's Python emulator in place of the C engine (fc_emul_kernel): the plans with kFormFloat
 //   kFormEmulInt8   the emulator on int8 rows [n][in_bytes] that are already scaled (fc_emul_i8_kernel), every plan
+//   kFormEngines    both engines on float32 images (fc_engines_kernel): one input scaling and one layer 1, then the C engine's
+//                   and the emulator's hidden layers; both labels and the EngineTally counts, no logits.  The plans with kFormFloat
 // The emulator forms have the emulator's hidden-layer rule and float64 logits = last layer's accumulators x 2^-level_shift (0 or 1).
-enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFcForms };
+enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFormEngines, kFcForms };
 bool fc_chain_has_form(const FcChainPlan *p, FcForm f);
 // the template arguments of the kernel of a form the plan has, e.g. "<192,1,emul>"
 const char *fc_chain_form_name(const FcChainPlan *p, FcForm f);
+// kFormEngines outputs besides `labels` (the C engine's): the emulator's labels uint32 [n], truth uint32 [n] and counts (each may be
+// null; truth only with counts)
+struct EngineOutputs {
+    uint32_t *labels_py;
+    const uint32_t *truth;
+    unsigned long long *counts;
+};
 // one launch of form f on n images `in` -> logits (int32 [n][n_classes], float64 for the emulator forms) and labels uint32 [n];
 // each may be null.  gather (kFormInt8 only, may be null): extra destination buffers every row is also stored to (peer memory),
-// fused into the epilogue.  0, or a negative code (-6: the plan has no form f)
+// fused into the epilogue.  engines: kFormEngines only, and required there (no logits).  0, or a negative code (-6: the plan
+// has no form f)
 int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
-                    const GatherDst *gather, cudaStream_t st);
+                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines = nullptr);
 // the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
 // [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
 constexpr uint32_t kCnnEmulMaxChannels = 128;

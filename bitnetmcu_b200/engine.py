@@ -158,6 +158,26 @@ class Engine:
         _lib.check(self.lib.bnm_infer_batch_device_f32(self.handle, C.c_void_p(images.data_ptr()), n, self._logits_ptr(logits, n),
                                                        self._labels_ptr(labels, n), C.c_void_p(stream)), "bnm_infer_batch_device_f32")
 
+    def compare_engines_device(self, images, truth=None, labels_c=None, labels_py=None, counts=None, stream: Optional[int] = None) -> None:
+        """Both engines on the same float images in one call (test_inference.py:130-175): images torch.float32 [n, img_bytes] on
+        this GPU -> labels_c [n] (what ``infer_device_f32`` returns), labels_py [n] (what ``inference_quantized_device`` returns)
+        and counts, a torch.int64 [4] tensor (images, correct_c, correct_py, mismatches) that the call ADDS to.  truth: [n] true
+        classes (4-byte elements), counted into correct_c / correct_py, and only with counts.  Any of labels_c, labels_py and
+        counts may be None, not all three.  Asynchronous on ``stream`` (default: torch's current stream).  FC models up to 64
+        wide: one kernel."""
+        import torch
+        n = images.shape[0]
+        if stream is None:
+            stream = torch.cuda.current_stream(images.device).cuda_stream
+        assert images.is_contiguous() and images.dtype == torch.float32 and images.shape[1] == self.img_bytes
+        cp = None
+        if counts is not None:
+            assert counts.is_contiguous() and counts.dtype == torch.int64 and tuple(counts.shape) == (4,)
+            cp = C.c_void_p(counts.data_ptr())
+        _lib.check(self.lib.bnm_compare_engines_device(self.handle, C.c_void_p(images.data_ptr()), n, self._labels_ptr(truth, n),
+                                                       self._labels_ptr(labels_c, n), self._labels_ptr(labels_py, n), cp,
+                                                       C.c_void_p(stream)), "bnm_compare_engines_device")
+
     def infer_tensor(self, images, want_logits: bool = True):
         """images: torch.int8 [n, img_bytes] on this engine's GPU -> (logits torch.int32 [n, n_classes], labels torch.int32 [n]) on
         the same GPU, asynchronous on torch's current stream (device memory end to end; plumbing for ``dist.sharded_infer``).

@@ -15,6 +15,7 @@
  * Section 3 is the batched entry the reference lacks (its caller loops lib.Inference() per image,
  *   /root/reference/test_inference.py:136-150): millions of 16x16 int8 images per call.
  * Section 4 exposes the four kernels batched, for parity tests and partial integration.
+ * Sections 5 to 7 take float images: the C engine (5), the reference's Python emulator (6), and both at once, scored (7).
  *
  * Pointers are plain host (or, where the name says _device, CUDA device) pointers; sizes are element
  * counts unless named *_bytes.  All-integer arithmetic: results are bit-exact with the reference.
@@ -228,6 +229,34 @@ BNM_API int bnm_emulate_inference_quantized(bnm_model *m, const float *images, s
  * the first large call, then reused): calls on one model must then not overlap in time on different streams.  Either way the
  * call makes no host synchronisation once its scratch has grown. */
 BNM_API int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 7. Both engines in one call: the reference's verification loop (test_inference.py:130-175) scores every
+ *    image with the C engine (lib.Inference()) and with the Python emulator (np.argmax(inference_quantized(x))) on the same
+ *    scaled input, then reports both accuracies and the number of images on which the engines disagree.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct bnm_engine_counts {
+    uint64_t images;      /* images scored                                   */
+    uint64_t correct_c;   /* C-engine label == truth                         */
+    uint64_t correct_py;  /* emulator label == truth                         */
+    uint64_t mismatches;  /* C-engine label != emulator label                */
+} bnm_engine_counts;
+/* images float32 [n][img_bytes], device memory, 16-byte aligned.  labels_c uint32 [n] = what bnm_infer_batch_device_f32 returns,
+ * labels_py uint32 [n] = what bnm_emulate_batch_device returns (np.argmax of the emulator's logits, first maximum), both device
+ * memory.  counts is device memory (8-byte aligned) and the call ADDS to it, it never overwrites: zero it once, then score a data
+ * set in several calls (or per rank).  Every call adds n to images and #(label_c != label_py) to mismatches; with truth (uint32
+ * [n], device memory) also #(label_c == truth) to correct_c and #(label_py == truth) to correct_py.  A truth value of n_classes or
+ * more never matches.  labels_c, labels_py and counts may each be NULL, not all three (BNM_E_ARG); truth without counts is
+ * BNM_E_ARG.  n == 0 returns 0 and leaves counts unchanged.  There are no logits: bnm_infer_batch_device_f32 and
+ * bnm_emulate_batch_device serve them.
+ * On the fused path, FC models with image rows of <= 256 elements, <= 16 classes and <= 64 wide (the one-kernel models of both
+ * entries) run ONE kernel: each float image is read and scaled once, layer 1 runs once (both engines' layer-1 accumulators are
+ * the same), then the C engine's and the emulator's hidden layers run from it, and the epilogue writes both labels and counts
+ * warp by warp.  Every other model runs the two entries' routes in chunks of 2^20 images, then a counting kernel.  Asynchronous
+ * on `stream`, no host synchronisation once the model's scratch has grown; like the emulator's routes, calls on one model must
+ * not overlap in time on different streams. */
+BNM_API int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth,
+                                       uint32_t *labels_c, uint32_t *labels_py, bnm_engine_counts *counts, void *stream);
 
 #ifdef __cplusplus
 }
