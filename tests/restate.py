@@ -1,0 +1,175 @@
+"""NumPy restatements the tests compare the GPU against, one copy of each: the reference caller's input scaling, the reference
+Python emulator's FC and CNN paths, and the fused FC kernels' tile schedule.  Pure NumPy: no torch, no CUDA library."""
+from typing import NamedTuple
+
+import numpy as np
+
+from bitnetmcu_b200 import model as M, pack as P
+
+LEVEL_SHIFT = {2: 1, 4: 1}          # 2bitsym / 4bitsym levels are half the engine's integer weights (BitNetMCU.py:155-164)
+TILE = 128                          # images per tile (kTileM)
+
+
+# ---- the emulator ---------------------------------------------------------------------------------------------------------
+
+def scale_images(x):
+    """float32 images -> int8, test_inference.py:140-141 and BitNetMCU.py:435-436 in float32:
+    round_half_even(x * 127 / max(max|x|, 1e-5)).clip(-128, 127)"""
+    x = np.asarray(x, dtype=np.float32)
+    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
+    return np.round(x * scale).clip(-128, 127).astype(np.int8)
+
+
+def bitlinear(model, act):
+    """the BitLinear layers (BitNetMCU.py:452-457, 527-530) on activations [n, k] -> float64 logits: per layer a float64
+    product with the weight levels, a power-of-two rescale of every row to a maximum of at most 127 with round-half-even and
+    ReLU, and no rescale after the last layer"""
+    fc = [l for l in model.layers if l.kind == M.LAYER_FC]
+    act = act.astype(np.float64)
+    for i, l in enumerate(fc):
+        # weight levels over the columns the previous layer delivers (Ternary pads n_in with zero trits)
+        w = P.decode_int_weights(l).astype(np.float64)[:, :act.shape[1]] / 2.0 ** LEVEL_SHIFT.get(l.bitperweight, 0)
+        conv = act @ w.T
+        if i + 1 == len(fc):
+            return conv
+        top = np.maximum(conv.max(axis=-1, keepdims=True), 1e-5)
+        act = np.round(conv * np.exp2(np.floor(np.log2(127.0 / top)))).clip(0, 127)
+
+
+def emulate_fc(model, x):
+    """float32 images [n, img_bytes] of an FC model -> the emulator's float64 logits [n, n_classes]"""
+    return bitlinear(model, scale_images(x))
+
+
+def _conv_relu(a, w):
+    """depthwise 3x3 (k_conv33relu's indices, no shift) + ReLU: a int64 [n, 1 or C, H, W], w int8 [C * 9] -> [n, C, H-2, W-2]"""
+    n, _, h, wd = a.shape
+    k = w.reshape(-1, 3, 3).astype(np.int64)
+    out = np.zeros((n, k.shape[0], h - 2, wd - 2), dtype=np.int64)
+    for dr in range(3):
+        for dc in range(3):
+            out += k[None, :, dr, dc, None, None] * a[:, :, dr:dr + h - 2, dc:dc + wd - 2]
+    return np.maximum(out, 0)
+
+
+def _renorm(v):
+    """BitConv2d's renormalisation over each image's C*H*W outputs (float64); an all-zero image stays zero"""
+    m = v.reshape(v.shape[0], -1).max(axis=1)
+    scale = np.where(m > 0, 127.0 / np.maximum(m, 1), 0.0)[:, None, None, None]
+    return np.round(v * scale).clip(0, 127).astype(np.int64)
+
+
+def _pool(v):
+    n, c, h, w = v.shape
+    return v.reshape(n, c, h // 2, 2, w // 2, 2).max(axis=(3, 5))
+
+
+def cnn_features(model, x):
+    """float32 images [n, 256] -> int64 features [n, C*4], the (C, 2, 2) flatten"""
+    w1, w2, w3 = [l.weights for l in model.layers if l.kind == M.LAYER_CONV33]
+    a = scale_images(x).astype(np.int64).reshape(-1, 1, 16, 16)
+    a = _renorm(_conv_relu(a, w1))
+    a = _pool(_renorm(_conv_relu(a, w2)))
+    a = _pool(_renorm(_conv_relu(a, w3)))
+    return a.reshape(a.shape[0], -1)
+
+
+def emulate(model, x, block=512):
+    """float32 images -> the emulator's float64 logits, FC and CNN models"""
+    if model.model_class == 0:
+        return emulate_fc(model, x)
+    return np.concatenate([bitlinear(model, cnn_features(model, x[i:i + block])) for i in range(0, len(x), block)])
+
+
+# ---- the fused FC kernels' tile schedule (tests/test_fc_ring_rounds.py) -----------------------------------------------------
+
+class Schedule(NamedTuple):
+    """One launch of n images; the per-tile arrays are indexed by global tile."""
+    n: int
+    grid: int
+    cta: np.ndarray
+    local: np.ndarray       # index among the CTA's tiles
+    pipe: np.ndarray
+    slot: np.ndarray        # 0 = slot A, 1 = slot B
+    stage: np.ndarray       # stage inside the pipe
+    phase: np.ndarray
+    round: np.ndarray
+    ragged: int             # the tile that holds fewer than 128 images, -1 when n is a multiple of 128
+    per_pipe: np.ndarray    # [grid, pipes]: tiles of each CTA's pipe
+    end_slot: np.ndarray    # [grid, pipes]: slot of the last of them (-1: the pipe has no tile)
+
+
+def tile_schedule(n, sm, pipes, stages, slots):
+    n_tiles = -(-n // TILE)
+    grid = min(n_tiles, sm)
+    t = np.arange(n_tiles)
+    cta, local = t % grid, t // grid
+    pipe, j = local % pipes, local // pipes
+    rnd = j // stages
+    per_pipe = np.zeros((grid, pipes), dtype=np.int64)
+    np.add.at(per_pipe, (cta, pipe), 1)
+    end_slot = np.where(per_pipe > 0, (per_pipe - 1) % slots, -1)
+    return Schedule(n, grid, cta, local, pipe, j % slots, j % stages, rnd & 1, rnd, n_tiles - 1 if n % TILE else -1,
+                    per_pipe, end_slot)
+
+
+def top_tiles(pipes, stages, slots):
+    """tiles per CTA that take every stage of every pipe (and so every slot that meets it) through rounds 0, 1 and 2: each phase
+    parity of every stage is waited on at least twice, counting the full and the empty barrier.  That is at least
+    pipes (2 stages + 1) + pipes slots whenever a pipe of two slots has three or more stages."""
+    return 3 * stages * pipes
+
+
+def batch_size(sm, t, r, tail):
+    """n for (t - 1) sm + r tiles, the last of them holding `tail` images (0: a full tile).  With r <= sm that last tile is
+    local tile t - 1 of CTA r - 1."""
+    return ((t - 1) * sm + r) * TILE - ((TILE - tail) if tail else 0)
+
+
+def ring_sweep(sm, pipes, stages, slots):
+    """ascending batch sizes that, launched one after the other, cover the ring: see sweep_gaps"""
+    launches = [(1, max(1, sm // 2), 1),        # fewer tiles than SMs, one per CTA; n % 128 = 1
+                (2, max(1, sm // 3), 127)]      # CTAs from r on hold one tile, the others two; n % 128 = 127
+    k, ends = 0, pipes * slots
+    for p in range(pipes):
+        for x in range(slots):
+            j = stages + (x - stages) % slots   # the first place of round 1 that slot x takes
+            launches.append((j * pipes + p + 1, 1 + (sm - 1) * (k + 1) // (ends + 1), 40 + 23 * k))   # ragged last tile there
+            k += 1
+    launches.append((top_tiles(pipes, stages, slots), sm // 2 + 1, 0))   # rounds 0 to 2 everywhere; n % 128 = 0
+    return sorted({batch_size(sm, t, min(r, sm), tail) for t, r, tail in launches})
+
+
+def sweep_gaps(sizes, sm, pipes, stages, slots):
+    """what a sweep of launches leaves uncovered (empty: nothing):
+      * every (pipe, slot, stage) the schedule puts in rounds 0, 1 and 2;
+      * the ragged last tile on every (pipe, slot), in an odd round;
+      * a CTA with one tile, and a launch with fewer tiles than SMs;
+      * a CTA's pipe with an odd tile count (slot B idles at the end) and one with an even count (slot A idles);
+      * n % 128 in {0, 1, 127}."""
+    want = {(p, j % slots, j % stages, j // stages) for p in range(pipes) for j in range(3 * stages)}
+    want_ragged = {(p, x) for p in range(pipes) for x in range(slots)}
+    seen, ragged, misc = set(), set(), set()
+    for n in sizes:
+        s = tile_schedule(n, sm, pipes, stages, slots)
+        seen |= set(zip(s.pipe.tolist(), s.slot.tolist(), s.stage.tolist(), s.round.tolist()))
+        if s.ragged >= 0 and s.round[s.ragged] % 2:
+            ragged.add((int(s.pipe[s.ragged]), int(s.slot[s.ragged])))
+        if (s.per_pipe.sum(axis=1) == 1).any():
+            misc.add("a CTA with one tile")
+        if s.grid < sm:
+            misc.add("fewer tiles than SMs")
+        if ((s.per_pipe % 2 == 1) & (s.end_slot == 0)).any():
+            misc.add("odd per-pipe count")
+        if ((s.per_pipe % 2 == 0) & (s.per_pipe > 0) & (s.end_slot == slots - 1)).any():
+            misc.add("even per-pipe count")
+        misc.add(f"n % 128 = {n % TILE}")
+    gaps = [f"round position {w}" for w in sorted(want - seen)]
+    gaps += [f"ragged last tile on (pipe, slot) {w} in an odd round" for w in sorted(want_ragged - ragged)]
+    gaps += [m for m in ("a CTA with one tile", "fewer tiles than SMs", "odd per-pipe count", "even per-pipe count",
+                         "n % 128 = 0", "n % 128 = 1", "n % 128 = 127") if m not in misc]
+    return gaps
+
+
+def most_tiles_per_cta(sizes, sm, pipes, stages, slots):
+    return max(int(tile_schedule(n, sm, pipes, stages, slots).local.max()) + 1 for n in sizes)

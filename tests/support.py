@@ -1,0 +1,256 @@
+"""Plumbing more than one test module uses: the library fixture, engine factories, the BNM_VERBOSE lines, the library's SASS
+dumped once, the ring sweep on this GPU, and the models, inputs and device calls that several modules feed.
+
+Test modules import the fixture by name (`from support import lib`): pytest finds fixtures in a module's globals."""
+import functools
+import os
+import re
+import subprocess
+
+import numpy as np
+import pytest
+
+from conftest import GOLDEN, ROOT, load_model
+from restate import TILE, most_tiles_per_cta, ring_sweep, sweep_gaps, tile_schedule
+
+N_MANY = 148 * 128 * 2 + 77          # several tiles per CTA, a ragged last tile
+
+
+@pytest.fixture(scope="module")
+def lib(built):
+    from bitnetmcu_b200 import _lib
+    l = _lib.load()
+    assert l.bnm_device_count() > 0, "no CUDA device"
+    return l
+
+
+# ---- engines ---------------------------------------------------------------------------------------------------------------
+
+def engine(model, path=0, cnn_frontend=None):
+    from bitnetmcu_b200 import _lib
+    from bitnetmcu_b200.engine import Engine
+    e = Engine(model, device=0, path=path)
+    if cnn_frontend is not None:
+        e.set_option(_lib.OPT_CNN_FRONTEND, cnn_frontend)
+    return e
+
+
+def frontends(model):
+    """CNN models run once per front-end kernel (BNM_OPT_CNN_FRONTEND): CUDA cores and conv1-on-wgmma; FC models once."""
+    from bitnetmcu_b200 import _lib
+    if model.model_class != 1:
+        return [None]
+    return [_lib.CNN_CUDA_CORES, _lib.CNN_TENSOR_CORES] if model.channels % 16 == 0 else [_lib.CNN_CUDA_CORES]
+
+
+def verbose_engine(capfd, monkeypatch, make):
+    """the engine make() builds with BNM_VERBOSE set, and the lines it printed to stderr"""
+    monkeypatch.setenv("BNM_VERBOSE", "1")
+    capfd.readouterr()
+    e = make()
+    err = capfd.readouterr().err.splitlines()
+    monkeypatch.delenv("BNM_VERBOSE")
+    return e, err
+
+
+def plan_line(err):
+    """the last `fused FC plan` line, None when there is none"""
+    plan = [l for l in err if "fused FC plan" in l]
+    return plan[-1] if plan else None
+
+
+def route(err, what):
+    """the route of the one `<what> route:` line ("emulator" or "engines")"""
+    lines = [l for l in err if f"{what} route: " in l]
+    assert len(lines) == 1, lines
+    return lines[0].split(f"{what} route: ")[1]
+
+
+# ---- the library's SASS -----------------------------------------------------------------------------------------------------
+
+@functools.lru_cache(maxsize=None)
+def sass():
+    """the SASS of the whole library, dumped once per session; take the `built` fixture before the first call"""
+    from bitnetmcu_b200 import _lib
+    return subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+
+
+@functools.lru_cache(maxsize=None)
+def sass_functions():
+    """{mangled name: SASS text} of every function in the library"""
+    return {k.split()[0]: k for k in re.split(r"\n\s*Function : ", sass())[1:]}
+
+
+def instructions(text):
+    return [i.strip() for i in re.findall(r"/\*[0-9a-f]{4,}\*/\s+([^;]*);", text)]
+
+
+def local_memory(ins):
+    """the instructions that load or store local memory"""
+    return [i for i in ins if re.match(r"(@\S+\s+)?(LDL|STL)\b", i)]
+
+
+# ---- the ring sweep on this GPU ---------------------------------------------------------------------------------------------
+
+class Sweep:
+    """the sweep of one case on this GPU, and the tag every assertion message of the case carries"""
+
+    def __init__(self, row, ring):
+        import torch
+        self.ring = ring
+        self.sm = torch.cuda.get_device_properties(0).multi_processor_count
+        self.sizes = ring_sweep(self.sm, *ring)
+        self.top = most_tiles_per_cta(self.sizes, self.sm, *ring)
+        self.tag = "%s: %d pipes x %d stages, %d slots, %d SMs, up to %d tiles per CTA" % ((row,) + ring + (self.sm, self.top))
+        print(self.tag, "batch sizes", self.sizes)
+        assert self.top >= ring[0] * (2 * ring[1] + 1), self.tag
+        assert not sweep_gaps(self.sizes, self.sm, *ring), self.tag
+
+    def where(self, n, rows):
+        """(tile, CTA, local index, pipe, slot, stage, round) of the tiles that hold the given rows of launch n"""
+        s = tile_schedule(n, self.sm, *self.ring)
+        return [(int(t), int(s.cta[t]), int(s.local[t]), int(s.pipe[t]), "AB"[s.slot[t]], int(s.stage[t]), int(s.round[t]))
+                for t in np.unique(np.asarray(rows) // TILE)[:6]]
+
+    def check(self, n, got, want, sentinel, what):
+        """rows :n of the (n + 128)-row device buffer `got` equal `want`; rows n: still hold the sentinel"""
+        g = got.cpu().numpy()
+        if what == "labels":
+            g = g.astype(np.uint32) if want.dtype == np.uint32 else g.astype(np.int64)
+        bad = np.flatnonzero((g[:n] != want[:n]).reshape(n, -1).any(axis=1))
+        assert bad.size == 0, (self.tag, n, what, f"{bad.size} rows wrong, first {bad[:4].tolist()}",
+                               "(tile, cta, local, pipe, slot, stage, round):", self.where(n, bad))
+        assert (got[n:].cpu().numpy() == sentinel).all(), (self.tag, n, what, "written past row n")
+
+
+# ---- models ------------------------------------------------------------------------------------------------------------------
+
+def random_fc(enc, widths, seed):
+    """a random FC model whose images are widths[0] bytes"""
+    from bitnetmcu_b200 import pack as P
+    m = P.random_fc_model(enc, widths, seed=seed)
+    m.img_bytes = widths[0]
+    return m
+
+
+# every row of kChainKernels (fc_wgmma.cu), with a model that selects it (checked against the plan's BNM_VERBOSE line)
+CHAIN_ROWS = [
+    ("<64,1>", lambda: random_fc(4, (512, 64, 64, 10), 1)),           # 512-byte rows: room for three 64 kB stages, one pipe
+    ("<64,2,2,64>", lambda: random_fc(4, (256, 64, 64, 37), 2)),      # 37 classes: the last layer is wider than 16
+    ("<64,2,2,16>", lambda: load_model("1k")),                        # 16-wide layers, three of them: not the fixed class
+    ("<64,2,2,16,fixed>", lambda: load_model("fc")),
+    ("<128,1>", lambda: load_model("2bitsym96")),
+    ("<192,1>", lambda: load_model("binary160")),
+    ("<256,1>", lambda: random_fc(4, (256, 256, 10), 3)),
+]
+
+
+def cnn_model(channels, n_classes, seed, w=(None, None, None)):
+    """a random CNN model: conv weights uniform in [-128, 127] with +-127 taps in every layer (or the given weights), a 64-wide
+    4bitsym hidden layer and an n_classes head"""
+    from bitnetmcu_b200 import model as M, pack as P
+    rng = np.random.default_rng(seed)
+
+    def conv_w(i):
+        if w[i] is not None:
+            return np.asarray(w[i], dtype=np.int8).reshape(channels * 9)
+        k = rng.integers(-128, 128, size=channels * 9).astype(np.int8)
+        k[rng.integers(0, channels * 9, size=max(2, channels))] = 127
+        k[rng.integers(0, channels * 9, size=max(2, channels))] = -127
+        return k
+    layers = [M.Layer(kind=M.LAYER_CONV33, name="L2", bitperweight=8, n_in=16, n_out=channels, in_channels=1, groups=1, weights=conv_w(0)),
+              M.Layer(kind=M.LAYER_CONV33, name="L4", bitperweight=8, n_in=14, n_out=channels, in_channels=channels, groups=channels,
+                      weights=conv_w(1)),
+              M.Layer(kind=M.LAYER_MAXPOOL22, name="L6", n_in=12, n_out=6),
+              M.Layer(kind=M.LAYER_CONV33, name="L7", bitperweight=8, n_in=6, n_out=channels, in_channels=channels, groups=channels,
+                      weights=conv_w(2)),
+              M.Layer(kind=M.LAYER_MAXPOOL22, name="L9", n_in=4, n_out=2)]
+    fc = P.random_fc_model(M.ENC_4BITSYM, (channels * 4, 64, n_classes), seed=seed)
+    for i, l in enumerate(fc.layers):
+        l.name = f"L{11 + 2 * i}"
+        layers.append(l)
+    m = M.Model(model_class=M.MODEL_CNNMNIST, layers=layers)
+    m.validate()
+    return m
+
+
+# ---- inputs -------------------------------------------------------------------------------------------------------------------
+
+def normal_images(n, seed, elems=256):
+    """normal float32 rows, the first 40 of them MNIST-normalised"""
+    rng = np.random.default_rng(seed)
+    x = rng.normal(size=(n, elems)).astype(np.float32)
+    k = min(n, 40)
+    x[:k] = (rng.integers(0, 256, size=(k, elems)) / 255.0 - 0.1307).astype(np.float32) / np.float32(0.3081)
+    return x
+
+
+def scattered_edge_images(n, elems, seed):
+    """normal rows with, scattered through the whole batch, MNIST-normalised rows and rows at the edges of the input scaling:
+    all zero (the 1e-5 floor), exact .5 ties after scaling, one huge pixel, constant negative rows"""
+    rng = np.random.default_rng(seed)
+    x = rng.standard_normal(size=(n, elems), dtype=np.float32)
+    kind = rng.integers(0, 10, size=n)
+    mn = np.flatnonzero(kind >= 6)
+    x[mn] = (rng.integers(0, 256, size=(mn.size, elems)) / 255.0 - 0.1307).astype(np.float32) / np.float32(0.3081)
+    x[kind == 0] = 0.0
+    x[kind == 1] = np.float32(0.5) / np.float32(127.0) * np.arange(elems, dtype=np.float32)
+    x[kind == 2, 0] = np.float32(3e38)
+    x[kind == 3] = -1.0
+    return x
+
+
+def crafted_cnn_case():
+    """images: all zero, and one negative pixel among zeros, then normal rows; models: a random CNN and two whose conv2 or
+    conv3 taps are all <= 0 (no positive output on non-negative inputs).  -> (images, [(model, what)])"""
+    x = normal_images(700, seed=5)
+    x[:110] = 0.0
+    x[100:110, 7] = np.float32(-3.0)
+    rng = np.random.default_rng(3)
+    neg = -rng.integers(0, 129, size=48 * 9)
+    return x, [(cnn_model(48, 10, seed=4, w=w), what)
+               for w, what in (((None, None, None), "random"), ((None, neg, None), "conv2 <= 0"), ((None, None, neg), "conv3 <= 0"))]
+
+
+# ---- device calls -------------------------------------------------------------------------------------------------------------
+
+def run_emulator(e, x, want_logits=True, want_labels=True, stream=None):
+    """the emulator's device entry -> (logits, labels) as NumPy, None for what was not asked for; x NumPy or a CUDA tensor"""
+    import torch
+    d_x = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).cuda()
+    n = d_x.shape[0]
+    lo = torch.full((n, e.n_classes), np.nan, dtype=torch.float64, device="cuda") if want_logits else None
+    la = torch.full((n,), -1, dtype=torch.int32, device="cuda") if want_labels else None
+    e.inference_quantized_device(d_x, lo, la, stream=stream)
+    torch.cuda.synchronize()
+    return (lo.cpu().numpy() if want_logits else None), (la.cpu().numpy().astype(np.int64) if want_labels else None)
+
+
+# ---- the plain-C host side ----------------------------------------------------------------------------------------------------
+
+def _write_test_data_header(path, images, labels):
+    with open(path, "w") as f:
+        for i in range(images.shape[0]):
+            f.write(f"int8_t input_data_{i}[256] = {{" + ", ".join(str(int(v)) for v in images[i]) + "};\n")
+            f.write(f"uint8_t label_{i} = {int(labels[i])};\n")
+
+
+def build_c_shim(tmp, name):
+    """gcc-build host/'s DLL shim and MNIST test program for a fixture model in tmp -> (dll, exe, digits.npz)"""
+    from bitnetmcu_b200 import _lib
+    from bitnetmcu_b200.pack import write_header
+    m = load_model(name)
+    # Model.load names the layers as the reference's dll.c expects: FC L1..L4 / CNN L2..L15 (dll.c:48-121)
+    want = ["L2", "L4", "L6", "L7", "L9", "L11", "L13", "L15"] if m.model_class == 1 else ["L1", "L2", "L3", "L4"]
+    assert [l.name for l in m.layers] == want[:len(m.layers)]
+    write_header(m, os.path.join(tmp, "BitNetMCU_model.h"))
+    d = np.load(os.path.join(GOLDEN, "digits.npz"))
+    _write_test_data_header(os.path.join(tmp, "BitNetMCU_MNIST_test_data.h"), d["images"], d["labels"])
+    libdir = os.path.dirname(_lib.LIB_PATH)
+    common = ["-I" + tmp, "-I" + os.path.join(ROOT, "include"), "-L" + libdir, "-lbitnetmcu_b200", "-Wl,-rpath," + libdir]
+    dll = os.path.join(tmp, "Bitnet_inf.dll")
+    exe = os.path.join(tmp, "mnist_test")
+    subprocess.run(["gcc", "-fPIC", "-shared", "-D_DLL", "-o", dll, os.path.join(ROOT, "host", "bitnetmcu_b200_dll.c")] + common, check=True)
+    subprocess.run(["gcc", "-o", exe, os.path.join(ROOT, "host", "bitnetmcu_b200_test.c"), os.path.join(ROOT, "host", "bitnetmcu_b200_dll.c")] + common,
+                   check=True)
+    return dll, exe, d

@@ -8,6 +8,8 @@ import struct
 import numpy as np
 import pytest
 
+from restate import scale_images
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
 
@@ -52,8 +54,7 @@ def test_idx_and_npz_loaders(tmp_path):
 def test_scaling_recipe_matches_reference_expression():
     """The CPU-side statement of test_inference.py:140-141 used as the expectation in the GPU test."""
     x, _, digits = _float_set(3)
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    q = np.round(x * scale).clip(-128, 127).astype(np.int8)
+    q = scale_images(x)
     # every shipped test digit has a +127 pixel, so the recipe returns the digit itself
     assert np.array_equal(q, digits)
 

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from conftest import ROOT, load_model
+from support import sass
 
 
 def _declared():
@@ -33,11 +34,10 @@ def test_library_exports_every_declared_symbol(built):
 
 def test_library_contains_hopper_sass(built):
     """wgmma s8 / TMA / bulk copies show up as IGMMA / UTMALDG / UBLKCP in the sm_90a SASS."""
-    from bitnetmcu_b200 import _lib
-    sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    assert "sm_90a" in sass
+    text = sass()
+    assert "sm_90a" in text
     for mnemonic in ("IGMMA", "WARPGROUP.ARRIVE", "UTMALDG", "UBLKCP", "VIADDMNMX", "VIMNMX3", "IDP.4A"):
-        assert mnemonic in sass, mnemonic
+        assert mnemonic in text, mnemonic
 
 
 def test_no_cpu_fallback_without_gpu(built):

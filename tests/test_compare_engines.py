@@ -8,15 +8,15 @@ scaled images for the C engine, the NumPy restatement of the emulator for the ot
 import ctypes as C
 import os
 import re
-import subprocess
 import zlib
 
 import numpy as np
 import pytest
 
 from conftest import GOLDEN, load_model
-from test_emulator_routes import _images, _scale, cnn_features, cnn_model, emulate
-from test_fc_ring_rounds import TILE, _float_images, _Sweep
+from restate import TILE, cnn_features, emulate, scale_images
+from support import N_MANY, Sweep, crafted_cnn_case, cnn_model, engine, instructions, lib, local_memory, normal_images, \
+    plan_line, route, sass_functions, scattered_edge_images, verbose_engine
 
 GOLDEN_NAMES = ["fc", "1k", "12k_FP130", "8bit64", "ternary64", "binary160", "2bitsym96", "cnn", "cnn_48", "cnn_16small"]
 FUSED = {"fc", "1k", "12k_FP130", "8bit64", "ternary64"}          # the float-input row's models
@@ -39,16 +39,14 @@ def expected_counts(lc, lp, truth=None, n_classes=10):
 
 def test_engines_kernels_sass(built):
     """exactly one fc_engines_kernel (IGMMA, no local memory) and k_engine_counts (no local memory)"""
-    from bitnetmcu_b200 import _lib
-    out = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    kernels = {k.split()[0]: k for k in re.split(r"\n\s*Function : ", out)[1:]}
+    kernels = sass_functions()
     fused = [k for k in kernels if k.startswith("_ZN3bnm17fc_engines_kernel")]
     counts = [k for k in kernels if k.startswith("_ZN3bnm15k_engine_counts")]
     assert len(fused) == 1 and len(counts) == 1, (fused, counts)
     for k in fused + counts:
-        ins = [i.strip() for i in re.findall(r"/\*[0-9a-f]{4,}\*/\s+([^;]*);", kernels[k])]
+        ins = instructions(kernels[k])
         assert len(ins) > 20, k
-        assert not [i for i in ins if re.match(r"(@\S+\s+)?(LDL|STL)\b", i)], f"local memory in {k}"
+        assert not local_memory(ins), f"local memory in {k}"
         assert (k in fused) == any(i.startswith("IGMMA") for i in ins), k
     assert "VOTE.ANY" in kernels[counts[0]] and "POPC" in kernels[counts[0]]
 
@@ -73,7 +71,7 @@ def test_expectations(oracle):
     total = 0
     for name in GOLDEN_NAMES:
         m = load_model(name)
-        _, lc = oracle.infer(m, _scale(g["images"]).astype(np.int8))
+        _, lc = oracle.infer(m, scale_images(g["images"]))
         lp = np.argmax(emulate(m, g["images"]), axis=1)
         assert np.array_equal(lp, np.argmax(g[name], axis=1)), name
         c = expected_counts(lc, lp, np.arange(64) % 12)
@@ -83,28 +81,6 @@ def test_expectations(oracle):
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def lib(built):
-    from bitnetmcu_b200 import _lib
-    l = _lib.load()
-    assert l.bnm_device_count() > 0, "no CUDA device"
-    return l
-
-
-def _engine_and_route(model, capfd, monkeypatch):
-    """an engine built with BNM_VERBOSE set, its engines route line and its fused FC plan line (or None)"""
-    from bitnetmcu_b200.engine import Engine
-    monkeypatch.setenv("BNM_VERBOSE", "1")
-    capfd.readouterr()
-    e = Engine(model, device=0)
-    err = capfd.readouterr().err.splitlines()
-    monkeypatch.delenv("BNM_VERBOSE")
-    lines = [l for l in err if "engines route:" in l]
-    plan = [l for l in err if "fused FC plan" in l]
-    assert len(lines) == 1, lines
-    return e, lines[0].split("engines route: ")[1], (plan[-1] if plan else None)
-
 
 def _compare(e, d_x, truth=None, want=("c", "py", "counts"), counts=None, stream=None, sentinel=-7):
     """one call -> (labels_c, labels_py, counts) as NumPy (None for what was not asked for)"""
@@ -149,11 +125,11 @@ def test_golden_models(lib, oracle, capfd, monkeypatch, name):
     """labels_c == the oracle on the scaled images, labels_py == np.argmax of the reference emulator's logits, counts == NumPy's
     against a seeded truth; the route names the fused kernel exactly for the float-row models"""
     g = np.load(os.path.join(GOLDEN, "emulator.npz"))
-    x = np.concatenate([g["images"], _images(4000, seed=21)])
+    x = np.concatenate([g["images"], normal_images(4000, seed=21)])
     m = load_model(name)
-    e, route, _ = _engine_and_route(m, capfd, monkeypatch)
-    assert route == (ENGINES_ROW if name in FUSED else FALLBACK), (name, route)
-    _, want_c = oracle.infer(m, _scale(x).astype(np.int8))
+    e, err = verbose_engine(capfd, monkeypatch, lambda: engine(m))
+    assert route(err, "engines") == (ENGINES_ROW if name in FUSED else FALLBACK), (name, err)
+    _, want_c = oracle.infer(m, scale_images(x))
     want_py = np.argmax(emulate(m, x), axis=1)
     assert np.array_equal(want_py[:64], np.argmax(g[name], axis=1))
     truth = _truth(len(x), m.n_classes, seed=len(name))
@@ -173,17 +149,14 @@ def _fc_models():
             ("ternary-d8", P.random_fc_model(M.ENC_TERNARY, (256,) + (64,) * 7 + (12,), seed=8))]
 
 
-N_MANY = 148 * 128 * 2 + 77        # several tiles per CTA, a ragged last tile
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("idx", range(4))
 def test_random_fc_models(lib, capfd, monkeypatch, idx):
     """one call == the two entries, at 1, 127, 128, 129 and N_MANY images; normal-distributed images make the engines disagree"""
     tag, m = _fc_models()[idx]
-    e, route, _ = _engine_and_route(m, capfd, monkeypatch)
-    assert route == ENGINES_ROW, (tag, route)
-    d_all = _cuda(_images(N_MANY, seed=idx + 40))
+    e, err = verbose_engine(capfd, monkeypatch, lambda: engine(m))
+    assert route(err, "engines") == ENGINES_ROW, (tag, err)
+    d_all = _cuda(normal_images(N_MANY, seed=idx + 40))
     truth = _truth(N_MANY, m.n_classes, seed=idx)
     for n in (1, 127, 128, 129, N_MANY):
         d_x = d_all[:n]
@@ -200,9 +173,9 @@ def test_random_fc_models(lib, capfd, monkeypatch, idx):
 @pytest.mark.parametrize("channels,n_classes", [(16, 10), (48, 37), (128, 10)])
 def test_random_cnn_models(lib, capfd, monkeypatch, channels, n_classes):
     m = cnn_model(channels, n_classes, seed=channels + n_classes)
-    e, route, _ = _engine_and_route(m, capfd, monkeypatch)
-    assert route == FALLBACK, route
-    d_all = _cuda(_images(4000, seed=channels))
+    e, err = verbose_engine(capfd, monkeypatch, lambda: engine(m))
+    assert route(err, "engines") == FALLBACK, err
+    d_all = _cuda(normal_images(4000, seed=channels))
     truth = _truth(4000, n_classes, seed=channels)
     for n in (1, 129, 4000):
         want_c, want_py = _two_entries(e, d_all[:n])
@@ -220,12 +193,13 @@ def test_engines_row_past_two_ring_rounds(lib, oracle, capfd, monkeypatch, name)
     oracle and the restatement, nothing written past row n, and the counts"""
     import torch
     m = load_model(name)
-    e, route, line = _engine_and_route(m, capfd, monkeypatch)
-    assert route == ENGINES_ROW and line, route
+    e, err = verbose_engine(capfd, monkeypatch, lambda: engine(m))
+    line = plan_line(err)
+    assert route(err, "engines") == ENGINES_ROW and line, err
     stages = int(re.search(r"float input stages (\d+)", line).group(1))
-    sw = _Sweep(f"<64,1,float,engines> ({name})", (1, stages, 1))
-    x = _float_images(sw.sizes[-1], m.img_bytes, zlib.crc32(name.encode()) + 2)
-    _, want_c = oracle.infer(m, _scale(x).astype(np.int8))
+    sw = Sweep(f"<64,1,float,engines> ({name})", (1, stages, 1))
+    x = scattered_edge_images(sw.sizes[-1], m.img_bytes, zlib.crc32(name.encode()) + 2)
+    _, want_c = oracle.infer(m, scale_images(x))
     want_c = want_c.astype(np.int64)
     want_py = np.argmax(emulate(m, x), axis=1)
     truth = _truth(len(x), m.n_classes, seed=3)
@@ -248,11 +222,10 @@ def test_output_combinations(lib, name):
     """each output NULL in turn leaves the others unchanged; all three NULL, truth without counts and misaligned images are
     BNM_E_ARG; n == 0 leaves the counts alone"""
     import torch
-    from bitnetmcu_b200.engine import Engine
     m = load_model(name)
-    e = Engine(m, device=0)
+    e = engine(m)
     n = 3001
-    d_x = _cuda(_images(n, seed=9))
+    d_x = _cuda(normal_images(n, seed=9))
     truth = _truth(n, m.n_classes, seed=9)
     full = _compare(e, d_x, truth)
     no_truth = full[2][:1] + [0, 0] + full[2][3:]
@@ -291,11 +264,10 @@ def test_output_combinations(lib, name):
 def test_counts_accumulate(lib, name):
     """two calls on the halves of a batch add up to one call on the whole, into the same counts"""
     import torch
-    from bitnetmcu_b200.engine import Engine
     m = load_model(name)
-    e = Engine(m, device=0)
+    e = engine(m)
     n = 148 * 128 + 1001
-    d_x = _cuda(_images(n, seed=12))
+    d_x = _cuda(normal_images(n, seed=12))
     d_t = torch.from_numpy(_truth(n, m.n_classes, seed=12)).cuda()
     whole = torch.zeros(4, dtype=torch.int64, device="cuda")
     halves = torch.zeros(4, dtype=torch.int64, device="cuda")
@@ -313,10 +285,9 @@ def test_counts_accumulate(lib, name):
 def test_layered_path(lib, name):
     """BNM_PATH_LAYERS gives the labels and counts of the default path"""
     from bitnetmcu_b200 import _lib
-    from bitnetmcu_b200.engine import Engine
     m = load_model(name)
-    e = Engine(m, device=0)
-    x = _images(5000, seed=13)
+    e = engine(m)
+    x = normal_images(5000, seed=13)
     truth = _truth(5000, m.n_classes, seed=13)
     d_x = _cuda(x)
     default = _compare(e, d_x, truth)
@@ -332,12 +303,11 @@ def test_layered_path(lib, name):
 def test_non_default_stream(lib, name):
     """images copied from pinned memory on a side stream and the call on that stream, ordered by it alone"""
     import torch
-    from bitnetmcu_b200.engine import Engine
     m = load_model(name)
     n = 148 * 128 * 3 + 5
-    x = _images(n, seed=3)
+    x = normal_images(n, seed=3)
     truth = _truth(n, m.n_classes, seed=3)
-    e = Engine(m, device=0)
+    e = engine(m)
     h_x = torch.from_numpy(x).pin_memory()
     d_t = torch.from_numpy(truth).cuda()
     s = torch.cuda.Stream()
@@ -360,21 +330,14 @@ def test_non_default_stream(lib, name):
 def test_crafted_inputs(lib, oracle):
     """all-zero images, one negative pixel, and CNN models whose conv2 or conv3 outputs are never positive (the inputs of
     test_emulator_routes.test_crafted_inputs); and the fused row on the same images"""
-    from bitnetmcu_b200.engine import Engine
-    x = _images(700, seed=5)
-    x[:110] = 0.0
-    x[100:110, 7] = np.float32(-3.0)
-    rng = np.random.default_rng(3)
-    neg = -rng.integers(0, 129, size=48 * 9)
+    x, models = crafted_cnn_case()
     truth = _truth(700, 10, seed=5)
-    models = [(cnn_model(48, 10, seed=4, w=w), what) for w, what in (((None, None, None), "random"), ((None, neg, None), "conv2 <= 0"),
-                                                                     ((None, None, neg), "conv3 <= 0"))]
     models.append((load_model("fc"), "fc"))
     for m, what in models:
         if what.startswith("conv"):
             assert not cnn_features(m, x).any(), what
-        e = Engine(m, device=0)
-        _, want_c = oracle.infer(m, _scale(x).astype(np.int8))
+        e = engine(m)
+        _, want_c = oracle.infer(m, scale_images(x))
         want_py = np.argmax(emulate(m, x), axis=1)
         lc, lp, cnt = _compare(e, _cuda(x), truth)
         assert np.array_equal(lc, want_c.astype(np.int64)) and np.array_equal(lp, want_py), what

@@ -7,38 +7,17 @@ expectation of the GPU tests) against the reference's own logits, and the emulat
 import ctypes as C
 import importlib.util
 import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 
 from conftest import GOLDEN, ROOT, load_model
+from restate import emulate_fc, scale_images
+from support import N_MANY, engine, instructions, lib, local_memory, normal_images, plan_line, random_fc, run_emulator, \
+    sass_functions, verbose_engine
 
 FC_GOLDEN = ["fc", "1k", "12k_FP130", "2bitsym96", "8bit64", "binary160", "ternary64"]
 ALL_GOLDEN = FC_GOLDEN + ["cnn", "cnn_48", "cnn_16small"]
-LEVEL_SHIFT = {2: 1, 4: 1}          # 2bitsym / 4bitsym levels are half the engine's integer weights (BitNetMCU.py:155-164)
-
-
-# ---- NumPy restatement of the emulator's FC path --------------------------------------------------------------------------
-
-def emulate_fc(model, x):
-    """float32 images [n, img_bytes] -> float64 logits [n, n_classes], following BitNetMCU.py:435-457 and 527-530: the float32
-    input scaling, then per BitLinear layer a float64 product with the weight levels, a power-of-two rescale of every row to a
-    maximum of at most 127 with round-half-even and ReLU, and no rescale after the last layer."""
-    from bitnetmcu_b200 import model as M, pack as P
-    x = np.asarray(x, dtype=np.float32)
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    act = np.round(x * scale).clip(-128, 127).astype(np.float64)
-    fc = [l for l in model.layers if l.kind == M.LAYER_FC]
-    for i, l in enumerate(fc):
-        # weight levels over the columns the previous layer delivers (Ternary pads n_in with zero trits)
-        w = P.decode_int_weights(l).astype(np.float64)[:, :act.shape[1]] / 2.0 ** LEVEL_SHIFT.get(l.bitperweight, 0)
-        conv = act @ w.T
-        if i + 1 == len(fc):
-            return conv
-        top = np.maximum(conv.max(axis=-1, keepdims=True), 1e-5)
-        act = np.round(conv * np.exp2(np.floor(np.log2(127.0 / top)))).clip(0, 127)
 
 
 def emul_exponent(m):
@@ -110,59 +89,20 @@ def test_restatement_reproduces_reference_emulator(name):
 
 def test_emulator_kernel_sass(built):
     """fc_emul_kernel is its own function (not a ninth fc_chain_kernel instantiation) and keeps everything in registers"""
-    from bitnetmcu_b200 import _lib
-    out = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    kernels = {k.split()[0]: k for k in re.split(r"\n\s*Function : ", out)[1:]}
+    kernels = sass_functions()
     emul = [k for k in kernels if k.startswith("_ZN3bnm14fc_emul_kernel")]
     assert len(emul) == 1, sorted(kernels)
-    ins = re.findall(r"/\*[0-9a-f]{4,}\*/\s+([^;]*);", kernels[emul[0]])
-    assert len(ins) > 100 and any(i.strip().startswith("IGMMA") for i in ins)
-    assert not [i for i in ins if re.match(r"(@\S+\s+)?(LDL|STL)\b", i.strip())], "local memory in fc_emul_kernel"
+    ins = instructions(kernels[emul[0]])
+    assert len(ins) > 100 and any(i.startswith("IGMMA") for i in ins)
+    assert not local_memory(ins), "local memory in fc_emul_kernel"
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------------
 
-@pytest.fixture(scope="module")
-def lib(built):
-    from bitnetmcu_b200 import _lib
-    l = _lib.load()
-    assert l.bnm_device_count() > 0, "no CUDA device"
-    return l
-
-
-def _engine(model, path=0):
-    from bitnetmcu_b200.engine import Engine
-    return Engine(model, device=0, path=path)
-
-
-def _run(e, x, want_logits=True, want_labels=True, stream=None):
-    """device call on host data -> (logits, labels) as NumPy, None for what was not asked for"""
-    import torch
-    n = x.shape[0]
-    d_x = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).cuda()
-    lo = torch.full((n, e.n_classes), np.nan, dtype=torch.float64, device="cuda") if want_logits else None
-    la = torch.full((n,), -1, dtype=torch.int32, device="cuda") if want_labels else None
-    e.inference_quantized_device(d_x, lo, la, stream=stream)
-    torch.cuda.synchronize()
-    return (lo.cpu().numpy() if want_logits else None), (la.cpu().numpy().astype(np.int64) if want_labels else None)
-
-
-def _fused_row(e_factory, capfd, monkeypatch):
-    """build an engine with BNM_VERBOSE set; True when its plan runs the fused emulator kernel"""
-    monkeypatch.setenv("BNM_VERBOSE", "1")
-    capfd.readouterr()
-    e = e_factory()
-    plan = [l for l in capfd.readouterr().err.splitlines() if "fused FC plan" in l]
-    monkeypatch.delenv("BNM_VERBOSE")
-    return e, bool(plan) and "emulator <64,1,float,emul>" in plan[-1]
-
-
-def _float_images(n, elems, seed):
-    rng = np.random.default_rng(seed)
-    x = rng.normal(size=(n, elems)).astype(np.float32)
-    k = min(n, 40)
-    x[:k] = (rng.integers(0, 256, size=(k, elems)) / 255.0 - 0.1307).astype(np.float32) / np.float32(0.3081)
-    return x
+def _fused_engine(capfd, monkeypatch, model):
+    """an engine, and whether its plan runs the fused emulator kernel"""
+    e, err = verbose_engine(capfd, monkeypatch, lambda: engine(model))
+    return e, "emulator <64,1,float,emul>" in (plan_line(err) or "")
 
 
 @pytest.mark.gpu
@@ -174,13 +114,13 @@ def test_device_entry_matches_reference_emulator(lib, capfd, monkeypatch, name):
     g = np.load(os.path.join(GOLDEN, "emulator.npz"))
     want = g[name]
     m = load_model(name)
-    e, fused = _fused_row(lambda: _engine(m), capfd, monkeypatch)
+    e, fused = _fused_engine(capfd, monkeypatch, m)
     # FC models up to 64 wide; a CNN model's plan has the kernel too (its FC part fits), but CNN models always take the fallback
     assert fused == (name in ("fc", "1k", "12k_FP130", "8bit64", "ternary64", "cnn_16small")), name
     for path in (None, _lib.PATH_LAYERS):
         if path is not None:
             e.set_option(_lib.OPT_PATH, path)
-        lo, la = _run(e, g["images"])
+        lo, la = run_emulator(e, g["images"])
         assert np.array_equal(lo, want), (name, path, np.argwhere(lo != want)[:5])
         assert np.array_equal(la, np.argmax(want, axis=1)), (name, path)
     e.close()
@@ -192,13 +132,8 @@ def _random_models():
     for enc in (M.ENC_BINARY, M.ENC_2BITSYM, M.ENC_4BITSYM, M.ENC_4BIT, M.ENC_8BIT, M.ENC_FP130, M.ENC_TERNARY):
         out.append((M.ENC_NAMES[enc], P.random_fc_model(enc, (256, 64, 64, 64, 10), seed=enc)))
     out.append(("2bitsym-16cls", P.random_fc_model(M.ENC_2BITSYM, (256, 48, 16), seed=3)))
-    out.append(("4bitsym-160in", _sized(P.random_fc_model(M.ENC_4BITSYM, (160, 64, 32, 7), seed=5), 160)))
+    out.append(("4bitsym-160in", random_fc(M.ENC_4BITSYM, (160, 64, 32, 7), 5)))
     return out
-
-
-def _sized(m, img_bytes):
-    m.img_bytes = img_bytes
-    return m
 
 
 @pytest.mark.gpu
@@ -208,30 +143,30 @@ def test_fused_equals_layered_and_restatement(lib, capfd, monkeypatch, idx):
     inputs): the fused emulator, the layer-by-layer emulator and the NumPy restatement agree exactly"""
     from bitnetmcu_b200 import _lib
     tag, m = _random_models()[idx]
-    x = _float_images(3001, m.img_bytes, seed=idx)
+    x = normal_images(3001, seed=idx, elems=m.img_bytes)
     want = emulate_fc(m, x)
-    e, fused = _fused_row(lambda: _engine(m), capfd, monkeypatch)
+    e, fused = _fused_engine(capfd, monkeypatch, m)
     assert fused, tag
-    lo, la = _run(e, x)
+    lo, la = run_emulator(e, x)
     assert np.array_equal(lo, want), (tag, np.argwhere(lo != want)[:5])
     assert np.array_equal(la, np.argmax(want, axis=1)), tag
     e.set_option(_lib.OPT_PATH, _lib.PATH_LAYERS)
-    lo2, la2 = _run(e, x)
+    lo2, la2 = run_emulator(e, x)
     assert np.array_equal(lo2, lo) and np.array_equal(la2, la), tag
     e.close()
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("n", [1, 127, 128, 129, 148 * 128 * 2 + 77])
+@pytest.mark.parametrize("n", [1, 127, 128, 129, N_MANY])
 def test_batch_sizes(lib, n):
     """ragged tiles, one tile, several tiles per CTA; twice in a row (the launch is repeatable: each one starts its ring at stage
     0, phase 0; tests/test_fc_ring_rounds.py runs the ring past its first rounds)"""
     m = load_model("fc")
-    x = _float_images(n, 256, seed=n)
+    x = normal_images(n, seed=n)
     want = emulate_fc(m, x)
-    e = _engine(m)
+    e = engine(m)
     for _ in range(2):
-        lo, la = _run(e, x)
+        lo, la = run_emulator(e, x)
         assert np.array_equal(lo, want) and np.array_equal(la, np.argmax(want, axis=1)), n
     e.close()
 
@@ -256,9 +191,7 @@ def _first_layer_stats(model, x):
     """layer-1 row maxima and whether round-half-even met an exact tie there, per the restatement"""
     from bitnetmcu_b200 import model as M, pack as P
     l = [l for l in model.layers if l.kind == M.LAYER_FC][0]
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    q = np.round(x * scale).clip(-128, 127).astype(np.int64)
-    acc = q @ P.decode_int_weights(l).astype(np.int64)[:, :x.shape[1]].T
+    acc = scale_images(x).astype(np.int64) @ P.decode_int_weights(l).astype(np.int64)[:, :x.shape[1]].T
     mx = acc.max(axis=1)
     e = emul_exponent(np.maximum(mx, 1))
     s = np.maximum(-e, 0)[:, None]
@@ -282,11 +215,11 @@ def test_crafted_rows(lib):
         else:
             assert (ex[mx > 0] >= 0).any() and (ex < 0).any() and ties and (mx <= 0).any()
         want = emulate_fc(m, xs)
-        e = _engine(m)
+        e = engine(m)
         for path in (None, _lib.PATH_LAYERS):
             if path is not None:
                 e.set_option(_lib.OPT_PATH, path)
-            lo, la = _run(e, xs)
+            lo, la = run_emulator(e, xs)
             assert np.array_equal(lo, want) and np.array_equal(la, np.argmax(want, axis=1)), (m.source, path)
         e.close()
 
@@ -297,11 +230,11 @@ def test_labels_only_and_logits_only(lib, name):
     m = load_model(name)
     g = np.load(os.path.join(GOLDEN, "emulator.npz"))
     x = np.concatenate([g["images"]] * 20)
-    e = _engine(m)
-    full, lab = _run(e, x)
-    lo, la = _run(e, x, want_logits=False)
+    e = engine(m)
+    full, lab = run_emulator(e, x)
+    lo, la = run_emulator(e, x, want_logits=False)
     assert lo is None and np.array_equal(la, lab)
-    lo, la = _run(e, x, want_labels=False)
+    lo, la = run_emulator(e, x, want_labels=False)
     assert la is None and np.array_equal(lo, full)
     assert np.array_equal(full[:64], g[name])
     e.close()
@@ -310,7 +243,7 @@ def test_labels_only_and_logits_only(lib, name):
 @pytest.mark.gpu
 def test_argument_errors(lib):
     import torch
-    e = _engine(load_model("fc"))
+    e = engine(load_model("fc"))
     h, n = e.handle, 300
     d_x = torch.zeros((n + 1, 256), dtype=torch.float32, device="cuda")
     d_lo = torch.zeros((n + 1, 10), dtype=torch.float64, device="cuda")
@@ -335,9 +268,9 @@ def test_non_default_stream(lib, name):
     import torch
     m = load_model(name)
     n = 148 * 128 * 3 + 5
-    x = _float_images(n, 256, seed=3)
+    x = normal_images(n, seed=3)
     want = emulate_fc(m, x) if m.model_class == 0 else None
-    e = _engine(m)
+    e = engine(m)
     h_x = torch.from_numpy(x).pin_memory()
     s = torch.cuda.Stream()
     with torch.cuda.stream(s):
@@ -357,10 +290,10 @@ def test_non_default_stream(lib, name):
 
 @pytest.mark.gpu
 def test_verbose_names_emulator_kernel(lib, capfd, monkeypatch):
-    e, fused = _fused_row(lambda: _engine(load_model("fc")), capfd, monkeypatch)
+    e, fused = _fused_engine(capfd, monkeypatch, load_model("fc"))
     assert fused
     e.close()
-    e, fused = _fused_row(lambda: _engine(load_model("binary160")), capfd, monkeypatch)
+    e, fused = _fused_engine(capfd, monkeypatch, load_model("binary160"))
     assert not fused
     e.close()
 
@@ -377,7 +310,7 @@ def _host_module(name):
 def test_driver_emulator_lines(lib, oracle, which):
     """host/evaluate_engines.py: the three lines of the C-engine driver unchanged, then the emulator's counters"""
     m = load_model(which)
-    x = _float_images(4000, 256, seed=21)
+    x = normal_images(4000, seed=21)
     labels = np.random.default_rng(5).integers(0, 10, size=4000)
     lines, c_lines = [], []
     res = _host_module("evaluate_engines").evaluate(m, x, labels, out=lines.append)

@@ -2,20 +2,19 @@
 its sm_90a SASS issues layer 1 as one unrolled run of wgmma, ReLUNorm without predicates, and its consumer warpgroups divide
 nothing per tile."""
 import re
-import subprocess
 
 import pytest
+
+from support import instructions, sass_functions
 
 FIXED = "_ZN3bnm15fc_chain_kernelILi64ELi2ELb0ELi2ELi16ELb1EEEv14CUtensorMap_stNS_11ChainParamsE"
 
 
 @pytest.fixture(scope="module")
 def fixed_sass(built):
-    from bitnetmcu_b200 import _lib
-    out = subprocess.run(["cuobjdump", "-sass", "-fun", FIXED, _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    ins = re.findall(r"/\*[0-9a-f]{4,}\*/\s+([^;]*);", out)
+    ins = instructions(sass_functions().get(FIXED, ""))
     assert len(ins) > 100, "fixed-shape instantiation missing from the library"
-    return [i.strip() for i in ins]
+    return ins
 
 
 def _consumer(ins):
@@ -59,10 +58,7 @@ def test_consumer_has_no_division(fixed_sass):
 def test_every_instantiation_divides_once(built):
     """every role of every fc_chain_kernel instantiation advances its ring position by counters: the one unsigned integer
     division left (I2F.U32.RP starts its sequence) is the entry code's count of the CTA's tiles"""
-    from bitnetmcu_b200 import _lib
-    out = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    kernels = re.split(r"\n\s*Function : ", out)[1:]
-    chain = {k.split()[0]: k for k in kernels if k.startswith("_ZN3bnm15fc_chain_kernel")}
+    chain = {name: text for name, text in sass_functions().items() if name.startswith("_ZN3bnm15fc_chain_kernel")}
     assert FIXED in chain and len(chain) == 8, sorted(chain)
     for name, sass in chain.items():
         assert sass.count("I2F.U32.RP") == 1, name

@@ -9,38 +9,10 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, load_model, model_names
+from restate import scale_images
+from support import N_MANY, engine, frontends, lib
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def lib(built):
-    from bitnetmcu_b200 import _lib
-    l = _lib.load()
-    assert l.bnm_device_count() > 0, "no CUDA device"
-    return l
-
-
-def _engine(name, path, nf4=False, cnn_frontend=None):
-    from bitnetmcu_b200 import _lib
-    from bitnetmcu_b200.engine import Engine
-    e = Engine(load_model(name), device=0, path=path, nf4_extension=nf4)
-    if cnn_frontend is not None:
-        e.set_option(_lib.OPT_CNN_FRONTEND, cnn_frontend)
-    return e
-
-
-def _frontends(model):
-    """CNN models run once per front-end kernel (BNM_OPT_CNN_FRONTEND): CUDA cores and conv1-on-wgmma; FC models once."""
-    from bitnetmcu_b200 import _lib
-    if model.model_class != 1:
-        return [None]
-    return [_lib.CNN_CUDA_CORES, _lib.CNN_TENSOR_CORES] if model.channels % 16 == 0 else [_lib.CNN_CUDA_CORES]
-
-
-def _paths(name):
-    from bitnetmcu_b200 import _lib
-    return [_lib.PATH_LAYERS, _lib.PATH_TCGEN05]
 
 
 def _rand_images(n, seed=0):
@@ -64,8 +36,8 @@ def test_model_matches_golden_and_oracle(lib, oracle, golden, digits, name, path
     n = 5000 + 37
     r = _rand_images(n, seed=len(name))
     oo, ol = oracle.infer(model, r)
-    for fe in _frontends(model):
-        e = _engine(name, _lib.PATH_LAYERS if path == "layers" else _lib.PATH_TCGEN05, cnn_frontend=fe)
+    for fe in frontends(model):
+        e = engine(model, _lib.PATH_LAYERS if path == "layers" else _lib.PATH_TCGEN05, cnn_frontend=fe)
         assert e.active_path == (_lib.PATH_LAYERS if path == "layers" else _lib.PATH_TCGEN05)
         imgs, _ = digits
         lo, la = e.infer(imgs)
@@ -88,8 +60,8 @@ def test_edge_batch_sizes(lib, oracle, n):
     for name in ("fc", "cnn_48"):
         m = load_model(name)
         for path in (_lib.PATH_LAYERS, _lib.PATH_TCGEN05):
-            for fe in _frontends(m):
-                e = _engine(name, path, cnn_frontend=fe)
+            for fe in frontends(m):
+                e = engine(m, path, cnn_frontend=fe)
                 imgs = _rand_images(n, seed=n)
                 lo, la = e.infer(imgs)
                 assert lo.shape == (n, m.n_classes)
@@ -102,14 +74,14 @@ def test_edge_batch_sizes(lib, oracle, n):
 def test_survey_kat_on_gpu(lib, oracle):
     """SURVEY.md 8c: CRC-32 of the first 1000x10 logits of the xorshift stream = fc621bad; label sums."""
     kat = json.load(open(os.path.join(GOLDEN, "kat.json")))
-    e = _engine("fc", 0)
+    e = engine(load_model("fc"))
     xs = oracle.xorshift_images(400000)
     lo, la = e.infer(xs)
     assert "%08x" % zlib.crc32(lo[:1000].astype("<i4").tobytes()) == kat["fc_xs_crc32_first1000"]
     assert int(la[:1000].sum()) == kat["fc_xs_sum_labels_1000"]
     assert int(la.sum()) == kat["fc_xs_sum_labels_400000"]
     e.close()
-    e = _engine("cnn", 0)
+    e = engine(load_model("cnn"))
     _, la = e.infer(xs[:40000])
     assert int(la.sum()) == kat["cnn_xs_sum_labels_40000"]
     e.close()
@@ -121,7 +93,7 @@ def test_nf4_extension(lib, oracle):
     m = load_model("rand_nf4_64")
     imgs = _rand_images(777)
     for path in (_lib.PATH_LAYERS, _lib.PATH_TCGEN05):
-        e = _engine("rand_nf4_64", path)
+        e = engine(m, path)
         lo, _ = e.infer(imgs)
         assert not lo.any()
         e.set_option(_lib.OPT_NF4_EXTENSION, 1)
@@ -140,7 +112,7 @@ def test_full_size_batch_properties(lib, oracle, name):
     n = 1 << 20
     rng = np.random.default_rng(5)
     imgs = rng.integers(-128, 128, size=(n, 256), dtype=np.int8)
-    e = _engine(name, 0)
+    e = engine(m)
     lo, la = e.infer(imgs)
     # shards of uneven size reproduce the same rows
     cut = 333333
@@ -165,7 +137,7 @@ def test_host_pipeline_chunks(lib, oracle):
     imgs = _rand_images(10000, seed=3)
     oo, ol = oracle.infer(m, imgs)
     for chunk in (128, 1024, 4096):
-        e = _engine("fc", 0)
+        e = engine(m)
         e.set_option(_lib.OPT_CHUNK_IMAGES, chunk)
         lo, la = e.infer(imgs)
         assert np.array_equal(lo, oo) and np.array_equal(la, ol)
@@ -179,7 +151,7 @@ def test_device_api_torch(lib, oracle):
     m = load_model("fc")
     imgs = _rand_images(3000, seed=4)
     oo, ol = oracle.infer(m, imgs)
-    e = _engine("fc", 0)
+    e = engine(m)
     d_img = torch.from_numpy(imgs).cuda()
     d_log = torch.empty((3000, 10), dtype=torch.int32, device="cuda")
     d_lab = torch.empty(3000, dtype=torch.int32, device="cuda")
@@ -203,7 +175,7 @@ def test_launch_overlap_modes(lib, oracle, mode, n):
     # n: several tiles per SM + a ragged last tile; the small n does not fill the GPU -> no early trigger even in mode 2
     batches = [_rand_images(n, seed=20 + k) for k in range(4)]
     want = [oracle.infer(m, b) for b in batches]
-    e = _engine("fc", 0)
+    e = engine(m)
     e.set_option(_lib.OPT_LAUNCH_OVERLAP, mode)
     s = torch.cuda.Stream()
     src = [torch.from_numpy(b).cuda() for b in batches]
@@ -374,7 +346,7 @@ def test_extreme_weights_cnn(lib, oracle):
     imgs = _extreme_images()
     want_logits, want_labels = oracle.infer(base, imgs)
     from bitnetmcu_b200 import _lib
-    for fe in _frontends(base):
+    for fe in frontends(base):
         e = Engine(base)
         e.set_option(_lib.OPT_CNN_FRONTEND, fe)
         lo_, la_ = e.infer(imgs)
@@ -394,8 +366,7 @@ def test_quantize_images_matches_numpy(lib):
     x[52, :] = np.float32(0.5) / np.float32(127.0) * np.arange(256, dtype=np.float32)   # many exact .5 ties
     x[53] = -x[52]
     x[54, 0] = 3e38
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    want = np.round(x * scale).clip(-128, 127).astype(np.int8)
+    want = scale_images(x)
     got = E.quantize_images(x)
     assert got.dtype == np.int8 and np.array_equal(got, want)
 
@@ -408,10 +379,9 @@ def test_float_images_to_labels_on_device(lib, oracle):
     m = load_model("fc")
     rng = np.random.default_rng(9)
     x = rng.normal(size=(5000, 256)).astype(np.float32)
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    q = np.round(x * scale).clip(-128, 127).astype(np.int8)
+    q = scale_images(x)
     want_logits, want_labels = oracle.infer(m, q)
-    e = _engine("fc", 0)
+    e = engine(m)
     d_x = torch.from_numpy(x).cuda()
     d_q = torch.empty((5000, 256), dtype=torch.int8, device="cuda")
     d_log = torch.empty((5000, 10), dtype=torch.int32, device="cuda")
@@ -492,8 +462,8 @@ def test_later_model_keeps_earlier_models_shared_memory(lib, oracle):
     """Creating a model must not lower the dynamic shared memory limit of a kernel another live model launches: FC 4bitsym-64's
     fused launch asks for more shared memory than Binary-160's."""
     from bitnetmcu_b200 import _lib
-    fc = _engine("fc", _lib.PATH_TCGEN05)
-    b160 = _engine("binary160", _lib.PATH_TCGEN05)
+    fc = engine(load_model("fc"), _lib.PATH_TCGEN05)
+    b160 = engine(load_model("binary160"), _lib.PATH_TCGEN05)
     imgs = _rand_images(5000 + 37, seed=3)
     lo, la = fc.infer(imgs)
     oo, ol = oracle.infer(load_model("fc"), imgs)
@@ -512,7 +482,7 @@ def test_launch_overlap_mode2_reused_buffers_keep_stream_order(lib, oracle):
     n = 148 * 128 * 5 + 3
     batches = [_rand_images(n, seed=40 + k) for k in range(4)]
     want = [oracle.infer(m, b) for b in batches]
-    e = _engine("fc", 0)
+    e = engine(m)
     e.set_option(_lib.OPT_LAUNCH_OVERLAP, 2)
     s = torch.cuda.Stream()
     src = [torch.from_numpy(b).cuda() for b in batches]
@@ -596,7 +566,7 @@ def _gather_case(lib, oracle, name, n, dst_device):
     m = load_model(name)
     imgs = _rand_images(n, seed=77)
     want, want_lab = oracle.infer(m, imgs)
-    e = _engine(name, _lib.PATH_TCGEN05)
+    e = engine(m, _lib.PATH_TCGEN05)
     if dst_device != 0:
         _lib.check(lib.bnm_enable_peer_access(0, dst_device), "bnm_enable_peer_access")
     C_ = m.n_classes
@@ -637,7 +607,7 @@ def _gather_case(lib, oracle, name, n, dst_device):
     e.close()
 
 
-@pytest.mark.parametrize("name,n", [("fc", 148 * 128 * 2 + 77), ("fc", 1000), ("cnn_letters", 3000), ("binary160", 5000), ("cnn_48", 2049)])
+@pytest.mark.parametrize("name,n", [("fc", N_MANY), ("fc", 1000), ("cnn_letters", 3000), ("binary160", 5000), ("cnn_48", 2049)])
 def test_fused_gather_epilogue_same_gpu(lib, oracle, name, n):
     """bnm_infer_batch_device_gather with destinations on the same GPU: full tiles take the staged bulk-store path (16-byte
     aligned rows), the ragged last tile and > 16 classes (cnn_letters: 37) the direct stores; rows outside the call stay untouched."""
@@ -653,7 +623,7 @@ def test_fused_gather_epilogue_peer_gpu(lib, oracle):
 
 # ---- float input fused into the FC kernel's load stage (SURVEY.md 8f rank 3) ----------------------------------------------------------
 
-def _float_images(n, elems, seed):
+def _edge_row_images(n, elems, seed):
     rng = np.random.default_rng(seed)
     x = rng.normal(size=(n, elems)).astype(np.float32)
     k = min(n, 50)
@@ -668,18 +638,17 @@ def _float_images(n, elems, seed):
     return x
 
 
-@pytest.mark.parametrize("name,n", [("fc", 148 * 128 * 2 + 77), ("fc", 1), ("fc", 129), ("ternary64", 5000), ("1k", 4097), ("binary160", 3000), ("cnn_48", 2500)])
+@pytest.mark.parametrize("name,n", [("fc", N_MANY), ("fc", 1), ("fc", 129), ("ternary64", 5000), ("1k", 4097), ("binary160", 3000), ("cnn_48", 2500)])
 def test_float_input_fused_into_the_fc_kernel(lib, oracle, name, n):
     """bnm_infer_batch_device_f32: float32 images -> int32 logits in one kernel for FC models (four quantiser warps write the int8 A
     operand of layer 1 into shared memory, SWIZZLE_128B by hand), through the scaling kernel for CNN models; compared with the
     NumPy scaling of test_inference.py:140-141 followed by the oracle.  Tolerance 0."""
     import torch
     m = load_model(name)
-    x = _float_images(n, m.img_bytes, seed=n)
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    q = np.round(x * scale).clip(-128, 127).astype(np.int8)
+    x = _edge_row_images(n, m.img_bytes, seed=n)
+    q = scale_images(x)
     want, want_lab = oracle.infer(m, q)
-    e = _engine(name, 0)
+    e = engine(m)
     d_x = torch.from_numpy(x).cuda()
     d_log = torch.empty((n, m.n_classes), dtype=torch.int32, device="cuda")
     d_lab = torch.empty(n, dtype=torch.int32, device="cuda")
@@ -700,10 +669,8 @@ def test_float_input_odd_row_widths(lib, oracle):
     for n_in, n_out in [(160, 160), (64, 10), (32, 1), (128, 16)]:
         m = P.random_fc_model(4, (n_in, 64, n_out), seed=n_in)
         m.img_bytes = n_in
-        x = _float_images(1777, n_in, seed=n_in)
-        scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-        q = np.round(x * scale).clip(-128, 127).astype(np.int8)
-        want, want_lab = oracle.infer(m, q)
+        x = _edge_row_images(1777, n_in, seed=n_in)
+        want, want_lab = oracle.infer(m, scale_images(x))
         e = Engine(m, path=_lib.PATH_TCGEN05)
         d_x = torch.from_numpy(x).cuda()
         d_log = torch.empty((1777, n_out), dtype=torch.int32, device="cuda")

@@ -1,45 +1,17 @@
 """The plain-C host side (host/*.c): compiles against any exported BitNetMCU_model.h with gcc and, on a GPU, reproduces
 the reference's stdout for BASELINE.json config #1 (BitNetMCU_MNIST_test.c + 10 digits) and its ctypes protocol."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, ROOT, load_model
-
-
-def _write_test_data_header(path, images, labels):
-    with open(path, "w") as f:
-        for i in range(images.shape[0]):
-            f.write(f"int8_t input_data_{i}[256] = {{" + ", ".join(str(int(v)) for v in images[i]) + "};\n")
-            f.write(f"uint8_t label_{i} = {int(labels[i])};\n")
-
-
-def _build(tmp, name):
-    from bitnetmcu_b200 import _lib
-    from bitnetmcu_b200.pack import write_header
-    m = load_model(name)
-    # Model.load names the layers as the reference's dll.c expects: FC L1..L4 / CNN L2..L15 (dll.c:48-121)
-    want = ["L2", "L4", "L6", "L7", "L9", "L11", "L13", "L15"] if m.model_class == 1 else ["L1", "L2", "L3", "L4"]
-    assert [l.name for l in m.layers] == want[:len(m.layers)]
-    write_header(m, os.path.join(tmp, "BitNetMCU_model.h"))
-    d = np.load(os.path.join(GOLDEN, "digits.npz"))
-    _write_test_data_header(os.path.join(tmp, "BitNetMCU_MNIST_test_data.h"), d["images"], d["labels"])
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    common = ["-I" + tmp, "-I" + os.path.join(ROOT, "include"), "-L" + libdir, "-lbitnetmcu_b200", "-Wl,-rpath," + libdir]
-    dll = os.path.join(tmp, "Bitnet_inf.dll")
-    exe = os.path.join(tmp, "mnist_test")
-    subprocess.run(["gcc", "-fPIC", "-shared", "-D_DLL", "-o", dll, os.path.join(ROOT, "host", "bitnetmcu_b200_dll.c")] + common, check=True)
-    subprocess.run(["gcc", "-o", exe, os.path.join(ROOT, "host", "bitnetmcu_b200_test.c"), os.path.join(ROOT, "host", "bitnetmcu_b200_dll.c")] + common,
-                   check=True)
-    return dll, exe, d
+from support import build_c_shim
 
 
 @pytest.mark.parametrize("name", ["fc", "cnn", "1k"])
 def test_shim_compiles_and_exports_inference(built, tmp_path, name):
-    dll, exe, _ = _build(str(tmp_path), name)
+    dll, exe, _ = build_c_shim(str(tmp_path), name)
     out = subprocess.run(["nm", "-D", "--defined-only", dll], capture_output=True, text=True, check=True).stdout
     for sym in ("Inference", "InferenceBatch", "BitMnistInference"):
         assert f" T {sym}" in out
@@ -48,7 +20,7 @@ def test_shim_compiles_and_exports_inference(built, tmp_path, name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["fc", "cnn"])
 def test_shim_reproduces_reference_stdout(built, tmp_path, name):
-    dll, exe, d = _build(str(tmp_path), name)
+    dll, exe, d = build_c_shim(str(tmp_path), name)
     out = subprocess.run([exe], capture_output=True, text=True, check=True, timeout=120).stdout
     want = "".join(f"label: {int(l)} predicted: {int(l)}\n" for l in d["labels"])   # reference: 10/10 for both shipped models
     assert out == want

@@ -7,16 +7,10 @@ import numpy as np
 import pytest
 
 from conftest import load_model, model_names
+from restate import scale_images
+from support import CHAIN_ROWS, N_MANY, build_c_shim, engine, frontends, lib, plan_line, verbose_engine
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def lib(built):
-    from bitnetmcu_b200 import _lib
-    l = _lib.load()
-    assert l.bnm_device_count() > 0, "no CUDA device"
-    return l
 
 
 def _images(n, img_bytes=256, seed=0):
@@ -24,22 +18,6 @@ def _images(n, img_bytes=256, seed=0):
     imgs = rng.integers(-128, 128, size=(n, img_bytes)).astype(np.int8)
     imgs[: min(n, 64)] = np.clip(imgs[: min(n, 64)], -20, 127)   # MNIST-like rows: background ~ -20, strokes to 127
     return imgs
-
-
-def _frontends(model):
-    from bitnetmcu_b200 import _lib
-    if model.model_class != 1:
-        return [None]
-    return [_lib.CNN_CUDA_CORES, _lib.CNN_TENSOR_CORES] if model.channels % 16 == 0 else [_lib.CNN_CUDA_CORES]
-
-
-def _engine(model, path=0, cnn_frontend=None):
-    from bitnetmcu_b200 import _lib
-    from bitnetmcu_b200.engine import Engine
-    e = Engine(model, device=0, path=path)
-    if cnn_frontend is not None:
-        e.set_option(_lib.OPT_CNN_FRONTEND, cnn_frontend)
-    return e
 
 
 @pytest.mark.parametrize("path", ["layers", "tcgen05"])
@@ -51,8 +29,8 @@ def test_golden_models_labels_only(lib, oracle, name, path):
     imgs = _images(5037, seed=len(name))
     _, want = oracle.infer(m, imgs)
     p = _lib.PATH_LAYERS if path == "layers" else _lib.PATH_TCGEN05
-    for fe in _frontends(m):
-        e = _engine(m, p, fe)
+    for fe in frontends(m):
+        e = engine(m, p, fe)
         assert e.active_path == p
         lo, la = e.infer(imgs, want_logits=False)
         assert lo is None and np.array_equal(la, want), (name, path, fe)
@@ -67,42 +45,21 @@ def test_edge_batch_sizes_labels_only(lib, oracle, n):
         m = load_model(name)
         want = oracle.infer(m, imgs)[1] if n else np.empty(0, dtype=np.uint32)
         for path in (_lib.PATH_LAYERS, _lib.PATH_TCGEN05):
-            for fe in _frontends(m):
-                e = _engine(m, path, fe)
+            for fe in frontends(m):
+                e = engine(m, path, fe)
                 lo, la = e.infer(imgs, want_logits=False)
                 assert lo is None and la.shape == (n,) and np.array_equal(la, want), (name, path, fe)
                 e.close()
 
 
-def _random(enc, widths, seed):
-    from bitnetmcu_b200 import pack as P
-    m = P.random_fc_model(enc, widths, seed=seed)
-    m.img_bytes = widths[0]
-    return m
-
-
-# every row of kChainKernels (fc_wgmma.cu), with a model that selects it (checked against the plan's BNM_VERBOSE line)
-_ROWS = [
-    ("<64,1>", lambda: _random(4, (512, 64, 64, 10), 1)),           # 512-byte rows: room for three 64 kB stages, one pipe
-    ("<64,2,2,64>", lambda: _random(4, (256, 64, 64, 37), 2)),      # 37 classes: the last layer is wider than 16
-    ("<64,2,2,16>", lambda: load_model("1k")),                      # 16-wide layers, three of them: not the fixed class
-    ("<64,2,2,16,fixed>", lambda: load_model("fc")),
-    ("<128,1>", lambda: load_model("2bitsym96")),
-    ("<192,1>", lambda: load_model("binary160")),
-    ("<256,1>", lambda: _random(4, (256, 256, 10), 3)),
-]
-
-
-@pytest.mark.parametrize("row", [r for r, _ in _ROWS])
+@pytest.mark.parametrize("row", [r for r, _ in CHAIN_ROWS])
 def test_every_chain_kernel_row_labels_only(lib, oracle, capfd, monkeypatch, row):
     from bitnetmcu_b200 import _lib
-    monkeypatch.setenv("BNM_VERBOSE", "1")
-    m = dict(_ROWS)[row]()
-    capfd.readouterr()
-    e = _engine(m, _lib.PATH_TCGEN05)
-    plan = [l for l in capfd.readouterr().err.splitlines() if "fused FC plan" in l]
-    assert plan and re.search(r"fc_chain_kernel(<[^>]*>)", plan[-1]).group(1) == row, plan
-    n = 148 * 128 * 2 + 77                 # several tiles per CTA and a ragged last tile
+    m = dict(CHAIN_ROWS)[row]()
+    e, err = verbose_engine(capfd, monkeypatch, lambda: engine(m, _lib.PATH_TCGEN05))
+    plan = plan_line(err)
+    assert plan and re.search(r"fc_chain_kernel(<[^>]*>)", plan).group(1) == row, err
+    n = N_MANY
     imgs = _images(n, m.img_bytes, seed=len(row))
     _, want = oracle.infer(m, imgs)
     lo, la = e.infer(imgs, want_logits=False)
@@ -112,14 +69,11 @@ def test_every_chain_kernel_row_labels_only(lib, oracle, capfd, monkeypatch, row
 
 def test_float_input_row_labels_only(lib, oracle, capfd, monkeypatch):
     """the fused float-input row (<64,1,float>) through bnm_infer_batch_device_f32 with NULL logits"""
-    import torch
     from bitnetmcu_b200 import _lib
-    monkeypatch.setenv("BNM_VERBOSE", "1")
     m = load_model("fc")
-    capfd.readouterr()
-    e = _engine(m, _lib.PATH_TCGEN05)
-    assert "float input <64,1,float>" in capfd.readouterr().err
-    _float_case(e, m, oracle, 148 * 128 * 2 + 77)
+    e, err = verbose_engine(capfd, monkeypatch, lambda: engine(m, _lib.PATH_TCGEN05))
+    assert any("float input <64,1,float>" in l for l in err)
+    _float_case(e, m, oracle, N_MANY)
     e.close()
 
 
@@ -127,9 +81,7 @@ def _float_case(e, m, oracle, n):
     import torch
     rng = np.random.default_rng(n)
     x = rng.normal(size=(n, m.img_bytes)).astype(np.float32)
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    q = np.round(x * scale).clip(-128, 127).astype(np.int8)
-    _, want = oracle.infer(m, q)
+    _, want = oracle.infer(m, scale_images(x))
     d_x = torch.from_numpy(x).cuda()
     d_lab = torch.full((n,), -1, dtype=torch.int32, device="cuda")
     for _ in range(2):                      # twice: the launch is repeatable (each one starts its ring at stage 0, phase 0)
@@ -142,7 +94,7 @@ def _float_case(e, m, oracle, n):
 def test_float_input_labels_only(lib, oracle, name):
     """fc: the fused float kernel; binary160 (192 columns): the scaling kernel into scratch, then the int8 entry"""
     m = load_model(name)
-    e = _engine(m)
+    e = engine(m)
     _float_case(e, m, oracle, 3001)
     e.close()
 
@@ -153,7 +105,7 @@ def test_device_labels_only_on_torch_stream(lib, oracle, name):
     m = load_model(name)
     imgs = _images(3000, seed=4)
     _, want = oracle.infer(m, imgs)
-    e = _engine(m)
+    e = engine(m)
     d_img = torch.from_numpy(imgs).cuda()
     d_lab = torch.full((3000,), -1, dtype=torch.int32, device="cuda")
     s = torch.cuda.Stream()
@@ -172,12 +124,12 @@ def test_host_pipeline_labels_only(lib, oracle, name):
     imgs = _images(10000, seed=3)
     _, want = oracle.infer(m, imgs)
     for chunk in (128, 1024, 4096):
-        e = _engine(m)
+        e = engine(m)
         e.set_option(_lib.OPT_CHUNK_IMAGES, chunk)
         lo, la = e.infer(imgs, want_logits=False)
         assert lo is None and np.array_equal(la, want), chunk
         e.close()
-    e = _engine(m)
+    e = engine(m)
     for n in (1, 777, 1024):               # n <= 1024: staged through the small-batch buffers
         lo, la = e.infer(imgs[:n], want_logits=False)
         assert lo is None and np.array_equal(la, want[:n]), n
@@ -197,7 +149,7 @@ def test_launch_overlap_labels_only(lib, oracle, mode):
     n = 148 * 128 * 7 + 77                  # fills the GPU: launches trigger early
     batches = [_images(n, seed=60 + k) for k in range(4)]
     want = [oracle.infer(m, b)[1] for b in batches]
-    e = _engine(m)
+    e = engine(m)
     e.set_option(_lib.OPT_LAUNCH_OVERLAP, mode)
     src = [torch.from_numpy(b).cuda() for b in batches]     # resident inputs: consecutive launches never share a buffer
     d_lab = [torch.full((n,), -1, dtype=torch.int32, device="cuda") for _ in range(2)]
@@ -228,10 +180,10 @@ def test_gather_labels_only(lib, oracle):
     import torch
     from bitnetmcu_b200 import _lib
     m = load_model("fc")
-    n, rows, off = 148 * 128 * 2 + 77, 148 * 128 * 2 + 77 + 640, 512
+    n, rows, off = N_MANY, N_MANY + 640, 512
     imgs = _images(n, seed=77)
     _, want = oracle.infer(m, imgs)
-    e = _engine(m, _lib.PATH_TCGEN05)
+    e = engine(m, _lib.PATH_TCGEN05)
     d_img = torch.from_numpy(imgs).cuda()
     d_lab = torch.full((n,), -1, dtype=torch.int32, device="cuda")
     dst = [torch.full((rows,), -7, dtype=torch.int32, device="cuda") for _ in range(2)]
@@ -255,7 +207,7 @@ def test_no_output_is_an_error(lib):
     """every entry needs at least one output; the emulation entry keeps its logits mandatory"""
     import torch
     from bitnetmcu_b200 import _lib
-    e = _engine(load_model("fc"))
+    e = engine(load_model("fc"))
     imgs = _images(300)
     d_img = torch.from_numpy(imgs).cuda()
     d_x = torch.zeros((300, 256), dtype=torch.float32, device="cuda")
@@ -277,8 +229,7 @@ def test_no_output_is_an_error(lib):
 @pytest.mark.parametrize("name", ["fc", "cnn"])
 def test_c_shim_inference_batch_labels_only(built, oracle, tmp_path, name):
     """InferenceBatch(images, n, NULL, labels) through the gcc-built plain-C shim"""
-    from test_host_c_shim import _build
-    dll, _, d = _build(str(tmp_path), name)
+    dll, _, d = build_c_shim(str(tmp_path), name)
     lib = C.CDLL(dll)
     lib.InferenceBatch.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     lib.InferenceBatch.restype = C.c_int
