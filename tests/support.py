@@ -59,6 +59,23 @@ def plan_line(err):
     return plan[-1] if plan else None
 
 
+def plan_ring(line, kind):
+    """(row, (pipes, stages, slots)) of one form of a `fused FC plan` line: kind "int8" (fc_chain_kernel), "float" (the
+    float-input row), "emul" (the float-input emulator row) or "emul_i8" (fc_emul_i8_kernel).  The slots are the third field
+    of a two-pipe row's name <kN,pipes,slots,...>; a one-pipe row runs one."""
+    if kind == "int8":
+        row = re.search(r"fc_chain_kernel(<[^>]*>)", line).group(1)
+        pipes, stages = map(int, re.search(r"(\d+) pipes x (\d+) stages", line).groups())
+        fields = row[1:-1].split(",")
+        assert int(fields[1]) == pipes, line
+        return row, (pipes, stages, int(fields[2]) if pipes == 2 else 1)
+    if kind == "emul_i8":
+        row, stages = re.search(r"int8 emulator fc_emul_i8_kernel(<[^>]*>) x (\d+) stages", line).groups()
+        return row, (1, int(stages), 1)
+    row = re.search(r"float input (<[^>]*>)" if kind == "float" else r"emulator (<[^>]*>)", line).group(1)
+    return row, (1, int(re.search(r"float input stages (\d+)", line).group(1)), 1)
+
+
 def route(err, what):
     """the route of the one `<what> route:` line ("emulator" or "engines")"""
     lines = [l for l in err if f"{what} route: " in l]
@@ -224,6 +241,19 @@ def run_emulator(e, x, want_logits=True, want_labels=True, stream=None):
     e.inference_quantized_device(d_x, lo, la, stream=stream)
     torch.cuda.synchronize()
     return (lo.cpu().numpy() if want_logits else None), (la.cpu().numpy().astype(np.int64) if want_labels else None)
+
+
+def gather_call(lib, e, d_img, d_log, d_lab, g, stream):
+    """bnm_infer_batch_device_gather of the engine on GPU 0 (images d_img, own outputs d_log / d_lab, either None, and the
+    destinations of the BnmGather g) on `stream`, then waits for the stream -> the entry's return code"""
+    import ctypes as Ct
+    import torch
+    ptr = lambda t: Ct.c_void_p(t.data_ptr()) if t is not None else None
+    with torch.cuda.device(0):
+        rc = lib.bnm_infer_batch_device_gather(e.handle, ptr(d_img), d_img.shape[0], ptr(d_log), ptr(d_lab), Ct.byref(g),
+                                               Ct.c_void_p(stream.cuda_stream))
+        stream.synchronize()
+    return rc
 
 
 # ---- the plain-C host side ----------------------------------------------------------------------------------------------------

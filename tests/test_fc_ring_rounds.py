@@ -10,7 +10,6 @@ CPU: the restatement of that schedule in restate.py (checked against the kernel'
 batch sizes whose coverage is checked.  GPU (tolerance 0): every kernel row, its ring shape read from the plan's BNM_VERBOSE line
 and the SM count from the device, over its sweep -- one launch per batch size on a prefix of one device buffer -- against the
 oracle (int8 and float input) or the NumPy restatement of the emulator."""
-import re
 import zlib
 
 import numpy as np
@@ -19,7 +18,7 @@ import pytest
 from conftest import load_model
 from restate import LEVEL_SHIFT, TILE, batch_size, emulate_fc, most_tiles_per_cta, ring_sweep, scale_images, sweep_gaps, \
     tile_schedule
-from support import CHAIN_ROWS, Sweep, engine, lib, plan_line, random_fc, scattered_edge_images, verbose_engine
+from support import CHAIN_ROWS, Sweep, engine, lib, plan_line, plan_ring, random_fc, scattered_edge_images, verbose_engine
 
 # ---- CPU -------------------------------------------------------------------------------------------------------------------
 
@@ -113,14 +112,9 @@ def _plan(capfd, monkeypatch, model):
 
 def _ring(line, row, kind):
     """(pipes, stages, slots) of `kind` ("int8", "float" or "emul") from the plan line, which must name `row` for it"""
-    if kind == "int8":
-        assert re.search(r"fc_chain_kernel(<[^>]*>)", line).group(1) == row, line
-        pipes, stages = map(int, re.search(r"(\d+) pipes x (\d+) stages", line).groups())
-        fields = row[1:-1].split(",")
-        assert int(fields[1]) == pipes, line
-        return pipes, stages, int(fields[2]) if pipes == 2 else 1
-    assert (f"float input {row}" if kind == "float" else f"emulator {row}") in line, line
-    return 1, int(re.search(r"float input stages (\d+)", line).group(1)), 1
+    got, ring = plan_ring(line, kind)
+    assert got == row, line
+    return ring
 
 
 def _int8_images(n, img_bytes, seed):

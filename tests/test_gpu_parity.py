@@ -10,7 +10,7 @@ import pytest
 
 from conftest import GOLDEN, load_model, model_names
 from restate import scale_images
-from support import N_MANY, engine, frontends, lib
+from support import N_MANY, engine, frontends, gather_call, lib
 
 pytestmark = pytest.mark.gpu
 
@@ -562,7 +562,6 @@ def _gather_case(lib, oracle, name, n, dst_device):
     """One engine on GPU 0; destination buffers on `dst_device` (0: plain second buffers; 1: peer memory over NVLink)."""
     import torch
     from bitnetmcu_b200 import _lib
-    import ctypes as Ct
     m = load_model(name)
     imgs = _rand_images(n, seed=77)
     want, want_lab = oracle.infer(m, imgs)
@@ -582,21 +581,15 @@ def _gather_case(lib, oracle, name, n, dst_device):
         g.labels_dst[k] = dst_lab[k].data_ptr()
         g.logits_dst[k] = dst_log[k].data_ptr()
     torch.cuda.synchronize()
-    with torch.cuda.device(0):
-        s = torch.cuda.current_stream()
-        _lib.check(lib.bnm_infer_batch_device_gather(e.handle, Ct.c_void_p(d_img.data_ptr()), n, Ct.c_void_p(d_log.data_ptr()),
-                                                     Ct.c_void_p(d_lab.data_ptr()), Ct.byref(g), Ct.c_void_p(s.cuda_stream)), "gather")
-        s.synchronize()
+    s = torch.cuda.current_stream(0)
+    _lib.check(gather_call(lib, e, d_img, d_log, d_lab, g, s), "gather")
     assert np.array_equal(d_log.cpu().numpy(), want) and np.array_equal(d_lab.cpu().numpy().astype(np.uint32), want_lab)
     # one byte per label (bnm_gather.labels_u8)
     dst8 = torch.full((rows,), 201, dtype=torch.uint8, device=f"cuda:{dst_device}")
     g8 = _lib.BnmGather()
     g8.n_labels_dst, g8.n_logits_dst, g8.row_offset, g8.labels_u8 = 1, 0, off, 1
     g8.labels_dst[0] = dst8.data_ptr()
-    with torch.cuda.device(0):
-        _lib.check(lib.bnm_infer_batch_device_gather(e.handle, Ct.c_void_p(d_img.data_ptr()), n, Ct.c_void_p(d_log.data_ptr()),
-                                                     Ct.c_void_p(d_lab.data_ptr()), Ct.byref(g8), Ct.c_void_p(s.cuda_stream)), "gather u8")
-        s.synchronize()
+    _lib.check(gather_call(lib, e, d_img, d_log, d_lab, g8, s), "gather u8")
     g8h = dst8.cpu().numpy()
     assert np.array_equal(g8h[off:off + n], want_lab.astype(np.uint8)) and (g8h[:off] == 201).all() and (g8h[off + n:] == 201).all()
     for k in range(2):
