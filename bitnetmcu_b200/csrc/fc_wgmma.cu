@@ -98,7 +98,7 @@ struct FcChainPlan {
     FormLayout forms[kFcForms];
     int sm_count = 0;
     int device = 0;
-    int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 plain launch, 1 dependent launch + wait, 2 independent launches
+    int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 and 1 dependent launch + wait, 2 independent launches
     struct TmapSlot { const void *ptr = nullptr; size_t n = 0; CUtensorMap map; };
     TmapSlot tmaps[4];                // tensor maps of the most recent (pointer, n) pairs: double/triple-buffered callers hit every time
     unsigned tmap_next = 0;
@@ -349,6 +349,16 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
             for (uint32_t off = 0; off < P.w_bytes; off += 32768)
                 bulk_load_1d(smem + P.off_w + off, P.w_image + off, min(32768u, P.w_bytes - off), &bar_w);
             if (!kFloatIn) {
+                // kFixed: the first tile of each of the CTA's four slots is prefetched into L2 ahead of the grid-dependency wait,
+                // so that the first loads after it do not wait on HBM.  A prefetch hands no data to the CTA: the loads below
+                // read the images through L2, the point of coherence that every write of an earlier kernel has reached once
+                // the wait returns.
+                if constexpr (kFixed) {
+                    for (uint32_t i = 0; i < min(my_tiles, (uint32_t)(kPipes * kSlots)); i++)
+#pragma unroll
+                        for (uint32_t a = 0; a < kFixedInAtoms; a++)
+                            tma_prefetch_l2_2d(&tmap_in, (int32_t)(a * 128), (int32_t)((tile0 + i * tile_step) * kTileM));
+                }
                 // everything else this kernel reads or writes may belong to the kernel launched before it
                 if (P.wait_prior_grid) asm volatile("griddepcontrol.wait;" ::: "memory");
                 const uint64_t l2_policy = policy_evict_first();   // images are read exactly once
@@ -1138,20 +1148,23 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void 
     cfg.dynamicSmemBytes = form.smem_bytes;
     cfg.stream = st;
     // Only the C engine's int8 form overlaps launches; every other form is a plain launch, ordered by the stream alone, whose
-    // grid-dependency wait returns at once.  Mode 2 drops the wait, i.e. EVERY ordering against the work enqueued before this
-    // launch on the stream (the previous bnm launch and any producer kernel of `images` alike).  The library keeps the wait
-    // whenever it can see the promise being broken: first launch on this plan / another stream / a buffer of the previous launch
-    // reused / a launch of another form in between.  A null output is no buffer: it neither reuses nor differs from one.
+    // grid-dependency wait returns at once.  The int8 form is always a programmatic dependent launch: modes 0 and 1 are one
+    // launch, whose CTAs take each SM as the kernel before them leaves it and run their prologue (barriers, setmaxnreg, weight
+    // copy) there, but read images and write results only after the grid-dependency wait -- ordinary stream semantics.
+    // Mode 2 drops the wait, i.e. EVERY ordering against the work enqueued before this launch on the stream (the previous bnm
+    // launch and any producer kernel of `images` alike).  The library keeps the wait whenever it can see the promise being
+    // broken: first launch on this plan / another stream / a buffer of the previous launch reused / a launch of another form
+    // in between.  A null output is no buffer: it neither reuses nor differs from one.
     const bool independent = engine_i8 && plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && in != plan->prev_in &&
                              (logits == nullptr || logits != plan->prev_logits) && (labels == nullptr || labels != plan->prev_labels);
     p.wait_prior_grid = !independent;
-    p.early_trigger = engine_i8 && plan->overlap != 0 && cfg.gridDim.x == (unsigned)plan->sm_count;
+    p.early_trigger = engine_i8 && cfg.gridDim.x == (unsigned)plan->sm_count;
     plan->prev_in = in; plan->prev_logits = logits; plan->prev_labels = labels; plan->prev_stream = st; plan->prev_valid = engine_i8;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = engine_i8 && plan->overlap ? 1 : 0;
+    cfg.numAttrs = engine_i8 ? 1 : 0;
     trace_before(st);
     if (cudaLaunchKernelEx(&cfg, form.kernel->fn, *tmap_p, p) != cudaSuccess) return -4;
     trace_after(st);

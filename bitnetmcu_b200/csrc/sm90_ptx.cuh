@@ -114,6 +114,11 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const void *tmap, in
                  ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
+// 2D tiled prefetch global -> L2 (no data reaches the CTA, no barrier)
+__device__ __forceinline__ void tma_prefetch_l2_2d(const void *tmap, int32_t c0, int32_t c1) {
+    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
+                 ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1) : "memory");
+}
 // same with an L2 cache-policy operand (createpolicy-style 64-bit hint)
 __device__ __forceinline__ void tma_load_2d_hint(void *smem_dst, const void *tmap, int32_t c0, int32_t c1, uint64_t *bar,
                                                  uint64_t policy) {

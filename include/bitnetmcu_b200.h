@@ -89,10 +89,10 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  * (wgmma, depthwise tail fed from shared memory) when the channel count is a multiple of 16 and <= 128, else the CUDA-core kernel;
  * 1 CUDA-core kernel; 2 tensor-core kernel or fail.  Results are identical. */
 /* BNM_OPT_LAUNCH_OVERLAP (fused kernel, consecutive bnm_infer_batch_device calls on one stream):
- *   0  (default) plain launches, ordinary stream semantics.
- *   1  programmatic dependent launch with a grid-dependency wait: the next launch's prologue (barriers, weights) runs
- *      under the tail of the previous one; inputs are read and outputs written only after the previous kernel has
- *      completed.  Ordinary stream semantics.
+ *   0  (default) ordinary stream semantics.  Each launch is a programmatic dependent launch with a grid-dependency wait:
+ *      its prologue (barriers, weights, an L2 prefetch of its first tiles) runs under the tail of the kernel before it;
+ *      inputs are read into the kernel and outputs written only after that kernel has completed.
+ *   1  the same as 0 (kept as a separate value for callers that set it).
  *   2  the caller declares consecutive launches independent -- the images / logits / labels of one call are not the
  *      buffers of the call right before it (e.g. double-buffered batches), exactly what issuing them on two streams would
  *      promise.  The next launch's tiles then start on each SM as the previous launch leaves it.
