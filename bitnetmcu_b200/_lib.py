@@ -22,6 +22,7 @@ EXPORTED = [
     "bnm_infer_batch_device_gather", "bnm_device_alloc", "bnm_device_free", "bnm_ipc_export", "bnm_ipc_open", "bnm_ipc_close",
     "bnm_enable_peer_access", "bnm_emulate_inference_quantized", "bnm_infer_batch_device_f32", "bnm_emulate_batch_device",
     "bnm_compare_engines_device",
+    "bnm_infer_topk", "bnm_infer_topk_device", "bnm_infer_topk_device_f32", "bnm_emulate_topk_device",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
@@ -35,6 +36,7 @@ class BnmLayer(C.Structure):
 
 
 MAX_GATHER_DST = 8
+MAX_TOPK = 16   # BNM_MAX_TOPK
 
 
 class BnmGather(C.Structure):
@@ -82,6 +84,10 @@ def load() -> C.CDLL:
         "bnm_emulate_batch_device": (C.c_int, [vp, vp, sz, vp, vp, vp]),
         "bnm_infer_batch_device_f32": (C.c_int, [vp, vp, sz, vp, vp, vp]),
         "bnm_compare_engines_device": (C.c_int, [vp, vp, sz, vp, vp, vp, vp, vp]),
+        "bnm_infer_topk": (C.c_int, [vp, vp, sz, u32, vp, vp]),
+        "bnm_infer_topk_device": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
+        "bnm_infer_topk_device_f32": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
+        "bnm_emulate_topk_device": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

@@ -83,6 +83,7 @@ struct PipeSlot {
     DevBuf<int32_t> d_logits;
     DevBuf<uint32_t> d_labels;
     DevBuf<int8_t> d_feat;   // CNN models: this slot's own feature buffer, so that the slots' chunks may overlap in time
+    DevBuf<uint32_t> d_classes;   // bnm_infer_topk: the chunk's classes (its scores go to d_logits)
 };
 
 struct bnm_model {
@@ -127,6 +128,8 @@ struct bnm_model {
     DevBuf<double> d_emul_out;
     DevBuf<int8_t> d_emul_rows;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
     DevBuf<uint32_t> d_engine_labels[2];   // bnm_compare_engines_device's two routes: C / emulator labels the caller does not take
+    DevBuf<double> d_topk_logits;   // bnm_emulate_topk_device's layer-by-layer route: the emulator's logits of a chunk
+    bool verbose = false;           // BNM_VERBOSE at model creation: the top-k entries name their route on every call
     int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
                                // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
 };
@@ -319,7 +322,8 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
             if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaStreamCreate failed"); break; }
     }
     if (rc != 0) { std::string keep = g_err; bnm_model_destroy(m); g_err = keep; return rc; }
-    if (getenv("BNM_VERBOSE")) {   // diagnostics: the kernels bnm_emulate_batch_device runs on the default path
+    m->verbose = getenv("BNM_VERBOSE") != nullptr;
+    if (m->verbose) {   // diagnostics: the kernels bnm_emulate_batch_device runs on the default path
         const EmulRoute r = emul_route(m);
         fprintf(stderr, "bitnetmcu_b200: emulator route: %s%s\n",
                 r == kEmulLayers ? "layer by layer" : r == kEmulFloatRow ? "fc_emul_kernel" :
@@ -990,6 +994,172 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
     }
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+}
+
+// -----------------------------------------------------------------------------------------------
+// Top-k (section 8): the k best classes of every image and their scores -- the classes ranked by logit, highest first, ties to the
+// lower class, so rank 0 is the label of the matching entry -- and no logits written anywhere.
+//   * FC models on the fused path: one launch of fc_topk_kernel, whose epilogue ranks the classes in registers;
+//   * CNN models on the fused path: the front-end into the feature scratch, then that kernel, in chunks of 2^20 images;
+//   * BNM_PATH_LAYERS and models without a fused plan: the layer-by-layer chain into its int32 scratch (the emulator: its float64
+//     logits into d_topk_logits), then k_topk_rows.
+// The float entry scales the images into d_f32_scratch first; the emulator runs its own front-end (scaling kernel or CNN
+// front-end) into d_emul_rows, then fc_topk_kernel with its rule.
+// -----------------------------------------------------------------------------------------------
+static int topk_check(const bnm_model *m, const char *fn, const void *images, size_t n, uint32_t k, const uint32_t *classes,
+                      const void *scores, uintptr_t score_align, uintptr_t image_align) {
+    if (!m || (n && (!images || !classes))) return fail(BNM_E_ARG, "%s: null argument", fn);
+    if (k < 1 || k > std::min<uint32_t>(m->n_classes, BNM_MAX_TOPK))
+        return fail(BNM_E_ARG, "%s: k = %u, must be 1 .. min(n_classes = %u, %d)", fn, k, m->n_classes, BNM_MAX_TOPK);
+    if ((uintptr_t)images & (image_align - 1)) return fail(BNM_E_ARG, "%s: the device image buffer must be %zu-byte aligned", fn, (size_t)image_align);
+    if ((uintptr_t)classes & 3) return fail(BNM_E_ARG, "%s: the classes buffer must be 4-byte aligned", fn);
+    if ((uintptr_t)scores & (score_align - 1)) return fail(BNM_E_ARG, "%s: the scores buffer must be %zu-byte aligned", fn, (size_t)score_align);
+    return 0;
+}
+
+// the kernels of the C engine's top-k on int8 images, for the route line
+static std::string topk_c_route(const bnm_model *m) {
+    std::string s;
+    if (m->model_class == BNM_MODEL_CNNMNIST)
+        s = m->cnn_frontend != 1 && cnn_frontend_tc_supported(m->channels, m->xy0) ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
+    if (bnm_model_active_path(m) == BNM_PATH_TCGEN05) return s + "fc_topk_kernel" + fc_chain_form_name(m->plan, kFormTopK);
+    return s + "layer by layer + k_topk_rows<int32>";
+}
+
+// the C engine's top-k of int8 images on st, arguments checked.  slot_feat as in infer_device_impl.
+static int topk_device_impl(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, cudaStream_t st,
+                            int8_t *slot_feat = nullptr) {
+    const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
+    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
+    if (fused && !cnn) {
+        const TopKOutputs out{k, classes, scores};
+        int rc = fc_chain_launch(m->plan, kFormTopK, images, n, nullptr, nullptr, 0, nullptr, st, nullptr, &out);
+        return rc ? fail(BNM_E_CUDA, "fused top-k kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
+    }
+    const size_t chunk = slot_feat ? n : std::min(n, fused ? kFusedCnnChunk : kLayeredChunk);
+    int rc = (slot_feat && fused) ? 0 : ensure_scratch(m, chunk, !fused);
+    if (rc) return rc;
+    int8_t *feat = slot_feat ? slot_feat : m->d_feat.p;
+    for (size_t b = 0; b < n; b += chunk) {
+        const size_t nb = std::min(chunk, n - b);
+        const TopKOutputs out{k, classes + b * k, scores ? scores + b * k : nullptr};
+        const int8_t *fc_in = images + b * m->img_bytes;
+        uint32_t fc_stride = m->img_bytes;
+        if (cnn) {
+            if ((rc = run_cnn_front(m, fc_in, nb, feat, st))) return rc;
+            fc_in = feat;
+            fc_stride = m->feat_stride;
+        }
+        if (fused) {
+            if ((rc = fc_chain_launch(m->plan, kFormTopK, fc_in, nb, nullptr, nullptr, 0, nullptr, st, nullptr, &out)))
+                return fail(BNM_E_CUDA, "fused top-k kernel launch failed (%d)", rc);
+        } else {
+            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, nullptr, nullptr, st))) return rc;   // last layer's accumulators in d_acc
+            launch_topk_rows(m->d_acc.p, m->n_classes, k, out.classes, static_cast<int32_t *>(out.scores), nb, st);
+        }
+    }
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+}
+
+extern "C" int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
+    if (int rc = topk_check(m, "bnm_infer_topk_device", images, n, k, classes, scores, 4, 16)) return rc;
+    if (n == 0) return 0;
+    CU_TRY(cudaSetDevice(m->device));
+    if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk_device: %s\n", topk_c_route(m).c_str());
+    return topk_device_impl(m, images, n, k, classes, scores, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
+    if (int rc = topk_check(m, "bnm_infer_topk_device_f32", images, n, k, classes, scores, 4, 16)) return rc;
+    if (n == 0) return 0;
+    CU_TRY(cudaSetDevice(m->device));
+    if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk_device_f32: k_quantize_images + %s\n", topk_c_route(m).c_str());
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t chunk = std::min(n, kFusedCnnChunk), elems = m->img_bytes;
+    CU_TRY(m->d_f32_scratch.grow(chunk * elems));
+    for (size_t b = 0; b < n; b += chunk) {
+        const size_t nb = std::min(chunk, n - b);
+        launch_quantize_images(images + b * elems, (uint32_t)elems, m->d_f32_scratch.p, nb, st);
+        if (int rc = topk_device_impl(m, m->d_f32_scratch.p, nb, k, classes + b * k, scores ? scores + b * k : nullptr, st)) return rc;
+    }
+    return 0;
+}
+
+extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, double *scores, void *stream) {
+    if (int rc = topk_check(m, "bnm_emulate_topk_device", images, n, k, classes, scores, 8, 16)) return rc;
+    if (n == 0) return 0;
+    CU_TRY(cudaSetDevice(m->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
+    const size_t elems = m->img_bytes, ncls = m->n_classes;
+    if (emul_route(m) != kEmulLayers) {
+        if (m->verbose)
+            fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: %s + fc_topk_kernel%s\n",
+                    cnn ? "k_cnn_emul_frontend" : "k_quantize_images", fc_chain_form_name(m->plan, kFormEmulTopK));
+        const int out_shift = level_shift_of(m->fc.back().enc);
+        const size_t chunk = std::min(n, kFusedCnnChunk);
+        CU_TRY(m->d_emul_rows.grow(chunk * (cnn ? m->feat_stride : elems)));
+        int8_t *rows = m->d_emul_rows.p;
+        for (size_t b = 0; b < n; b += chunk) {
+            const size_t nb = std::min(chunk, n - b);
+            if (!cnn) launch_quantize_images(images + b * elems, (uint32_t)elems, rows, nb, st);   // BitNetMCU.py:435-436
+            else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, m->channels, rows, m->feat_stride, nb, st))
+                return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
+            const TopKOutputs out{k, classes + b * k, scores ? scores + b * k : nullptr};
+            int rc = fc_chain_launch(m->plan, kFormEmulTopK, rows, nb, nullptr, nullptr, out_shift, nullptr, st, nullptr, &out);
+            if (rc) return fail(BNM_E_CUDA, "fused emulator top-k kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+        }
+    } else {
+        if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: layer by layer + k_topk_rows<double>\n");
+        const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
+        CU_TRY(m->d_topk_logits.grow(chunk * ncls * sizeof(double)));
+        for (size_t b = 0; b < n; b += chunk) {
+            const size_t nb = std::min(chunk, n - b);
+            if (int rc = emulate_device(m, images + b * elems, nb, m->d_topk_logits.p, nullptr, st)) return rc;
+            launch_topk_rows(m->d_topk_logits.p, (uint32_t)ncls, k, classes + b * k, scores ? scores + b * k : nullptr, nb, st);
+        }
+    }
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+}
+
+// host buffers: the chunked pipeline of bnm_infer_batch, k classes (and k scores) per image copied back
+extern "C" int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores) {
+    if (int rc = topk_check(m, "bnm_infer_topk", images, n, k, classes, scores, 1, 1)) return rc;
+    if (n == 0) return 0;
+    CU_TRY(cudaSetDevice(m->device));
+    if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk: %s\n", topk_c_route(m).c_str());
+    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
+    const size_t chunk = std::min(n, m->chunk_images), out_bytes = chunk * k * sizeof(uint32_t);
+    bool small = false;
+    for (auto &s : m->slots)
+        small = small || s.d_images.bytes < chunk * m->img_bytes || s.d_classes.bytes < out_bytes || (scores && s.d_logits.bytes < out_bytes) ||
+                (cnn && s.d_feat.bytes < chunk * m->feat_stride);
+    if (small) {
+        CU_TRY(cudaDeviceSynchronize());   // no chunk of an earlier call may still use a buffer that is reallocated
+        for (auto &s : m->slots) {
+            if (cnn) CU_TRY(s.d_feat.grow(chunk * (size_t)m->feat_stride, true));
+            CU_TRY(s.d_images.grow(chunk * (size_t)m->img_bytes));
+            CU_TRY(s.d_classes.grow(out_bytes));
+            if (scores) CU_TRY(s.d_logits.grow(out_bytes));   // the scores of a chunk: k <= n_classes int32 per image
+        }
+    }
+    // as in bnm_infer_batch: the layer-by-layer path's shared scratch allows one stream, the fused path takes all three
+    const bool shared_scratch = bnm_model_active_path(m) != BNM_PATH_TCGEN05;
+    size_t c = 0;
+    for (size_t b = 0; b < n; b += chunk, c++) {
+        const size_t nb = std::min(chunk, n - b);
+        PipeSlot &s = m->slots[shared_scratch ? 0 : c % 3];
+        CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
+        int rc = topk_device_impl(m, s.d_images.p, nb, k, s.d_classes.p, scores ? s.d_logits.p : nullptr, s.stream,
+                                  shared_scratch ? nullptr : s.d_feat.p);
+        if (rc) return rc;
+        CU_TRY(cudaMemcpyAsync(classes + b * k, s.d_classes.p, nb * k * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
+        if (scores) CU_TRY(cudaMemcpyAsync(scores + b * k, s.d_logits.p, nb * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
+    }
+    for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
+    return 0;
 }
 
 // -----------------------------------------------------------------------------------------------

@@ -77,6 +77,12 @@ struct ChainParams {
     uint32_t *labels_py;
     const uint32_t *truth;
     unsigned long long *counts;
+    // top-k launches (fc_topk_kernel): the k best classes of every row, uint32 [n][k], and their logits, int32 [n][k] (C engine)
+    // or float64 [n][k] (emulator: accumulators x emul_logit_scale), or null; no logits, no labels, no result exchange
+    uint32_t k;
+    uint32_t *classes;
+    int32_t *scores_i32;
+    double *scores_f64;
 };
 
 struct ChainKernel;
@@ -285,14 +291,18 @@ struct RingPos {
 // logits (P.emul_logits); no result exchange.
 // kEngines: both engines on one tile (fc_engines_kernel): layer 1 once, its accumulators through both hidden-layer rules, the C
 // chain and then the emulator's chain, both labels and their EngineTally counts; no logits, no result exchange.
+// kTopK: the k best classes of every row and their scores (fc_topk_kernel) in place of logits and label: k rounds of the
+// epilogue's argmax, each over the columns ranked below the previous round's pick.
 // The body of the kernels below; tmap_in and P are their __grid_constant__ parameters (TMA reads the tensor map by address).
-template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, bool kEmul, bool kEngines = false>
+template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, bool kEmul, bool kEngines = false, bool kTopK = false>
 __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const ChainParams &P) {
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
     static_assert(!kEmul || (kPipes == 1 && kSlots == 1 && kLastN == kN && !kFixed && (kN == 64 || !kFloatIn)),
                   "emulator: the 64-wide float-input launch, or one-pipe one-slot int8 launches at full width");
     static_assert(!kEngines || (kN == 64 && kPipes == 1 && kFloatIn && kSlots == 1 && kLastN == kN && !kFixed && !kEmul),
                   "both engines: the 64-wide float-input launch");
+    static_assert(!kTopK || (kPipes == 1 && kSlots == 1 && !kFloatIn && kLastN == kN && !kFixed && !kEngines),
+                  "top-k: one-pipe one-slot int8 launches at full width");
     static_assert(!kFloatIn || kPipes == 1, "float input: one pipe, whose stages the quantiser warps fill");
     static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
     static_assert(!kFixed || (kSlots == 2 && kLastN == fixed_n_pad(kFixedLayers - 1)), "fixed shape: two-slot launches of its class");
@@ -515,6 +525,56 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                         wgmma_rs_n64(a + c0 / 2, f + 4 * k, b_desc((uint32_t)c0 < n_pad ? bt : w_zero, c0), (pl | k) != 0);
                 }
         };
+        // ---- kTopK: the k best classes of tile i and their scores from the last layer's accumulators a, in place of the epilogue
+        // below.  k rounds of its argmax: round 0 is that argmax; round t > 0 takes the first maximum of the columns ranked after
+        // round t - 1's pick (v, p) -- x < v, or x == v at a column >= q = p + 1.  So the picks are the row's classes by logit,
+        // highest first, ties to the lower class (np.argsort(-x, kind="stable")), with no exclusion mask: (v, q) per row is all the
+        // state.  Rounds t > 0 start from INT32_MIN, below every logit (|logit| <= 1024 x 127 x 255 < 2^25).  Quad lane t % 4
+        // keeps round t's pick; after every fourth round and after the last, the quad stores its picks: up to four consecutive
+        // classes (and scores) of the row, 16 contiguous bytes.
+        auto topk_epilogue = [&](const uint32_t *a, uint32_t i) {
+            const uint32_t tile = tile0 + i * tile_step;
+            const uint32_t k = P.k;
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                const size_t img = (size_t)tile * kTileM + row_in_tile + 8 * r;
+                int v = INT32_MAX;
+                uint32_t q = 0;
+                uint32_t my_cls = 0;
+                int my_score = 0;
+#pragma unroll 1
+                for (uint32_t t = 0; t < k; t++) {
+                    int best = t ? INT32_MIN : -INT32_MAX;
+                    uint32_t pos = 255;
+#pragma unroll
+                    for (int j = 0; j < kLastN / 8; j++)
+#pragma unroll
+                        for (int e = 0; e < 2; e++) {
+                            const uint32_t col = 8 * j + 2 * quad + e;
+                            const int x = (int)a[4 * j + 2 * r + e];
+                            if (col < ncls && (x < v || (x == v && col >= q)) && x > best) { best = x; pos = col; }
+                        }
+#pragma unroll
+                    for (int sh = 1; sh <= 2; sh <<= 1) {
+                        const int ob = __shfl_xor_sync(0xffffffffu, best, sh);
+                        const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, sh);
+                        if (ob > best || (ob == best && op < pos)) { best = ob; pos = op; }
+                    }
+                    v = best;
+                    q = pos + 1;
+                    if (quad == (t & 3)) { my_cls = pos; my_score = best; }
+                    if (((t & 3) == 3 || t + 1 == k) && img < P.n && quad <= (t & 3)) {
+                        const size_t o = img * k + (t & ~3u) + quad;
+                        P.classes[o] = my_cls;
+                        if constexpr (kEmul) {
+                            if (P.scores_f64) P.scores_f64[o] = (double)my_score * P.emul_logit_scale;   // exact, as the logits
+                        } else {
+                            if (P.scores_i32) P.scores_i32[o] = my_score;
+                        }
+                    }
+                }
+            }
+        };
         // ---- logits + label of tile i from the last layer's accumulators a (dll.c:115-116: the last ReLUNorm's argmax is what
         // Inference() returns).  argmax = first maximum (strict '>' from -INT32_MAX, pos 255, inference.c:32-37): in column order
         // per thread, then over the quad.  The last layer has at most kLastN columns.
@@ -696,7 +756,8 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                         BNM_TRACE(TR_WAIT_END, 0, l + 1);
                         continue;
                     }
-                    epilogue(acc[0], i);
+                    if constexpr (kTopK) topk_epilogue(acc[0], i);
+                    else epilogue(acc[0], i);
                     BNM_TRACE(TR_EPI_END, 0, 0);
                     break;
                 }
@@ -864,6 +925,14 @@ fc_engines_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
     fc_chain_body<64, 1, true, 1, 64, false, false, true>(tmap_in, P);
 }
 
+// Top-k on int8 rows: the chain of fc_chain_kernel (kEmul false) or of fc_emul_i8_kernel (true) on one pipe and one slot at the
+// full width kN, with an epilogue that writes the k best classes of every row and their scores instead of logits and label.
+template <int kN, bool kEmul>
+__global__ void __launch_bounds__(chain_threads<kN, 1, false, 1>(), 1)
+fc_topk_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<kN, 1, false, 1, kN, false, kEmul, false, true>(tmap_in, P);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -907,8 +976,8 @@ static void trace_before(cudaStream_t) {}
 static void trace_after(cudaStream_t) {}
 #endif
 
-// the instantiations of fc_chain_kernel, fc_emul_kernel, fc_emul_i8_kernel and fc_engines_kernel, one row each, named by their
-// template arguments <kN, kPipes, kSlots, kLastN>
+// the instantiations of fc_chain_kernel, fc_emul_kernel, fc_emul_i8_kernel, fc_engines_kernel and fc_topk_kernel, one row each,
+// named by their template arguments <kN, kPipes, kSlots, kLastN>
 struct ChainKernel {
     const char *name;
     void (*fn)(CUtensorMap, ChainParams);
@@ -920,11 +989,15 @@ static ChainKernel chain_kernel(const char *name) {
 }
 template <int kN>
 static ChainKernel emul_i8_kernel(const char *name) { return {name, fc_emul_i8_kernel<kN>, chain_threads<kN, 1, false, 1>()}; }
+template <int kN, bool kEmul>
+static ChainKernel topk_kernel(const char *name) { return {name, fc_topk_kernel<kN, kEmul>, chain_threads<kN, 1, false, 1>()}; }
 enum ChainRow {
     kRow64, kRow64x2, kRow64x2Last16, kRowFixed, kRow128, kRow192, kRow256, kRowFloat,
     kRowEmulFloat,
     kRowEmul64, kRowEmul128, kRowEmul192, kRowEmul256,   // row kRowEmul64 + max_n / 64 - 1
     kRowEngines,
+    kRowTopK64, kRowTopK128, kRowTopK192, kRowTopK256,   // likewise from kRowTopK64 / kRowEmulTopK64
+    kRowEmulTopK64, kRowEmulTopK128, kRowEmulTopK192, kRowEmulTopK256,
     kChainRows
 };
 static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
@@ -943,6 +1016,14 @@ static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
     t[kRowEmul192] = emul_i8_kernel<192>("<192,1,emul>");
     t[kRowEmul256] = emul_i8_kernel<256>("<256,1,emul>");
     t[kRowEngines] = {"<64,1,float,engines>", fc_engines_kernel, chain_threads<64, 1, true, 1>()};
+    t[kRowTopK64] = topk_kernel<64, false>("<64,1,topk>");
+    t[kRowTopK128] = topk_kernel<128, false>("<128,1,topk>");
+    t[kRowTopK192] = topk_kernel<192, false>("<192,1,topk>");
+    t[kRowTopK256] = topk_kernel<256, false>("<256,1,topk>");
+    t[kRowEmulTopK64] = topk_kernel<64, true>("<64,1,emul,topk>");
+    t[kRowEmulTopK128] = topk_kernel<128, true>("<128,1,emul,topk>");
+    t[kRowEmulTopK192] = topk_kernel<192, true>("<192,1,emul,topk>");
+    t[kRowEmulTopK256] = topk_kernel<256, true>("<256,1,emul,topk>");
     return t;
 }();
 
@@ -1015,6 +1096,9 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     }
     // the emulator on int8 rows runs one pipe at every width, so a 64-wide plan, whose int8 form runs two, has its own layout
     forms[kFormEmulInt8] = layout(kRowEmul64 + max_n / 64 - 1, 1, 6, 0);
+    // top-k forms: the same one-pipe layout, for either rule
+    forms[kFormTopK] = layout(kRowTopK64 + max_n / 64 - 1, 1, 6, 0);
+    forms[kFormEmulTopK] = layout(kRowEmulTopK64 + max_n / 64 - 1, 1, 6, 0);
     if (getenv("BNM_VERBOSE")) {   // diagnostics: the shapes this plan launches
         const bool has_float = forms[kFormFloat].kernel;
         char f_stages[32] = "";
@@ -1025,6 +1109,9 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
                 has_float ? forms[kFormFloat].kernel->name : "", has_float ? ", emulator " : "",
                 has_float ? forms[kFormEmulFloat].kernel->name : "", f_stages, forms[kFormEmulInt8].kernel->name,
                 forms[kFormEmulInt8].n_stages);
+        fprintf(stderr, "bitnetmcu_b200: fused FC top-k forms: fc_topk_kernel%s x %u stages, emulator fc_topk_kernel%s x %u stages, %zu B smem\n",
+                forms[kFormTopK].kernel->name, forms[kFormTopK].n_stages, forms[kFormEmulTopK].kernel->name, forms[kFormEmulTopK].n_stages,
+                forms[kFormTopK].smem_bytes);
     }
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
@@ -1098,18 +1185,27 @@ const char *fc_chain_form_name(const FcChainPlan *plan, FcForm f) { return plan-
 static const CUtensorMap kNoTensorMap{};   // the float-input forms' tensor map: not used (no TMA image loads)
 
 int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
-                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines) {
+                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines, const TopKOutputs *topk) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
     const FormLayout &form = plan->forms[f];
     if (!form.kernel) return -6;
     if ((f == kFormEngines) != (engines != nullptr) || (engines && logits)) return -5;
+    const bool topk_form = f == kFormTopK || f == kFormEmulTopK;
+    if (topk_form != (topk != nullptr) || (topk && (logits || labels || !topk->classes || topk->k == 0 || topk->k > plan->p.n_classes)))
+        return -5;
     const bool engine_i8 = f == kFormInt8, float_in = f == kFormFloat || f == kFormEmulFloat || f == kFormEngines;
     ChainParams p = plan->p;   // the model's shapes; null outputs, no result exchange
     p.n_stages = form.n_stages;
     p.off_w = form.off_w;
     p.off_fring = form.off_fring;
-    if (f == kFormEmulFloat || f == kFormEmulInt8) {
+    if (topk) {
+        p.k = topk->k;
+        p.classes = topk->classes;
+        if (f == kFormEmulTopK) p.scores_f64 = static_cast<double *>(topk->scores);
+        else p.scores_i32 = static_cast<int32_t *>(topk->scores);
+    }
+    if (f == kFormEmulFloat || f == kFormEmulInt8 || f == kFormEmulTopK) {
         p.emul_logits = static_cast<double *>(logits);
         p.emul_logit_scale = level_shift ? 0.5 : 1.0;
     } else {

@@ -373,6 +373,51 @@ void launch_emul_logits(const int32_t *acc, uint32_t n_cls, int level_shift, dou
     if (n && n_cls) k_emul_logits<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(acc, n_cls, level_shift ? 0.5 : 1.0, logits, labels, n);
 }
 
+// Top-k of the layer-by-layer routes: one warp per row, k rounds.  Round t takes the first maximum of the columns ranked after
+// round t - 1's pick (v, p) -- x < v, or x == v at a column > p; round 0 takes every column -- by a strided scan and a shfl.xor
+// reduction, as fc_topk_kernel's epilogue does over its quads.  Lane t % 32 keeps round t's pick and stores it with the others
+// after every 32nd and the last round.
+template <class T>
+__global__ void __launch_bounds__(256) k_topk_rows(const T *__restrict__ rows, uint32_t n_cls, uint32_t k, uint32_t *__restrict__ classes,
+                                                   T *__restrict__ scores, size_t n) {
+    constexpr uint32_t kNone = 0xffffffffu;
+    const uint32_t lane = threadIdx.x & 31;
+    const size_t row = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= n) return;
+    const T *x = rows + row * n_cls;
+    T v = 0, my_score = 0;
+    uint32_t p = kNone, my_cls = 0;
+    for (uint32_t t = 0; t < k; t++) {
+        T best = 0;
+        uint32_t pos = kNone;
+        for (uint32_t i = lane; i < n_cls; i += 32) {
+            const T y = x[i];
+            if ((p == kNone || y < v || (y == v && i > p)) && (pos == kNone || y > best)) { best = y; pos = i; }
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            const T ob = __shfl_xor_sync(0xffffffffu, best, off);
+            const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, off);
+            if (op != kNone && (pos == kNone || ob > best || (ob == best && op < pos))) { best = ob; pos = op; }
+        }
+        v = best;
+        p = pos;
+        if (lane == (t & 31)) { my_cls = pos; my_score = best; }
+        if (((t & 31) == 31 || t + 1 == k) && lane <= (t & 31)) {
+            const size_t o = row * k + (t & ~31u) + lane;
+            classes[o] = my_cls;
+            if (scores) scores[o] = my_score;
+        }
+    }
+}
+
+void launch_topk_rows(const int32_t *rows, uint32_t n_cls, uint32_t k, uint32_t *classes, int32_t *scores, size_t n, cudaStream_t st) {
+    if (n) k_topk_rows<int32_t><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(rows, n_cls, k, classes, scores, n);
+}
+void launch_topk_rows(const double *rows, uint32_t n_cls, uint32_t k, uint32_t *classes, double *scores, size_t n, cudaStream_t st) {
+    if (n) k_topk_rows<double><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(rows, n_cls, k, classes, scores, n);
+}
+
 void launch_relunorm_emul(const int32_t *in, uint32_t n_in, int level_shift, int8_t *out, uint32_t out_stride, size_t n, cudaStream_t st) {
     if (n) k_relunorm_emul<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(in, n_in, level_shift, out, out_stride, n);
 }

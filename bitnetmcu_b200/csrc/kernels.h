@@ -75,6 +75,10 @@ void launch_i32_to_i8(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t ou
 // the last layer's int32 accumulators [n][n_cls] -> float64 logits x 2^-level_shift and first-maximum labels (np.argmax); either
 // output may be null
 void launch_emul_logits(const int32_t *acc, uint32_t n_cls, int level_shift, double *logits, uint32_t *labels, size_t n, cudaStream_t st);
+// top-k of rows [n][n_cls] (int32 or float64) -> classes uint32 [n][k] and scores [n][k] (may be null): the classes by value,
+// highest first, ties to the lower class; 1 <= k <= n_cls
+void launch_topk_rows(const int32_t *rows, uint32_t n_cls, uint32_t k, uint32_t *classes, int32_t *scores, size_t n, cudaStream_t st);
+void launch_topk_rows(const double *rows, uint32_t n_cls, uint32_t k, uint32_t *classes, double *scores, size_t n, cudaStream_t st);
 
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
@@ -118,8 +122,10 @@ void fc_chain_plan_set_overlap(FcChainPlan *p, int mode);
 //   kFormEmulInt8   the emulator on int8 rows [n][in_bytes] that are already scaled (fc_emul_i8_kernel), every plan
 //   kFormEngines    both engines on float32 images (fc_engines_kernel): one input scaling and one layer 1, then the C engine's
 //                   and the emulator's hidden layers; both labels and the EngineTally counts, no logits.  The plans with kFormFloat
+//   kFormTopK       the C engine on int8 images, the k best classes of every row and their int32 logits (fc_topk_kernel), every plan
+//   kFormEmulTopK   the same with the emulator's rule and float64 scores, every plan
 // The emulator forms have the emulator's hidden-layer rule and float64 logits = last layer's accumulators x 2^-level_shift (0 or 1).
-enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFormEngines, kFcForms };
+enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFormEngines, kFormTopK, kFormEmulTopK, kFcForms };
 bool fc_chain_has_form(const FcChainPlan *p, FcForm f);
 // the template arguments of the kernel of a form the plan has, e.g. "<192,1,emul>"
 const char *fc_chain_form_name(const FcChainPlan *p, FcForm f);
@@ -130,12 +136,19 @@ struct EngineOutputs {
     const uint32_t *truth;
     unsigned long long *counts;
 };
+// top-k form outputs: k (1 .. n_classes) classes uint32 [n][k], required, and their scores [n][k] (int32, float64 for kFormEmulTopK)
+// or null
+struct TopKOutputs {
+    uint32_t k;
+    uint32_t *classes;
+    void *scores;
+};
 // one launch of form f on n images `in` -> logits (int32 [n][n_classes], float64 for the emulator forms) and labels uint32 [n];
 // each may be null.  gather (kFormInt8 only, may be null): extra destination buffers every row is also stored to (peer memory),
-// fused into the epilogue.  engines: kFormEngines only, and required there (no logits).  0, or a negative code (-6: the plan
-// has no form f)
+// fused into the epilogue.  engines: kFormEngines only, and required there (no logits).  topk: the top-k forms only, and required
+// there (no logits, no labels).  0, or a negative code (-6: the plan has no form f)
 int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
-                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines = nullptr);
+                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines = nullptr, const TopKOutputs *topk = nullptr);
 // the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
 // [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
 constexpr uint32_t kCnnEmulMaxChannels = 128;

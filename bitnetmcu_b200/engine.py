@@ -178,6 +178,58 @@ class Engine:
                                                        self._labels_ptr(labels_c, n), self._labels_ptr(labels_py, n), cp,
                                                        C.c_void_p(stream)), "bnm_compare_engines_device")
 
+    # ---- top-k: each image's k best classes and their scores (include/bitnetmcu_b200.h section 8) ------------------------------
+    # Classes are ranked by logit, highest first, ties to the lower class: np.argsort(-logits, kind="stable")[:, :k].  Rank 0 is
+    # the label of the matching entry.  1 <= k <= min(n_classes, 16).
+    def topk(self, images: np.ndarray, k: int, want_scores: bool = True) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+        """images int8 [n, img_bytes] (host) -> (classes uint32 [n, k], scores int32 [n, k] = the C engine's logits of those
+        classes, or None with ``want_scores=False``).  No logits are written or copied back."""
+        imgs = np.ascontiguousarray(images, dtype=np.int8).reshape(-1, self.img_bytes)
+        n = imgs.shape[0]
+        classes = np.empty((n, k), dtype=np.uint32)
+        scores = np.empty((n, k), dtype=np.int32) if want_scores else None
+        _lib.check(self.lib.bnm_infer_topk(self.handle, _ptr(imgs), n, int(k), _ptr(classes), _ptr(scores)), "bnm_infer_topk")
+        return classes, scores
+
+    @staticmethod
+    def _topk_ptrs(images, k: int, classes, scores, score_dtype):
+        """the pointer arguments of a top-k device call: classes [n, k] (4-byte elements), scores [n, k] of score_dtype or None"""
+        n = images.shape[0]
+        assert images.is_contiguous() and images.dim() == 2
+        assert classes.is_contiguous() and classes.element_size() == 4 and tuple(classes.shape) == (n, k)
+        sp = None
+        if scores is not None:
+            assert scores.is_contiguous() and scores.dtype == score_dtype and tuple(scores.shape) == (n, k)
+            sp = C.c_void_p(scores.data_ptr())
+        return C.c_void_p(images.data_ptr()), n, C.c_void_p(classes.data_ptr()), sp
+
+    def _topk_device(self, fn, what, images, in_dtype, k, classes, scores, score_dtype, stream):
+        import torch
+        if stream is None:
+            stream = torch.cuda.current_stream(images.device).cuda_stream
+        assert images.dtype == in_dtype and images.shape[1] == self.img_bytes
+        ip, n, cp, sp = self._topk_ptrs(images, k, classes, scores, score_dtype)
+        _lib.check(fn(self.handle, ip, n, int(k), cp, sp, C.c_void_p(stream)), what)
+
+    def topk_device(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
+        """images torch.int8 [n, img_bytes] on this GPU -> classes [n, k] (torch.int32 / uint32) and scores torch.int32 [n, k] or
+        None.  Asynchronous on ``stream`` (a cudaStream_t as int; default: torch's current stream)."""
+        import torch
+        self._topk_device(self.lib.bnm_infer_topk_device, "bnm_infer_topk_device", images, torch.int8, k, classes, scores, torch.int32, stream)
+
+    def topk_device_f32(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
+        """``topk_device`` on torch.float32 [n, img_bytes] images, scaled to int8 as ``infer_device_f32`` does."""
+        import torch
+        self._topk_device(self.lib.bnm_infer_topk_device_f32, "bnm_infer_topk_device_f32", images, torch.float32, k, classes, scores,
+                          torch.int32, stream)
+
+    def emulate_topk_device(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
+        """The emulator's top-k: images torch.float32 [n, img_bytes] -> classes [n, k] and scores torch.float64 [n, k] (the
+        logits ``inference_quantized_device`` writes, at those classes) or None."""
+        import torch
+        self._topk_device(self.lib.bnm_emulate_topk_device, "bnm_emulate_topk_device", images, torch.float32, k, classes, scores,
+                          torch.float64, stream)
+
     def infer_tensor(self, images, want_logits: bool = True):
         """images: torch.int8 [n, img_bytes] on this engine's GPU -> (logits torch.int32 [n, n_classes], labels torch.int32 [n]) on
         the same GPU, asynchronous on torch's current stream (device memory end to end; plumbing for ``dist.sharded_infer``).

@@ -16,6 +16,7 @@
  *   /root/reference/test_inference.py:136-150): millions of 16x16 int8 images per call.
  * Section 4 exposes the four kernels batched, for parity tests and partial integration.
  * Sections 5 to 7 take float images: the C engine (5), the reference's Python emulator (6), and both at once, scored (7).
+ * Section 8 returns each image's k best classes and their scores (top-k) from either engine.
  *
  * Pointers are plain host (or, where the name says _device, CUDA device) pointers; sizes are element
  * counts unless named *_bytes.  All-integer arithmetic: results are bit-exact with the reference.
@@ -257,6 +258,32 @@ typedef struct bnm_engine_counts {
  * not overlap in time on different streams. */
 BNM_API int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth,
                                        uint32_t *labels_c, uint32_t *labels_py, bnm_engine_counts *counts, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 8. Top-k: each image's k best classes and their scores, between the label (section 3) and the whole logits row.  What
+ *    top-k accuracy and ranked predictions need, without writing or copying n_classes logits per image.
+ * ------------------------------------------------------------------------------------------- */
+#define BNM_MAX_TOPK 16
+/* Order: the classes of a row ranked by logit, highest first, ties to the lower class index -- np.argsort(-logits,
+ * kind="stable")[:, :k].  Rank 0 is exactly the label of the matching entry: the C engine's first maximum (Inference()), or
+ * np.argmax of the emulator's logits.
+ * k: 1 <= k <= min(n_classes, BNM_MAX_TOPK), anything else is BNM_E_ARG.  classes: uint32 [n][k], required (BNM_E_ARG when NULL).
+ * scores: the logits of those classes [n][k], or NULL: int32 = layer_out after the last processfclayer (the C engine), float64 =
+ * what bnm_emulate_batch_device writes as logits (the emulator).  No logits are written anywhere.  n == 0 returns 0 and writes
+ * nothing.  Device entries: device memory on the model's GPU, images 16-byte, classes 4-byte, float64 scores 8-byte aligned,
+ * asynchronous on `stream` (NULL = default stream), no host synchronisation once the model's scratch has grown.
+ * On the fused path, FC models run ONE kernel (bnm_infer_topk_device): the int8 chain of bnm_infer_batch_device on one pipe, whose
+ * epilogue ranks each row's logits in registers.  CNN models run the front-end selected by BNM_OPT_CNN_FRONTEND, then that kernel,
+ * in chunks of 2^20 images.  BNM_PATH_LAYERS and models without a fused plan run the layer-by-layer chain, then a ranking kernel.
+ * The float entry scales the images first (the scaling kernel into the model's scratch, chunks of 2^20), then takes the int8
+ * route; the emulator takes the scaling kernel (FC) or its CNN front-end (CNN up to 128 channels), then the kernel with the
+ * emulator's rule, else its layer-by-layer route.  Every route but the first uses scratch the model owns: calls on one model
+ * must not overlap in time on different streams.  A top-k launch is an ordinary stream-ordered launch (no BNM_OPT_LAUNCH_OVERLAP
+ * mode 2, no result exchange). */
+BNM_API int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores);   /* host buffers */
+BNM_API int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream);
+BNM_API int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream);
+BNM_API int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, double *scores, void *stream);
 
 #ifdef __cplusplus
 }
