@@ -95,6 +95,31 @@ struct FormLayout {
     size_t smem_bytes = 0;                 // dynamic shared memory
 };
 
+// the device buffers one int8-form launch reads or writes, for the mode-2 check: images, logits and labels (null: none), and the
+// gather destinations, which it writes from row row0 on
+struct LaunchBuffers {
+    const void *io[3] = {};
+    const void *dst[2 * kMaxGatherDst] = {};
+    uint32_t n_dst = 0;
+    size_t row0 = 0;
+};
+
+// Does launch b touch a buffer of launch a?  Any non-null pointer of one equal to any of the other, whatever the roles, except
+// that a destination both write counts only at the same row offset: the exchange's callers write their own rows of a shared
+// destination, which the library cannot tell from overlapping ones (the caller's promise, like any aliasing at an offset).
+static bool shares_buffer(const LaunchBuffers &a, const LaunchBuffers &b) {
+    auto seen = [](const void *x, const void *const *set, uint32_t n) {
+        for (uint32_t i = 0; i < n; i++)
+            if (x && x == set[i]) return true;
+        return false;
+    };
+    for (const void *x : b.io)
+        if (seen(x, a.io, 3) || seen(x, a.dst, a.n_dst)) return true;
+    for (uint32_t i = 0; i < b.n_dst; i++)
+        if (seen(b.dst[i], a.io, 3) || (a.row0 == b.row0 && seen(b.dst[i], a.dst, a.n_dst))) return true;
+    return false;
+}
+
 struct FcChainPlan {
     ChainParams p{};
     uint8_t *d_w_image = nullptr;
@@ -109,10 +134,11 @@ struct FcChainPlan {
     TmapSlot tmaps[4];                // tensor maps of the most recent (pointer, n) pairs: double/triple-buffered callers hit every time
     unsigned tmap_next = 0;
     // mode 2 bookkeeping: the buffers of the previous launch on this plan (the promise "consecutive launches are independent" is
-    // checked as far as the library can see it: a launch that reuses a buffer of the one before keeps the grid-dependency wait)
-    const void *prev_in = nullptr, *prev_logits = nullptr, *prev_labels = nullptr;
+    // checked as far as the library can see it: a launch that touches a buffer of the one before keeps the grid-dependency wait)
+    LaunchBuffers prev;
     cudaStream_t prev_stream = nullptr;
     bool prev_valid = false;
+    bool verbose = false;             // BNM_VERBOSE at plan creation: every int8-form launch names its wait decision
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -1113,6 +1139,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
                 forms[kFormTopK].kernel->name, forms[kFormTopK].n_stages, forms[kFormEmulTopK].kernel->name, forms[kFormEmulTopK].n_stages,
                 forms[kFormTopK].smem_bytes);
     }
+    plan->verbose = getenv("BNM_VERBOSE") != nullptr;
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
     plan->device = device;
@@ -1249,13 +1276,21 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void 
     // copy) there, but read images and write results only after the grid-dependency wait -- ordinary stream semantics.
     // Mode 2 drops the wait, i.e. EVERY ordering against the work enqueued before this launch on the stream (the previous bnm
     // launch and any producer kernel of `images` alike).  The library keeps the wait whenever it can see the promise being
-    // broken: first launch on this plan / another stream / a buffer of the previous launch reused / a launch of another form
-    // in between.  A null output is no buffer: it neither reuses nor differs from one.
-    const bool independent = engine_i8 && plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && in != plan->prev_in &&
-                             (logits == nullptr || logits != plan->prev_logits) && (labels == nullptr || labels != plan->prev_labels);
+    // broken: first launch on this plan / another stream / a buffer of the previous launch touched again, in any role (one
+    // launch's logits the next one's images, say) / a launch of another form in between.  A null output is no buffer: it
+    // neither reuses nor differs from one.
+    LaunchBuffers bufs;
+    bufs.io[0] = in; bufs.io[1] = logits; bufs.io[2] = labels;
+    if (gather) {
+        for (uint32_t d = 0; d < p.n_lab_dst; d++) bufs.dst[bufs.n_dst++] = p.lab_dst[d];
+        for (uint32_t d = 0; d < p.n_log_dst; d++) bufs.dst[bufs.n_dst++] = p.log_dst[d];
+        bufs.row0 = p.row0;
+    }
+    const bool independent = engine_i8 && plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && !shares_buffer(plan->prev, bufs);
     p.wait_prior_grid = !independent;
     p.early_trigger = engine_i8 && cfg.gridDim.x == (unsigned)plan->sm_count;
-    plan->prev_in = in; plan->prev_logits = logits; plan->prev_labels = labels; plan->prev_stream = st; plan->prev_valid = engine_i8;
+    plan->prev = bufs; plan->prev_stream = st; plan->prev_valid = engine_i8;
+    if (engine_i8 && plan->verbose) fprintf(stderr, "bitnetmcu_b200: fused launch: %s\n", independent ? "independent" : "wait");
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;

@@ -102,9 +102,15 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      call k must therefore be complete before call k-1 was enqueued (resident inputs, or produced on another stream and
  *      joined by an event before call k-1).  The library keeps ordinary stream semantics (the wait) for every launch where it
  *      can see the promise broken: the first launch after the option is set, a launch on another stream than the one before,
- *      and a launch that reuses the images, logits or labels pointer of the one before.  A NULL logits or labels pointer is
- *      no buffer: two labels-only launches in a row do not share their (absent) logits.  Producer -> inference chains on one
- *      stream (bnm_quantize_images_device then bnm_infer_batch_device) belong to mode 0 or 1.
+ *      a launch right after a launch of another kind (float input, emulator, top-k, ...), and a launch that touches a buffer
+ *      of the one before.  That is: one of its images, logits, labels or gather destination pointers equals one of the
+ *      previous launch's, whatever the roles (the logits of call k-1 passed as the images of call k count), except that a
+ *      gather destination both write counts only at the same row_offset.  A NULL pointer is no buffer: two labels-only
+ *      launches in a row do not share their (absent) logits.  The check compares pointers only: buffers that overlap at an
+ *      offset (a slice of the previous call's logits as images, destination rows of two offsets that overlap) stay the
+ *      caller's promise.  Producer -> inference chains on one stream (bnm_quantize_images_device then
+ *      bnm_infer_batch_device) belong to mode 0 or 1.  With BNM_VERBOSE set at model creation every such launch prints
+ *      "bitnetmcu_b200: fused launch: wait" or "... independent".
  *      Only launches that fill the GPU (>= one 128-image tile per SM) trigger early, and every launch occupies its SM
  *      exclusively (more than half of the shared memory): at most two consecutive launches are ever in flight together.
  *      CNN models are held at mode 1 (the front-end kernel really feeds the FC kernel). */

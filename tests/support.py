@@ -256,6 +256,52 @@ def gather_call(lib, e, d_img, d_log, d_lab, g, stream):
     return rc
 
 
+# ---- kernel neighbours of a launch -------------------------------------------------------------------------------------------
+# A dependent launch relaxes the ordering between two kernels only: after a cudaMemcpyAsync, which is what ATen makes of
+# Tensor.copy_ and Tensor.clone on contiguous tensors of one dtype, the fused FC launch runs fully serialised and its
+# grid-dependency wait is never put to the test.  Tests that place a producer or consumer next to a launch use these.
+
+def kernel_copy(dst, src):
+    """dst <- src (same dtype, an integer type) by an elementwise CUDA kernel, never a memory copy"""
+    import torch
+    torch.bitwise_xor(src, 0, out=dst)
+    return dst
+
+
+def kernel_clone(src):
+    """a new tensor equal to src (an integer type), written by an elementwise CUDA kernel"""
+    import torch
+    return torch.bitwise_xor(src, 0)
+
+
+@functools.lru_cache(maxsize=None)
+def _kernel_copy_profile():
+    """the CUDA activities torch.profiler records for one kernel_copy and one kernel_clone, and whether both copied.  Once per
+    process: a later profiler session in the same process can miss activities."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    src = torch.arange(-128, 128, dtype=torch.int32, device="cuda").to(torch.int8).repeat(64)
+    dst = torch.full_like(src, 5)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA], acc_events=True) as prof:
+        kernel_copy(dst, src)
+        out = kernel_clone(dst)
+        torch.cuda.synchronize()
+    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+    return names, bool(torch.equal(dst, src) and torch.equal(out, src))
+
+
+@pytest.fixture(scope="session")
+def kernel_copies_are_kernels(built):
+    """kernel_copy and kernel_clone record a CUDA kernel each and no memcpy (torch.profiler); fails if torch ever turns them
+    into copies"""
+    names, copied = _kernel_copy_profile()
+    assert not [n for n in names if "memcpy" in n.lower() or "memset" in n.lower()], names
+    assert len([n for n in names if "BitwiseXor" in n]) == 2, names
+    assert copied
+    return True
+
+
 # ---- the plain-C host side ----------------------------------------------------------------------------------------------------
 
 def _write_test_data_header(path, images, labels):

@@ -10,7 +10,7 @@ import pytest
 
 from conftest import GOLDEN, load_model, model_names
 from restate import scale_images
-from support import N_MANY, engine, frontends, gather_call, lib
+from support import N_MANY, engine, frontends, gather_call, kernel_clone, kernel_copies_are_kernels, kernel_copy, lib
 
 pytestmark = pytest.mark.gpu
 
@@ -165,10 +165,12 @@ def test_device_api_torch(lib, oracle):
 
 
 @pytest.mark.parametrize("mode,n", [(0, 148 * 128 * 7 + 77), (1, 148 * 128 * 7 + 77), (2, 148 * 128 * 7 + 77), (2, 1000)])
-def test_launch_overlap_modes(lib, oracle, mode, n):
-    """BNM_OPT_LAUNCH_OVERLAP: back-to-back launches on one stream stay bit-exact.  Mode 1 (dependent launch + wait) with
-    the SAME buffers reused by every launch and a producer kernel (a torch copy) feeding each launch -- ordinary stream
-    semantics must hold; mode 2 with double-buffered inputs and outputs, the promise it asks for."""
+def test_launch_overlap_modes(lib, oracle, kernel_copies_are_kernels, mode, n):
+    """BNM_OPT_LAUNCH_OVERLAP: back-to-back launches on one stream stay bit-exact.  Modes 0 and 1 (dependent launch + wait)
+    with the SAME buffers reused by every launch, a producer kernel (kernel_copy, an elementwise kernel: a copy_ would be a
+    memcpy, which a dependent launch never overlaps) writing the images right before each launch and a consumer kernel
+    (kernel_clone) reading the outputs right after -- ordinary stream semantics must hold; mode 2 with double-buffered
+    inputs and outputs, the promise it asks for."""
     import torch
     from bitnetmcu_b200 import _lib
     m = load_model("fc")
@@ -197,9 +199,9 @@ def test_launch_overlap_modes(lib, oracle, mode, n):
         else:
             ref = []
             for k in range(4):                      # producer kernel -> our kernel -> consumer kernel, same buffers every time
-                d_img[0].copy_(src[k])
+                kernel_copy(d_img[0], src[k])
                 e.infer_device(d_img[0], d_log[0], d_lab[0])
-                got.append((d_log[0].clone(), d_lab[0].clone()))
+                got.append((kernel_clone(d_log[0]), kernel_clone(d_lab[0])))
                 ref.append(want[k])
             s.synchronize()
             got = [(a.cpu().numpy(), b.cpu().numpy()) for a, b in got]
@@ -472,10 +474,11 @@ def test_later_model_keeps_earlier_models_shared_memory(lib, oracle):
     fc.close()
 
 
-def test_launch_overlap_mode2_reused_buffers_keep_stream_order(lib, oracle):
-    """ADVICE r1: mode 2 drops the grid-dependency wait only for launches whose buffers differ from the previous call's.
-    Reusing the SAME buffers with a producer copy in front of every launch (the pattern mode 2 does not promise) must still
-    be ordered: the library falls back to the wait when it sees a pointer of the previous launch again."""
+def test_launch_overlap_mode2_reused_buffers_keep_stream_order(lib, oracle, kernel_copies_are_kernels):
+    """Mode 2 drops the grid-dependency wait only for launches whose buffers differ from the previous call's.  Reusing the
+    SAME buffers with a producer kernel (kernel_copy) in front of every launch and a consumer kernel (kernel_clone) after it
+    (the pattern mode 2 does not promise) must still be ordered: the library falls back to the wait when it sees a pointer
+    of the previous launch again."""
     import torch
     from bitnetmcu_b200 import _lib
     m = load_model("fc")
@@ -494,10 +497,10 @@ def test_launch_overlap_mode2_reused_buffers_keep_stream_order(lib, oracle):
     with torch.cuda.stream(s):
         for rep in range(3):
             for k in range(4):
-                d_img.copy_(src[k])
+                kernel_copy(d_img, src[k])
                 e.infer_device(d_img, d_log, d_lab)
                 if rep == 2:
-                    got.append((d_log.clone(), d_lab.clone()))
+                    got.append((kernel_clone(d_log), kernel_clone(d_lab)))
         s.synchronize()
     for (gl, gb), (wl, wb) in zip(got, want):
         assert np.array_equal(gl.cpu().numpy(), wl) and np.array_equal(gb.cpu().numpy().astype(np.uint32), wb)

@@ -8,7 +8,8 @@ import pytest
 
 from conftest import load_model, model_names
 from restate import scale_images
-from support import CHAIN_ROWS, N_MANY, build_c_shim, engine, frontends, lib, plan_line, verbose_engine
+from support import CHAIN_ROWS, N_MANY, build_c_shim, engine, frontends, kernel_clone, kernel_copies_are_kernels, lib, plan_line, \
+    verbose_engine
 
 pytestmark = pytest.mark.gpu
 
@@ -139,10 +140,11 @@ def test_host_pipeline_labels_only(lib, oracle, name):
 
 
 @pytest.mark.parametrize("mode", [1, 2])
-def test_launch_overlap_labels_only(lib, oracle, mode):
+def test_launch_overlap_labels_only(lib, oracle, kernel_copies_are_kernels, mode):
     """BNM_OPT_LAUNCH_OVERLAP with NULL logits: back-to-back launches on one stream, images and labels double-buffered, stay
-    bit-exact.  Then one labels buffer reused by every launch (resident images, a consumer copy after each): the library must see
-    the reuse and keep the launches ordered, whatever the absent logits."""
+    bit-exact.  Then one labels buffer reused by every launch (resident images, a consumer kernel -- kernel_clone, not a
+    memcpy -- reading it right after each): the library must see the reuse and keep the launches ordered, whatever the
+    absent logits."""
     import torch
     from bitnetmcu_b200 import _lib
     m = load_model("fc")
@@ -168,7 +170,7 @@ def test_launch_overlap_labels_only(lib, oracle, mode):
         for rep in range(3):
             for k in range(4):
                 e.infer_device(src[k], None, one)
-                seen.append(one.clone())
+                seen.append(kernel_clone(one))
         s.synchronize()
     for i, t in enumerate(seen):
         assert np.array_equal(t.cpu().numpy().astype(np.uint32), want[i % 4]), i
