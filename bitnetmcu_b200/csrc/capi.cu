@@ -101,7 +101,8 @@ struct bnm_model {
     size_t chunk_images = 1 << 16;   // host pipeline chunk
     int launch_overlap = 0;
     int cnn_frontend = 0;            // BNM_OPT_CNN_FRONTEND
-    bool conv3_fits_u16 = false;     // static range of conv3's inputs for this model's weights (cnn_conv3_fits_u16)
+    long long conv3_bound = 0;       // static range of conv3's inputs for this model's weights (cnn_conv3_bound)
+    bool conv3_fits_u16 = false;     // conv3_bound <= 65535: the tensor-core front-end runs conv3 on IDP.2A
     std::vector<int8_t> h_conv[3];   // host copies of the conv weights (range analysis)
     DevBuf<int> d_err;               // error word of the bounded device-side waits
     // fused plan
@@ -309,7 +310,8 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         else {
             uint32_t f = ((m->xy0 - 4) / 2 - 2) / 2;   // 16 -> 2
             m->feat_stride = round_up(m->channels * f * f, 16);
-            m->conv3_fits_u16 = cnn_conv3_fits_u16(m->h_conv[0].data(), m->h_conv[1].data(), m->channels);
+            m->conv3_bound = cnn_conv3_bound(m->h_conv[0].data(), m->h_conv[1].data(), m->channels);
+            m->conv3_fits_u16 = m->conv3_bound <= 65535;
         }
     }
     if (rc == 0 && model_class == BNM_MODEL_FCMNIST && !front.empty()) rc = fail(BNM_E_ARG, "MODEL_FCMNIST with conv/pool layers");
@@ -332,6 +334,10 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         // and the kernels of bnm_compare_engines_device
         if (engines_fused(m)) fprintf(stderr, "bitnetmcu_b200: engines route: fc_engines_kernel%s\n", fc_chain_form_name(m->plan, kFormEngines));
         else fprintf(stderr, "bitnetmcu_b200: engines route: bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts\n");
+        // and which conv3 the tensor-core CNN front-end runs
+        if (m->model_class == BNM_MODEL_CNNMNIST)
+            fprintf(stderr, "bitnetmcu_b200: cnn front-end: conv3 bound %lld, conv3 on %s\n", m->conv3_bound,
+                    m->conv3_fits_u16 ? "IDP.2A" : "IMAD");
     }
     *out = m;
     return 0;

@@ -816,8 +816,10 @@ __global__ void __launch_bounds__(kCnnThreads) k_cnn_frontend16(const int8_t *__
 
 // Static range of conv3's inputs for given HOST weights (int8 [C][9] each): conv1 sums are at most 127 * (sum of positive taps) +
 // 128 * (sum of |negative taps|) for int8 pixels, ReLU >> 4 of that bounds conv2's inputs (all >= 0), so only conv2's positive taps
-// raise its maximum; ReLU >> 4 again bounds the pooled values.  (SURVEY.md section 7: per-channel static range proofs.)
-bool cnn_conv3_fits_u16(const int8_t *w1, const int8_t *w2, uint32_t channels) {
+// raise its maximum; ReLU >> 4 again bounds the pooled values.  Returns the largest bound over the channels.  (SURVEY.md
+// section 7: per-channel static range proofs.)
+long long cnn_conv3_bound(const int8_t *w1, const int8_t *w2, uint32_t channels) {
+    long long bound = 0;
     for (uint32_t c = 0; c < channels; c++) {
         long long pos1 = 0, neg1 = 0, pos2 = 0;
         for (int k = 0; k < 9; k++) {
@@ -826,9 +828,9 @@ bool cnn_conv3_fits_u16(const int8_t *w1, const int8_t *w2, uint32_t channels) {
             if (b > 0) pos2 += b;
         }
         const long long b1 = (127 * pos1 + 128 * neg1) >> 4;
-        if (((b1 * pos2) >> 4) > 65535) return false;
+        bound = std::max(bound, (b1 * pos2) >> 4);
     }
-    return true;
+    return bound;
 }
 
 bool launch_cnn_frontend(const int8_t *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,

@@ -57,8 +57,8 @@ bool launch_cnn_frontend(const int8_t *images, const int8_t *w1, const int8_t *w
                          uint32_t xy, int8_t *features, uint32_t feat_stride, size_t n, int sm_count, int frontend, int *d_err,
                          bool conv3_fits_u16, cudaStream_t st);
 // conv3_fits_u16: the pooled conv2 outputs (conv3's inputs) cannot exceed 65535 for this model's conv1 / conv2 weights
-// (cnn_conv3_fits_u16, computed once per model): conv3 may then run on IDP.2A
-bool cnn_conv3_fits_u16(const int8_t *w1, const int8_t *w2, uint32_t channels);
+// (cnn_conv3_bound <= 65535, computed once per model): conv3 may then run on IDP.2A
+long long cnn_conv3_bound(const int8_t *w1, const int8_t *w2, uint32_t channels);
 bool cnn_frontend_tc_supported(uint32_t channels, uint32_t xy);
 
 // same front-end with conv1 on wgmma and the depthwise tail fed from shared memory (cnn_wgmma.cu); false when the shape is not

@@ -1,5 +1,6 @@
 """NumPy restatements the tests compare the GPU against, one copy of each: the reference caller's input scaling, the reference
-Python emulator's FC and CNN paths, and the fused FC kernels' tile schedule.  Pure NumPy: no torch, no CUDA library."""
+Python emulator's FC and CNN paths, the C engine's CNN front-end stages and conv3 input bound, and the fused FC kernels' tile
+schedule.  Pure NumPy: no torch, no CUDA library."""
 from typing import NamedTuple
 
 import numpy as np
@@ -52,11 +53,11 @@ def _conv_relu(a, w):
     return np.maximum(out, 0)
 
 
-def _renorm(v):
+def _renorm(v, rounding=np.round):
     """BitConv2d's renormalisation over each image's C*H*W outputs (float64); an all-zero image stays zero"""
     m = v.reshape(v.shape[0], -1).max(axis=1)
     scale = np.where(m > 0, 127.0 / np.maximum(m, 1), 0.0)[:, None, None, None]
-    return np.round(v * scale).clip(0, 127).astype(np.int64)
+    return rounding(v * scale).clip(0, 127).astype(np.int64)
 
 
 def _pool(v):
@@ -64,14 +65,25 @@ def _pool(v):
     return v.reshape(n, c, h // 2, 2, w // 2, 2).max(axis=(3, 5))
 
 
+def _conv_weights(model):
+    return [l.weights for l in model.layers if l.kind == M.LAYER_CONV33]
+
+
+def cnn_stages(model, x, rounding=np.round):
+    """float32 images [n, 256] -> (conv1, conv2, conv3, features): the ReLU output of each convolution before its
+    renormalisation (int64 [n, C, H, W]) and the int64 features [n, C*4], the (C, 2, 2) flatten.  rounding: the
+    renormalisation's (np.round, half to even, is the emulator's)"""
+    w1, w2, w3 = _conv_weights(model)
+    c1 = _conv_relu(scale_images(x).astype(np.int64).reshape(-1, 1, 16, 16), w1)
+    c2 = _conv_relu(_renorm(c1, rounding), w2)
+    c3 = _conv_relu(_pool(_renorm(c2, rounding)), w3)
+    f = _pool(_renorm(c3, rounding))
+    return c1, c2, c3, f.reshape(f.shape[0], -1)
+
+
 def cnn_features(model, x):
     """float32 images [n, 256] -> int64 features [n, C*4], the (C, 2, 2) flatten"""
-    w1, w2, w3 = [l.weights for l in model.layers if l.kind == M.LAYER_CONV33]
-    a = scale_images(x).astype(np.int64).reshape(-1, 1, 16, 16)
-    a = _renorm(_conv_relu(a, w1))
-    a = _pool(_renorm(_conv_relu(a, w2)))
-    a = _pool(_renorm(_conv_relu(a, w3)))
-    return a.reshape(a.shape[0], -1)
+    return cnn_stages(model, x)[3]
 
 
 def emulate(model, x, block=512):
@@ -79,6 +91,49 @@ def emulate(model, x, block=512):
     if model.model_class == 0:
         return emulate_fc(model, x)
     return np.concatenate([bitlinear(model, cnn_features(model, x[i:i + block])) for i in range(0, len(x), block)])
+
+
+# ---- the C engine's CNN front-end (dll.c:64-80) ------------------------------------------------------------------------------
+
+def conv3_channel_bounds(model):
+    """per channel, the largest pooled conv2 output (conv3's input) any int8 image can give, from the conv1 / conv2 weights:
+    ((127 sum(w1 > 0) + 128 sum|w1 < 0|) >> 4) sum(w2 > 0) >> 4 -> int64 [C]"""
+    w1, w2, _ = (w.astype(np.int64).reshape(-1, 9) for w in _conv_weights(model))
+    b1 = (127 * np.where(w1 > 0, w1, 0).sum(axis=1) + 128 * np.where(w1 < 0, -w1, 0).sum(axis=1)) >> 4
+    return (b1 * np.where(w2 > 0, w2, 0).sum(axis=1)) >> 4
+
+
+def conv3_bound(model):
+    """cnn_conv3_bound (generic_kernels.cu): the maximum of conv3_channel_bounds"""
+    return int(conv3_channel_bounds(model).max())
+
+
+def relunorm(v):
+    """orc_ReLUNorm (inference.c:23-72) on rows int64 [n, k] without the argmax: shift = bit length of (max >> 7), then
+    min(127, (x + rounding) >> shift) with rounding = (1 << shift) >> 1, negatives to 0"""
+    m = v.max(axis=1)
+    shift = np.array([int(t).bit_length() if t > 0 else 0 for t in m >> 7], dtype=np.int64)[:, None]
+    return np.where(v < 0, 0, np.minimum(127, (v + ((1 << shift) >> 1)) >> shift))
+
+
+class Frontend(NamedTuple):
+    conv1: np.ndarray       # int64 [n, C, 14, 14]: processconv33ReLU(image, w1, 16, 4)
+    conv2: np.ndarray       # [n, C, 6, 6]: processconv33ReLU(conv1, w2, 14, 4), pooled -- conv3's inputs
+    conv3: np.ndarray       # [n, C, 2, 2]: processconv33ReLU(conv2, w3, 6, 4), pooled
+    raw: np.ndarray         # [n, C*4]: the features before ReLUNorm, channel-major
+    features: np.ndarray    # [n, C*4]: after ReLUNorm (dll.c:80)
+
+
+def c_frontend(model, images):
+    """the C engine's front-end (orc_processconv33ReLU / orc_processmaxpool22, bitnet_oracle.c) on int8 images [n, 256], int64
+    throughout: conv = ReLU(sum) >> 4 with no rounding or clip"""
+    w1, w2, w3 = _conv_weights(model)
+    a = np.asarray(images, dtype=np.int8).astype(np.int64).reshape(-1, 1, 16, 16)
+    c1 = _conv_relu(a, w1) >> 4
+    c2 = _pool(_conv_relu(c1, w2) >> 4)
+    c3 = _pool(_conv_relu(c2, w3) >> 4)
+    raw = c3.reshape(c3.shape[0], -1)
+    return Frontend(c1, c2, c3, raw, relunorm(raw))
 
 
 # ---- the fused FC kernels' tile schedule (tests/test_fc_ring_rounds.py) -----------------------------------------------------

@@ -36,11 +36,13 @@ def engine(model, path=0, cnn_frontend=None):
 
 
 def frontends(model):
-    """CNN models run once per front-end kernel (BNM_OPT_CNN_FRONTEND): CUDA cores and conv1-on-wgmma; FC models once."""
+    """CNN models run once per front-end kernel (BNM_OPT_CNN_FRONTEND): CUDA cores and conv1-on-wgmma, which takes multiples of
+    16 channels up to 128; FC models once."""
     from bitnetmcu_b200 import _lib
     if model.model_class != 1:
         return [None]
-    return [_lib.CNN_CUDA_CORES, _lib.CNN_TENSOR_CORES] if model.channels % 16 == 0 else [_lib.CNN_CUDA_CORES]
+    tc = model.channels % 16 == 0 and model.channels <= 128
+    return [_lib.CNN_CUDA_CORES, _lib.CNN_TENSOR_CORES] if tc else [_lib.CNN_CUDA_CORES]
 
 
 def verbose_engine(capfd, monkeypatch, make):
@@ -162,9 +164,9 @@ CHAIN_ROWS = [
 ]
 
 
-def cnn_model(channels, n_classes, seed, w=(None, None, None)):
-    """a random CNN model: conv weights uniform in [-128, 127] with +-127 taps in every layer (or the given weights), a 64-wide
-    4bitsym hidden layer and an n_classes head"""
+def cnn_model(channels, n_classes, seed, w=(None, None, None), hidden=(64,)):
+    """a random CNN model: conv weights uniform in [-128, 127] with +-127 taps in every layer (or the given weights), 4bitsym
+    hidden layers of the given widths (default one, 64 wide; none: the features feed the head directly) and an n_classes head"""
     from bitnetmcu_b200 import model as M, pack as P
     rng = np.random.default_rng(seed)
 
@@ -182,7 +184,7 @@ def cnn_model(channels, n_classes, seed, w=(None, None, None)):
               M.Layer(kind=M.LAYER_CONV33, name="L7", bitperweight=8, n_in=6, n_out=channels, in_channels=channels, groups=channels,
                       weights=conv_w(2)),
               M.Layer(kind=M.LAYER_MAXPOOL22, name="L9", n_in=4, n_out=2)]
-    fc = P.random_fc_model(M.ENC_4BITSYM, (channels * 4, 64, n_classes), seed=seed)
+    fc = P.random_fc_model(M.ENC_4BITSYM, (channels * 4,) + tuple(hidden) + (n_classes,), seed=seed)
     for i, l in enumerate(fc.layers):
         l.name = f"L{11 + 2 * i}"
         layers.append(l)
@@ -241,6 +243,16 @@ def run_emulator(e, x, want_logits=True, want_labels=True, stream=None):
     e.inference_quantized_device(d_x, lo, la, stream=stream)
     torch.cuda.synchronize()
     return (lo.cpu().numpy() if want_logits else None), (la.cpu().numpy().astype(np.int64) if want_labels else None)
+
+
+def run_emulator_layered(e, x):
+    """run_emulator on the layer-by-layer route (BNM_PATH_LAYERS), then back to the default path"""
+    from bitnetmcu_b200 import _lib
+    e.set_option(_lib.OPT_PATH, _lib.PATH_LAYERS)
+    try:
+        return run_emulator(e, x)
+    finally:
+        e.set_option(_lib.OPT_PATH, _lib.PATH_AUTO)
 
 
 def gather_call(lib, e, d_img, d_log, d_lab, g, stream):

@@ -2,7 +2,7 @@
 
 * FC models wider than 64 or with more than 16 classes: k_quantize_images, then fc_emul_i8_kernel<max_n> (int8 TMA input, one
   pipe, one slot, the last layer at full width, the emulator's hidden-layer rule and float64 logits);
-* CNN models up to 128 channels: k_cnn_emul_frontend (input scaling, three convolutions with the per-image renormalisation, two
+* CNN models up to 128 channels (beyond that: layer by layer): k_cnn_emul_frontend (input scaling, three convolutions with the per-image renormalisation, two
   pools; BitNetMCU.py:435-445, 459-526), then fc_emul_i8_kernel on its features.
 
 CPU tests: a NumPy restatement of the emulator's CNN path against the reference emulator's own logits (the expectation of the
@@ -16,7 +16,7 @@ import pytest
 from conftest import GOLDEN, load_model
 from restate import cnn_features, emulate
 from support import N_MANY, cnn_model, crafted_cnn_case, engine, instructions, lib, local_memory, normal_images, route, \
-    run_emulator, sass_functions, verbose_engine
+    run_emulator, run_emulator_layered, sass_functions, verbose_engine
 
 CHUNK = 1 << 20                     # images per front-end / FC launch pair of the new routes
 
@@ -48,21 +48,12 @@ def test_new_kernels_sass(built):
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------------
 
-def _layered(e, x):
-    from bitnetmcu_b200 import _lib
-    e.set_option(_lib.OPT_PATH, _lib.PATH_LAYERS)
-    try:
-        return run_emulator(e, x)
-    finally:
-        e.set_option(_lib.OPT_PATH, _lib.PATH_AUTO)
-
-
 def _check(e, x, want, tag):
     """default path == restatement (logits and np.argmax labels), and == the layered emulator"""
     lo, la = run_emulator(e, x)
     assert np.array_equal(lo, want), (tag, np.argwhere(lo != want)[:5])
     assert np.array_equal(la, np.argmax(want, axis=1)), tag
-    lo2, la2 = _layered(e, x)
+    lo2, la2 = run_emulator_layered(e, x)
     assert np.array_equal(lo2, lo) and np.array_equal(la2, la), tag
 
 
@@ -122,13 +113,17 @@ def test_random_fc_models(lib, capfd, monkeypatch, idx):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("channels", [16, 24, 48, 64, 128])
+@pytest.mark.parametrize("channels", [16, 24, 48, 64, 128, 144, 256])
 @pytest.mark.parametrize("n_classes", [10, 37])
 def test_random_cnn_models(lib, capfd, monkeypatch, channels, n_classes):
+    """up to 128 channels k_cnn_emul_frontend, beyond that the layer-by-layer route"""
     m = cnn_model(channels, n_classes, seed=channels + n_classes)
     x = normal_images(1500, seed=channels)
     e, err = verbose_engine(capfd, monkeypatch, lambda: engine(m))
-    assert route(err, "emulator").startswith("k_cnn_emul_frontend + fc_emul_i8_kernel<64,"), err
+    if channels <= 128:
+        assert route(err, "emulator").startswith("k_cnn_emul_frontend + fc_emul_i8_kernel<64,"), err
+    else:
+        assert route(err, "emulator") == "layer by layer", err
     _check(e, x, emulate(m, x), (channels, n_classes))
     e.close()
 
@@ -161,7 +156,7 @@ def test_batch_sizes(lib, name, n):
     for _ in range(2):
         lo, la = run_emulator(e, x)
         assert np.array_equal(lo[idx], want) and np.array_equal(la[idx], np.argmax(want, axis=1)), (name, n)
-    lo2, la2 = _layered(e, x)
+    lo2, la2 = run_emulator_layered(e, x)
     assert np.array_equal(lo2, lo) and np.array_equal(la2, la), (name, n)
     e.close()
 
@@ -181,7 +176,7 @@ def test_one_past_the_chunk(lib, name):
     d_x = _device_images(CHUNK + 1, seed=2)
     e = engine(m)
     lo, la = run_emulator(e, d_x)
-    lo2, la2 = _layered(e, d_x)
+    lo2, la2 = run_emulator_layered(e, d_x)
     assert np.array_equal(lo, lo2) and np.array_equal(la, la2)
     import torch
     idx = np.r_[0:200, CHUNK - 200:CHUNK + 1]
@@ -205,7 +200,7 @@ def test_ring_rounds(lib, capfd, monkeypatch, width):
     n = sms * 128 * (3 * max_stages + 1) + 77
     d_x = _device_images(n, seed=width)
     lo, la = run_emulator(e, d_x)
-    lo2, la2 = _layered(e, d_x)
+    lo2, la2 = run_emulator_layered(e, d_x)
     assert np.array_equal(lo, lo2) and np.array_equal(la, la2), width
     idx = np.r_[0:300, n - 2 * sms * 128:n]
     want = emulate(m, d_x[torch.as_tensor(idx, device="cuda")].cpu().numpy())

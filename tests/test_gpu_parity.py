@@ -507,11 +507,12 @@ def test_launch_overlap_mode2_reused_buffers_keep_stream_order(lib, oracle, kern
     e.close()
 
 
-@pytest.mark.parametrize("channels", [16, 32, 48, 64, 80, 96, 112, 128])
+@pytest.mark.parametrize("channels", [8, 16, 24, 32, 40, 48, 64, 80, 96, 100, 112, 128, 144, 200, 256])
 def test_cnn_frontends_agree_for_every_channel_count(lib, oracle, channels):
     """Random conv weights for every channel count the tensor-core front-end takes (multiples of 16 up to 128: tiles that
     straddle images for C = 48 / 80 / 96, eight images per tile for C = 16) against the oracle, both front-end kernels, ragged
-    batch sizes around the group size."""
+    batch sizes around the group size; and counts only the CUDA-core kernel runs: not a multiple of 16 (idle threads in its
+    CTA of 256 / C images), and more than 128 (one image per CTA)."""
     from bitnetmcu_b200 import _lib, model as M, pack as P
     from bitnetmcu_b200.engine import Engine
     rng = np.random.default_rng(channels)
@@ -532,7 +533,7 @@ def test_cnn_frontends_agree_for_every_channel_count(lib, oracle, channels):
     for n in (1, 7, 8, 9, 300, 4099):
         imgs = _rand_images(n, seed=n + channels)
         want, want_lab = oracle.infer(m, imgs)
-        for fe in (_lib.CNN_CUDA_CORES, _lib.CNN_TENSOR_CORES):
+        for fe in frontends(m):
             e = Engine(m)
             e.set_option(_lib.OPT_CNN_FRONTEND, fe)
             lo, la = e.infer(imgs)
