@@ -34,6 +34,12 @@ static int fail(int code, const char *fmt, ...) {
 
 enum { BNM_E_ARG = -1, BNM_E_NODEV = -2, BNM_E_UNSUPPORTED = -3, BNM_E_CUDA = -4 };
 
+// the status of the kernels just launched: 0, or the launch error
+static int launch_status() {
+    cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+}
+
 static uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
 // One allocation of T and its only owner, which frees it: device memory, or mapped pinned host memory (kPinned).  grow(need) makes
@@ -136,13 +142,61 @@ struct bnm_model {
 };
 static const size_t kSmallBatch = 1024;
 
-static void free_fc_dev(bnm_model *m) {
-    for (auto &L : m->fc) {
-        cudaFree(L.dense_a);
-        cudaFree(L.dense_b);
-        cudaFree(L.quad_a);
-        cudaFree(L.quad_b);
+// bytes of an FC layer's packed weights, what the reference reads: n_out * ceil(n_in / weights per word) 32-bit words (ternary:
+// n_out * (n_in / 10) uint16) -- inference.c:88-208.  An unknown encoding reads nothing and decodes as zeros (inference.c:202).
+static size_t packed_weight_bytes(int32_t enc, uint32_t n_in, uint32_t n_out) {
+    switch (enc) {
+    case BNM_ENC_BINARY: return (size_t)n_out * ((n_in + 31) / 32) * 4;
+    case BNM_ENC_2BITSYM: return (size_t)n_out * ((n_in + 15) / 16) * 4;
+    case BNM_ENC_4BITSYM: case BNM_ENC_4BIT: case BNM_ENC_FP130: case BNM_ENC_NF4: return (size_t)n_out * ((n_in + 7) / 8) * 4;
+    case BNM_ENC_8BIT: return (size_t)n_out * ((n_in + 3) / 4) * 4;
+    case BNM_ENC_TERNARY: return (size_t)n_out * (n_in / 10) * 2;
+    default: return 0;
     }
+}
+
+static void free_fc_layer(FcLayerDev &L) {
+    cudaFree(L.dense_a);
+    cudaFree(L.dense_b);
+    cudaFree(L.quad_a);
+    cudaFree(L.quad_b);
+    L.dense_a = L.dense_b = nullptr;
+    L.quad_a = L.quad_b = nullptr;
+}
+
+// one FC layer's packed weights (device, zero padded past the end) decoded into its int8 planes, the residual ones only where they
+// are needed.  On failure nothing stays allocated.
+static cudaError_t decode_fc_layer(const void *d_packed, int32_t enc, uint32_t n_in, uint32_t n_out, int nf4_ext, FcLayerDev &L) {
+    L.enc = enc;
+    L.n_in = n_in;
+    L.n_out = n_out;
+    L.k_pad = round_up(std::max(n_in, 1u), 32);
+    L.n_pad = round_up(n_out, 16);
+    const size_t plane = (size_t)L.k_pad * L.n_pad;
+    DevBuf<int> d_flag;
+    int flag = 0;
+    cudaError_t e = cudaMalloc(&L.dense_a, plane);
+    if (e == cudaSuccess) e = cudaMalloc(&L.dense_b, plane);
+    if (e == cudaSuccess) e = cudaMalloc(&L.quad_a, plane);
+    if (e == cudaSuccess) e = cudaMalloc(&L.quad_b, plane);
+    if (e == cudaSuccess) e = d_flag.grow(sizeof(int), true);
+    if (e == cudaSuccess) {
+        launch_decode_fc(d_packed, enc, n_in, n_out, L.k_pad, L.n_pad, L.dense_a, L.dense_b, L.quad_a, L.quad_b, nf4_ext, d_flag.p, 0);
+        e = cudaMemcpy(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost);
+    }
+    if (e != cudaSuccess) {
+        free_fc_layer(L);
+    } else if (!flag) {   // no residual plane needed (everything but FP130 layers that contain +128)
+        cudaFree(L.dense_b);
+        cudaFree(L.quad_b);
+        L.dense_b = nullptr;
+        L.quad_b = nullptr;
+    }
+    return e;
+}
+
+static void free_fc_dev(bnm_model *m) {
+    for (auto &L : m->fc) free_fc_layer(L);
     m->fc.clear();
     if (m->plan) fc_chain_plan_destroy(m->plan);
     m->plan = nullptr;
@@ -156,46 +210,18 @@ static int effective_overlap(const bnm_model *m) {
 // decode all FC layers into int8 planes and (re)build the fused plan
 static int build_fc_dev(bnm_model *m) {
     free_fc_dev(m);
-    int *d_flag = nullptr;
-    CU_TRY(cudaMalloc(&d_flag, sizeof(int)));
     m->max_kpad = round_up(std::max(m->img_bytes, m->feat_stride), 32);
     m->max_nout = 0;
     for (auto &H : m->fc_host) {
         FcLayerDev L;
-        L.enc = H.enc;
-        L.n_in = H.n_in;
-        L.n_out = H.n_out;
-        L.k_pad = round_up(H.n_in, 32);
-        L.n_pad = round_up(H.n_out, 16);
-        size_t plane = (size_t)L.k_pad * L.n_pad;
-        int flag = 0;
-        cudaError_t e = cudaMalloc(&L.dense_a, plane);
-        if (e == cudaSuccess) e = cudaMalloc(&L.dense_b, plane);
-        if (e == cudaSuccess) e = cudaMalloc(&L.quad_a, plane);
-        if (e == cudaSuccess) e = cudaMalloc(&L.quad_b, plane);
-        if (e == cudaSuccess) e = cudaMemset(d_flag, 0, sizeof(int));
-        if (e == cudaSuccess) {
-            launch_decode_fc(H.d_packed, H.enc, H.n_in, H.n_out, L.k_pad, L.n_pad, L.dense_a, L.dense_b, L.quad_a, L.quad_b,
-                             m->nf4_ext, d_flag, 0);
-            e = cudaMemcpy(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost);
-        }
-        if (e != cudaSuccess) {   // nothing half-built stays behind
-            cudaFree(L.dense_a); cudaFree(L.dense_b); cudaFree(L.quad_a); cudaFree(L.quad_b);
-            cudaFree(d_flag);
+        if (cudaError_t e = decode_fc_layer(H.d_packed, H.enc, H.n_in, H.n_out, m->nf4_ext, L)) {   // nothing half-built stays behind
             free_fc_dev(m);
             return fail(BNM_E_CUDA, "weight decode of an FC layer failed: %s", cudaGetErrorString(e));
-        }
-        if (!flag) {   // no residual plane needed (everything but FP130 layers that contain +128)
-            cudaFree(L.dense_b);
-            cudaFree(L.quad_b);
-            L.dense_b = nullptr;
-            L.quad_b = nullptr;
         }
         m->max_kpad = std::max(m->max_kpad, L.k_pad);
         m->max_nout = std::max(m->max_nout, L.n_out);
         m->fc.push_back(L);
     }
-    cudaFree(d_flag);
     m->n_classes = m->fc.back().n_out;
     // fused plan (may legitimately be unavailable for exotic shapes: the layered path then serves the model)
     char err[256] = {0};
@@ -226,6 +252,10 @@ static EmulRoute emul_route(const bnm_model *m) {
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
     if (bnm_model_active_path(m) != BNM_PATH_TCGEN05 || (cnn && m->channels > kCnnEmulMaxChannels)) return kEmulLayers;
     return !cnn && fc_chain_has_form(m->plan, kFormEmulFloat) ? kEmulFloatRow : kEmulInt8Row;
+}
+// the kernel that makes the emulator's int8 rows from float images on its row routes (emulate_device)
+static const char *emul_rows_kernel(const bnm_model *m) {
+    return m->model_class == BNM_MODEL_CNNMNIST ? "k_cnn_emul_frontend" : "k_quantize_images";
 }
 
 // bnm_compare_engines_device: fc_engines_kernel for the models both float-input rows serve, else the two entries' routes and
@@ -268,16 +298,7 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         const bnm_layer &L = layers[i];
         if (L.kind == BNM_LAYER_FC) {
             if (!L.weights || L.n_in == 0 || L.n_out == 0) { rc = fail(BNM_E_ARG, "FC layer %u: empty", i); break; }
-            // the reference reads n_out * ceil(n_in/wpw) words (ternary: n_out*(n_in/10) uint16) -- inference.c:88-208
-            size_t need = 0;
-            switch (L.bitperweight) {
-            case BNM_ENC_BINARY: need = (size_t)L.n_out * ((L.n_in + 31) / 32) * 4; break;
-            case BNM_ENC_2BITSYM: need = (size_t)L.n_out * ((L.n_in + 15) / 16) * 4; break;
-            case BNM_ENC_4BITSYM: case BNM_ENC_4BIT: case BNM_ENC_FP130: case BNM_ENC_NF4: need = (size_t)L.n_out * ((L.n_in + 7) / 8) * 4; break;
-            case BNM_ENC_8BIT: need = (size_t)L.n_out * ((L.n_in + 3) / 4) * 4; break;
-            case BNM_ENC_TERNARY: need = (size_t)L.n_out * (L.n_in / 10) * 2; break;
-            default: need = 0; break;   // unknown id: decoded as zeros like inference.c:202, nothing is read
-            }
+            const size_t need = packed_weight_bytes(L.bitperweight, L.n_in, L.n_out);
             if (L.weight_bytes < need) { rc = fail(BNM_E_ARG, "FC layer %u: %zu weight bytes, reference reads %zu", i, L.weight_bytes, need); break; }
             FcLayerHost H{L.bitperweight, L.n_in, L.n_out, nullptr, std::max<size_t>(need, 16)};
             if (cudaMalloc(&H.d_packed, H.packed_bytes + 16) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaMalloc failed"); break; }
@@ -327,10 +348,9 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
     m->verbose = getenv("BNM_VERBOSE") != nullptr;
     if (m->verbose) {   // diagnostics: the kernels bnm_emulate_batch_device runs on the default path
         const EmulRoute r = emul_route(m);
-        fprintf(stderr, "bitnetmcu_b200: emulator route: %s%s\n",
-                r == kEmulLayers ? "layer by layer" : r == kEmulFloatRow ? "fc_emul_kernel" :
-                m->model_class == BNM_MODEL_CNNMNIST ? "k_cnn_emul_frontend + fc_emul_i8_kernel" : "k_quantize_images + fc_emul_i8_kernel",
-                r == kEmulLayers ? "" : fc_chain_form_name(m->plan, r == kEmulFloatRow ? kFormEmulFloat : kFormEmulInt8));
+        if (r == kEmulLayers) fprintf(stderr, "bitnetmcu_b200: emulator route: layer by layer\n");
+        else if (r == kEmulFloatRow) fprintf(stderr, "bitnetmcu_b200: emulator route: fc_emul_kernel%s\n", fc_chain_form_name(m->plan, kFormEmulFloat));
+        else fprintf(stderr, "bitnetmcu_b200: emulator route: %s + fc_emul_i8_kernel%s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulInt8));
         // and the kernels of bnm_compare_engines_device
         if (engines_fused(m)) fprintf(stderr, "bitnetmcu_b200: engines route: fc_engines_kernel%s\n", fc_chain_form_name(m->plan, kFormEngines));
         else fprintf(stderr, "bitnetmcu_b200: engines route: bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts\n");
@@ -465,16 +485,20 @@ static int run_cnn_front(bnm_model *m, const int8_t *images, size_t n, int8_t *f
                 m->channels, m->xy0, m->xy0);
 }
 
+// images per chunk of the C engine on int8 images; 0: one launch whatever the batch (FC models on the fused path)
+static size_t c_engine_chunk(const bnm_model *m, bool fused) {
+    if (!fused) return kLayeredChunk;
+    return m->model_class == BNM_MODEL_CNNMNIST ? kFusedCnnChunk : 0;
+}
+
 extern "C" int bnm_infer_launch_count(const bnm_model *m, size_t n) {
     if (!m || n == 0) return 0;
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    if (fused && !cnn) return 1;
-    const size_t chunk_images = fused ? kFusedCnnChunk : kLayeredChunk;
-    size_t chunks = (n + chunk_images - 1) / chunk_images;
-    int per = cnn ? 1 : 0;
+    const size_t chunk = c_engine_chunk(m, fused);
+    if (!chunk) return 1;
+    int per = m->model_class == BNM_MODEL_CNNMNIST ? 1 : 0;
     per += fused ? 1 : (int)(2 * m->fc.size());   // fc + relunorm per layer (last relunorm = labels)
-    return (int)(chunks * per);
+    return (int)((n + chunk - 1) / chunk * per);
 }
 
 // a call must produce something: logits, labels or (gather) a destination in another buffer
@@ -482,53 +506,74 @@ static bool has_output(const int32_t *logits, const uint32_t *labels, const Gath
     return logits || labels || (gather && (gather->n_labels_dst || gather->n_logits_dst));
 }
 
+// What a call of the C engine produces: logits int32 [n][n_classes] and labels uint32 [n], each may be null, and the fused result
+// exchange's destinations (gather, may be null); or, with topk.k > 0, instead of all these the k best classes of every image and
+// their int32 scores (may be null).
+struct InferOut {
+    int32_t *logits;
+    uint32_t *labels;
+    const GatherDst *gather;
+    TopKOutputs topk;
+};
+
+// the top-k outputs of a call from image b on (T: the type of its scores)
+template <class T> static TopKOutputs topk_from(const TopKOutputs &t, size_t b) {
+    return TopKOutputs{t.k, t.classes ? t.classes + b * t.k : nullptr, t.scores ? static_cast<T *>(t.scores) + b * t.k : nullptr};
+}
+
+// The C engine on int8 images on st, arguments checked: FC models on the fused path in one launch, every other model in chunks
+// (CNN front-end, then the fused launch, or the layer-by-layer chain and for top-k k_topk_rows on its int32 accumulators).
 // slot_feat: a caller-owned feature buffer for n images (the host pipeline's per-slot buffers); null = the model's own scratch.
-// logits and labels may each be null.
-static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather, void *stream,
-                             int8_t *slot_feat = nullptr) {
+static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const InferOut &out, cudaStream_t st, int8_t *slot_feat = nullptr) {
+    const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
+    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
+    const uint32_t k = out.topk.k;
+    const FcForm form = k ? kFormTopK : kFormInt8;
+    const char *kernel = k ? "top-k" : "FC";
+    const size_t chunk_max = c_engine_chunk(m, fused);
+    if (!chunk_max) {
+        int rc = fc_chain_launch(m->plan, form, images, n, out.logits, out.labels, 0, out.gather, st, nullptr, k ? &out.topk : nullptr);
+        return rc ? fail(BNM_E_CUDA, "fused %s kernel launch failed (%d): %s", kernel, rc, cudaGetErrorString(cudaGetLastError())) : 0;
+    }
+    const size_t chunk = slot_feat ? n : std::min(n, chunk_max);
+    int rc = (slot_feat && fused) ? 0 : ensure_scratch(m, chunk, !fused);
+    if (rc) return rc;
+    int8_t *feat = slot_feat ? slot_feat : m->d_feat.p;
+    for (size_t b = 0; b < n; b += chunk) {
+        const size_t nb = std::min(chunk, n - b);
+        const int8_t *fc_in = images + b * m->img_bytes;
+        uint32_t fc_stride = m->img_bytes;
+        if (cnn) {
+            if ((rc = run_cnn_front(m, fc_in, nb, feat, st))) return rc;
+            fc_in = feat;
+            fc_stride = m->feat_stride;
+        }
+        int32_t *lg = out.logits ? out.logits + b * m->n_classes : nullptr;
+        uint32_t *lb = out.labels ? out.labels + b : nullptr;
+        const TopKOutputs topk = topk_from<int32_t>(out.topk, b);
+        if (fused) {
+            GatherDst gchunk;
+            if (out.gather) { gchunk = *out.gather; gchunk.row_offset += b; }
+            if ((rc = fc_chain_launch(m->plan, form, fc_in, nb, lg, lb, 0, out.gather ? &gchunk : nullptr, st, nullptr, k ? &topk : nullptr)))
+                return fail(BNM_E_CUDA, "fused %s kernel launch failed (%d)", kernel, rc);
+        } else {
+            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, lb, st))) return rc;
+            if (k) launch_topk_rows(m->d_acc.p, m->n_classes, k, topk.classes, static_cast<int32_t *>(topk.scores), nb, st);   // last layer's accumulators
+        }
+    }
+    return launch_status();
+}
+
+static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather, void *stream) {
     if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch_device: null argument");
     if (n && !has_output(logits, labels, gather)) return fail(BNM_E_ARG, "bnm_infer_batch_device: no output (logits, labels and gather destinations all absent)");
     if (n == 0) return 0;
     if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned (TMA)");
     if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
     CU_TRY(cudaSetDevice(m->device));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    if (gather && !fused) return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
-    if (fused && !cnn) {
-        int rc = fc_chain_launch(m->plan, kFormInt8, images, n, logits, labels, 0, gather, st);
-        return rc ? fail(BNM_E_CUDA, "fused FC kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
-    }
-    const size_t chunk = slot_feat ? n : std::min(n, fused ? kFusedCnnChunk : kLayeredChunk);
-    int rc = (slot_feat && fused) ? 0 : ensure_scratch(m, chunk, !fused);
-    if (rc) return rc;
-    int8_t *feat = slot_feat ? slot_feat : m->d_feat.p;
-    for (size_t b = 0; b < n; b += chunk) {
-        const size_t nb = std::min(chunk, n - b);
-        const int8_t *img = images + b * m->img_bytes;
-        int32_t *lg = logits ? logits + b * m->n_classes : nullptr;
-        uint32_t *lb = labels ? labels + b : nullptr;
-        const int8_t *fc_in = img;
-        uint32_t fc_stride = m->img_bytes;
-        if (cnn) {
-            rc = run_cnn_front(m, img, nb, feat, st);
-            if (rc) return rc;
-            fc_in = feat;
-            fc_stride = m->feat_stride;
-        }
-        if (fused) {
-            GatherDst gchunk;
-            if (gather) { gchunk = *gather; gchunk.row_offset += b; }
-            rc = fc_chain_launch(m->plan, kFormInt8, fc_in, nb, lg, lb, 0, gather ? &gchunk : nullptr, st);
-            if (rc) return fail(BNM_E_CUDA, "fused FC kernel launch failed (%d)", rc);
-        } else {
-            rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, lb, st);
-            if (rc) return rc;
-        }
-    }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+    if (gather && bnm_model_active_path(m) != BNM_PATH_TCGEN05)
+        return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
+    return run_c_engine(m, images, n, InferOut{logits, labels, gather, {}}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
@@ -628,39 +673,55 @@ static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *lo
     return 0;
 }
 
+// the C engine on host buffers in chunks of chunk_images, each through one slot's buffers: images in, run_c_engine, out's arrays
+// back.  Synchronous.
+static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const InferOut &out) {
+    const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
+    // per image, in 4-byte words: d_logits holds the logits or the top-k scores (bnm_infer_batch sizes it and d_labels whether or
+    // not it takes them), d_classes the top-k classes
+    const size_t n_logits = k ? (out.topk.scores ? k : 0) : m->n_classes, n_labels = k ? 0 : 1;
+    const size_t feat_bytes = m->model_class == BNM_MODEL_CNNMNIST ? m->feat_stride : 0;
+    bool small = false;
+    for (auto &s : m->slots)
+        small = small || s.d_feat.bytes < chunk * feat_bytes || s.d_images.bytes < chunk * m->img_bytes || s.d_classes.bytes < chunk * k * 4 ||
+                s.d_logits.bytes < chunk * n_logits * 4 || s.d_labels.bytes < chunk * n_labels * 4;
+    if (small) {
+        CU_TRY(cudaDeviceSynchronize());   // no chunk of an earlier call may still use a buffer that is reallocated
+        for (auto &s : m->slots) {
+            CU_TRY(s.d_feat.grow(chunk * feat_bytes, true));
+            CU_TRY(s.d_images.grow(chunk * (size_t)m->img_bytes));
+            CU_TRY(s.d_classes.grow(chunk * k * 4));
+            CU_TRY(s.d_logits.grow(chunk * n_logits * 4));
+            CU_TRY(s.d_labels.grow(chunk * n_labels * 4));
+        }
+    }
+    // the layer-by-layer path shares one scratch arena (accumulators / activations): its chunks must not overlap in time -> one
+    // stream.  The fused path has no shared state (CNN models: one feature buffer per slot) and uses all three.
+    const bool shared_scratch = bnm_model_active_path(m) != BNM_PATH_TCGEN05;
+    int32_t *h_logits = k ? static_cast<int32_t *>(out.topk.scores) : out.logits;   // where d_logits goes
+    size_t c = 0;
+    for (size_t b = 0; b < n; b += chunk, c++) {
+        const size_t nb = std::min(chunk, n - b);
+        PipeSlot &s = m->slots[shared_scratch ? 0 : c % 3];
+        CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
+        const InferOut d{out.logits ? s.d_logits.p : nullptr, out.labels ? s.d_labels.p : nullptr, nullptr,
+                         {(uint32_t)k, s.d_classes.p, out.topk.scores ? s.d_logits.p : nullptr}};
+        if (int rc = run_c_engine(m, s.d_images.p, nb, d, s.stream, shared_scratch ? nullptr : s.d_feat.p)) return rc;
+        if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, s.d_classes.p, nb * k * 4, cudaMemcpyDeviceToHost, s.stream));
+        if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * n_logits, s.d_logits.p, nb * n_logits * 4, cudaMemcpyDeviceToHost, s.stream));
+        if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, s.d_labels.p, nb * 4, cudaMemcpyDeviceToHost, s.stream));
+    }
+    for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
+    return 0;
+}
+
 extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
     if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch: null argument");
     if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_infer_batch: no output (logits and labels both NULL)");
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);
-    const size_t chunk = std::min(n, m->chunk_images);
-    // the last slot's labels are the last buffer grown: smaller than a chunk's until every slot has all of its buffers
-    if (m->slots[2].d_labels.bytes < chunk * sizeof(uint32_t)) {
-        CU_TRY(cudaDeviceSynchronize());   // no chunk of an earlier call may still use a buffer that is reallocated
-        for (auto &s : m->slots) {
-            if (m->model_class == BNM_MODEL_CNNMNIST) CU_TRY(s.d_feat.grow(chunk * (size_t)m->feat_stride, true));
-            CU_TRY(s.d_images.grow(chunk * (size_t)m->img_bytes));
-            CU_TRY(s.d_logits.grow(chunk * (size_t)m->n_classes * sizeof(int32_t)));
-            CU_TRY(s.d_labels.grow(chunk * sizeof(uint32_t)));
-        }
-    }
-    // the layer-by-layer path shares one scratch arena (accumulators / activations): its chunks must not overlap in time -> one
-    // stream.  The fused path has no shared state (CNN models: one feature buffer per slot) and uses all three.
-    const bool shared_scratch = bnm_model_active_path(m) != BNM_PATH_TCGEN05;
-    size_t k = 0;
-    for (size_t b = 0; b < n; b += chunk, k++) {
-        const size_t nb = std::min(chunk, n - b);
-        PipeSlot &s = m->slots[shared_scratch ? 0 : k % 3];
-        CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
-        int rc = infer_device_impl(m, s.d_images.p, nb, logits ? s.d_logits.p : nullptr, labels ? s.d_labels.p : nullptr, nullptr, s.stream,
-                                   shared_scratch ? nullptr : s.d_feat.p);
-        if (rc) return rc;
-        if (logits) CU_TRY(cudaMemcpyAsync(logits + b * m->n_classes, s.d_logits.p, nb * (size_t)m->n_classes * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
-        if (labels) CU_TRY(cudaMemcpyAsync(labels + b, s.d_labels.p, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-    }
-    for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
-    return 0;
+    return infer_pipelined(m, images, n, InferOut{logits, labels, nullptr, {}});
 }
 
 extern "C" void *bnm_host_alloc(size_t bytes) {
@@ -689,36 +750,18 @@ extern "C" int bnm_processfclayer_batch(const int8_t *activations, const uint32_
     if (int rc = require_device()) return rc;
     if (n == 0 || n_output == 0) return 0;
     if (!activations || !weights || !output) return fail(BNM_E_ARG, "bnm_processfclayer_batch: null argument");
-    size_t need = 0;
-    switch (enc) {
-    case BNM_ENC_BINARY: need = (size_t)n_output * ((n_input + 31) / 32) * 4; break;
-    case BNM_ENC_2BITSYM: need = (size_t)n_output * ((n_input + 15) / 16) * 4; break;
-    case BNM_ENC_4BITSYM: case BNM_ENC_4BIT: case BNM_ENC_FP130: case BNM_ENC_NF4: need = (size_t)n_output * ((n_input + 7) / 8) * 4; break;
-    case BNM_ENC_8BIT: need = (size_t)n_output * ((n_input + 3) / 4) * 4; break;
-    case BNM_ENC_TERNARY: need = (size_t)n_output * (n_input / 10) * 2; break;
-    default: need = 0;
-    }
-    FcLayerDev L;
-    L.enc = enc; L.n_in = n_input; L.n_out = n_output;
-    L.k_pad = round_up(std::max(n_input, 1u), 32);
-    L.n_pad = round_up(n_output, 16);
-    const size_t plane = (size_t)L.k_pad * L.n_pad;
+    const size_t need = packed_weight_bytes(enc, n_input, n_output);
     DevBuf<uint8_t> packed;
-    DevBuf<int8_t> da, db, act;
-    DevBuf<int4> qa, qb;
-    DevBuf<int> flag;
-    DevBuf<int32_t> out;
-    if (packed.grow(need + 16) || da.grow(plane) || db.grow(plane) || qa.grow(plane) || qb.grow(plane) || flag.grow(4) ||
-        act.grow(n * (size_t)L.k_pad) || out.grow(n * (size_t)n_output * 4))
-        return fail(BNM_E_CUDA, "cudaMalloc failed");
+    if (packed.grow(need + 16)) return fail(BNM_E_CUDA, "cudaMalloc failed");
     CU_TRY(cudaMemset(packed.p, 0, need + 16));
     if (need) CU_TRY(cudaMemcpy(packed.p, weights, need, cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemset(flag.p, 0, 4));
-    L.dense_a = da.p; L.quad_a = qa.p;
-    launch_decode_fc(packed.p, enc, n_input, n_output, L.k_pad, L.n_pad, L.dense_a, db.p, L.quad_a, qb.p, nf4_extension, flag.p, 0);
-    int f = 0;
-    CU_TRY(cudaMemcpy(&f, flag.p, 4, cudaMemcpyDeviceToHost));
-    if (f) { L.dense_b = db.p; L.quad_b = qb.p; }
+    FcLayerDev L;
+    if (cudaError_t e = decode_fc_layer(packed.p, enc, n_input, n_output, nf4_extension, L))
+        return fail(BNM_E_CUDA, "weight decode of an FC layer failed: %s", cudaGetErrorString(e));
+    struct Planes { FcLayerDev &L; ~Planes() { free_fc_layer(L); } } planes{L};   // L's planes are freed on every return below
+    DevBuf<int8_t> act;
+    DevBuf<int32_t> out;
+    if (act.grow(n * (size_t)L.k_pad) || out.grow(n * (size_t)n_output * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
     CU_TRY(cudaMemset(act.p, 0, n * (size_t)L.k_pad));
     // Ternary layers declare n_input padded to a multiple of 10 with zero trits (exportquant.py:132-137,166) and the
     // reference never reads the activations under a zero trit (inference.c:128): a caller may hand in a 256-byte row for
@@ -804,8 +847,7 @@ extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_
     if (n == 0 || elems == 0) return 0;
     if (!images || !out) return fail(BNM_E_ARG, "bnm_quantize_images_device: null argument");
     launch_quantize_images(images, elems, out, n, static_cast<cudaStream_t>(stream));
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+    return launch_status();
 }
 
 // float images -> logits / labels on the device.  FC models on the fused path (rows of <= 256 elements, <= 16 classes): ONE kernel, the
@@ -858,36 +900,39 @@ static int level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc =
 static const size_t kEmulChunkFc = 65536, kEmulChunkCnn = 2048;   // images per pass of the layer kernels (CNN: 2 x C kB of planes each)
 
 // The emulator on device buffers, asynchronous on st: images float32 [n][img_bytes] -> logits float64 [n][n_classes] and / or labels
-// (first maximum).  The routes other than fc_emul_kernel run in chunks through scratch the model owns (grow-only), which the
-// layer-by-layer path shares: like that path, one stream at a time per model.
-static int emulate_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, cudaStream_t st) {
+// (first maximum); or, with topk.k > 0, instead of both the k best classes of every image and their float64 scores (may be null).
+// The routes other than fc_emul_kernel run in chunks through scratch the model owns (grow-only), which the layer-by-layer path
+// shares: like that path, one stream at a time per model.
+static int emulate_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, cudaStream_t st,
+                          const TopKOutputs &topk = {}) {
     const size_t nl = m->fc.size();
     const int out_shift = level_shift_of(m->fc[nl - 1].enc);   // logits = last layer's accumulators / its level scale
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    const uint32_t C = m->channels, elems = m->img_bytes;
+    const uint32_t C = m->channels, elems = m->img_bytes, k = topk.k;
     const EmulRoute route = emul_route(m);
-    if (route == kEmulFloatRow) {
+    if (route == kEmulFloatRow && !k) {   // fc_emul_kernel has no top-k form: top-k takes the int8 rows
         int rc = fc_chain_launch(m->plan, kFormEmulFloat, images, n, logits, labels, out_shift, nullptr, st);
         return rc ? fail(BNM_E_CUDA, "fused emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
-    if (route == kEmulInt8Row) {
+    if (route != kEmulLayers) {
         const size_t chunk = std::min(n, kFusedCnnChunk);
-        const size_t row_bytes = cnn ? m->feat_stride : elems;
-        CU_TRY(m->d_emul_rows.grow(chunk * row_bytes));
+        CU_TRY(m->d_emul_rows.grow(chunk * (cnn ? m->feat_stride : elems)));
         int8_t *rows = m->d_emul_rows.p;
         for (size_t b = 0; b < n; b += chunk) {
             const size_t nb = std::min(chunk, n - b);
             if (!cnn) launch_quantize_images(images + b * elems, elems, rows, nb, st);   // BitNetMCU.py:435-436
             else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, rows, m->feat_stride, nb, st))
                 return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
-            int rc = fc_chain_launch(m->plan, kFormEmulInt8, rows, nb, logits ? logits + b * m->n_classes : nullptr,
-                                     labels ? labels + b : nullptr, out_shift, nullptr, st);
-            if (rc) return fail(BNM_E_CUDA, "fused int8 emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+            const TopKOutputs tk = topk_from<double>(topk, b);
+            int rc = fc_chain_launch(m->plan, k ? kFormEmulTopK : kFormEmulInt8, rows, nb, logits ? logits + b * m->n_classes : nullptr,
+                                     labels ? labels + b : nullptr, out_shift, nullptr, st, nullptr, k ? &tk : nullptr);
+            if (rc) return fail(BNM_E_CUDA, "fused %s kernel launch failed (%d): %s", k ? "emulator top-k" : "int8 emulator", rc,
+                                cudaGetErrorString(cudaGetLastError()));
         }
-        cudaError_t e = cudaGetLastError();
-        return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+        return launch_status();
     }
     const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
+    if (k) CU_TRY(m->d_topk_logits.grow(chunk * m->n_classes * sizeof(double)));   // top-k: the logits of a chunk
     if (int rc = ensure_scratch(m, chunk, true)) return rc;   // accumulators and the two int8 activation buffers
     CU_TRY(m->d_emul_q.grow(chunk * elems));
     if (cnn)
@@ -923,10 +968,14 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
             act = next;
             stride = next_stride;
         }
-        launch_emul_logits(m->d_acc.p, m->n_classes, out_shift, logits ? logits + b * m->n_classes : nullptr, labels ? labels + b : nullptr, nb, st);
+        double *lg = k ? m->d_topk_logits.p : logits ? logits + b * m->n_classes : nullptr;
+        launch_emul_logits(m->d_acc.p, m->n_classes, out_shift, lg, labels ? labels + b : nullptr, nb, st);
+        if (k) {
+            const TopKOutputs tk = topk_from<double>(topk, b);
+            launch_topk_rows(lg, m->n_classes, k, tk.classes, static_cast<double *>(tk.scores), nb, st);
+        }
     }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+    return launch_status();
 }
 
 extern "C" int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream) {
@@ -998,8 +1047,7 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
             if (int rc = emulate_device(m, img, nb, nullptr, lp, st)) return rc;
         if (counts) launch_engine_counts(lc, lp, truth ? truth + b : nullptr, nb, m->n_classes, cnt, st);
     }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+    return launch_status();
 }
 
 // -----------------------------------------------------------------------------------------------
@@ -1027,45 +1075,9 @@ static int topk_check(const bnm_model *m, const char *fn, const void *images, si
 static std::string topk_c_route(const bnm_model *m) {
     std::string s;
     if (m->model_class == BNM_MODEL_CNNMNIST)
-        s = m->cnn_frontend != 1 && cnn_frontend_tc_supported(m->channels, m->xy0) ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
+        s = cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
     if (bnm_model_active_path(m) == BNM_PATH_TCGEN05) return s + "fc_topk_kernel" + fc_chain_form_name(m->plan, kFormTopK);
     return s + "layer by layer + k_topk_rows<int32>";
-}
-
-// the C engine's top-k of int8 images on st, arguments checked.  slot_feat as in infer_device_impl.
-static int topk_device_impl(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, cudaStream_t st,
-                            int8_t *slot_feat = nullptr) {
-    const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    if (fused && !cnn) {
-        const TopKOutputs out{k, classes, scores};
-        int rc = fc_chain_launch(m->plan, kFormTopK, images, n, nullptr, nullptr, 0, nullptr, st, nullptr, &out);
-        return rc ? fail(BNM_E_CUDA, "fused top-k kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
-    }
-    const size_t chunk = slot_feat ? n : std::min(n, fused ? kFusedCnnChunk : kLayeredChunk);
-    int rc = (slot_feat && fused) ? 0 : ensure_scratch(m, chunk, !fused);
-    if (rc) return rc;
-    int8_t *feat = slot_feat ? slot_feat : m->d_feat.p;
-    for (size_t b = 0; b < n; b += chunk) {
-        const size_t nb = std::min(chunk, n - b);
-        const TopKOutputs out{k, classes + b * k, scores ? scores + b * k : nullptr};
-        const int8_t *fc_in = images + b * m->img_bytes;
-        uint32_t fc_stride = m->img_bytes;
-        if (cnn) {
-            if ((rc = run_cnn_front(m, fc_in, nb, feat, st))) return rc;
-            fc_in = feat;
-            fc_stride = m->feat_stride;
-        }
-        if (fused) {
-            if ((rc = fc_chain_launch(m->plan, kFormTopK, fc_in, nb, nullptr, nullptr, 0, nullptr, st, nullptr, &out)))
-                return fail(BNM_E_CUDA, "fused top-k kernel launch failed (%d)", rc);
-        } else {
-            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, nullptr, nullptr, st))) return rc;   // last layer's accumulators in d_acc
-            launch_topk_rows(m->d_acc.p, m->n_classes, k, out.classes, static_cast<int32_t *>(out.scores), nb, st);
-        }
-    }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
 }
 
 extern "C" int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
@@ -1073,7 +1085,7 @@ extern "C" int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t 
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk_device: %s\n", topk_c_route(m).c_str());
-    return topk_device_impl(m, images, n, k, classes, scores, static_cast<cudaStream_t>(stream));
+    return run_c_engine(m, images, n, InferOut{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
@@ -1087,7 +1099,8 @@ extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         launch_quantize_images(images + b * elems, (uint32_t)elems, m->d_f32_scratch.p, nb, st);
-        if (int rc = topk_device_impl(m, m->d_f32_scratch.p, nb, k, classes + b * k, scores ? scores + b * k : nullptr, st)) return rc;
+        const InferOut out{nullptr, nullptr, nullptr, {k, classes + b * k, scores ? scores + b * k : nullptr}};
+        if (int rc = run_c_engine(m, m->d_f32_scratch.p, nb, out, st)) return rc;
     }
     return 0;
 }
@@ -1096,38 +1109,9 @@ extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t
     if (int rc = topk_check(m, "bnm_emulate_topk_device", images, n, k, classes, scores, 8, 16)) return rc;
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    const size_t elems = m->img_bytes, ncls = m->n_classes;
-    if (emul_route(m) != kEmulLayers) {
-        if (m->verbose)
-            fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: %s + fc_topk_kernel%s\n",
-                    cnn ? "k_cnn_emul_frontend" : "k_quantize_images", fc_chain_form_name(m->plan, kFormEmulTopK));
-        const int out_shift = level_shift_of(m->fc.back().enc);
-        const size_t chunk = std::min(n, kFusedCnnChunk);
-        CU_TRY(m->d_emul_rows.grow(chunk * (cnn ? m->feat_stride : elems)));
-        int8_t *rows = m->d_emul_rows.p;
-        for (size_t b = 0; b < n; b += chunk) {
-            const size_t nb = std::min(chunk, n - b);
-            if (!cnn) launch_quantize_images(images + b * elems, (uint32_t)elems, rows, nb, st);   // BitNetMCU.py:435-436
-            else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, m->channels, rows, m->feat_stride, nb, st))
-                return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
-            const TopKOutputs out{k, classes + b * k, scores ? scores + b * k : nullptr};
-            int rc = fc_chain_launch(m->plan, kFormEmulTopK, rows, nb, nullptr, nullptr, out_shift, nullptr, st, nullptr, &out);
-            if (rc) return fail(BNM_E_CUDA, "fused emulator top-k kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
-        }
-    } else {
-        if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: layer by layer + k_topk_rows<double>\n");
-        const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
-        CU_TRY(m->d_topk_logits.grow(chunk * ncls * sizeof(double)));
-        for (size_t b = 0; b < n; b += chunk) {
-            const size_t nb = std::min(chunk, n - b);
-            if (int rc = emulate_device(m, images + b * elems, nb, m->d_topk_logits.p, nullptr, st)) return rc;
-            launch_topk_rows(m->d_topk_logits.p, (uint32_t)ncls, k, classes + b * k, scores ? scores + b * k : nullptr, nb, st);
-        }
-    }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : fail(BNM_E_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+    if (m->verbose && emul_route(m) == kEmulLayers) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: layer by layer + k_topk_rows<double>\n");
+    else if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: %s + fc_topk_kernel%s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulTopK));
+    return emulate_device(m, images, n, nullptr, nullptr, static_cast<cudaStream_t>(stream), TopKOutputs{k, classes, scores});
 }
 
 // host buffers: the chunked pipeline of bnm_infer_batch, k classes (and k scores) per image copied back
@@ -1136,36 +1120,7 @@ extern "C" int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk: %s\n", topk_c_route(m).c_str());
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    const size_t chunk = std::min(n, m->chunk_images), out_bytes = chunk * k * sizeof(uint32_t);
-    bool small = false;
-    for (auto &s : m->slots)
-        small = small || s.d_images.bytes < chunk * m->img_bytes || s.d_classes.bytes < out_bytes || (scores && s.d_logits.bytes < out_bytes) ||
-                (cnn && s.d_feat.bytes < chunk * m->feat_stride);
-    if (small) {
-        CU_TRY(cudaDeviceSynchronize());   // no chunk of an earlier call may still use a buffer that is reallocated
-        for (auto &s : m->slots) {
-            if (cnn) CU_TRY(s.d_feat.grow(chunk * (size_t)m->feat_stride, true));
-            CU_TRY(s.d_images.grow(chunk * (size_t)m->img_bytes));
-            CU_TRY(s.d_classes.grow(out_bytes));
-            if (scores) CU_TRY(s.d_logits.grow(out_bytes));   // the scores of a chunk: k <= n_classes int32 per image
-        }
-    }
-    // as in bnm_infer_batch: the layer-by-layer path's shared scratch allows one stream, the fused path takes all three
-    const bool shared_scratch = bnm_model_active_path(m) != BNM_PATH_TCGEN05;
-    size_t c = 0;
-    for (size_t b = 0; b < n; b += chunk, c++) {
-        const size_t nb = std::min(chunk, n - b);
-        PipeSlot &s = m->slots[shared_scratch ? 0 : c % 3];
-        CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
-        int rc = topk_device_impl(m, s.d_images.p, nb, k, s.d_classes.p, scores ? s.d_logits.p : nullptr, s.stream,
-                                  shared_scratch ? nullptr : s.d_feat.p);
-        if (rc) return rc;
-        CU_TRY(cudaMemcpyAsync(classes + b * k, s.d_classes.p, nb * k * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-        if (scores) CU_TRY(cudaMemcpyAsync(scores + b * k, s.d_logits.p, nb * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
-    }
-    for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
-    return 0;
+    return infer_pipelined(m, images, n, InferOut{nullptr, nullptr, nullptr, {k, classes, scores}});
 }
 
 // -----------------------------------------------------------------------------------------------

@@ -833,13 +833,20 @@ long long cnn_conv3_bound(const int8_t *w1, const int8_t *w2, uint32_t channels)
     return bound;
 }
 
+CnnFrontendKernel cnn_frontend_kernel(uint32_t channels, uint32_t xy, int frontend) {
+    if (xy != 16 || channels == 0) return kCnnFrontendNone;
+    if (frontend != 1 && cnn_frontend_tc_supported(channels, xy)) return kCnnFrontendTensorCores;
+    return frontend == 2 || channels > kCnnThreads ? kCnnFrontendNone : kCnnFrontendCudaCores;
+}
+
 bool launch_cnn_frontend(const int8_t *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
                          uint32_t xy, int8_t *features, uint32_t feat_stride, size_t n, int sm_count, int frontend, int *d_err,
                          bool conv3_fits_u16, cudaStream_t st) {
-    if (xy != 16 || channels == 0) return false;
+    const CnnFrontendKernel kernel = cnn_frontend_kernel(channels, xy, frontend);
+    if (kernel == kCnnFrontendNone) return false;
     if (n == 0) return true;
-    if (frontend != 1 && launch_cnn_frontend_tc(images, w1, w2, w3, channels, xy, features, feat_stride, n, sm_count, d_err, conv3_fits_u16, st)) return true;
-    if (frontend == 2 || channels > kCnnThreads) return false;
+    if (kernel == kCnnFrontendTensorCores)
+        return launch_cnn_frontend_tc(images, w1, w2, w3, channels, xy, features, feat_stride, n, sm_count, d_err, conv3_fits_u16, st);
     uint32_t ipb = kCnnThreads / channels;
     size_t smem = (size_t)ipb * (64 + 224) * 4 + ipb * 4;
     size_t n_groups = (n + ipb - 1) / ipb;

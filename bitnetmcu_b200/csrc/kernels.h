@@ -56,6 +56,9 @@ void launch_maxpool22(const int32_t *act, uint32_t xy, int32_t *out, size_t n, c
 bool launch_cnn_frontend(const int8_t *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
                          uint32_t xy, int8_t *features, uint32_t feat_stride, size_t n, int sm_count, int frontend, int *d_err,
                          bool conv3_fits_u16, cudaStream_t st);
+// the kernel launch_cnn_frontend runs for frontend and a model's shape (none: it returns false)
+enum CnnFrontendKernel { kCnnFrontendNone, kCnnFrontendCudaCores, kCnnFrontendTensorCores };
+CnnFrontendKernel cnn_frontend_kernel(uint32_t channels, uint32_t xy, int frontend);
 // conv3_fits_u16: the pooled conv2 outputs (conv3's inputs) cannot exceed 65535 for this model's conv1 / conv2 weights
 // (cnn_conv3_bound <= 65535, computed once per model): conv3 may then run on IDP.2A
 long long cnn_conv3_bound(const int8_t *w1, const int8_t *w2, uint32_t channels);
