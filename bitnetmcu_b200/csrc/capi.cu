@@ -349,10 +349,10 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
     if (m->verbose) {   // diagnostics: the kernels bnm_emulate_batch_device runs on the default path
         const EmulRoute r = emul_route(m);
         if (r == kEmulLayers) fprintf(stderr, "bitnetmcu_b200: emulator route: layer by layer\n");
-        else if (r == kEmulFloatRow) fprintf(stderr, "bitnetmcu_b200: emulator route: fc_emul_kernel%s\n", fc_chain_form_name(m->plan, kFormEmulFloat));
-        else fprintf(stderr, "bitnetmcu_b200: emulator route: %s + fc_emul_i8_kernel%s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulInt8));
+        else if (r == kEmulFloatRow) fprintf(stderr, "bitnetmcu_b200: emulator route: %s\n", fc_chain_form_name(m->plan, kFormEmulFloat));
+        else fprintf(stderr, "bitnetmcu_b200: emulator route: %s + %s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulInt8));
         // and the kernels of bnm_compare_engines_device
-        if (engines_fused(m)) fprintf(stderr, "bitnetmcu_b200: engines route: fc_engines_kernel%s\n", fc_chain_form_name(m->plan, kFormEngines));
+        if (engines_fused(m)) fprintf(stderr, "bitnetmcu_b200: engines route: %s\n", fc_chain_form_name(m->plan, kFormEngines));
         else fprintf(stderr, "bitnetmcu_b200: engines route: bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts\n");
         // and which conv3 the tensor-core CNN front-end runs
         if (m->model_class == BNM_MODEL_CNNMNIST)
@@ -506,25 +506,16 @@ static bool has_output(const int32_t *logits, const uint32_t *labels, const Gath
     return logits || labels || (gather && (gather->n_labels_dst || gather->n_logits_dst));
 }
 
-// What a call of the C engine produces: logits int32 [n][n_classes] and labels uint32 [n], each may be null, and the fused result
-// exchange's destinations (gather, may be null); or, with topk.k > 0, instead of all these the k best classes of every image and
-// their int32 scores (may be null).
-struct InferOut {
-    int32_t *logits;
-    uint32_t *labels;
-    const GatherDst *gather;
-    TopKOutputs topk;
-};
-
 // the top-k outputs of a call from image b on (T: the type of its scores)
 template <class T> static TopKOutputs topk_from(const TopKOutputs &t, size_t b) {
     return TopKOutputs{t.k, t.classes ? t.classes + b * t.k : nullptr, t.scores ? static_cast<T *>(t.scores) + b * t.k : nullptr};
 }
 
-// The C engine on int8 images on st, arguments checked: FC models on the fused path in one launch, every other model in chunks
+// The C engine on int8 images on st, arguments checked -> out: logits int32 [n][n_classes], labels and gather, or with topk.k > 0
+// the k best classes of every image and their int32 scores.  FC models on the fused path in one launch, every other model in chunks
 // (CNN front-end, then the fused launch, or the layer-by-layer chain and for top-k k_topk_rows on its int32 accumulators).
 // slot_feat: a caller-owned feature buffer for n images (the host pipeline's per-slot buffers); null = the model's own scratch.
-static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const InferOut &out, cudaStream_t st, int8_t *slot_feat = nullptr) {
+static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const FcOutputs &out, cudaStream_t st, int8_t *slot_feat = nullptr) {
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
     const uint32_t k = out.topk.k;
@@ -532,7 +523,7 @@ static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const Infe
     const char *kernel = k ? "top-k" : "FC";
     const size_t chunk_max = c_engine_chunk(m, fused);
     if (!chunk_max) {
-        int rc = fc_chain_launch(m->plan, form, images, n, out.logits, out.labels, 0, out.gather, st, nullptr, k ? &out.topk : nullptr);
+        int rc = fc_chain_launch(m->plan, form, images, n, out, st);
         return rc ? fail(BNM_E_CUDA, "fused %s kernel launch failed (%d): %s", kernel, rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
     const size_t chunk = slot_feat ? n : std::min(n, chunk_max);
@@ -548,17 +539,16 @@ static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const Infe
             fc_in = feat;
             fc_stride = m->feat_stride;
         }
-        int32_t *lg = out.logits ? out.logits + b * m->n_classes : nullptr;
-        uint32_t *lb = out.labels ? out.labels + b : nullptr;
-        const TopKOutputs topk = topk_from<int32_t>(out.topk, b);
+        int32_t *lg = out.logits ? static_cast<int32_t *>(out.logits) + b * m->n_classes : nullptr;
+        FcOutputs o{lg, out.labels ? out.labels + b : nullptr, nullptr, topk_from<int32_t>(out.topk, b)};
         if (fused) {
             GatherDst gchunk;
-            if (out.gather) { gchunk = *out.gather; gchunk.row_offset += b; }
-            if ((rc = fc_chain_launch(m->plan, form, fc_in, nb, lg, lb, 0, out.gather ? &gchunk : nullptr, st, nullptr, k ? &topk : nullptr)))
+            if (out.gather) { gchunk = *out.gather; gchunk.row_offset += b; o.gather = &gchunk; }
+            if ((rc = fc_chain_launch(m->plan, form, fc_in, nb, o, st)))
                 return fail(BNM_E_CUDA, "fused %s kernel launch failed (%d)", kernel, rc);
         } else {
-            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, lb, st))) return rc;
-            if (k) launch_topk_rows(m->d_acc.p, m->n_classes, k, topk.classes, static_cast<int32_t *>(topk.scores), nb, st);   // last layer's accumulators
+            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, o.labels, st))) return rc;
+            if (k) launch_topk_rows(m->d_acc.p, m->n_classes, k, o.topk.classes, static_cast<int32_t *>(o.topk.scores), nb, st);   // last layer's accumulators
         }
     }
     return launch_status();
@@ -573,7 +563,7 @@ static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32
     CU_TRY(cudaSetDevice(m->device));
     if (gather && bnm_model_active_path(m) != BNM_PATH_TCGEN05)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
-    return run_c_engine(m, images, n, InferOut{logits, labels, gather, {}}, static_cast<cudaStream_t>(stream));
+    return run_c_engine(m, images, n, FcOutputs{logits, labels, gather}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
@@ -675,7 +665,7 @@ static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *lo
 
 // the C engine on host buffers in chunks of chunk_images, each through one slot's buffers: images in, run_c_engine, out's arrays
 // back.  Synchronous.
-static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const InferOut &out) {
+static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const FcOutputs &out) {
     const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
     // per image, in 4-byte words: d_logits holds the logits or the top-k scores (bnm_infer_batch sizes it and d_labels whether or
     // not it takes them), d_classes the top-k classes
@@ -698,13 +688,13 @@ static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const I
     // the layer-by-layer path shares one scratch arena (accumulators / activations): its chunks must not overlap in time -> one
     // stream.  The fused path has no shared state (CNN models: one feature buffer per slot) and uses all three.
     const bool shared_scratch = bnm_model_active_path(m) != BNM_PATH_TCGEN05;
-    int32_t *h_logits = k ? static_cast<int32_t *>(out.topk.scores) : out.logits;   // where d_logits goes
+    int32_t *h_logits = static_cast<int32_t *>(k ? out.topk.scores : out.logits);   // where d_logits goes
     size_t c = 0;
     for (size_t b = 0; b < n; b += chunk, c++) {
         const size_t nb = std::min(chunk, n - b);
         PipeSlot &s = m->slots[shared_scratch ? 0 : c % 3];
         CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
-        const InferOut d{out.logits ? s.d_logits.p : nullptr, out.labels ? s.d_labels.p : nullptr, nullptr,
+        const FcOutputs d{out.logits ? s.d_logits.p : nullptr, out.labels ? s.d_labels.p : nullptr, nullptr,
                          {(uint32_t)k, s.d_classes.p, out.topk.scores ? s.d_logits.p : nullptr}};
         if (int rc = run_c_engine(m, s.d_images.p, nb, d, s.stream, shared_scratch ? nullptr : s.d_feat.p)) return rc;
         if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, s.d_classes.p, nb * k * 4, cudaMemcpyDeviceToHost, s.stream));
@@ -721,7 +711,7 @@ extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);
-    return infer_pipelined(m, images, n, InferOut{logits, labels, nullptr, {}});
+    return infer_pipelined(m, images, n, FcOutputs{logits, labels});
 }
 
 extern "C" void *bnm_host_alloc(size_t bytes) {
@@ -862,7 +852,7 @@ extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, siz
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool fused_fc = bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST;
     if (fused_fc && fc_chain_has_form(m->plan, kFormFloat)) {
-        int rc = fc_chain_launch(m->plan, kFormFloat, images, n, logits, labels, 0, nullptr, st);
+        int rc = fc_chain_launch(m->plan, kFormFloat, images, n, FcOutputs{logits, labels}, st);
         return rc ? fail(BNM_E_CUDA, "fused float-input kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
     CU_TRY(m->d_f32_scratch.grow(n * (size_t)m->img_bytes));
@@ -896,7 +886,7 @@ extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems
 //   * CNN models up to kCnnEmulMaxChannels channels: the front-end kernel k_cnn_emul_frontend, then fc_emul_i8_kernel on its features.
 // BNM_PATH_LAYERS, models without a fused plan and wider CNN models run the emulation kernels layer by layer.
 // -----------------------------------------------------------------------------------------------
-static int level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
+int bnm::level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
 static const size_t kEmulChunkFc = 65536, kEmulChunkCnn = 2048;   // images per pass of the layer kernels (CNN: 2 x C kB of planes each)
 
 // The emulator on device buffers, asynchronous on st: images float32 [n][img_bytes] -> logits float64 [n][n_classes] and / or labels
@@ -906,12 +896,11 @@ static const size_t kEmulChunkFc = 65536, kEmulChunkCnn = 2048;   // images per 
 static int emulate_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, cudaStream_t st,
                           const TopKOutputs &topk = {}) {
     const size_t nl = m->fc.size();
-    const int out_shift = level_shift_of(m->fc[nl - 1].enc);   // logits = last layer's accumulators / its level scale
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
     const uint32_t C = m->channels, elems = m->img_bytes, k = topk.k;
     const EmulRoute route = emul_route(m);
     if (route == kEmulFloatRow && !k) {   // fc_emul_kernel has no top-k form: top-k takes the int8 rows
-        int rc = fc_chain_launch(m->plan, kFormEmulFloat, images, n, logits, labels, out_shift, nullptr, st);
+        int rc = fc_chain_launch(m->plan, kFormEmulFloat, images, n, FcOutputs{logits, labels}, st);
         return rc ? fail(BNM_E_CUDA, "fused emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
     if (route != kEmulLayers) {
@@ -923,9 +912,8 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
             if (!cnn) launch_quantize_images(images + b * elems, elems, rows, nb, st);   // BitNetMCU.py:435-436
             else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, rows, m->feat_stride, nb, st))
                 return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
-            const TopKOutputs tk = topk_from<double>(topk, b);
-            int rc = fc_chain_launch(m->plan, k ? kFormEmulTopK : kFormEmulInt8, rows, nb, logits ? logits + b * m->n_classes : nullptr,
-                                     labels ? labels + b : nullptr, out_shift, nullptr, st, nullptr, k ? &tk : nullptr);
+            const FcOutputs out{logits ? logits + b * m->n_classes : nullptr, labels ? labels + b : nullptr, nullptr, topk_from<double>(topk, b)};
+            int rc = fc_chain_launch(m->plan, k ? kFormEmulTopK : kFormEmulInt8, rows, nb, out, st);
             if (rc) return fail(BNM_E_CUDA, "fused %s kernel launch failed (%d): %s", k ? "emulator top-k" : "int8 emulator", rc,
                                 cudaGetErrorString(cudaGetLastError()));
         }
@@ -969,7 +957,7 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
             stride = next_stride;
         }
         double *lg = k ? m->d_topk_logits.p : logits ? logits + b * m->n_classes : nullptr;
-        launch_emul_logits(m->d_acc.p, m->n_classes, out_shift, lg, labels ? labels + b : nullptr, nb, st);
+        launch_emul_logits(m->d_acc.p, m->n_classes, level_shift_of(m->fc[nl - 1].enc), lg, labels ? labels + b : nullptr, nb, st);
         if (k) {
             const TopKOutputs tk = topk_from<double>(topk, b);
             launch_topk_rows(lg, m->n_classes, k, tk.classes, static_cast<double *>(tk.scores), nb, st);
@@ -1029,8 +1017,7 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     auto *cnt = reinterpret_cast<unsigned long long *>(counts);
     if (engines_fused(m)) {
-        const EngineOutputs out{labels_py, truth, cnt};
-        int rc = fc_chain_launch(m->plan, kFormEngines, images, n, nullptr, labels_c, 0, nullptr, st, &out);
+        int rc = fc_chain_launch(m->plan, kFormEngines, images, n, FcOutputs{nullptr, labels_c, nullptr, {}, {labels_py, truth, cnt}}, st);
         return rc ? fail(BNM_E_CUDA, "fused two-engine kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
     const size_t chunk = std::min(n, kEnginesChunk), elems = m->img_bytes;
@@ -1076,7 +1063,7 @@ static std::string topk_c_route(const bnm_model *m) {
     std::string s;
     if (m->model_class == BNM_MODEL_CNNMNIST)
         s = cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
-    if (bnm_model_active_path(m) == BNM_PATH_TCGEN05) return s + "fc_topk_kernel" + fc_chain_form_name(m->plan, kFormTopK);
+    if (bnm_model_active_path(m) == BNM_PATH_TCGEN05) return s + fc_chain_form_name(m->plan, kFormTopK);
     return s + "layer by layer + k_topk_rows<int32>";
 }
 
@@ -1085,7 +1072,7 @@ extern "C" int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t 
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk_device: %s\n", topk_c_route(m).c_str());
-    return run_c_engine(m, images, n, InferOut{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
+    return run_c_engine(m, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
@@ -1099,7 +1086,7 @@ extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         launch_quantize_images(images + b * elems, (uint32_t)elems, m->d_f32_scratch.p, nb, st);
-        const InferOut out{nullptr, nullptr, nullptr, {k, classes + b * k, scores ? scores + b * k : nullptr}};
+        const FcOutputs out{nullptr, nullptr, nullptr, {k, classes + b * k, scores ? scores + b * k : nullptr}};
         if (int rc = run_c_engine(m, m->d_f32_scratch.p, nb, out, st)) return rc;
     }
     return 0;
@@ -1110,7 +1097,7 @@ extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (m->verbose && emul_route(m) == kEmulLayers) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: layer by layer + k_topk_rows<double>\n");
-    else if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: %s + fc_topk_kernel%s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulTopK));
+    else if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: %s + %s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulTopK));
     return emulate_device(m, images, n, nullptr, nullptr, static_cast<cudaStream_t>(stream), TopKOutputs{k, classes, scores});
 }
 
@@ -1120,7 +1107,7 @@ extern "C" int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk: %s\n", topk_c_route(m).c_str());
-    return infer_pipelined(m, images, n, InferOut{nullptr, nullptr, nullptr, {k, classes, scores}});
+    return infer_pipelined(m, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}});
 }
 
 // -----------------------------------------------------------------------------------------------

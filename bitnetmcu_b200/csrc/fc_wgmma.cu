@@ -18,7 +18,7 @@
 // work of ReLUNorm, which bounds this kernel.  Weights of every encoding are pre-decoded once per model into int8 planes
 // (kernels.h FcLayerDev); FP130's +128 does not fit s8 and is carried by a second residual plane accumulated into the same D.
 // All arithmetic is integer: results are bit-exact with the reference.
-#include <array>
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -36,6 +36,14 @@ constexpr uint32_t kEmptyArrivals = 8;     // a stage is free once the 8 warps o
 constexpr uint32_t kFloatQuantWarps = 8;   // float-input path: quantiser warps per CTA (one pipe next to them)
 constexpr uint32_t kFloatRowsPerWarp = 128 / kFloatQuantWarps;   // rows of every tile per quantiser warp
 constexpr uint32_t kFloatGroupRows = 4;    // rows per bulk copy of a quantiser warp (4 kB for 256-element rows) = rows per pass
+
+// What a launch form computes (the form table, host side below).  Rule: the hidden-layer rule -- the C engine's (inference.c),
+// the reference's Python emulator's (emul_coef, float64 logits), or both on one tile (layer 1 once, its accumulators through
+// both rules, then the C chain and the emulator's chain).  Outputs: logits and labels (the C engine on int8 rows also stores
+// them to the result exchange's destinations); both engines' labels and their EngineTally counts; or the k best classes of
+// every row and their scores, from k rounds of the epilogue's argmax.
+enum FcRule { kRuleC, kRuleEmul, kRuleBoth };
+enum FcOut { kOutLogits, kOutEngines, kOutTopK };
 
 struct ChainParams {
     int n_layers;
@@ -313,23 +321,16 @@ struct RingPos {
 // kLastN: wgmma width of the last layer -- 16 when the plan's last layer is at most 16 wide (every classifier head), else kN.
 // kFixed: the two-slot kernel specialised for the shape class above: no plane loop, no zero-tile selects, layer 1 issued as
 // one unrolled run of MMAs at compile-time descriptor offsets, ReLUNorm without predicates.
-// kEmul: the reference's Python emulator instead of the C engine (fc_emul_kernel): its hidden-layer rule (emul_coef) and float64
-// logits (P.emul_logits); no result exchange.
-// kEngines: both engines on one tile (fc_engines_kernel): layer 1 once, its accumulators through both hidden-layer rules, the C
-// chain and then the emulator's chain, both labels and their EngineTally counts; no logits, no result exchange.
-// kTopK: the k best classes of every row and their scores (fc_topk_kernel) in place of logits and label: k rounds of the
-// epilogue's argmax, each over the columns ranked below the previous round's pick.
+// kRule, kOut: the rule and the outputs of the launch form (the form table, host side below).
 // The body of the kernels below; tmap_in and P are their __grid_constant__ parameters (TMA reads the tensor map by address).
-template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, bool kEmul, bool kEngines = false, bool kTopK = false>
+template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, FcRule kRule, FcOut kOut>
 __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const ChainParams &P) {
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
-    static_assert(!kEmul || (kPipes == 1 && kSlots == 1 && kLastN == kN && !kFixed && (kN == 64 || !kFloatIn)),
-                  "emulator: the 64-wide float-input launch, or one-pipe one-slot int8 launches at full width");
-    static_assert(!kEngines || (kN == 64 && kPipes == 1 && kFloatIn && kSlots == 1 && kLastN == kN && !kFixed && !kEmul),
-                  "both engines: the 64-wide float-input launch");
-    static_assert(!kTopK || (kPipes == 1 && kSlots == 1 && !kFloatIn && kLastN == kN && !kFixed && !kEngines),
-                  "top-k: one-pipe one-slot int8 launches at full width");
-    static_assert(!kFloatIn || kPipes == 1, "float input: one pipe, whose stages the quantiser warps fill");
+    static_assert((kRule == kRuleC && kOut == kOutLogits) || (kPipes == 1 && kSlots == 1 && kLastN == kN && !kFixed),
+                  "the emulator, both engines and top-k: one-pipe one-slot launches at full width");
+    static_assert((kRule == kRuleBoth) == (kOut == kOutEngines), "both rules: the engines' outputs, which need both");
+    static_assert(!kFloatIn || (kPipes == 1 && kN == 64),
+                  "float input: one pipe, whose stages the quantiser warps fill; 17 warps leave 96 registers, enough for 64 wide");
     static_assert(kLastN == kN || (kLastN == 16 && kSlots == 2), "narrow last layer: two-slot launches");
     static_assert(!kFixed || (kSlots == 2 && kLastN == fixed_n_pad(kFixedLayers - 1)), "fixed shape: two-slot launches of its class");
     constexpr bool kProducerWG = producer_warpgroup<kN, kSlots>();
@@ -432,7 +433,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
         const uint32_t ncls = P.n_classes;
         // labels-only launches pass no logits buffer.  The shuffle is a value no-op (a uniform flag), kept for ptxas: testing
         // P.logits at the store instead serialises the fixed-shape kernel's wgmma pipeline (C7511, CUDA 12.9).
-        const bool has_logits = __shfl_sync(0xffffffffu, (uint32_t)(kEmul ? P.emul_logits != nullptr : P.logits != nullptr), 0);
+        const bool has_logits = __shfl_sync(0xffffffffu, (uint32_t)(kRule == kRuleEmul ? P.emul_logits != nullptr : P.logits != nullptr), 0);
         mbar_wait(&bar_w, 0, P.err, 6);   // weight tiles are in shared memory
         // B descriptor of the 64 columns from c0 of the K-step tile at smem address t (no-swizzle K-major: 8-row groups 256 B apart).
         // Every wgmma is issued at the kernel's full width kN, with no condition around it (a conditional wgmma cannot stay in
@@ -510,7 +511,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                 }
             }
         };
-        auto relunorm = [&](const uint32_t *a, uint32_t *f, int l) { relunorm_rule(a, f, l, std::bool_constant<kEmul>{}); };
+        auto relunorm = [&](const uint32_t *a, uint32_t *f, int l) { relunorm_rule(a, f, l, std::bool_constant<kRule == kRuleEmul>{}); };
         // ---- layer l >= 1 into a (A: the fragments f)
         auto issue_layer = [&](uint32_t *a, const uint32_t *f, int l) {
             if constexpr (kFixed) {
@@ -551,7 +552,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                         wgmma_rs_n64(a + c0 / 2, f + 4 * k, b_desc((uint32_t)c0 < n_pad ? bt : w_zero, c0), (pl | k) != 0);
                 }
         };
-        // ---- kTopK: the k best classes of tile i and their scores from the last layer's accumulators a, in place of the epilogue
+        // ---- kOutTopK: the k best classes of tile i and their scores from the last layer's accumulators a, in place of the epilogue
         // below.  k rounds of its argmax: round 0 is that argmax; round t > 0 takes the first maximum of the columns ranked after
         // round t - 1's pick (v, p) -- x < v, or x == v at a column >= q = p + 1.  So the picks are the row's classes by logit,
         // highest first, ties to the lower class (np.argsort(-x, kind="stable")), with no exclusion mask: (v, q) per row is all the
@@ -592,7 +593,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                     if (((t & 3) == 3 || t + 1 == k) && img < P.n && quad <= (t & 3)) {
                         const size_t o = img * k + (t & ~3u) + quad;
                         P.classes[o] = my_cls;
-                        if constexpr (kEmul) {
+                        if constexpr (kRule == kRuleEmul) {
                             if (P.scores_f64) P.scores_f64[o] = (double)my_score * P.emul_logit_scale;   // exact, as the logits
                         } else {
                             if (P.scores_i32) P.scores_i32[o] = my_score;
@@ -627,7 +628,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                     const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, sh);
                     if (ob > best || (ob == best && op < pos)) { best = ob; pos = op; }
                 }
-                if (kEmul && img < P.n) {
+                if (kRule == kRuleEmul && img < P.n) {
                     // float64 logits: (double)acc x 2^-level_shift is exact, and argmax of the int32 accumulators is that of them
                     if (has_logits) {
                         double *d = P.emul_logits + img * ncls;
@@ -678,7 +679,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
         };
 
         RingPos ring;   // ring position of the pipe's next tile
-        if constexpr (kEngines) {
+        if constexpr (kOut == kOutEngines) {
             // Both engines scale the image alike and multiply it by the same weights (the emulator's level scale cancels, see
             // emul_coef), so their layer-1 accumulators are the same: layer 1 runs once and feeds both hidden-layer rules, the
             // emulator's fragments in afr_py.  Then the C chain and the emulator's chain run one after the other from their own
@@ -782,7 +783,7 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                         BNM_TRACE(TR_WAIT_END, 0, l + 1);
                         continue;
                     }
-                    if constexpr (kTopK) topk_epilogue(acc[0], i);
+                    if constexpr (kOut == kOutTopK) topk_epilogue(acc[0], i);
                     else epilogue(acc[0], i);
                     BNM_TRACE(TR_EPI_END, 0, 0);
                     break;
@@ -926,14 +927,14 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
 template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
 __global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn, kSlots>(), 1)
 fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed, false>(tmap_in, P);
+    fc_chain_body<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed, kRuleC, kOutLogits>(tmap_in, P);
 }
 
 // QuantizedModel.inference_quantized (BitNetMCU.py:420-535) of FC models: the float-input launch <64,1,float> with the emulator's
 // hidden-layer rule and float64 logits.  The input scaling of BitNetMCU.py:435-436 is the quantiser warps' (test_inference.py:140-141).
 __global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
 fc_emul_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<64, 1, true, 1, 64, false, true>(tmap_in, P);
+    fc_chain_body<64, 1, true, 1, 64, false, kRuleEmul, kOutLogits>(tmap_in, P);
 }
 
 // The same emulator on int8 rows that are already scaled (k_quantize_images, or the features of k_cnn_emul_frontend): TMA
@@ -941,14 +942,14 @@ fc_emul_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
 template <int kN>
 __global__ void __launch_bounds__(chain_threads<kN, 1, false, 1>(), 1)
 fc_emul_i8_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<kN, 1, false, 1, kN, false, true>(tmap_in, P);
+    fc_chain_body<kN, 1, false, 1, kN, false, kRuleEmul, kOutLogits>(tmap_in, P);
 }
 
 // The reference's check of its two engines (test_inference.py:130-175) in one pass: the float-input launch <64,1,float> that
 // runs the C engine's chain and the emulator's after one shared layer 1, and writes both labels and their counts.
 __global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
 fc_engines_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<64, 1, true, 1, 64, false, false, true>(tmap_in, P);
+    fc_chain_body<64, 1, true, 1, 64, false, kRuleBoth, kOutEngines>(tmap_in, P);
 }
 
 // Top-k on int8 rows: the chain of fc_chain_kernel (kEmul false) or of fc_emul_i8_kernel (true) on one pipe and one slot at the
@@ -956,7 +957,7 @@ fc_engines_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
 template <int kN, bool kEmul>
 __global__ void __launch_bounds__(chain_threads<kN, 1, false, 1>(), 1)
 fc_topk_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<kN, 1, false, 1, kN, false, kEmul, false, true>(tmap_in, P);
+    fc_chain_body<kN, 1, false, 1, kN, false, kEmul ? kRuleEmul : kRuleC, kOutTopK>(tmap_in, P);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1002,56 +1003,57 @@ static void trace_before(cudaStream_t) {}
 static void trace_after(cudaStream_t) {}
 #endif
 
-// the instantiations of fc_chain_kernel, fc_emul_kernel, fc_emul_i8_kernel, fc_engines_kernel and fc_topk_kernel, one row each,
-// named by their template arguments <kN, kPipes, kSlots, kLastN>
+// a kernel row: one __global__ instantiation, named by its function and its template arguments <kN, kPipes, kSlots, kLastN>
 struct ChainKernel {
     const char *name;
     void (*fn)(CUtensorMap, ChainParams);
     int threads;
 };
-template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
-static ChainKernel chain_kernel(const char *name) {
-    return {name, fc_chain_kernel<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed>, chain_threads<kN, kPipes, kFloatIn, kSlots>()};
+template <int kN, int kPipes = 1, bool kFloatIn = false, int kSlots = 1>
+static constexpr ChainKernel row(const char *name, void (*fn)(CUtensorMap, ChainParams)) {
+    return {name, fn, chain_threads<kN, kPipes, kFloatIn, kSlots>()};
 }
-template <int kN>
-static ChainKernel emul_i8_kernel(const char *name) { return {name, fc_emul_i8_kernel<kN>, chain_threads<kN, 1, false, 1>()}; }
-template <int kN, bool kEmul>
-static ChainKernel topk_kernel(const char *name) { return {name, fc_topk_kernel<kN, kEmul>, chain_threads<kN, 1, false, 1>()}; }
-enum ChainRow {
-    kRow64, kRow64x2, kRow64x2Last16, kRowFixed, kRow128, kRow192, kRow256, kRowFloat,
-    kRowEmulFloat,
-    kRowEmul64, kRowEmul128, kRowEmul192, kRowEmul256,   // row kRowEmul64 + max_n / 64 - 1
-    kRowEngines,
-    kRowTopK64, kRowTopK128, kRowTopK192, kRowTopK256,   // likewise from kRowTopK64 / kRowEmulTopK64
-    kRowEmulTopK64, kRowEmulTopK128, kRowEmulTopK192, kRowEmulTopK256,
-    kChainRows
+
+// The launch forms, indexed by FcForm.  A launch takes everything but its buffers from its form's entry.
+struct FormSpec {
+    bool float_in;           // float32 rows through the quantiser warps, else int8 rows over TMA
+    FcRule rule;
+    FcOut out;               // kOutLogits: the C engine on int8 rows alone also takes result-exchange destinations
+    uint32_t stage_cap;      // stages per pipe at most
+    ChainKernel rows[4];     // by accumulator width 64, 128, 192, 256; fn null: the form has no row at that width
 };
-static const std::array<ChainKernel, kChainRows> kChainKernels = [] {
-    std::array<ChainKernel, kChainRows> t{};
-    t[kRow64] = chain_kernel<64, 1, false>("<64,1>");
-    t[kRow64x2] = chain_kernel<64, 2, false, 2>("<64,2,2,64>");
-    t[kRow64x2Last16] = chain_kernel<64, 2, false, 2, 16>("<64,2,2,16>");
-    t[kRowFixed] = chain_kernel<64, 2, false, 2, 16, true>("<64,2,2,16,fixed>");
-    t[kRow128] = chain_kernel<128, 1, false>("<128,1>");
-    t[kRow192] = chain_kernel<192, 1, false>("<192,1>");
-    t[kRow256] = chain_kernel<256, 1, false>("<256,1>");
-    t[kRowFloat] = chain_kernel<64, 1, true>("<64,1,float>");
-    t[kRowEmulFloat] = {"<64,1,float,emul>", fc_emul_kernel, chain_threads<64, 1, true, 1>()};
-    t[kRowEmul64] = emul_i8_kernel<64>("<64,1,emul>");
-    t[kRowEmul128] = emul_i8_kernel<128>("<128,1,emul>");
-    t[kRowEmul192] = emul_i8_kernel<192>("<192,1,emul>");
-    t[kRowEmul256] = emul_i8_kernel<256>("<256,1,emul>");
-    t[kRowEngines] = {"<64,1,float,engines>", fc_engines_kernel, chain_threads<64, 1, true, 1>()};
-    t[kRowTopK64] = topk_kernel<64, false>("<64,1,topk>");
-    t[kRowTopK128] = topk_kernel<128, false>("<128,1,topk>");
-    t[kRowTopK192] = topk_kernel<192, false>("<192,1,topk>");
-    t[kRowTopK256] = topk_kernel<256, false>("<256,1,topk>");
-    t[kRowEmulTopK64] = topk_kernel<64, true>("<64,1,emul,topk>");
-    t[kRowEmulTopK128] = topk_kernel<128, true>("<128,1,emul,topk>");
-    t[kRowEmulTopK192] = topk_kernel<192, true>("<192,1,emul,topk>");
-    t[kRowEmulTopK256] = topk_kernel<256, true>("<256,1,emul,topk>");
-    return t;
-}();
+// The float-input forms have a 64-wide row only: the eight quantiser warps make 17 warps, so at most 96 registers per thread.
+static const FormSpec kForms[kFcForms] = {
+    // kFormInt8; a 64-wide plan with room for two pipes takes one of kTwoPipeRows instead of the one-pipe row
+    {false, kRuleC, kOutLogits, 6,
+     {row<64>("fc_chain_kernel<64,1>", fc_chain_kernel<64, 1, false>), row<128>("fc_chain_kernel<128,1>", fc_chain_kernel<128, 1, false>),
+      row<192>("fc_chain_kernel<192,1>", fc_chain_kernel<192, 1, false>), row<256>("fc_chain_kernel<256,1>", fc_chain_kernel<256, 1, false>)}},
+    // kFormFloat
+    {true, kRuleC, kOutLogits, 4, {row<64, 1, true>("fc_chain_kernel<64,1,float>", fc_chain_kernel<64, 1, true>)}},
+    // kFormEmulFloat
+    {true, kRuleEmul, kOutLogits, 4, {row<64, 1, true>("fc_emul_kernel<64,1,float,emul>", fc_emul_kernel)}},
+    // kFormEmulInt8
+    {false, kRuleEmul, kOutLogits, 6,
+     {row<64>("fc_emul_i8_kernel<64,1,emul>", fc_emul_i8_kernel<64>), row<128>("fc_emul_i8_kernel<128,1,emul>", fc_emul_i8_kernel<128>),
+      row<192>("fc_emul_i8_kernel<192,1,emul>", fc_emul_i8_kernel<192>), row<256>("fc_emul_i8_kernel<256,1,emul>", fc_emul_i8_kernel<256>)}},
+    // kFormEngines
+    {true, kRuleBoth, kOutEngines, 4, {row<64, 1, true>("fc_engines_kernel<64,1,float,engines>", fc_engines_kernel)}},
+    // kFormTopK
+    {false, kRuleC, kOutTopK, 6,
+     {row<64>("fc_topk_kernel<64,1,topk>", fc_topk_kernel<64, false>), row<128>("fc_topk_kernel<128,1,topk>", fc_topk_kernel<128, false>),
+      row<192>("fc_topk_kernel<192,1,topk>", fc_topk_kernel<192, false>), row<256>("fc_topk_kernel<256,1,topk>", fc_topk_kernel<256, false>)}},
+    // kFormEmulTopK
+    {false, kRuleEmul, kOutTopK, 6,
+     {row<64>("fc_topk_kernel<64,1,emul,topk>", fc_topk_kernel<64, true>), row<128>("fc_topk_kernel<128,1,emul,topk>", fc_topk_kernel<128, true>),
+      row<192>("fc_topk_kernel<192,1,emul,topk>", fc_topk_kernel<192, true>), row<256>("fc_topk_kernel<256,1,emul,topk>", fc_topk_kernel<256, true>)}},
+};
+// kFormInt8's two-pipe two-slot rows: the last layer at full width, 16 wide (kLastN, for heads of at most 16 classes), or the
+// fixed-shape kernel
+static const ChainKernel kTwoPipeRows[3] = {
+    row<64, 2, false, 2>("fc_chain_kernel<64,2,2,64>", fc_chain_kernel<64, 2, false, 2>),
+    row<64, 2, false, 2>("fc_chain_kernel<64,2,2,16>", fc_chain_kernel<64, 2, false, 2, 16>),
+    row<64, 2, false, 2>("fc_chain_kernel<64,2,2,16,fixed>", fc_chain_kernel<64, 2, false, 2, 16, true>),
+};
 
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
                                   char *err, size_t err_len) {
@@ -1084,58 +1086,51 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     p.zero_off = w_off;                    // [max_n x 32 B] of zeros behind the layers (cudaMemset below)
     p.w_bytes = w_off + max_n * 32;
     p.n_classes = layers[n_layers - 1].n_out;
+    p.emul_logit_scale = level_shift_of(layers[n_layers - 1].enc) ? 0.5 : 1.0;
     const uint32_t smem_limit = 227 * 1024 - 1024 /*alignment slack*/ - 1024 /*static: barriers*/;
     const uint32_t w_fixed = round_up(p.w_bytes, 128);
     if (w_fixed + 2 * p.stage_bytes > smem_limit) { delete plan; return fail("fused path: weights do not fit in shared memory"); }
-    // the layout of a form: `pipes` rings of at most `cap` stages each in what the weight image and `extra` bytes (the float-input
-    // forms' quantiser rings) leave, then the weights, then the extra bytes
-    auto layout = [&](int row, uint32_t pipes, uint32_t cap, uint32_t extra) {
-        FormLayout f;
-        f.kernel = &kChainKernels[row];
-        f.n_stages = std::min<uint32_t>(cap, (smem_limit - w_fixed - extra) / p.stage_bytes / pipes);
-        f.off_w = pipes * f.n_stages * p.stage_bytes;
-        f.off_fring = extra ? f.off_w + w_fixed : 0;
-        // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared
-        // memory enforces it once a CTA asks for more than half of the SM's 227 kB.
-        f.smem_bytes = std::max<size_t>((size_t)f.off_w + w_fixed + extra + 1024, 116 * 1024);
-        return f;
-    };
+    // the int8 C-engine form of a 64-wide model runs two pipes where four stages fit.  Two pipes run two slots, which issue a last
+    // layer of at most 16 columns 16 wide (kLastN); plans of exactly the fixed shape class (kFixedLayers and the fixed_* shapes)
+    // run the fixed-shape kernel
     const uint32_t pipes = (max_n == 64 && (smem_limit - w_fixed) / p.stage_bytes >= 4) ? 2 : 1;
-    // two pipes run two slots, which issue a last layer of at most 16 columns 16 wide (kLastN); plans of exactly the fixed
-    // shape class (kFixedLayers and the fixed_* shapes) run the fixed-shape kernel
     const bool last16 = layers[n_layers - 1].n_pad <= 16;
     bool fixed = pipes == 2 && last16 && n_layers == kFixedLayers && p.in_atoms == kFixedInAtoms;
     for (int l = 0; l < n_layers && fixed; l++)
         fixed = p.planes[l] == 1 && p.n_pad[l] == fixed_n_pad(l) && p.k_steps[l] == fixed_k_steps(l) && p.b_off[l] == fixed_b_off(l);
-    int row = max_n == 64 ? kRow64 : max_n == 128 ? kRow128 : max_n == 192 ? kRow192 : kRow256;
-    if (pipes == 2) row = fixed ? kRowFixed : last16 ? kRow64x2Last16 : kRow64x2;
-    FormLayout *forms = plan->forms;
-    // at most kMaxStages over the pipes and 6 per pipe; >= 2 with two pipes: two tile slots need it
-    forms[kFormInt8] = layout(row, pipes, std::min<uint32_t>(kMaxStages / pipes, 6), 0);
-    // float-input forms: the eight quantiser warps make 17 warps, so at most 96 registers per thread -- models up to 64 wide.
-    // One pipe, fewer int8 stages, the freed shared memory holds the quantiser warps' float rings
+    // the float-input forms (one pipe, fewer int8 stages) hold the quantiser warps' float rings in the shared memory they free:
+    // rows of at most 256 elements and at most 16 classes
     const uint32_t fring = kFloatQuantWarps * 2 * kFloatGroupRows * 1024;
-    if (in_bytes <= 256 && p.n_classes <= 16 && max_n == 64 && w_fixed + fring + 2 * p.stage_bytes <= smem_limit) {
-        forms[kFormFloat] = layout(kRowFloat, 1, 4, fring);
-        forms[kFormEmulFloat] = layout(kRowEmulFloat, 1, 4, fring);
-        forms[kFormEngines] = layout(kRowEngines, 1, 4, fring);
+    const bool float_fits = in_bytes <= 256 && p.n_classes <= 16 && w_fixed + fring + 2 * p.stage_bytes <= smem_limit;
+    FormLayout *forms = plan->forms;
+    for (int f = 0; f < kFcForms; f++) {
+        const FormSpec &s = kForms[f];
+        const uint32_t np = f == kFormInt8 ? pipes : 1;
+        const ChainKernel *k = np == 2 ? &kTwoPipeRows[fixed ? 2 : last16 ? 1 : 0] : &s.rows[max_n / 64 - 1];
+        if (!k->fn || (s.float_in && !float_fits)) continue;
+        // the layout: np rings of stages in what the weight image and `extra` bytes (the float rings) leave, at most kMaxStages
+        // over the pipes (>= 2 per pipe with two: two tile slots need it), then the weights, then the extra bytes
+        FormLayout &l = forms[f];
+        const uint32_t extra = s.float_in ? fring : 0;
+        l.kernel = k;
+        l.n_stages = std::min({s.stage_cap, kMaxStages / np, (smem_limit - w_fixed - extra) / p.stage_bytes / np});
+        l.off_w = np * l.n_stages * p.stage_bytes;
+        l.off_fring = extra ? l.off_w + w_fixed : 0;
+        // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared
+        // memory enforces it once a CTA asks for more than half of the SM's 227 kB.
+        l.smem_bytes = std::max<size_t>((size_t)l.off_w + w_fixed + extra + 1024, 116 * 1024);
     }
-    // the emulator on int8 rows runs one pipe at every width, so a 64-wide plan, whose int8 form runs two, has its own layout
-    forms[kFormEmulInt8] = layout(kRowEmul64 + max_n / 64 - 1, 1, 6, 0);
-    // top-k forms: the same one-pipe layout, for either rule
-    forms[kFormTopK] = layout(kRowTopK64 + max_n / 64 - 1, 1, 6, 0);
-    forms[kFormEmulTopK] = layout(kRowEmulTopK64 + max_n / 64 - 1, 1, 6, 0);
     if (getenv("BNM_VERBOSE")) {   // diagnostics: the shapes this plan launches
         const bool has_float = forms[kFormFloat].kernel;
+        auto args = [&](FcForm f) { return has_float ? strchr(forms[f].kernel->name, '<') : ""; };   // the template arguments
         char f_stages[32] = "";
         if (has_float) snprintf(f_stages, sizeof(f_stages), ", float input stages %u", forms[kFormFloat].n_stages);
         fprintf(stderr, "bitnetmcu_b200: fused FC plan: %u accumulator columns, %u pipes x %u stages, %u weight bytes, %zu B smem, "
-                "fc_chain_kernel%s%s%s%s%s%s, int8 emulator fc_emul_i8_kernel%s x %u stages\n", max_n, pipes, forms[kFormInt8].n_stages,
-                p.w_bytes, forms[kFormInt8].smem_bytes, forms[kFormInt8].kernel->name, has_float ? ", float input " : "",
-                has_float ? forms[kFormFloat].kernel->name : "", has_float ? ", emulator " : "",
-                has_float ? forms[kFormEmulFloat].kernel->name : "", f_stages, forms[kFormEmulInt8].kernel->name,
+                "%s%s%s%s%s%s, int8 emulator %s x %u stages\n", max_n, pipes, forms[kFormInt8].n_stages, p.w_bytes,
+                forms[kFormInt8].smem_bytes, forms[kFormInt8].kernel->name, has_float ? ", float input " : "", args(kFormFloat),
+                has_float ? ", emulator " : "", args(kFormEmulFloat), f_stages, forms[kFormEmulInt8].kernel->name,
                 forms[kFormEmulInt8].n_stages);
-        fprintf(stderr, "bitnetmcu_b200: fused FC top-k forms: fc_topk_kernel%s x %u stages, emulator fc_topk_kernel%s x %u stages, %zu B smem\n",
+        fprintf(stderr, "bitnetmcu_b200: fused FC top-k forms: %s x %u stages, emulator %s x %u stages, %zu B smem\n",
                 forms[kFormTopK].kernel->name, forms[kFormTopK].n_stages, forms[kFormEmulTopK].kernel->name, forms[kFormEmulTopK].n_stages,
                 forms[kFormTopK].smem_bytes);
     }
@@ -1211,43 +1206,40 @@ const char *fc_chain_form_name(const FcChainPlan *plan, FcForm f) { return plan-
 
 static const CUtensorMap kNoTensorMap{};   // the float-input forms' tensor map: not used (no TMA image loads)
 
-int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
-                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines, const TopKOutputs *topk) {
+int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
     const FormLayout &form = plan->forms[f];
     if (!form.kernel) return -6;
-    if ((f == kFormEngines) != (engines != nullptr) || (engines && logits)) return -5;
-    const bool topk_form = f == kFormTopK || f == kFormEmulTopK;
-    if (topk_form != (topk != nullptr) || (topk && (logits || labels || !topk->classes || topk->k == 0 || topk->k > plan->p.n_classes)))
+    const FormSpec &s = kForms[f];
+    // the C engine on int8 rows: the one form with result-exchange destinations and overlapping launches
+    const bool engine_i8 = !s.float_in && s.rule == kRuleC && s.out == kOutLogits;
+    const EngineOutputs &e = out.engines;
+    const TopKOutputs &t = out.topk;
+    if ((out.logits && s.out != kOutLogits) || (out.gather && !engine_i8) || ((e.labels_py || e.truth || e.counts) && s.out != kOutEngines) ||
+        (s.out == kOutTopK) != (t.k != 0) || (t.k && (out.labels || !t.classes || t.k > plan->p.n_classes)))
         return -5;
-    const bool engine_i8 = f == kFormInt8, float_in = f == kFormFloat || f == kFormEmulFloat || f == kFormEngines;
-    ChainParams p = plan->p;   // the model's shapes; null outputs, no result exchange
+    ChainParams p = plan->p;   // the model's shapes and the emulator's logit scale; null outputs, no result exchange
     p.n_stages = form.n_stages;
     p.off_w = form.off_w;
     p.off_fring = form.off_fring;
-    if (topk) {
-        p.k = topk->k;
-        p.classes = topk->classes;
-        if (f == kFormEmulTopK) p.scores_f64 = static_cast<double *>(topk->scores);
-        else p.scores_i32 = static_cast<int32_t *>(topk->scores);
-    }
-    if (f == kFormEmulFloat || f == kFormEmulInt8 || f == kFormEmulTopK) {
-        p.emul_logits = static_cast<double *>(logits);
-        p.emul_logit_scale = level_shift ? 0.5 : 1.0;
+    if (s.rule == kRuleEmul) {
+        p.emul_logits = static_cast<double *>(out.logits);
+        p.scores_f64 = static_cast<double *>(t.scores);
     } else {
-        p.logits = static_cast<int32_t *>(logits);
+        p.logits = static_cast<int32_t *>(out.logits);
+        p.scores_i32 = static_cast<int32_t *>(t.scores);
     }
-    p.labels = labels;
-    if (engines) {
-        p.labels_py = engines->labels_py;
-        p.truth = engines->truth;
-        p.counts = engines->counts;
-    }
+    p.labels = out.labels;
+    p.labels_py = e.labels_py;
+    p.truth = e.truth;
+    p.counts = e.counts;
+    p.k = t.k;
+    p.classes = t.classes;
     p.n = n;
     p.n_tiles = (uint32_t)((n + kTileM - 1) / kTileM);
-    if (gather) {
-        if (!engine_i8 || gather->n_labels_dst > (uint32_t)kMaxGatherDst || gather->n_logits_dst > (uint32_t)kMaxGatherDst) return -5;
+    if (const GatherDst *gather = out.gather) {
+        if (gather->n_labels_dst > (uint32_t)kMaxGatherDst || gather->n_logits_dst > (uint32_t)kMaxGatherDst) return -5;
         p.n_lab_dst = gather->n_labels_dst;
         p.n_log_dst = gather->n_logits_dst;
         p.row0 = gather->row_offset;
@@ -1257,7 +1249,7 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void 
         for (uint32_t d = 0; d < p.n_log_dst; d++) p.log_dst[d] = gather->logits_dst[d];
     }
     const CUtensorMap *tmap_p = &kNoTensorMap;
-    if (float_in) {
+    if (s.float_in) {
         p.fimages = static_cast<const float *>(in);
         p.in_elems = plan->in_bytes;
     } else if (!(tmap_p = plan_tensor_map(plan, static_cast<const int8_t *>(in), n))) {
@@ -1280,8 +1272,8 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, void 
     // launch's logits the next one's images, say) / a launch of another form in between.  A null output is no buffer: it
     // neither reuses nor differs from one.
     LaunchBuffers bufs;
-    bufs.io[0] = in; bufs.io[1] = logits; bufs.io[2] = labels;
-    if (gather) {
+    bufs.io[0] = in; bufs.io[1] = out.logits; bufs.io[2] = out.labels;
+    if (out.gather) {
         for (uint32_t d = 0; d < p.n_lab_dst; d++) bufs.dst[bufs.n_dst++] = p.lab_dst[d];
         for (uint32_t d = 0; d < p.n_log_dst; d++) bufs.dst[bufs.n_dst++] = p.log_dst[d];
         bufs.row0 = p.row0;

@@ -117,41 +117,44 @@ void fc_chain_plan_destroy(FcChainPlan *p);
 // kFormInt8 launches: 0 plain launches, 1 programmatic dependent launch (inputs read after the previous kernel completed), 2 launches
 // declared independent
 void fc_chain_plan_set_overlap(FcChainPlan *p, int mode);
-// The launch forms of a plan, by input and by rule:
-//   kFormInt8       the C engine on int8 images [n][in_bytes] (device, 16B aligned): fc_chain_kernel, every plan
-//   kFormFloat      the C engine on float32 images [n][in_bytes elements], the input scaling of test_inference.py:140-141 fused
-//                   into the kernel's load stage: FC rows of up to 256 elements, models up to 64 wide with up to 16 classes
-//   kFormEmulFloat  the reference's Python emulator in place of the C engine (fc_emul_kernel): the plans with kFormFloat
-//   kFormEmulInt8   the emulator on int8 rows [n][in_bytes] that are already scaled (fc_emul_i8_kernel), every plan
-//   kFormEngines    both engines on float32 images (fc_engines_kernel): one input scaling and one layer 1, then the C engine's
-//                   and the emulator's hidden layers; both labels and the EngineTally counts, no logits.  The plans with kFormFloat
-//   kFormTopK       the C engine on int8 images, the k best classes of every row and their int32 logits (fc_topk_kernel), every plan
-//   kFormEmulTopK   the same with the emulator's rule and float64 scores, every plan
-// The emulator forms have the emulator's hidden-layer rule and float64 logits = last layer's accumulators x 2^-level_shift (0 or 1).
+// The launch forms of a plan.  fc_wgmma.cu's form table (kForms) says what each is: its input (int8 rows [n][in_bytes] over
+// TMA, device, 16B aligned; or float32 rows [n][in_bytes elements] with the input scaling of test_inference.py:140-141 fused
+// into the load stage), its rule (the C engine's, the reference's Python emulator's, or both), its outputs and its kernel rows.
+// A plan has every int8 form; the float-input forms only for models up to 64 wide with rows of up to 256 elements and up to
+// 16 classes.  The emulator's logits are the last layer's accumulators x 2^-level_shift_of(its encoding), in float64.
 enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFormEngines, kFormTopK, kFormEmulTopK, kFcForms };
 bool fc_chain_has_form(const FcChainPlan *p, FcForm f);
-// the template arguments of the kernel of a form the plan has, e.g. "<192,1,emul>"
+// the kernel of a form the plan has, e.g. "fc_emul_i8_kernel<192,1,emul>"
 const char *fc_chain_form_name(const FcChainPlan *p, FcForm f);
-// kFormEngines outputs besides `labels` (the C engine's): the emulator's labels uint32 [n], truth uint32 [n] and counts (each may be
-// null; truth only with counts)
+// the emulator's level scale of a layer is 2^level_shift_of(its encoding): 2 for 2bitsym / 4bitsym, else 1 (capi.cu)
+int level_shift_of(int32_t enc);
+// both engines' outputs besides `labels` (the C engine's): the emulator's labels uint32 [n], truth uint32 [n] and counts (each may
+// be null; truth only with counts)
 struct EngineOutputs {
     uint32_t *labels_py;
     const uint32_t *truth;
     unsigned long long *counts;
 };
-// top-k form outputs: k (1 .. n_classes) classes uint32 [n][k], required, and their scores [n][k] (int32, float64 for kFormEmulTopK)
-// or null
+// top-k outputs: k (1 .. n_classes) classes uint32 [n][k], required, and their scores [n][k] (int32, float64 for the emulator) or null
 struct TopKOutputs {
     uint32_t k;
     uint32_t *classes;
     void *scores;
 };
-// one launch of form f on n images `in` -> logits (int32 [n][n_classes], float64 for the emulator forms) and labels uint32 [n];
-// each may be null.  gather (kFormInt8 only, may be null): extra destination buffers every row is also stored to (peer memory),
-// fused into the epilogue.  engines: kFormEngines only, and required there (no logits).  topk: the top-k forms only, and required
-// there (no logits, no labels).  0, or a negative code (-6: the plan has no form f)
-int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, void *logits, uint32_t *labels, int level_shift,
-                    const GatherDst *gather, cudaStream_t st, const EngineOutputs *engines = nullptr, const TopKOutputs *topk = nullptr);
+// What a call writes, each buffer possibly null: logits (int32 [n][n_classes], float64 for the emulator) and labels uint32 [n],
+// and gather: extra destination buffers every row is also stored to (peer memory), fused into the epilogue (the C engine on int8
+// rows only).  Both engines' forms take labels and engines, no logits.  The top-k forms take topk alone, with k > 0; every other
+// form takes none (k = 0).
+struct FcOutputs {
+    void *logits;
+    uint32_t *labels;
+    const GatherDst *gather;
+    TopKOutputs topk;
+    EngineOutputs engines;
+};
+// one launch of form f on n images `in` -> out.  0, or a negative code (-5: an output the form does not take, or a missing one;
+// -6: the plan has no form f)
+int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st);
 // the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
 // [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
 constexpr uint32_t kCnnEmulMaxChannels = 128;
