@@ -4,8 +4,13 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
+#include <atomic>
+#include <chrono>
+#include <condition_variable>
 #include <cstring>
+#include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../../include/bitnetmcu_b200.h"
@@ -88,8 +93,35 @@ struct PipeSlot {
     DevBuf<int8_t> d_images;
     DevBuf<int32_t> d_logits;
     DevBuf<uint32_t> d_labels;
-    DevBuf<int8_t> d_feat;   // CNN models: this slot's own feature buffer, so that the slots' chunks may overlap in time
     DevBuf<uint32_t> d_classes;   // bnm_infer_topk: the chunk's classes (its scores go to d_logits)
+};
+
+// One staging generation of the small-batch path (infer_small): the rows of every call that joined it, in arrival order.
+struct SmallGen {
+    PinnedBuf<int8_t> h_in;     // [kSmallBatch][img_bytes]
+    PinnedBuf<int32_t> h_out;   // logits [rows][n_classes] when a member asks for them, then labels [rows]
+    DevBuf<int8_t> d_in;        // their device counterparts
+    DevBuf<int32_t> d_out;
+    enum State { kOpen, kLaunched, kDone };
+    // written under the batcher's lock; atomic so that a waiting caller may poll them without it (small_wait)
+    std::atomic<int> state{kOpen};
+    std::atomic<size_t> rows{0};   // rows reserved so far
+    std::atomic<int> calls{0}, copied_in{0};
+    int copied_out = 0;
+    bool logits = false, labels = false;   // what the launch writes: what any member asks for
+    int rc = 0;                 // the launch's result, and its error text, for every member
+    std::string err;
+};
+
+// The small-batch path's shared state: calls that arrive while one generation's launch is in flight join the other, and the
+// first of them launches it for all once that launch has completed.  All fields under mu.
+struct SmallBatcher {
+    std::mutex mu;
+    std::condition_variable cv;
+    SmallGen gen[2];
+    std::atomic<int> open{0};             // the generation callers join
+    std::atomic<bool> in_flight{false};   // a generation is launched and not yet complete
+    cudaStream_t stream = nullptr;
 };
 
 struct bnm_model {
@@ -114,28 +146,15 @@ struct bnm_model {
     // fused plan
     FcChainPlan *plan = nullptr;
     std::string plan_err;
-    // device scratch (grow-only): layered path accumulators / activations, CNN features
-    DevBuf<int32_t> d_acc;
-    DevBuf<int8_t> d_act[2], d_feat;
-    uint32_t max_kpad = 0, max_nout = 0;
-    // host pipeline
+    uint32_t max_kpad = 0, max_nout = 0;   // the layer-by-layer path's scratch per image (LayerScratch)
+    // every call's device scratch comes from this pool, stream-ordered on the call's stream (Scratch)
+    cudaMemPool_t pool = nullptr;
+    // host pipeline: the large host calls take turns on host_mu
+    std::mutex host_mu;
     PipeSlot slots[3];
     // small-batch path of bnm_infer_batch (the reference's own calling pattern: one image per Inference() call,
-    // test_inference.py:146-150): pinned staging buffers, one stream, one synchronisation
-    PinnedBuf<int8_t> small_h_in;    // [kSmallBatch][img_bytes]
-    PinnedBuf<int32_t> small_h_out;  // logits [n][n_classes] then labels [n]
-    DevBuf<int8_t> small_d_in;       // their device counterparts
-    DevBuf<int32_t> small_d_out;
-    DevBuf<int8_t> d_f32_scratch;   // bnm_infer_batch_device_f32 fallback: quantised images
-    // emulation mode (grow-only): the fallback's quantised images and CNN int32 planes, next to the layered path's scratch;
-    // the host entry's device copies of its images and logits
-    DevBuf<int8_t> d_emul_q;
-    DevBuf<int32_t> d_emul_planes[2];
-    DevBuf<float> d_emul_in;
-    DevBuf<double> d_emul_out;
-    DevBuf<int8_t> d_emul_rows;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
-    DevBuf<uint32_t> d_engine_labels[2];   // bnm_compare_engines_device's two routes: C / emulator labels the caller does not take
-    DevBuf<double> d_topk_logits;   // bnm_emulate_topk_device's layer-by-layer route: the emulator's logits of a chunk
+    // test_inference.py:146-150): pinned staging buffers, one stream, one synchronisation per shared launch
+    SmallBatcher small;
     bool verbose = false;           // BNM_VERBOSE at model creation: the top-k entries name their route on every call
     int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
                                // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
@@ -232,15 +251,40 @@ static int build_fc_dev(bnm_model *m) {
     return 0;
 }
 
-// scratch for n images: CNN features, and with `layered` the layer-by-layer path's int32 accumulators and ping-pong int8
-// activations, which the fused path needs neither of
-static int ensure_scratch(bnm_model *m, size_t n, bool layered) {
-    if (layered) {
-        CU_TRY(m->d_acc.grow(n * (size_t)std::max(m->max_nout, 1u) * sizeof(int32_t)));
-        for (auto &a : m->d_act) CU_TRY(a.grow(n * (size_t)m->max_kpad, true));
+// One call's device scratch: stream-ordered allocations from the model's pool on the call's stream, handed back on that stream
+// once the call has enqueued the work that uses them (the destructor).  Two calls in flight never share a byte of it, whatever
+// their threads and streams, and no call waits on the host for another.  The pool keeps what it has (its release threshold
+// is unbounded), so in steady state an allocation neither reaches the driver nor synchronises.
+struct Scratch {
+    cudaMemPool_t pool;
+    cudaStream_t st;
+    std::vector<void *> held;
+    Scratch(const bnm_model *m, cudaStream_t s) : pool(m->pool), st(s) {}
+    Scratch(const Scratch &) = delete;
+    Scratch &operator=(const Scratch &) = delete;
+    ~Scratch() { for (void *p : held) cudaFreeAsync(p, st); }
+    template <class T> cudaError_t get(T **p, size_t count) {   // count elements of T, null for none
+        *p = nullptr;
+        if (!count) return cudaSuccess;
+        void *q = nullptr;
+        cudaError_t e = cudaMallocFromPoolAsync(&q, count * sizeof(T), pool, st);
+        if (e != cudaSuccess) return e;
+        held.push_back(q);
+        *p = static_cast<T *>(q);
+        return cudaSuccess;
     }
-    if (m->model_class == BNM_MODEL_CNNMNIST) CU_TRY(m->d_feat.grow(n * (size_t)m->feat_stride, true));
-    return 0;
+};
+
+// the layer-by-layer path's scratch for n images: int32 accumulators of the widest layer, ping-pong int8 activations
+struct LayerScratch {
+    int32_t *acc = nullptr;
+    int8_t *act[2] = {nullptr, nullptr};
+};
+static cudaError_t layer_scratch(const bnm_model *m, Scratch &s, size_t n, LayerScratch &L) {
+    cudaError_t e = s.get(&L.acc, n * std::max(m->max_nout, 1u));
+    for (auto &a : L.act)
+        if (e == cudaSuccess) e = s.get(&a, n * m->max_kpad);
+    return e;
 }
 
 static int require_device_index(int device);
@@ -339,10 +383,20 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
     if (rc == 0) rc = build_fc_dev(m);
     if (rc == 0 && m->d_err.grow(sizeof(int), true) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaMalloc failed");
     if (rc == 0) {
+        cudaMemPoolProps props = {};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = device;
+        uint64_t keep = UINT64_MAX;   // never hand memory back to the device: steady-state calls neither allocate nor synchronise
+        if (cudaMemPoolCreate(&m->pool, &props) != cudaSuccess || cudaMemPoolSetAttribute(m->pool, cudaMemPoolAttrReleaseThreshold, &keep) != cudaSuccess)
+            rc = fail(BNM_E_CUDA, "scratch memory pool: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    if (rc == 0) {
         if (const char *e = getenv("BNM_CNN_FRONTEND")) m->cnn_frontend = std::max(0, std::min(2, atoi(e)));   // development override, read once per model
         if (const char *e = getenv("BNM_SMALL_ZC")) m->small_zero_copy = std::max(0, std::min(2, atoi(e)));     // development knob, likewise
         for (auto &s : m->slots)
             if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaStreamCreate failed"); break; }
+        if (rc == 0 && cudaStreamCreateWithFlags(&m->small.stream, cudaStreamNonBlocking) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaStreamCreate failed");
     }
     if (rc != 0) { std::string keep = g_err; bnm_model_destroy(m); g_err = keep; return rc; }
     m->verbose = getenv("BNM_VERBOSE") != nullptr;
@@ -389,6 +443,8 @@ extern "C" void bnm_model_destroy(bnm_model *m) {
     for (auto &H : m->fc_host) cudaFree(H.d_packed);
     for (auto &s : m->slots)
         if (s.stream) cudaStreamDestroy(s.stream);
+    if (m->small.stream) cudaStreamDestroy(m->small.stream);
+    if (m->pool) cudaMemPoolDestroy(m->pool);   // every call's scratch went back to it before the synchronisation above
     delete m;   // and with it the buffers it owns as members
 }
 
@@ -454,19 +510,20 @@ static const size_t kFusedCnnChunk = 1 << 20;  // fused path, CNN models: images
 
 // FC chain, one CUDA-core kernel per layer: input int8 [n][in_stride].  Without logits the last layer's accumulators go to the
 // scratch (n x max_nout) like every other layer's, and only its ReLUNorm's argmax leaves it.
-static int run_fc_layers(bnm_model *m, const int8_t *in, uint32_t in_stride, size_t n, int32_t *logits, uint32_t *labels, cudaStream_t st) {
+static int run_fc_layers(bnm_model *m, const int8_t *in, uint32_t in_stride, size_t n, int32_t *logits, uint32_t *labels,
+                         const LayerScratch &ls, cudaStream_t st) {
     const int8_t *act = in;
     uint32_t stride = in_stride;
     const size_t nl = m->fc.size();
     for (size_t l = 0; l < nl; l++) {
         const bool last = l + 1 == nl;
-        int32_t *acc = last && logits ? logits : m->d_acc.p;
+        int32_t *acc = last && logits ? logits : ls.acc;
         if (!launch_fc_dp4a(act, stride, m->fc[l], acc, n, st))
             return fail(BNM_E_UNSUPPORTED, "FC layer %zu: %u inputs need more shared memory than an SM has (layer kernel stages 128 rows)", l, m->fc[l].n_in);
         if (last) {
             if (labels) launch_relunorm(acc, m->fc[l].n_out, nullptr, 0, labels, n, st);
         } else {
-            int8_t *next = m->d_act[l & 1].p;
+            int8_t *next = ls.act[l & 1];
             uint32_t next_stride = m->fc[l + 1].k_pad;
             launch_relunorm(acc, m->fc[l].n_out, next, next_stride, nullptr, n, st);
             act = next;
@@ -514,8 +571,8 @@ template <class T> static TopKOutputs topk_from(const TopKOutputs &t, size_t b) 
 // The C engine on int8 images on st, arguments checked -> out: logits int32 [n][n_classes], labels and gather, or with topk.k > 0
 // the k best classes of every image and their int32 scores.  FC models on the fused path in one launch, every other model in chunks
 // (CNN front-end, then the fused launch, or the layer-by-layer chain and for top-k k_topk_rows on its int32 accumulators).
-// slot_feat: a caller-owned feature buffer for n images (the host pipeline's per-slot buffers); null = the model's own scratch.
-static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const FcOutputs &out, cudaStream_t st, int8_t *slot_feat = nullptr) {
+// The chunks' scratch (CNN features, the layer-by-layer path's buffers) is this call's own, for one chunk.
+static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const FcOutputs &out, cudaStream_t st) {
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
     const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
     const uint32_t k = out.topk.k;
@@ -526,10 +583,13 @@ static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const FcOu
         int rc = fc_chain_launch(m->plan, form, images, n, out, st);
         return rc ? fail(BNM_E_CUDA, "fused %s kernel launch failed (%d): %s", kernel, rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
-    const size_t chunk = slot_feat ? n : std::min(n, chunk_max);
-    int rc = (slot_feat && fused) ? 0 : ensure_scratch(m, chunk, !fused);
-    if (rc) return rc;
-    int8_t *feat = slot_feat ? slot_feat : m->d_feat.p;
+    const size_t chunk = std::min(n, chunk_max);
+    Scratch scratch(m, st);
+    LayerScratch ls;
+    int8_t *feat = nullptr;
+    if (!fused) CU_TRY(layer_scratch(m, scratch, chunk, ls));
+    if (cnn) CU_TRY(scratch.get(&feat, chunk * m->feat_stride));
+    int rc = 0;
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         const int8_t *fc_in = images + b * m->img_bytes;
@@ -547,8 +607,8 @@ static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const FcOu
             if ((rc = fc_chain_launch(m->plan, form, fc_in, nb, o, st)))
                 return fail(BNM_E_CUDA, "fused %s kernel launch failed (%d)", kernel, rc);
         } else {
-            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, o.labels, st))) return rc;
-            if (k) launch_topk_rows(m->d_acc.p, m->n_classes, k, o.topk.classes, static_cast<int32_t *>(o.topk.scores), nb, st);   // last layer's accumulators
+            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, o.labels, ls, st))) return rc;
+            if (k) launch_topk_rows(ls.acc, m->n_classes, k, o.topk.classes, static_cast<int32_t *>(o.topk.scores), nb, st);   // last layer's accumulators
         }
     }
     return launch_status();
@@ -634,69 +694,143 @@ extern "C" int bnm_enable_peer_access(int device, int peer) {
 // -----------------------------------------------------------------------------------------------
 // batched inference, host pointers: chunks round-robin over three streams so H2D, kernels and D2H overlap
 // -----------------------------------------------------------------------------------------------
-// n <= kSmallBatch images: staging buffers allocated once, one stream, one synchronisation per call
-static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
+// Both generations' staging buffers, allocated by the first small call (under the batcher's lock): all of them or none.
+static int small_buffers(bnm_model *m) {
+    SmallGen *g = m->small.gen;
+    if (g[1].d_out.p) return 0;
+    CU_TRY(cudaSetDevice(m->device));
     const size_t in_bytes = kSmallBatch * (size_t)m->img_bytes, out_bytes = kSmallBatch * ((size_t)m->n_classes + 1) * 4;
-    cudaError_t e = m->small_h_in.grow(in_bytes);
-    if (e == cudaSuccess) e = m->small_h_out.grow(out_bytes);
-    if (e == cudaSuccess) e = m->small_d_in.grow(in_bytes);
-    if (e == cudaSuccess) e = m->small_d_out.grow(out_bytes);
-    if (e != cudaSuccess) {   // all four buffers or none
-        m->small_h_in.release(); m->small_h_out.release(); m->small_d_in.release(); m->small_d_out.release();
-        return fail(-100 - (int)e, "small-batch staging buffers: %s", cudaGetErrorString(e));
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
+        e = g[i].h_in.grow(in_bytes);
+        if (e == cudaSuccess) e = g[i].h_out.grow(out_bytes);
+        if (e == cudaSuccess) e = g[i].d_in.grow(in_bytes);
+        if (e == cudaSuccess) e = g[i].d_out.grow(out_bytes);
     }
-    cudaStream_t st = m->slots[0].stream;
-    memcpy(m->small_h_in.p, images, n * (size_t)m->img_bytes);
-    const int8_t *d_in = m->small_d_in.p;
-    int32_t *d_out = m->small_d_out.p;
-    if (m->small_zero_copy >= 2) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(const_cast<int8_t **>(&d_in)), m->small_h_in.p, 0));
-    else CU_TRY(cudaMemcpyAsync(m->small_d_in.p, m->small_h_in.p, n * (size_t)m->img_bytes, cudaMemcpyHostToDevice, st));
-    if (m->small_zero_copy >= 1) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), m->small_h_out.p, 0));
-    const size_t n_log = logits ? n * (size_t)m->n_classes : 0;   // labels-only calls: the labels start the staging buffer
+    if (e == cudaSuccess) return 0;
+    for (int i = 0; i < 2; i++) { g[i].h_in.release(); g[i].h_out.release(); g[i].d_in.release(); g[i].d_out.release(); }
+    return fail(-100 - (int)e, "small-batch staging buffers: %s", cudaGetErrorString(e));
+}
+
+// One generation's rows through the GPU: one copy in, one launch, one copy out (or zero-copy), one synchronisation.
+static int small_launch(bnm_model *m, SmallGen &g) {
+    CU_TRY(cudaSetDevice(m->device));
+    cudaStream_t st = m->small.stream;
+    const size_t n = g.rows;
+    const int8_t *d_in = g.d_in.p;
+    int32_t *d_out = g.d_out.p;
+    if (m->small_zero_copy >= 2) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(const_cast<int8_t **>(&d_in)), g.h_in.p, 0));
+    else CU_TRY(cudaMemcpyAsync(g.d_in.p, g.h_in.p, n * (size_t)m->img_bytes, cudaMemcpyHostToDevice, st));
+    if (m->small_zero_copy >= 1) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), g.h_out.p, 0));
+    const size_t n_log = g.logits ? n * (size_t)m->n_classes : 0;   // labels-only batches: the labels start the staging buffer
     uint32_t *d_lab = reinterpret_cast<uint32_t *>(d_out + n_log);
-    int rc = bnm_infer_batch_device(m, d_in, n, logits ? d_out : nullptr, labels ? d_lab : nullptr, st);
+    int rc = bnm_infer_batch_device(m, d_in, n, g.logits ? d_out : nullptr, g.labels ? d_lab : nullptr, st);
     if (rc) return rc;
-    if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(m->small_h_out.p, m->small_d_out.p, (n_log + (labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
+    if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(g.h_out.p, g.d_out.p, (n_log + (g.labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
-    if (logits) memcpy(logits, m->small_h_out.p, n_log * 4);
-    if (labels) memcpy(labels, m->small_h_out.p + n_log, n * 4);
     return 0;
+}
+
+// Wait under lk until ready() holds.  A launch takes tens of microseconds and waking a sleeping thread about as long, and a
+// sleeping caller that wakes must take the lock after every other one woken with it: so first poll ready() with the lock
+// released for up to kSmallSpin, yielding the core, and only then sleep on cv.  ready() reads atomics only.
+static const auto kSmallSpin = std::chrono::microseconds(200);
+template <class Ready> static void small_wait(std::unique_lock<std::mutex> &lk, std::condition_variable &cv, Ready ready) {
+    if (ready()) return;
+    lk.unlock();
+    const auto until = std::chrono::steady_clock::now() + kSmallSpin;
+    while (!ready() && std::chrono::steady_clock::now() < until) std::this_thread::yield();
+    lk.lock();
+    cv.wait(lk, ready);
+}
+
+// n <= kSmallBatch images.  A call reserves rows in the open generation, copies its images in, and waits; the generation's first
+// caller (its leader) launches it for all of them as soon as the other generation's launch has completed, so calls that arrive
+// while a launch is in flight share the next one.  Then every caller copies its own rows out.  A caller alone on the model makes
+// one copy, one launch and one synchronisation, as a plain call would; there is no timer.  Only the leader calls CUDA: a caller
+// that joins a generation must never wait on the runtime while the launch in flight is being synchronised.
+static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
+    SmallBatcher &B = m->small;
+    std::unique_lock<std::mutex> lk(B.mu);
+    if (int rc = small_buffers(m)) return rc;
+    small_wait(lk, B.cv, [&] { const SmallGen &o = B.gen[B.open]; return o.state == SmallGen::kOpen && o.rows + n <= kSmallBatch; });
+    SmallGen &g = B.gen[B.open];
+    const size_t row0 = g.rows;
+    g.rows += n;
+    const bool leader = g.calls++ == 0;
+    g.logits = g.logits || logits;
+    g.labels = g.labels || labels;
+    lk.unlock();
+    memcpy(g.h_in.p + row0 * m->img_bytes, images, n * (size_t)m->img_bytes);
+    lk.lock();
+    g.copied_in++;
+    B.cv.notify_all();
+    if (leader) {
+        small_wait(lk, B.cv, [&] { return !B.in_flight; });   // the generation takes callers until the launch before it has completed
+        g.state = SmallGen::kLaunched;
+        B.open ^= 1;
+        B.in_flight = true;
+        small_wait(lk, B.cv, [&] { return g.copied_in == g.calls; });
+        lk.unlock();
+        const int rc = small_launch(m, g);
+        lk.lock();
+        g.rc = rc;
+        g.err = rc ? g_err : std::string();
+        g.state = SmallGen::kDone;
+        B.in_flight = false;
+        if (m->verbose && g.calls > 1) fprintf(stderr, "bitnetmcu_b200: small batch: %zu images from %d calls\n", g.rows.load(), g.calls.load());
+        B.cv.notify_all();
+    } else {
+        small_wait(lk, B.cv, [&] { return g.state == SmallGen::kDone; });
+    }
+    const int rc = g.rc;
+    if (rc) g_err = g.err;   // every member reports the launch's failure in its own thread
+    const size_t n_log = g.logits ? g.rows * (size_t)m->n_classes : 0;
+    lk.unlock();
+    if (!rc && logits) memcpy(logits, g.h_out.p + row0 * m->n_classes, n * (size_t)m->n_classes * 4);
+    if (!rc && labels) memcpy(labels, g.h_out.p + n_log + row0, n * 4);
+    lk.lock();
+    if (++g.copied_out == g.calls) {   // the last member out opens the generation again
+        g.state = SmallGen::kOpen;
+        g.rows = 0;
+        g.calls = g.copied_in = g.copied_out = 0;
+        g.logits = g.labels = false;
+        B.cv.notify_all();
+    }
+    return rc;
 }
 
 // the C engine on host buffers in chunks of chunk_images, each through one slot's buffers: images in, run_c_engine, out's arrays
 // back.  Synchronous.
 static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const FcOutputs &out) {
+    std::lock_guard<std::mutex> turn(m->host_mu);   // large host calls take turns: each one keeps the copy engines busy alone
     const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
     // per image, in 4-byte words: d_logits holds the logits or the top-k scores (bnm_infer_batch sizes it and d_labels whether or
     // not it takes them), d_classes the top-k classes
     const size_t n_logits = k ? (out.topk.scores ? k : 0) : m->n_classes, n_labels = k ? 0 : 1;
-    const size_t feat_bytes = m->model_class == BNM_MODEL_CNNMNIST ? m->feat_stride : 0;
     bool small = false;
     for (auto &s : m->slots)
-        small = small || s.d_feat.bytes < chunk * feat_bytes || s.d_images.bytes < chunk * m->img_bytes || s.d_classes.bytes < chunk * k * 4 ||
+        small = small || s.d_images.bytes < chunk * m->img_bytes || s.d_classes.bytes < chunk * k * 4 ||
                 s.d_logits.bytes < chunk * n_logits * 4 || s.d_labels.bytes < chunk * n_labels * 4;
     if (small) {
-        CU_TRY(cudaDeviceSynchronize());   // no chunk of an earlier call may still use a buffer that is reallocated
+        for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));   // no chunk of an earlier call may still use a buffer that is reallocated
         for (auto &s : m->slots) {
-            CU_TRY(s.d_feat.grow(chunk * feat_bytes, true));
             CU_TRY(s.d_images.grow(chunk * (size_t)m->img_bytes));
             CU_TRY(s.d_classes.grow(chunk * k * 4));
             CU_TRY(s.d_logits.grow(chunk * n_logits * 4));
             CU_TRY(s.d_labels.grow(chunk * n_labels * 4));
         }
     }
-    // the layer-by-layer path shares one scratch arena (accumulators / activations): its chunks must not overlap in time -> one
-    // stream.  The fused path has no shared state (CNN models: one feature buffer per slot) and uses all three.
-    const bool shared_scratch = bnm_model_active_path(m) != BNM_PATH_TCGEN05;
+    // every chunk's scratch is its own (run_c_engine): the chunks of every path overlap in time on all three streams
     int32_t *h_logits = static_cast<int32_t *>(k ? out.topk.scores : out.logits);   // where d_logits goes
     size_t c = 0;
     for (size_t b = 0; b < n; b += chunk, c++) {
         const size_t nb = std::min(chunk, n - b);
-        PipeSlot &s = m->slots[shared_scratch ? 0 : c % 3];
+        PipeSlot &s = m->slots[c % 3];
         CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
         const FcOutputs d{out.logits ? s.d_logits.p : nullptr, out.labels ? s.d_labels.p : nullptr, nullptr,
                          {(uint32_t)k, s.d_classes.p, out.topk.scores ? s.d_logits.p : nullptr}};
-        if (int rc = run_c_engine(m, s.d_images.p, nb, d, s.stream, shared_scratch ? nullptr : s.d_feat.p)) return rc;
+        if (int rc = run_c_engine(m, s.d_images.p, nb, d, s.stream)) return rc;
         if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, s.d_classes.p, nb * k * 4, cudaMemcpyDeviceToHost, s.stream));
         if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * n_logits, s.d_logits.p, nb * n_logits * 4, cudaMemcpyDeviceToHost, s.stream));
         if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, s.d_labels.p, nb * 4, cudaMemcpyDeviceToHost, s.stream));
@@ -709,8 +843,8 @@ extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int
     if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch: null argument");
     if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_infer_batch: no output (logits and labels both NULL)");
     if (n == 0) return 0;
+    if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);   // sets the device where it launches
     CU_TRY(cudaSetDevice(m->device));
-    if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);
     return infer_pipelined(m, images, n, FcOutputs{logits, labels});
 }
 
@@ -855,9 +989,11 @@ extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, siz
         int rc = fc_chain_launch(m->plan, kFormFloat, images, n, FcOutputs{logits, labels}, st);
         return rc ? fail(BNM_E_CUDA, "fused float-input kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
-    CU_TRY(m->d_f32_scratch.grow(n * (size_t)m->img_bytes));
-    launch_quantize_images(images, m->img_bytes, m->d_f32_scratch.p, n, st);
-    return bnm_infer_batch_device(m, m->d_f32_scratch.p, n, logits, labels, stream);
+    Scratch scratch(m, st);
+    int8_t *q;
+    CU_TRY(scratch.get(&q, n * (size_t)m->img_bytes));
+    launch_quantize_images(images, m->img_bytes, q, n, st);
+    return bnm_infer_batch_device(m, q, n, logits, labels, stream);
 }
 
 extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out) {
@@ -891,8 +1027,7 @@ static const size_t kEmulChunkFc = 65536, kEmulChunkCnn = 2048;   // images per 
 
 // The emulator on device buffers, asynchronous on st: images float32 [n][img_bytes] -> logits float64 [n][n_classes] and / or labels
 // (first maximum); or, with topk.k > 0, instead of both the k best classes of every image and their float64 scores (may be null).
-// The routes other than fc_emul_kernel run in chunks through scratch the model owns (grow-only), which the layer-by-layer path
-// shares: like that path, one stream at a time per model.
+// The routes other than fc_emul_kernel run in chunks through scratch of their own, for one chunk.
 static int emulate_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, cudaStream_t st,
                           const TopKOutputs &topk = {}) {
     const size_t nl = m->fc.size();
@@ -905,8 +1040,9 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
     }
     if (route != kEmulLayers) {
         const size_t chunk = std::min(n, kFusedCnnChunk);
-        CU_TRY(m->d_emul_rows.grow(chunk * (cnn ? m->feat_stride : elems)));
-        int8_t *rows = m->d_emul_rows.p;
+        Scratch scratch(m, st);
+        int8_t *rows;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
+        CU_TRY(scratch.get(&rows, chunk * (cnn ? m->feat_stride : elems)));
         for (size_t b = 0; b < n; b += chunk) {
             const size_t nb = std::min(chunk, n - b);
             if (!cnn) launch_quantize_images(images + b * elems, elems, rows, nb, st);   // BitNetMCU.py:435-436
@@ -920,12 +1056,16 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
         return launch_status();
     }
     const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
-    if (k) CU_TRY(m->d_topk_logits.grow(chunk * m->n_classes * sizeof(double)));   // top-k: the logits of a chunk
-    if (int rc = ensure_scratch(m, chunk, true)) return rc;   // accumulators and the two int8 activation buffers
-    CU_TRY(m->d_emul_q.grow(chunk * elems));
-    if (cnn)
-        for (auto &p : m->d_emul_planes) CU_TRY(p.grow(chunk * C * 256 * 4));
-    int8_t *q = m->d_emul_q.p, *a0 = m->d_act[0].p, *a1 = m->d_act[1].p;
+    Scratch scratch(m, st);
+    LayerScratch ls;   // accumulators and the two int8 activation buffers
+    double *topk_logits;   // top-k: the logits of a chunk
+    int8_t *q;             // the quantised images
+    int32_t *planes[2];    // CNN models: int32 conv planes
+    CU_TRY(layer_scratch(m, scratch, chunk, ls));
+    CU_TRY(scratch.get(&topk_logits, k ? chunk * m->n_classes : 0));
+    CU_TRY(scratch.get(&q, chunk * elems));
+    for (auto &p : planes) CU_TRY(scratch.get(&p, cnn ? chunk * C * 256 : 0));
+    int8_t *a0 = ls.act[0], *a1 = ls.act[1];
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         launch_quantize_images(images + b * elems, elems, q, nb, st);   // BitNetMCU.py:435-436
@@ -933,7 +1073,7 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
         uint32_t stride = elems;
         if (cnn) {
             // conv (ReLU, no shift) -> per-image renormalisation, pools in between (BitNetMCU.py:459-526), planes [(image, channel)][xy*xy]
-            int32_t *p0 = m->d_emul_planes[0].p, *p1 = m->d_emul_planes[1].p;
+            int32_t *p0 = planes[0], *p1 = planes[1];
             launch_expand_image(q, p0, C, 256, nb, st);
             launch_conv33relu(p0, m->d_conv[0].p, C, 16, 0, p1, nb * C, st);
             launch_conv_renorm(p1, C * 196, nb, st);
@@ -948,16 +1088,16 @@ static int emulate_device(bnm_model *m, const float *images, size_t n, double *l
             stride = m->feat_stride;
         }
         for (size_t l = 0; l < nl; l++) {
-            if (!launch_fc_dp4a(act, stride, m->fc[l], m->d_acc.p, nb, st)) return fail(BNM_E_UNSUPPORTED, "FC layer %zu too wide for the layer kernel", l);
+            if (!launch_fc_dp4a(act, stride, m->fc[l], ls.acc, nb, st)) return fail(BNM_E_UNSUPPORTED, "FC layer %zu too wide for the layer kernel", l);
             if (l + 1 == nl) break;   // no renormalisation for the last layer (BitNetMCU.py:528-530)
             int8_t *next = (l & 1) ? a1 : a0;   // CNN features sit in a1 and are dead once layer 0 has run
             const uint32_t next_stride = m->fc[l + 1].k_pad;
-            launch_relunorm_emul(m->d_acc.p, m->fc[l].n_out, level_shift_of(m->fc[l].enc), next, next_stride, nb, st);
+            launch_relunorm_emul(ls.acc, m->fc[l].n_out, level_shift_of(m->fc[l].enc), next, next_stride, nb, st);
             act = next;
             stride = next_stride;
         }
-        double *lg = k ? m->d_topk_logits.p : logits ? logits + b * m->n_classes : nullptr;
-        launch_emul_logits(m->d_acc.p, m->n_classes, level_shift_of(m->fc[nl - 1].enc), lg, labels ? labels + b : nullptr, nb, st);
+        double *lg = k ? topk_logits : logits ? logits + b * m->n_classes : nullptr;
+        launch_emul_logits(ls.acc, m->n_classes, level_shift_of(m->fc[nl - 1].enc), lg, labels ? labels + b : nullptr, nb, st);
         if (k) {
             const TopKOutputs tk = topk_from<double>(topk, b);
             launch_topk_rows(lg, m->n_classes, k, tk.classes, static_cast<double *>(tk.scores), nb, st);
@@ -981,16 +1121,20 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
     if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_emulate_inference_quantized: null argument");
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
+    std::lock_guard<std::mutex> turn(m->host_mu);   // takes turns with the other large host calls, on the pipeline's first stream
     const size_t elems = m->img_bytes, ncls = m->n_classes;
     const size_t chunk = std::min(n, m->model_class == BNM_MODEL_CNNMNIST ? kEmulChunkCnn : kEmulChunkFc);
-    CU_TRY(m->d_emul_in.grow(chunk * elems * sizeof(float)));
-    CU_TRY(m->d_emul_out.grow(chunk * ncls * sizeof(double)));
     cudaStream_t st = m->slots[0].stream;
+    Scratch scratch(m, st);
+    float *d_in;      // the device copies of a chunk's images and logits
+    double *d_out;
+    CU_TRY(scratch.get(&d_in, chunk * elems));
+    CU_TRY(scratch.get(&d_out, chunk * ncls));
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
-        CU_TRY(cudaMemcpyAsync(m->d_emul_in.p, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
-        if (int rc = emulate_device(m, m->d_emul_in.p, nb, m->d_emul_out.p, nullptr, st)) return rc;
-        CU_TRY(cudaMemcpyAsync(logits + b * ncls, m->d_emul_out.p, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(d_in, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
+        if (int rc = emulate_device(m, d_in, nb, d_out, nullptr, st)) return rc;
+        CU_TRY(cudaMemcpyAsync(logits + b * ncls, d_out, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
     }
     return 0;
@@ -1000,7 +1144,7 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
 // Both engines in one call (test_inference.py:130-175): the C engine's and the emulator's labels of the same float images, and
 // counts of their agreement and of their accuracy against truth.  The one-pass kernel where both float-input rows exist; every
 // other model runs bnm_infer_batch_device_f32's and emulate_device's routes per chunk, into the caller's label buffers or the
-// model's scratch, then k_engine_counts.
+// call's scratch, then k_engine_counts.
 // -----------------------------------------------------------------------------------------------
 static const size_t kEnginesChunk = 1 << 20;   // images per pass of the two routes (bounds the label scratch)
 
@@ -1021,13 +1165,15 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
         return rc ? fail(BNM_E_CUDA, "fused two-engine kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
     }
     const size_t chunk = std::min(n, kEnginesChunk), elems = m->img_bytes;
-    if (counts && !labels_c) CU_TRY(m->d_engine_labels[0].grow(chunk * sizeof(uint32_t)));
-    if (counts && !labels_py) CU_TRY(m->d_engine_labels[1].grow(chunk * sizeof(uint32_t)));
+    Scratch scratch(m, st);
+    uint32_t *own[2];   // C / emulator labels the caller does not take
+    CU_TRY(scratch.get(&own[0], counts && !labels_c ? chunk : 0));
+    CU_TRY(scratch.get(&own[1], counts && !labels_py ? chunk : 0));
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         const float *img = images + b * elems;
-        uint32_t *lc = labels_c ? labels_c + b : counts ? m->d_engine_labels[0].p : nullptr;
-        uint32_t *lp = labels_py ? labels_py + b : counts ? m->d_engine_labels[1].p : nullptr;
+        uint32_t *lc = labels_c ? labels_c + b : own[0];
+        uint32_t *lp = labels_py ? labels_py + b : own[1];
         if (lc)
             if (int rc = bnm_infer_batch_device_f32(m, img, nb, nullptr, lc, st)) return rc;
         if (lp)
@@ -1043,9 +1189,9 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
 //   * FC models on the fused path: one launch of fc_topk_kernel, whose epilogue ranks the classes in registers;
 //   * CNN models on the fused path: the front-end into the feature scratch, then that kernel, in chunks of 2^20 images;
 //   * BNM_PATH_LAYERS and models without a fused plan: the layer-by-layer chain into its int32 scratch (the emulator: its float64
-//     logits into d_topk_logits), then k_topk_rows.
-// The float entry scales the images into d_f32_scratch first; the emulator runs its own front-end (scaling kernel or CNN
-// front-end) into d_emul_rows, then fc_topk_kernel with its rule.
+//     logits into a chunk of scratch), then k_topk_rows.
+// The float entry scales the images into its own scratch first; the emulator runs its own front-end (scaling kernel or CNN
+// front-end) into its scratch, then fc_topk_kernel with its rule.
 // -----------------------------------------------------------------------------------------------
 static int topk_check(const bnm_model *m, const char *fn, const void *images, size_t n, uint32_t k, const uint32_t *classes,
                       const void *scores, uintptr_t score_align, uintptr_t image_align) {
@@ -1082,12 +1228,14 @@ extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size
     if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk_device_f32: k_quantize_images + %s\n", topk_c_route(m).c_str());
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t chunk = std::min(n, kFusedCnnChunk), elems = m->img_bytes;
-    CU_TRY(m->d_f32_scratch.grow(chunk * elems));
+    Scratch scratch(m, st);
+    int8_t *q;
+    CU_TRY(scratch.get(&q, chunk * elems));
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
-        launch_quantize_images(images + b * elems, (uint32_t)elems, m->d_f32_scratch.p, nb, st);
+        launch_quantize_images(images + b * elems, (uint32_t)elems, q, nb, st);
         const FcOutputs out{nullptr, nullptr, nullptr, {k, classes + b * k, scores ? scores + b * k : nullptr}};
-        if (int rc = run_c_engine(m, m->d_f32_scratch.p, nb, out, st)) return rc;
+        if (int rc = run_c_engine(m, q, nb, out, st)) return rc;
     }
     return 0;
 }

@@ -22,6 +22,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -147,6 +148,9 @@ struct FcChainPlan {
     cudaStream_t prev_stream = nullptr;
     bool prev_valid = false;
     bool verbose = false;             // BNM_VERBOSE at plan creation: every int8-form launch names its wait decision
+    // guards the tensor-map cache and the bookkeeping above together with the launch they describe: launches from several host
+    // threads enqueue in the order the bookkeeping records
+    std::mutex mu;
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -967,13 +971,13 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
+    static const EncodeTiledFn fn = [] {   // initialised once, whichever thread creates the first plan
         void *p = nullptr;
         cudaDriverEntryPointQueryResult q;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
+            return (EncodeTiledFn)p;
+        return (EncodeTiledFn)nullptr;
+    }();
     return fn;
 }
 
@@ -1168,6 +1172,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
 
 void fc_chain_plan_set_overlap(FcChainPlan *p, int mode) {
     if (!p) return;
+    std::lock_guard<std::mutex> lock(p->mu);
     p->overlap = mode;
     p->prev_valid = false;
 }
@@ -1248,6 +1253,9 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
         for (uint32_t d = 0; d < p.n_lab_dst; d++) p.lab_dst[d] = gather->labels_dst[d];
         for (uint32_t d = 0; d < p.n_log_dst; d++) p.log_dst[d] = gather->logits_dst[d];
     }
+    // From the tensor-map lookup to the launch, one thread at a time per plan: the cached map must not be rewritten before the
+    // launch has copied it, and "the previous launch" of mode 2 is the previous launch enqueued on this plan, from any thread.
+    std::lock_guard<std::mutex> lock(plan->mu);
     const CUtensorMap *tmap_p = &kNoTensorMap;
     if (s.float_in) {
         p.fimages = static_cast<const float *>(in);

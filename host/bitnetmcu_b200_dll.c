@@ -8,6 +8,7 @@
  * unchanged -- plus the batched `InferenceBatch` the reference lacks.  All compute runs on the GPU through the C ABI;
  * there is no CPU path: a missing CUDA device aborts with a message.
  */
+#include <pthread.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -23,19 +24,25 @@
 #endif
 
 static bnm_model *g_model;
+static pthread_once_t g_model_once = PTHREAD_ONCE_INIT;
 
+static void create_model(void)
+{
+    static const bnm_layer layers[] = { BNM_MODEL_LAYERS };
+    const char *dev = getenv("BNM_DEVICE");
+    int rc = bnm_model_create(BNM_MODEL_CLASS, layers, (uint32_t)(sizeof layers / sizeof layers[0]), 256,
+                              dev ? atoi(dev) : 0, &g_model);
+    if (rc != 0) {
+        fprintf(stderr, "bitnetmcu_b200: cannot create the model (rc=%d): %s\n", rc, bnm_last_error());
+        abort();
+    }
+}
+
+/* created exactly once, by whichever thread calls first: Inference() may be called from any number of threads, and their
+ * concurrent calls share launches (bnm_infer_batch's small-batch path) */
 static bnm_model *model(void)
 {
-    if (!g_model) {
-        static const bnm_layer layers[] = { BNM_MODEL_LAYERS };
-        const char *dev = getenv("BNM_DEVICE");
-        int rc = bnm_model_create(BNM_MODEL_CLASS, layers, (uint32_t)(sizeof layers / sizeof layers[0]), 256,
-                                  dev ? atoi(dev) : 0, &g_model);
-        if (rc != 0) {
-            fprintf(stderr, "bitnetmcu_b200: cannot create the model (rc=%d): %s\n", rc, bnm_last_error());
-            abort();
-        }
-    }
+    pthread_once(&g_model_once, create_model);
     return g_model;
 }
 

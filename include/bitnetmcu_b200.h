@@ -20,6 +20,18 @@
  *
  * Pointers are plain host (or, where the name says _device, CUDA device) pointers; sizes are element
  * counts unless named *_bytes.  All-integer arithmetic: results are bit-exact with the reference.
+ *
+ * Threads.  Every entry point may be called concurrently from any number of host threads on one model, on the same stream or
+ * on different streams, and each call's results are exactly those of the same call made alone.  The exceptions are
+ * bnm_model_set_option and bnm_model_destroy: like any handle's, they must not overlap other calls on that model.  A call's
+ * device scratch (CNN features, the layer-by-layer path's buffers, scaled images, the emulator's planes) is its own, allocated
+ * stream-ordered on the call's stream from a memory pool of the model that keeps what it has: concurrency costs memory, as each
+ * call in flight holds its own chunk's scratch -- for example 256 MB of CNN features per 2^20-image chunk -- and the pool holds
+ * the most that was ever in flight at once until the model is destroyed.  No call synchronises the host with another.
+ * Small host calls (bnm_infer_batch with n <= 1024) that arrive while another one's launch is in flight share the next launch;
+ * the large host calls (bnm_infer_batch above 1024 images, bnm_infer_topk, bnm_emulate_inference_quantized) take turns.
+ * The fused kernel's launch-overlap bookkeeping (BNM_OPT_LAUNCH_OVERLAP) counts launches in the order they are enqueued on the
+ * model, from whichever thread.
  */
 #ifndef BITNETMCU_B200_H
 #define BITNETMCU_B200_H
@@ -144,7 +156,15 @@ BNM_API int bnm_model_active_path(const bnm_model *m);
  * destination buffer; otherwise it returns BNM_E_ARG (-1).  A labels-only call (logits NULL) writes and copies no logits at
  * all: 40 B per image less GPU memory traffic for 10 classes on the fused path, no logits copy over PCIe on the host path.
  * Host version: buffers are ordinary (ideally pinned, see bnm_host_alloc) host memory; the call streams them
- * through the GPU in chunks with copies overlapped and returns when the results are in `logits`/`labels`. */
+ * through the GPU in chunks with copies overlapped and returns when the results are in `logits`/`labels`.
+ * Calls of up to 1024 images go through pinned staging buffers in one copy, one launch and one synchronisation.  Such calls made
+ * from several threads at once are batched: each caller reserves rows in the open staging generation and copies its images in,
+ * the generation's first caller launches it for all of them once the launch before it has completed, and each caller copies its
+ * own results out.  A batch writes logits only if one of its calls asks for them; if its launch fails, every call in it returns
+ * the same code with the text in its own bnm_last_error().  There is no timer: a caller alone on the model is launched at once.
+ * With BNM_VERBOSE set at model creation, each launch that serves more than one call prints
+ * "bitnetmcu_b200: small batch: <images> images from <calls> calls".  Larger calls take turns on the model: each one keeps the
+ * host-device copies busy on its own. */
 BNM_API int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels);
 
 /* Device version: pointers are device memory on the model's GPU (images 16-byte, logits 8-byte aligned); asynchronous on `stream`
@@ -232,9 +252,8 @@ BNM_API int bnm_emulate_inference_quantized(bnm_model *m, const float *images, s
  * hidden-layer rule and float64 logits.  Other FC models run the input scaling kernel, then the int8-input FC kernel with the
  * emulator's rule at the model's width (up to 256); CNN models of up to 128 channels run the emulator's CNN front-end as one
  * kernel, then that FC kernel on its features; both in chunks of 2^20 images.  BNM_PATH_LAYERS, models without a fused plan and
- * wider CNN models run the emulation kernels layer by layer.  Every route but the first uses scratch the model owns (grown on
- * the first large call, then reused): calls on one model must then not overlap in time on different streams.  Either way the
- * call makes no host synchronisation once its scratch has grown. */
+ * wider CNN models run the emulation kernels layer by layer.  Every route but the first runs through scratch of the call's own
+ * (see "Threads" above).  The call makes no host synchronisation. */
 BNM_API int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
@@ -260,8 +279,7 @@ typedef struct bnm_engine_counts {
  * entries) run ONE kernel: each float image is read and scaled once, layer 1 runs once (both engines' layer-1 accumulators are
  * the same), then the C engine's and the emulator's hidden layers run from it, and the epilogue writes both labels and counts
  * warp by warp.  Every other model runs the two entries' routes in chunks of 2^20 images, then a counting kernel.  Asynchronous
- * on `stream`, no host synchronisation once the model's scratch has grown; like the emulator's routes, calls on one model must
- * not overlap in time on different streams. */
+ * on `stream`, no host synchronisation. */
 BNM_API int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth,
                                        uint32_t *labels_c, uint32_t *labels_py, bnm_engine_counts *counts, void *stream);
 
@@ -277,14 +295,13 @@ BNM_API int bnm_compare_engines_device(bnm_model *m, const float *images, size_t
  * scores: the logits of those classes [n][k], or NULL: int32 = layer_out after the last processfclayer (the C engine), float64 =
  * what bnm_emulate_batch_device writes as logits (the emulator).  No logits are written anywhere.  n == 0 returns 0 and writes
  * nothing.  Device entries: device memory on the model's GPU, images 16-byte, classes 4-byte, float64 scores 8-byte aligned,
- * asynchronous on `stream` (NULL = default stream), no host synchronisation once the model's scratch has grown.
+ * asynchronous on `stream` (NULL = default stream), no host synchronisation.
  * On the fused path, FC models run ONE kernel (bnm_infer_topk_device): the int8 chain of bnm_infer_batch_device on one pipe, whose
  * epilogue ranks each row's logits in registers.  CNN models run the front-end selected by BNM_OPT_CNN_FRONTEND, then that kernel,
  * in chunks of 2^20 images.  BNM_PATH_LAYERS and models without a fused plan run the layer-by-layer chain, then a ranking kernel.
- * The float entry scales the images first (the scaling kernel into the model's scratch, chunks of 2^20), then takes the int8
+ * The float entry scales the images first (the scaling kernel into the call's scratch, chunks of 2^20), then takes the int8
  * route; the emulator takes the scaling kernel (FC) or its CNN front-end (CNN up to 128 channels), then the kernel with the
- * emulator's rule, else its layer-by-layer route.  Every route but the first uses scratch the model owns: calls on one model
- * must not overlap in time on different streams.  A top-k launch is an ordinary stream-ordered launch (no BNM_OPT_LAUNCH_OVERLAP
+ * emulator's rule, else its layer-by-layer route.  A top-k launch is an ordinary stream-ordered launch (no BNM_OPT_LAUNCH_OVERLAP
  * mode 2, no result exchange). */
 BNM_API int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores);   /* host buffers */
 BNM_API int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream);
