@@ -289,23 +289,89 @@ static cudaError_t layer_scratch(const bnm_model *m, Scratch &s, size_t n, Layer
 
 static int require_device_index(int device);
 
-// the kernels of the emulator (emulate_device): fc_emul_kernel on float images; fc_emul_i8_kernel after the scaling kernel (FC)
-// or k_cnn_emul_frontend (CNN); or the emulation kernels layer by layer
-enum EmulRoute { kEmulFloatRow, kEmulInt8Row, kEmulLayers };
-static EmulRoute emul_route(const bnm_model *m) {
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    if (bnm_model_active_path(m) != BNM_PATH_TCGEN05 || (cnn && m->channels > kCnnEmulMaxChannels)) return kEmulLayers;
-    return !cnn && fc_chain_has_form(m->plan, kFormEmulFloat) ? kEmulFloatRow : kEmulInt8Row;
-}
-// the kernel that makes the emulator's int8 rows from float images on its row routes (emulate_device)
-static const char *emul_rows_kernel(const bnm_model *m) {
-    return m->model_class == BNM_MODEL_CNNMNIST ? "k_cnn_emul_frontend" : "k_quantize_images";
+// -----------------------------------------------------------------------------------------------
+// routes: the kernels a call runs on a model, and in what passes
+// -----------------------------------------------------------------------------------------------
+// Images per pass, each bounding the scratch of a call: 2^20 where a pass stages rows in scratch (scaled images, CNN features, the
+// two-engine entry's labels), 2^17 for the C engine layer by layer, 65 536 (FC) / 2 048 (CNN: 2 x C kB of conv planes per image)
+// for the emulator layer by layer
+static const size_t kPass = 1 << 20, kLayerPass = 1 << 17, kEmulLayerPass[2] = {65536, 2048};
+
+enum Engine { kEngineC, kEngineEmul, kEngineBoth };
+// the stage that turns a pass of (scaled) images into the FC stage's int8 rows: none, the C engine's CNN front-end (the kernel
+// cnn_frontend_kernel picks), k_cnn_emul_frontend, or the layered emulator's expand / conv / renorm / pool / k_i32_to_i8
+enum Front { kFrontNone, kFrontCnn, kFrontCnnEmul, kFrontCnnEmulLayers };
+
+// A route: which kernels one call runs, chosen once per call (choose_route), named (print_route) and run (run_route) from this
+// record alone.  Per pass of `pass` images (0: one pass), k_quantize_images into scratch when `scale`, then per `inner` images of
+// that pass (0: all of it) the front-end, the FC stage and for a layered top-k k_topk_rows.  The FC stage is one launch of `form`,
+// or the layer-by-layer chain with the engine's rule.  The two engines' route runs each engine's own route per pass instead.
+struct Route {
+    Engine engine;
+    bool f32, topk;   // float32 images in; the k best classes out
+    bool scale;
+    Front front;
+    bool fused;
+    FcForm form;
+    size_t pass, inner;
+};
+
+// the route of an entry of `engine` on float32 (f32) or int8 images, top-k or not, on this model with its options
+static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk) {
+    const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05, cnn = m->model_class == BNM_MODEL_CNNMNIST;
+    Route r{engine, f32, topk, false, kFrontNone, fused, kFormInt8, 0, 0};
+    // FC models whose plan has the engine's float-input form: one launch with the input scaling fused (no such top-k form)
+    const FcForm float_form = engine == kEngineC ? kFormFloat : engine == kEngineEmul ? kFormEmulFloat : kFormEngines;
+    if (f32 && !topk && fused && !cnn && fc_chain_has_form(m->plan, float_form)) {
+        r.form = float_form;
+        return r;
+    }
+    if (engine == kEngineBoth) {
+        r.fused = false;
+        r.pass = kPass;
+        return r;
+    }
+    if (engine == kEngineEmul) {   // float32 images only
+        if (!fused || (cnn && m->channels > kCnnEmulMaxChannels)) {
+            r.fused = false;
+            r.scale = true;
+            r.front = cnn ? kFrontCnnEmulLayers : kFrontNone;
+            r.pass = kEmulLayerPass[cnn];
+        } else {
+            r.form = topk ? kFormEmulTopK : kFormEmulInt8;
+            r.scale = !cnn;
+            r.front = cnn ? kFrontCnnEmul : kFrontNone;
+            r.pass = kPass;
+        }
+        return r;
+    }
+    r.form = topk ? kFormTopK : kFormInt8;
+    r.front = cnn ? kFrontCnn : kFrontNone;
+    r.pass = !fused ? kLayerPass : cnn ? kPass : 0;
+    if (f32) {   // the int8 route on each pass of scaled images
+        r.scale = true;
+        r.inner = r.pass;
+        r.pass = kPass;
+    }
+    return r;
 }
 
-// bnm_compare_engines_device: fc_engines_kernel for the models both float-input rows serve, else the two entries' routes and
-// k_engine_counts
-static bool engines_fused(const bnm_model *m) {
-    return bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST && fc_chain_has_form(m->plan, kFormEngines);
+// BNM_VERBOSE: "<what>: " and the kernels of route r.  The layered emulator names its chain only.
+static void print_route(const bnm_model *m, const char *what, const Route &r) {
+    if (!m->verbose) return;
+    std::string s;
+    if (r.engine == kEngineBoth && !r.fused) {
+        s = "bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts";
+    } else if (r.engine == kEngineEmul && !r.fused) {
+        s = r.topk ? "layer by layer + k_topk_rows<double>" : "layer by layer";
+    } else {
+        if (r.scale) s = "k_quantize_images + ";
+        if (r.front == kFrontCnn)
+            s += cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
+        if (r.front == kFrontCnnEmul) s += "k_cnn_emul_frontend + ";
+        s += r.fused ? fc_chain_form_name(m->plan, r.form) : r.topk ? "layer by layer + k_topk_rows<int32>" : "layer by layer";
+    }
+    fprintf(stderr, "bitnetmcu_b200: %s: %s\n", what, s.c_str());
 }
 
 extern "C" int bnm_version(void) { return BNM_VERSION; }
@@ -392,22 +458,16 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
             rc = fail(BNM_E_CUDA, "scratch memory pool: %s", cudaGetErrorString(cudaGetLastError()));
     }
     if (rc == 0) {
-        if (const char *e = getenv("BNM_CNN_FRONTEND")) m->cnn_frontend = std::max(0, std::min(2, atoi(e)));   // development override, read once per model
-        if (const char *e = getenv("BNM_SMALL_ZC")) m->small_zero_copy = std::max(0, std::min(2, atoi(e)));     // development knob, likewise
+        if (const char *e = getenv("BNM_SMALL_ZC")) m->small_zero_copy = std::max(0, std::min(2, atoi(e)));   // development knob, read once per model
         for (auto &s : m->slots)
             if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaStreamCreate failed"); break; }
         if (rc == 0 && cudaStreamCreateWithFlags(&m->small.stream, cudaStreamNonBlocking) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaStreamCreate failed");
     }
     if (rc != 0) { std::string keep = g_err; bnm_model_destroy(m); g_err = keep; return rc; }
     m->verbose = getenv("BNM_VERBOSE") != nullptr;
-    if (m->verbose) {   // diagnostics: the kernels bnm_emulate_batch_device runs on the default path
-        const EmulRoute r = emul_route(m);
-        if (r == kEmulLayers) fprintf(stderr, "bitnetmcu_b200: emulator route: layer by layer\n");
-        else if (r == kEmulFloatRow) fprintf(stderr, "bitnetmcu_b200: emulator route: %s\n", fc_chain_form_name(m->plan, kFormEmulFloat));
-        else fprintf(stderr, "bitnetmcu_b200: emulator route: %s + %s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulInt8));
-        // and the kernels of bnm_compare_engines_device
-        if (engines_fused(m)) fprintf(stderr, "bitnetmcu_b200: engines route: %s\n", fc_chain_form_name(m->plan, kFormEngines));
-        else fprintf(stderr, "bitnetmcu_b200: engines route: bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts\n");
+    if (m->verbose) {   // diagnostics: the routes of bnm_emulate_batch_device and bnm_compare_engines_device on the default path
+        print_route(m, "emulator route", choose_route(m, kEngineEmul, true, false));
+        print_route(m, "engines route", choose_route(m, kEngineBoth, true, false));
         // and which conv3 the tensor-core CNN front-end runs
         if (m->model_class == BNM_MODEL_CNNMNIST)
             fprintf(stderr, "bitnetmcu_b200: cnn front-end: conv3 bound %lld, conv3 on %s\n", m->conv3_bound,
@@ -505,31 +565,28 @@ extern "C" int64_t bnm_model_get_option(const bnm_model *m, int option) {
 // -----------------------------------------------------------------------------------------------
 // batched inference, device pointers
 // -----------------------------------------------------------------------------------------------
-static const size_t kLayeredChunk = 1 << 17;   // images per pass of the layer-by-layer path (bounds its scratch)
-static const size_t kFusedCnnChunk = 1 << 20;  // fused path, CNN models: images per front-end + FC launch pair (256 B of features each)
-
-// FC chain, one CUDA-core kernel per layer: input int8 [n][in_stride].  Without logits the last layer's accumulators go to the
-// scratch (n x max_nout) like every other layer's, and only its ReLUNorm's argmax leaves it.
-static int run_fc_layers(bnm_model *m, const int8_t *in, uint32_t in_stride, size_t n, int32_t *logits, uint32_t *labels,
-                         const LayerScratch &ls, cudaStream_t st) {
-    const int8_t *act = in;
-    uint32_t stride = in_stride;
+// The FC chain layer by layer on int8 rows [n][stride]: per layer the dp4a kernel, per hidden layer the engine's renormalisation
+// into the ping-pong activations.  The C engine writes the last layer's accumulators to logits (without them to the scratch, n x
+// max_nout) and, for labels, takes its ReLUNorm's argmax; the emulator ends with k_emul_logits (float64 logits, labels).
+static int run_layers(bnm_model *m, bool emul, const int8_t *act, uint32_t stride, size_t n, void *logits, uint32_t *labels,
+                      const LayerScratch &ls, cudaStream_t st) {
     const size_t nl = m->fc.size();
+    int32_t *acc = ls.acc;
     for (size_t l = 0; l < nl; l++) {
-        const bool last = l + 1 == nl;
-        int32_t *acc = last && logits ? logits : ls.acc;
-        if (!launch_fc_dp4a(act, stride, m->fc[l], acc, n, st))
-            return fail(BNM_E_UNSUPPORTED, "FC layer %zu: %u inputs need more shared memory than an SM has (layer kernel stages 128 rows)", l, m->fc[l].n_in);
-        if (last) {
-            if (labels) launch_relunorm(acc, m->fc[l].n_out, nullptr, 0, labels, n, st);
-        } else {
-            int8_t *next = ls.act[l & 1];
-            uint32_t next_stride = m->fc[l + 1].k_pad;
-            launch_relunorm(acc, m->fc[l].n_out, next, next_stride, nullptr, n, st);
-            act = next;
-            stride = next_stride;
-        }
+        const FcLayerDev &L = m->fc[l];
+        if (l + 1 == nl && logits && !emul) acc = static_cast<int32_t *>(logits);
+        if (!launch_fc_dp4a(act, stride, L, acc, n, st))
+            return fail(BNM_E_UNSUPPORTED, "FC layer %zu: %u inputs need more shared memory than an SM has (layer kernel stages 128 rows)", l, L.n_in);
+        if (l + 1 == nl) break;
+        int8_t *next = ls.act[l & 1];   // the layered CNN emulator's features sit in act[1], dead once layer 0 has run
+        stride = m->fc[l + 1].k_pad;
+        if (emul) launch_relunorm_emul(acc, L.n_out, level_shift_of(L.enc), next, stride, n, st);   // BitNetMCU.py:528-530
+        else launch_relunorm(acc, L.n_out, next, stride, nullptr, n, st);
+        act = next;
     }
+    const FcLayerDev &last = m->fc[nl - 1];
+    if (emul) launch_emul_logits(acc, last.n_out, level_shift_of(last.enc), static_cast<double *>(logits), labels, n, st);
+    else if (labels) launch_relunorm(acc, last.n_out, nullptr, 0, labels, n, st);
     return 0;
 }
 
@@ -542,76 +599,99 @@ static int run_cnn_front(bnm_model *m, const int8_t *images, size_t n, int8_t *f
                 m->channels, m->xy0, m->xy0);
 }
 
-// images per chunk of the C engine on int8 images; 0: one launch whatever the batch (FC models on the fused path)
-static size_t c_engine_chunk(const bnm_model *m, bool fused) {
-    if (!fused) return kLayeredChunk;
-    return m->model_class == BNM_MODEL_CNNMNIST ? kFusedCnnChunk : 0;
+// what a call writes from image b on (logits and scores: float64 for the emulator, else int32); its result-exchange rows in g
+static FcOutputs outputs_from(const FcOutputs &o, size_t b, uint32_t n_classes, bool emul, GatherDst &g) {
+    auto at = [&](void *p, size_t per_image) -> void * { return p ? static_cast<char *>(p) + b * per_image * (emul ? 8 : 4) : nullptr; };
+    if (o.gather) {
+        g = *o.gather;
+        g.row_offset += b;
+    }
+    return FcOutputs{at(o.logits, n_classes), o.labels ? o.labels + b : nullptr, o.gather ? &g : nullptr,
+                     {o.topk.k, o.topk.classes ? o.topk.classes + b * o.topk.k : nullptr, at(o.topk.scores, o.topk.k)}, o.engines};
+}
+
+// Route r (not the two engines' one) on n images on st, arguments checked -> out: logits (int32 [n][n_classes], float64 for the
+// emulator), labels and gather; or with topk.k > 0 the k best classes of every image and their scores.  A route of one pass and
+// one launch allocates nothing; every other one runs through scratch of this call's own, for one pass.
+static int run_route(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out, cudaStream_t st) {
+    const size_t pass = r.pass ? std::min(n, r.pass) : n, inner = r.inner ? std::min(pass, r.inner) : pass;
+    const bool emul = r.engine == kEngineEmul;
+    const uint32_t elems = m->img_bytes, C = m->channels, k = out.topk.k;
+    const size_t in_bytes = r.f32 ? elems * sizeof(float) : elems;   // per input image
+    Scratch s(m, st);
+    int8_t *q, *feat;     // a pass's scaled images; an inner pass's CNN features for the fused FC stage
+    LayerScratch ls;      // the layer-by-layer chain's accumulators and activations
+    double *lg;           // the layered emulator's top-k: its float64 logits
+    int32_t *planes[2];   // the layered CNN emulator's int32 conv planes [(image, channel)][xy*xy]
+    CU_TRY(s.get(&q, r.scale ? pass * elems : 0));
+    CU_TRY(s.get(&feat, r.front == kFrontCnn || r.front == kFrontCnnEmul ? inner * m->feat_stride : 0));
+    if (!r.fused) CU_TRY(layer_scratch(m, s, inner, ls));
+    CU_TRY(s.get(&lg, emul && !r.fused && k ? inner * m->n_classes : 0));
+    for (auto &p : planes) CU_TRY(s.get(&p, r.front == kFrontCnnEmulLayers ? inner * C * 256 : 0));
+    GatherDst g;
+    for (size_t b = 0; b < n; b += pass) {
+        const size_t nb = std::min(pass, n - b);
+        const char *in = static_cast<const char *>(images) + b * in_bytes;
+        size_t row_bytes = in_bytes;
+        if (r.scale) {   // test_inference.py:140-141, BitNetMCU.py:435-436
+            launch_quantize_images(reinterpret_cast<const float *>(in), elems, q, nb, st);
+            in = reinterpret_cast<const char *>(q);
+            row_bytes = elems;
+        }
+        for (size_t c = 0; c < nb; c += inner) {
+            const size_t nc = std::min(inner, nb - c);
+            const void *rows = in + c * row_bytes;   // the FC stage's input
+            uint32_t stride = elems;
+            int rc = 0;
+            if (r.front == kFrontCnn) {
+                if ((rc = run_cnn_front(m, static_cast<const int8_t *>(rows), nc, feat, st))) return rc;
+            } else if (r.front == kFrontCnnEmul) {
+                if (!launch_cnn_emul_frontend(static_cast<const float *>(rows), m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, feat, m->feat_stride, nc, st))
+                    return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
+            } else if (r.front == kFrontCnnEmulLayers) {
+                // conv (ReLU, no shift) -> per-image renormalisation, pools in between (BitNetMCU.py:459-526)
+                int32_t *p0 = planes[0], *p1 = planes[1];
+                launch_expand_image(static_cast<const int8_t *>(rows), p0, C, 256, nc, st);
+                launch_conv33relu(p0, m->d_conv[0].p, C, 16, 0, p1, nc * C, st);
+                launch_conv_renorm(p1, C * 196, nc, st);
+                launch_conv33relu(p1, m->d_conv[1].p, C, 14, 0, p0, nc * C, st);
+                launch_conv_renorm(p0, C * 144, nc, st);
+                launch_maxpool22(p0, 12, p1, nc * C, st);
+                launch_conv33relu(p1, m->d_conv[2].p, C, 6, 0, p0, nc * C, st);
+                launch_conv_renorm(p0, C * 16, nc, st);
+                launch_maxpool22(p0, 4, p1, nc * C, st);
+                launch_i32_to_i8(p1, C * 4, ls.act[1], m->feat_stride, nc, st);   // flatten (C, 2, 2) -> features (BitNetMCU.py:443-445)
+            }
+            if (r.front != kFrontNone) {
+                rows = r.front == kFrontCnnEmulLayers ? ls.act[1] : feat;
+                stride = m->feat_stride;
+            }
+            const FcOutputs o = outputs_from(out, b + c, m->n_classes, emul, g);
+            if (r.fused) {
+                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st)))
+                    return fail(BNM_E_CUDA, "fused launch of %s failed (%d): %s", fc_chain_form_name(m->plan, r.form), rc,
+                                cudaGetErrorString(cudaGetLastError()));
+                continue;
+            }
+            if ((rc = run_layers(m, emul, static_cast<const int8_t *>(rows), stride, nc, emul && k ? lg : o.logits, o.labels, ls, st))) return rc;
+            if (emul && k) launch_topk_rows(lg, m->n_classes, k, o.topk.classes, static_cast<double *>(o.topk.scores), nc, st);
+            else if (k) launch_topk_rows(ls.acc, m->n_classes, k, o.topk.classes, static_cast<int32_t *>(o.topk.scores), nc, st);   // last layer's accumulators
+        }
+    }
+    return launch_status();
 }
 
 extern "C" int bnm_infer_launch_count(const bnm_model *m, size_t n) {
     if (!m || n == 0) return 0;
-    const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
-    const size_t chunk = c_engine_chunk(m, fused);
-    if (!chunk) return 1;
-    int per = m->model_class == BNM_MODEL_CNNMNIST ? 1 : 0;
-    per += fused ? 1 : (int)(2 * m->fc.size());   // fc + relunorm per layer (last relunorm = labels)
-    return (int)((n + chunk - 1) / chunk * per);
+    const Route r = choose_route(m, kEngineC, false, false);
+    if (!r.pass) return 1;
+    const int per = (r.front != kFrontNone) + (r.fused ? 1 : (int)(2 * m->fc.size()));   // front-end, fc + relunorm per layer
+    return (int)((n + r.pass - 1) / r.pass * per);
 }
 
 // a call must produce something: logits, labels or (gather) a destination in another buffer
 static bool has_output(const int32_t *logits, const uint32_t *labels, const GatherDst *gather) {
     return logits || labels || (gather && (gather->n_labels_dst || gather->n_logits_dst));
-}
-
-// the top-k outputs of a call from image b on (T: the type of its scores)
-template <class T> static TopKOutputs topk_from(const TopKOutputs &t, size_t b) {
-    return TopKOutputs{t.k, t.classes ? t.classes + b * t.k : nullptr, t.scores ? static_cast<T *>(t.scores) + b * t.k : nullptr};
-}
-
-// The C engine on int8 images on st, arguments checked -> out: logits int32 [n][n_classes], labels and gather, or with topk.k > 0
-// the k best classes of every image and their int32 scores.  FC models on the fused path in one launch, every other model in chunks
-// (CNN front-end, then the fused launch, or the layer-by-layer chain and for top-k k_topk_rows on its int32 accumulators).
-// The chunks' scratch (CNN features, the layer-by-layer path's buffers) is this call's own, for one chunk.
-static int run_c_engine(bnm_model *m, const int8_t *images, size_t n, const FcOutputs &out, cudaStream_t st) {
-    const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05;
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    const uint32_t k = out.topk.k;
-    const FcForm form = k ? kFormTopK : kFormInt8;
-    const char *kernel = k ? "top-k" : "FC";
-    const size_t chunk_max = c_engine_chunk(m, fused);
-    if (!chunk_max) {
-        int rc = fc_chain_launch(m->plan, form, images, n, out, st);
-        return rc ? fail(BNM_E_CUDA, "fused %s kernel launch failed (%d): %s", kernel, rc, cudaGetErrorString(cudaGetLastError())) : 0;
-    }
-    const size_t chunk = std::min(n, chunk_max);
-    Scratch scratch(m, st);
-    LayerScratch ls;
-    int8_t *feat = nullptr;
-    if (!fused) CU_TRY(layer_scratch(m, scratch, chunk, ls));
-    if (cnn) CU_TRY(scratch.get(&feat, chunk * m->feat_stride));
-    int rc = 0;
-    for (size_t b = 0; b < n; b += chunk) {
-        const size_t nb = std::min(chunk, n - b);
-        const int8_t *fc_in = images + b * m->img_bytes;
-        uint32_t fc_stride = m->img_bytes;
-        if (cnn) {
-            if ((rc = run_cnn_front(m, fc_in, nb, feat, st))) return rc;
-            fc_in = feat;
-            fc_stride = m->feat_stride;
-        }
-        int32_t *lg = out.logits ? static_cast<int32_t *>(out.logits) + b * m->n_classes : nullptr;
-        FcOutputs o{lg, out.labels ? out.labels + b : nullptr, nullptr, topk_from<int32_t>(out.topk, b)};
-        if (fused) {
-            GatherDst gchunk;
-            if (out.gather) { gchunk = *out.gather; gchunk.row_offset += b; o.gather = &gchunk; }
-            if ((rc = fc_chain_launch(m->plan, form, fc_in, nb, o, st)))
-                return fail(BNM_E_CUDA, "fused %s kernel launch failed (%d)", kernel, rc);
-        } else {
-            if ((rc = run_fc_layers(m, fc_in, fc_stride, nb, lg, o.labels, ls, st))) return rc;
-            if (k) launch_topk_rows(ls.acc, m->n_classes, k, o.topk.classes, static_cast<int32_t *>(o.topk.scores), nb, st);   // last layer's accumulators
-        }
-    }
-    return launch_status();
 }
 
 static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather, void *stream) {
@@ -623,7 +703,7 @@ static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32
     CU_TRY(cudaSetDevice(m->device));
     if (gather && bnm_model_active_path(m) != BNM_PATH_TCGEN05)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
-    return run_c_engine(m, images, n, FcOutputs{logits, labels, gather}, static_cast<cudaStream_t>(stream));
+    return run_route(m, choose_route(m, kEngineC, false, false), images, n, FcOutputs{logits, labels, gather}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
@@ -724,8 +804,8 @@ static int small_launch(bnm_model *m, SmallGen &g) {
     if (m->small_zero_copy >= 1) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), g.h_out.p, 0));
     const size_t n_log = g.logits ? n * (size_t)m->n_classes : 0;   // labels-only batches: the labels start the staging buffer
     uint32_t *d_lab = reinterpret_cast<uint32_t *>(d_out + n_log);
-    int rc = bnm_infer_batch_device(m, d_in, n, g.logits ? d_out : nullptr, g.labels ? d_lab : nullptr, st);
-    if (rc) return rc;
+    const FcOutputs out{g.logits ? d_out : nullptr, g.labels ? d_lab : nullptr};
+    if (int rc = run_route(m, choose_route(m, kEngineC, false, false), d_in, n, out, st)) return rc;
     if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(g.h_out.p, g.d_out.p, (n_log + (g.labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
     return 0;
@@ -800,9 +880,9 @@ static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *lo
     return rc;
 }
 
-// the C engine on host buffers in chunks of chunk_images, each through one slot's buffers: images in, run_c_engine, out's arrays
-// back.  Synchronous.
-static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const FcOutputs &out) {
+// the C engine's int8 route r on host buffers in chunks of chunk_images, each through one slot's buffers: images in, run_route,
+// out's arrays back.  Synchronous.
+static int infer_pipelined(bnm_model *m, const Route &r, const int8_t *images, size_t n, const FcOutputs &out) {
     std::lock_guard<std::mutex> turn(m->host_mu);   // large host calls take turns: each one keeps the copy engines busy alone
     const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
     // per image, in 4-byte words: d_logits holds the logits or the top-k scores (bnm_infer_batch sizes it and d_labels whether or
@@ -821,7 +901,7 @@ static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const F
             CU_TRY(s.d_labels.grow(chunk * n_labels * 4));
         }
     }
-    // every chunk's scratch is its own (run_c_engine): the chunks of every path overlap in time on all three streams
+    // every chunk's scratch is its own (run_route): the chunks of every path overlap in time on all three streams
     int32_t *h_logits = static_cast<int32_t *>(k ? out.topk.scores : out.logits);   // where d_logits goes
     size_t c = 0;
     for (size_t b = 0; b < n; b += chunk, c++) {
@@ -830,7 +910,7 @@ static int infer_pipelined(bnm_model *m, const int8_t *images, size_t n, const F
         CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
         const FcOutputs d{out.logits ? s.d_logits.p : nullptr, out.labels ? s.d_labels.p : nullptr, nullptr,
                          {(uint32_t)k, s.d_classes.p, out.topk.scores ? s.d_logits.p : nullptr}};
-        if (int rc = run_c_engine(m, s.d_images.p, nb, d, s.stream)) return rc;
+        if (int rc = run_route(m, r, s.d_images.p, nb, d, s.stream)) return rc;
         if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, s.d_classes.p, nb * k * 4, cudaMemcpyDeviceToHost, s.stream));
         if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * n_logits, s.d_logits.p, nb * n_logits * 4, cudaMemcpyDeviceToHost, s.stream));
         if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, s.d_labels.p, nb * 4, cudaMemcpyDeviceToHost, s.stream));
@@ -845,7 +925,7 @@ extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int
     if (n == 0) return 0;
     if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);   // sets the device where it launches
     CU_TRY(cudaSetDevice(m->device));
-    return infer_pipelined(m, images, n, FcOutputs{logits, labels});
+    return infer_pipelined(m, choose_route(m, kEngineC, false, false), images, n, FcOutputs{logits, labels});
 }
 
 extern "C" void *bnm_host_alloc(size_t bytes) {
@@ -975,7 +1055,8 @@ extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_
 }
 
 // float images -> logits / labels on the device.  FC models on the fused path (rows of <= 256 elements, <= 16 classes): ONE kernel, the
-// input scaling fused into its load stage.  Everything else: the scaling kernel into a scratch buffer, then the ordinary path.
+// input scaling fused into its load stage.  Everything else: per pass of 2^20 images the scaling kernel into the call's scratch,
+// then the int8 route on it.
 extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
     if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch_device_f32: null argument");
     if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_infer_batch_device_f32: no output (logits and labels both NULL)");
@@ -983,17 +1064,7 @@ extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, siz
     if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
     if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
     CU_TRY(cudaSetDevice(m->device));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool fused_fc = bnm_model_active_path(m) == BNM_PATH_TCGEN05 && m->model_class == BNM_MODEL_FCMNIST;
-    if (fused_fc && fc_chain_has_form(m->plan, kFormFloat)) {
-        int rc = fc_chain_launch(m->plan, kFormFloat, images, n, FcOutputs{logits, labels}, st);
-        return rc ? fail(BNM_E_CUDA, "fused float-input kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
-    }
-    Scratch scratch(m, st);
-    int8_t *q;
-    CU_TRY(scratch.get(&q, n * (size_t)m->img_bytes));
-    launch_quantize_images(images, m->img_bytes, q, n, st);
-    return bnm_infer_batch_device(m, q, n, logits, labels, stream);
+    return run_route(m, choose_route(m, kEngineC, true, false), images, n, FcOutputs{logits, labels}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out) {
@@ -1020,91 +1091,9 @@ extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems
 //   * FC models whose rows have <= 256 elements, up to 64 wide with <= 16 classes: one kernel, fc_emul_kernel;
 //   * other FC models: the scaling kernel (k_quantize_images), then fc_emul_i8_kernel at the plan's width;
 //   * CNN models up to kCnnEmulMaxChannels channels: the front-end kernel k_cnn_emul_frontend, then fc_emul_i8_kernel on its features.
-// BNM_PATH_LAYERS, models without a fused plan and wider CNN models run the emulation kernels layer by layer.
+// BNM_PATH_LAYERS, models without a fused plan and wider CNN models run the emulation kernels layer by layer (choose_route).
 // -----------------------------------------------------------------------------------------------
 int bnm::level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
-static const size_t kEmulChunkFc = 65536, kEmulChunkCnn = 2048;   // images per pass of the layer kernels (CNN: 2 x C kB of planes each)
-
-// The emulator on device buffers, asynchronous on st: images float32 [n][img_bytes] -> logits float64 [n][n_classes] and / or labels
-// (first maximum); or, with topk.k > 0, instead of both the k best classes of every image and their float64 scores (may be null).
-// The routes other than fc_emul_kernel run in chunks through scratch of their own, for one chunk.
-static int emulate_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, cudaStream_t st,
-                          const TopKOutputs &topk = {}) {
-    const size_t nl = m->fc.size();
-    const bool cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    const uint32_t C = m->channels, elems = m->img_bytes, k = topk.k;
-    const EmulRoute route = emul_route(m);
-    if (route == kEmulFloatRow && !k) {   // fc_emul_kernel has no top-k form: top-k takes the int8 rows
-        int rc = fc_chain_launch(m->plan, kFormEmulFloat, images, n, FcOutputs{logits, labels}, st);
-        return rc ? fail(BNM_E_CUDA, "fused emulator kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
-    }
-    if (route != kEmulLayers) {
-        const size_t chunk = std::min(n, kFusedCnnChunk);
-        Scratch scratch(m, st);
-        int8_t *rows;   // the int8 emulator row's input: scaled images (FC) or front-end features (CNN)
-        CU_TRY(scratch.get(&rows, chunk * (cnn ? m->feat_stride : elems)));
-        for (size_t b = 0; b < n; b += chunk) {
-            const size_t nb = std::min(chunk, n - b);
-            if (!cnn) launch_quantize_images(images + b * elems, elems, rows, nb, st);   // BitNetMCU.py:435-436
-            else if (!launch_cnn_emul_frontend(images + b * elems, m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, rows, m->feat_stride, nb, st))
-                return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
-            const FcOutputs out{logits ? logits + b * m->n_classes : nullptr, labels ? labels + b : nullptr, nullptr, topk_from<double>(topk, b)};
-            int rc = fc_chain_launch(m->plan, k ? kFormEmulTopK : kFormEmulInt8, rows, nb, out, st);
-            if (rc) return fail(BNM_E_CUDA, "fused %s kernel launch failed (%d): %s", k ? "emulator top-k" : "int8 emulator", rc,
-                                cudaGetErrorString(cudaGetLastError()));
-        }
-        return launch_status();
-    }
-    const size_t chunk = std::min(n, cnn ? kEmulChunkCnn : kEmulChunkFc);
-    Scratch scratch(m, st);
-    LayerScratch ls;   // accumulators and the two int8 activation buffers
-    double *topk_logits;   // top-k: the logits of a chunk
-    int8_t *q;             // the quantised images
-    int32_t *planes[2];    // CNN models: int32 conv planes
-    CU_TRY(layer_scratch(m, scratch, chunk, ls));
-    CU_TRY(scratch.get(&topk_logits, k ? chunk * m->n_classes : 0));
-    CU_TRY(scratch.get(&q, chunk * elems));
-    for (auto &p : planes) CU_TRY(scratch.get(&p, cnn ? chunk * C * 256 : 0));
-    int8_t *a0 = ls.act[0], *a1 = ls.act[1];
-    for (size_t b = 0; b < n; b += chunk) {
-        const size_t nb = std::min(chunk, n - b);
-        launch_quantize_images(images + b * elems, elems, q, nb, st);   // BitNetMCU.py:435-436
-        const int8_t *act = q;
-        uint32_t stride = elems;
-        if (cnn) {
-            // conv (ReLU, no shift) -> per-image renormalisation, pools in between (BitNetMCU.py:459-526), planes [(image, channel)][xy*xy]
-            int32_t *p0 = planes[0], *p1 = planes[1];
-            launch_expand_image(q, p0, C, 256, nb, st);
-            launch_conv33relu(p0, m->d_conv[0].p, C, 16, 0, p1, nb * C, st);
-            launch_conv_renorm(p1, C * 196, nb, st);
-            launch_conv33relu(p1, m->d_conv[1].p, C, 14, 0, p0, nb * C, st);
-            launch_conv_renorm(p0, C * 144, nb, st);
-            launch_maxpool22(p0, 12, p1, nb * C, st);
-            launch_conv33relu(p1, m->d_conv[2].p, C, 6, 0, p0, nb * C, st);
-            launch_conv_renorm(p0, C * 16, nb, st);
-            launch_maxpool22(p0, 4, p1, nb * C, st);
-            launch_i32_to_i8(p1, C * 4, a1, m->feat_stride, nb, st);   // flatten (C, 2, 2) -> features (BitNetMCU.py:443-445)
-            act = a1;
-            stride = m->feat_stride;
-        }
-        for (size_t l = 0; l < nl; l++) {
-            if (!launch_fc_dp4a(act, stride, m->fc[l], ls.acc, nb, st)) return fail(BNM_E_UNSUPPORTED, "FC layer %zu too wide for the layer kernel", l);
-            if (l + 1 == nl) break;   // no renormalisation for the last layer (BitNetMCU.py:528-530)
-            int8_t *next = (l & 1) ? a1 : a0;   // CNN features sit in a1 and are dead once layer 0 has run
-            const uint32_t next_stride = m->fc[l + 1].k_pad;
-            launch_relunorm_emul(ls.acc, m->fc[l].n_out, level_shift_of(m->fc[l].enc), next, next_stride, nb, st);
-            act = next;
-            stride = next_stride;
-        }
-        double *lg = k ? topk_logits : logits ? logits + b * m->n_classes : nullptr;
-        launch_emul_logits(ls.acc, m->n_classes, level_shift_of(m->fc[nl - 1].enc), lg, labels ? labels + b : nullptr, nb, st);
-        if (k) {
-            const TopKOutputs tk = topk_from<double>(topk, b);
-            launch_topk_rows(lg, m->n_classes, k, tk.classes, static_cast<double *>(tk.scores), nb, st);
-        }
-    }
-    return launch_status();
-}
 
 extern "C" int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream) {
     if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_emulate_batch_device: null argument");
@@ -1113,17 +1102,18 @@ extern "C" int bnm_emulate_batch_device(bnm_model *m, const float *images, size_
     if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
     if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned");
     CU_TRY(cudaSetDevice(m->device));
-    return emulate_device(m, images, n, logits, labels, static_cast<cudaStream_t>(stream));
+    return run_route(m, choose_route(m, kEngineEmul, true, false), images, n, FcOutputs{logits, labels}, static_cast<cudaStream_t>(stream));
 }
 
-// host buffers: per chunk, images in -> emulate_device -> logits out, synchronously
+// host buffers: per chunk of the layered emulator's pass, images in -> the emulator's route -> logits out, synchronously
 extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits) {
     if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_emulate_inference_quantized: null argument");
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
     std::lock_guard<std::mutex> turn(m->host_mu);   // takes turns with the other large host calls, on the pipeline's first stream
     const size_t elems = m->img_bytes, ncls = m->n_classes;
-    const size_t chunk = std::min(n, m->model_class == BNM_MODEL_CNNMNIST ? kEmulChunkCnn : kEmulChunkFc);
+    const size_t chunk = std::min(n, kEmulLayerPass[m->model_class == BNM_MODEL_CNNMNIST]);
+    const Route r = choose_route(m, kEngineEmul, true, false);
     cudaStream_t st = m->slots[0].stream;
     Scratch scratch(m, st);
     float *d_in;      // the device copies of a chunk's images and logits
@@ -1133,7 +1123,7 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         CU_TRY(cudaMemcpyAsync(d_in, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
-        if (int rc = emulate_device(m, d_in, nb, d_out, nullptr, st)) return rc;
+        if (int rc = run_route(m, r, d_in, nb, FcOutputs{d_out, nullptr}, st)) return rc;
         CU_TRY(cudaMemcpyAsync(logits + b * ncls, d_out, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
     }
@@ -1143,11 +1133,9 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
 // -----------------------------------------------------------------------------------------------
 // Both engines in one call (test_inference.py:130-175): the C engine's and the emulator's labels of the same float images, and
 // counts of their agreement and of their accuracy against truth.  The one-pass kernel where both float-input rows exist; every
-// other model runs bnm_infer_batch_device_f32's and emulate_device's routes per chunk, into the caller's label buffers or the
-// call's scratch, then k_engine_counts.
+// other model runs the C engine's float route and the emulator's route per pass, into the caller's label buffers or the call's
+// scratch, then k_engine_counts.
 // -----------------------------------------------------------------------------------------------
-static const size_t kEnginesChunk = 1 << 20;   // images per pass of the two routes (bounds the label scratch)
-
 extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth, uint32_t *labels_c,
                                           uint32_t *labels_py, bnm_engine_counts *counts, void *stream) {
     static_assert(sizeof(bnm_engine_counts) == 4 * sizeof(unsigned long long), "bnm_engine_counts: four 64-bit counters");
@@ -1160,11 +1148,10 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
     CU_TRY(cudaSetDevice(m->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     auto *cnt = reinterpret_cast<unsigned long long *>(counts);
-    if (engines_fused(m)) {
-        int rc = fc_chain_launch(m->plan, kFormEngines, images, n, FcOutputs{nullptr, labels_c, nullptr, {}, {labels_py, truth, cnt}}, st);
-        return rc ? fail(BNM_E_CUDA, "fused two-engine kernel launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError())) : 0;
-    }
-    const size_t chunk = std::min(n, kEnginesChunk), elems = m->img_bytes;
+    const Route r = choose_route(m, kEngineBoth, true, false);
+    if (r.fused) return run_route(m, r, images, n, FcOutputs{nullptr, labels_c, nullptr, {}, {labels_py, truth, cnt}}, st);
+    const Route c_route = choose_route(m, kEngineC, true, false), py_route = choose_route(m, kEngineEmul, true, false);
+    const size_t chunk = std::min(n, r.pass), elems = m->img_bytes;
     Scratch scratch(m, st);
     uint32_t *own[2];   // C / emulator labels the caller does not take
     CU_TRY(scratch.get(&own[0], counts && !labels_c ? chunk : 0));
@@ -1175,9 +1162,9 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
         uint32_t *lc = labels_c ? labels_c + b : own[0];
         uint32_t *lp = labels_py ? labels_py + b : own[1];
         if (lc)
-            if (int rc = bnm_infer_batch_device_f32(m, img, nb, nullptr, lc, st)) return rc;
+            if (int rc = run_route(m, c_route, img, nb, FcOutputs{nullptr, lc}, st)) return rc;
         if (lp)
-            if (int rc = emulate_device(m, img, nb, nullptr, lp, st)) return rc;
+            if (int rc = run_route(m, py_route, img, nb, FcOutputs{nullptr, lp}, st)) return rc;
         if (counts) launch_engine_counts(lc, lp, truth ? truth + b : nullptr, nb, m->n_classes, cnt, st);
     }
     return launch_status();
@@ -1190,8 +1177,8 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
 //   * CNN models on the fused path: the front-end into the feature scratch, then that kernel, in chunks of 2^20 images;
 //   * BNM_PATH_LAYERS and models without a fused plan: the layer-by-layer chain into its int32 scratch (the emulator: its float64
 //     logits into a chunk of scratch), then k_topk_rows.
-// The float entry scales the images into its own scratch first; the emulator runs its own front-end (scaling kernel or CNN
-// front-end) into its scratch, then fc_topk_kernel with its rule.
+// The float entry scales each pass of 2^20 images into its own scratch, then runs the int8 route on it; the emulator runs its own
+// front-end (scaling kernel or CNN front-end) into its scratch, then fc_topk_kernel with its rule.  choose_route picks the route.
 // -----------------------------------------------------------------------------------------------
 static int topk_check(const bnm_model *m, const char *fn, const void *images, size_t n, uint32_t k, const uint32_t *classes,
                       const void *scores, uintptr_t score_align, uintptr_t image_align) {
@@ -1204,49 +1191,31 @@ static int topk_check(const bnm_model *m, const char *fn, const void *images, si
     return 0;
 }
 
-// the kernels of the C engine's top-k on int8 images, for the route line
-static std::string topk_c_route(const bnm_model *m) {
-    std::string s;
-    if (m->model_class == BNM_MODEL_CNNMNIST)
-        s = cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
-    if (bnm_model_active_path(m) == BNM_PATH_TCGEN05) return s + fc_chain_form_name(m->plan, kFormTopK);
-    return s + "layer by layer + k_topk_rows<int32>";
-}
-
 extern "C" int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
     if (int rc = topk_check(m, "bnm_infer_topk_device", images, n, k, classes, scores, 4, 16)) return rc;
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
-    if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk_device: %s\n", topk_c_route(m).c_str());
-    return run_c_engine(m, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
+    const Route r = choose_route(m, kEngineC, false, true);
+    print_route(m, "topk route: bnm_infer_topk_device", r);
+    return run_route(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
     if (int rc = topk_check(m, "bnm_infer_topk_device_f32", images, n, k, classes, scores, 4, 16)) return rc;
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
-    if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk_device_f32: k_quantize_images + %s\n", topk_c_route(m).c_str());
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t chunk = std::min(n, kFusedCnnChunk), elems = m->img_bytes;
-    Scratch scratch(m, st);
-    int8_t *q;
-    CU_TRY(scratch.get(&q, chunk * elems));
-    for (size_t b = 0; b < n; b += chunk) {
-        const size_t nb = std::min(chunk, n - b);
-        launch_quantize_images(images + b * elems, (uint32_t)elems, q, nb, st);
-        const FcOutputs out{nullptr, nullptr, nullptr, {k, classes + b * k, scores ? scores + b * k : nullptr}};
-        if (int rc = run_c_engine(m, q, nb, out, st)) return rc;
-    }
-    return 0;
+    const Route r = choose_route(m, kEngineC, true, true);
+    print_route(m, "topk route: bnm_infer_topk_device_f32", r);
+    return run_route(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, double *scores, void *stream) {
     if (int rc = topk_check(m, "bnm_emulate_topk_device", images, n, k, classes, scores, 8, 16)) return rc;
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
-    if (m->verbose && emul_route(m) == kEmulLayers) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: layer by layer + k_topk_rows<double>\n");
-    else if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_emulate_topk_device: %s + %s\n", emul_rows_kernel(m), fc_chain_form_name(m->plan, kFormEmulTopK));
-    return emulate_device(m, images, n, nullptr, nullptr, static_cast<cudaStream_t>(stream), TopKOutputs{k, classes, scores});
+    const Route r = choose_route(m, kEngineEmul, true, true);
+    print_route(m, "topk route: bnm_emulate_topk_device", r);
+    return run_route(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
 }
 
 // host buffers: the chunked pipeline of bnm_infer_batch, k classes (and k scores) per image copied back
@@ -1254,8 +1223,9 @@ extern "C" int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint
     if (int rc = topk_check(m, "bnm_infer_topk", images, n, k, classes, scores, 1, 1)) return rc;
     if (n == 0) return 0;
     CU_TRY(cudaSetDevice(m->device));
-    if (m->verbose) fprintf(stderr, "bitnetmcu_b200: topk route: bnm_infer_topk: %s\n", topk_c_route(m).c_str());
-    return infer_pipelined(m, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}});
+    const Route r = choose_route(m, kEngineC, false, true);
+    print_route(m, "topk route: bnm_infer_topk", r);
+    return infer_pipelined(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}});
 }
 
 // -----------------------------------------------------------------------------------------------

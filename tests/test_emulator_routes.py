@@ -1,4 +1,4 @@
-"""The emulator's fused routes beyond the float-input row (bnm_emulate_batch_device, emulate_device in capi.cu):
+"""The emulator's fused routes beyond the float-input row (bnm_emulate_batch_device, run_route in capi.cu):
 
 * FC models wider than 64 or with more than 16 classes: k_quantize_images, then fc_emul_i8_kernel<max_n> (int8 TMA input, one
   pipe, one slot, the last layer at full width, the emulator's hidden-layer rule and float64 logits);

@@ -635,11 +635,13 @@ def _edge_row_images(n, elems, seed):
     return x
 
 
-@pytest.mark.parametrize("name,n", [("fc", N_MANY), ("fc", 1), ("fc", 129), ("ternary64", 5000), ("1k", 4097), ("binary160", 3000), ("cnn_48", 2500)])
+@pytest.mark.parametrize("name,n", [("fc", N_MANY), ("fc", 1), ("fc", 129), ("ternary64", 5000), ("1k", 4097), ("binary160", 3000), ("cnn_48", 2500),
+                                    ("binary160", (1 << 20) + 77)])
 def test_float_input_fused_into_the_fc_kernel(lib, oracle, name, n):
     """bnm_infer_batch_device_f32: float32 images -> int32 logits in one kernel for FC models (four quantiser warps write the int8 A
-    operand of layer 1 into shared memory, SWIZZLE_128B by hand), through the scaling kernel for CNN models; compared with the
-    NumPy scaling of test_inference.py:140-141 followed by the oracle.  Tolerance 0."""
+    operand of layer 1 into shared memory, SWIZZLE_128B by hand), through the scaling kernel for CNN models and wider FC models,
+    per pass of 2^20 images (Binary-160 at 2^20 + 77 crosses a pass); compared with the NumPy scaling of test_inference.py:140-141
+    followed by the oracle.  Tolerance 0."""
     import torch
     m = load_model(name)
     x = _edge_row_images(n, m.img_bytes, seed=n)
