@@ -6,7 +6,8 @@
 //   ReLUNorm  on the accumulator registers: row max over the four threads that share a row (two shuffles) -> shift ->
 //             clamp(x+r,0,cap)>>shift -> int8x4 pack, straight into the register fragment of the next layer's A operand
 //   layer l>1 wgmma s8 (RS)  A = those registers, B = smem weights                                    -> int32 in registers
-//   last      int32 logits: first-maximum argmax over the quad + 64-bit stores straight to HBM
+//   last      int32 logits: first-maximum argmax over the quad + 64-bit stores straight to HBM (the fixed-shape kernel: through a
+//             per-warp staging buffer in smem, one bulk async copy per warp and tile)
 //
 // The accumulator fragment of a thread holds columns {2c, 2c+1, 8+2c, 9+2c} of every 16-column block (c = lane % 4), while the
 // A fragment wants K positions {4c .. 4c+3}: instead of shuffling activations, the K axis of every hidden layer's weights is
@@ -92,6 +93,7 @@ struct ChainParams {
     uint32_t *classes;
     int32_t *scores_i32;
     double *scores_f64;
+    uint32_t off_out;                 // fixed-shape launches: smem offset of the consumer warps' logits / labels staging buffers
 };
 
 struct ChainKernel;
@@ -101,6 +103,7 @@ struct FormLayout {
     const ChainKernel *kernel = nullptr;   // null: the plan has no such form
     uint32_t n_stages = 0;                 // stages per pipe
     uint32_t off_w = 0, off_fring = 0;     // as in ChainParams; off_fring only for the float-input forms
+    uint32_t off_out = 0;                  // as in ChainParams; only for the fixed-shape row
     size_t smem_bytes = 0;                 // dynamic shared memory
 };
 
@@ -136,6 +139,9 @@ struct FcChainPlan {
     int *h_err = nullptr;
     uint32_t in_bytes = 0;
     FormLayout forms[kFcForms];
+    // a fixed-shape plan's int8 form for the launches its bulk-copy epilogue cannot serve (result exchange, an odd class count,
+    // or logits or labels not 16-byte aligned): the 16-wide two-slot row with its own layout
+    FormLayout int8_general;
     int sm_count = 0;
     int device = 0;
     int overlap = 0;                  // BNM_OPT_LAUNCH_OVERLAP: 0 and 1 dependent launch + wait, 2 independent launches
@@ -303,6 +309,11 @@ constexpr uint32_t kFixedInAtoms = 2;
 __host__ __device__ constexpr uint32_t fixed_n_pad(int l) { return l + 1 < kFixedLayers ? 64u : 16u; }
 __host__ __device__ constexpr uint32_t fixed_k_steps(int l) { return l == 0 ? kFixedInAtoms * 4 : 2u; }
 __host__ __device__ constexpr uint32_t fixed_b_off(int l) { return l == 0 ? 0u : fixed_b_off(l - 1) + fixed_k_steps(l - 1) * fixed_n_pad(l - 1) * 32; }
+// The fixed-shape epilogue stages each consumer warp's 16 rows of logits (int32 [16][n_classes], at most 16 classes) and their
+// 16 labels in a buffer of its own, which one bulk async copy each writes to HBM
+constexpr uint32_t kFixedOutLabels = 16 * 16 * 4;                   // offset of the labels in a warp's buffer
+constexpr uint32_t kFixedOutWarpBytes = kFixedOutLabels + 16 * 4;   // a warp's buffer (a multiple of 16 bytes)
+constexpr uint32_t kFixedOutBytes = 2 * 8 * kFixedOutWarpBytes;     // all 16 consumer warps of the two pipes
 // a shared-memory descriptor advanced by `units` x 16 bytes: the 14-bit start field of an address inside the CTA's shared memory
 // does not carry into the fields above it, so a 32-bit add of the low word is enough
 __device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t units) {
@@ -611,8 +622,17 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
         // per thread, then over the quad.  The last layer has at most kLastN columns.
         // (row_label below is the same argmax for the two-engine kernel; the epilogue keeps its own copy, whose instruction
         // schedule in the other kernels a shared lambda would change.)
+        // kFixed: the warp's rows img0 .. img0 + 15 go through its staging buffer instead (its launches have an even class
+        // count, 16-byte aligned logits and labels and no result exchange: fc_chain_launch).  A row of
+        // logits is ncls x 4 bytes, so the warp's block is 64 ncls contiguous bytes at a multiple of 64 ncls: one bulk copy.
         auto epilogue = [&](const uint32_t *a, uint32_t i) {
             const uint32_t tile = tile0 + i * tile_step;
+            [[maybe_unused]] const uint32_t out_buf = smem_base + P.off_out + warp * kFixedOutWarpBytes;
+            [[maybe_unused]] const uint32_t out_row = out_buf + (lane >> 2) * ncls * 4 + quad * 8;   // row lane / 4, column 2 quad
+            if constexpr (kFixed) {
+                if (lane == 0) bulk_wait_read<0>();   // the warp's previous copies have read the buffer
+                __syncwarp();
+            }
 #pragma unroll
             for (int r = 0; r < 2; r++) {
                 const size_t img = (size_t)tile * kTileM + row_in_tile + 8 * r;
@@ -632,7 +652,14 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                     const uint32_t op = __shfl_xor_sync(0xffffffffu, pos, sh);
                     if (ob > best || (ob == best && op < pos)) { best = ob; pos = op; }
                 }
-                if (kRule == kRuleEmul && img < P.n) {
+                if constexpr (kFixed) {   // rows past P.n are staged too, and not copied
+                    if (has_logits) {
+#pragma unroll
+                        for (int j = 0; j < kLastN / 8; j++)
+                            if (8 * j + 2 * quad < ncls) st_shared_v2(out_row + r * 32 * ncls + 32 * j, a[4 * j + 2 * r], a[4 * j + 2 * r + 1]);
+                    }
+                    if (quad == 0) st_shared_u32(out_buf + kFixedOutLabels + (8 * r + (lane >> 2)) * 4, pos);
+                } else if (kRule == kRuleEmul && img < P.n) {
                     // float64 logits: (double)acc x 2^-level_shift is exact, and argmax of the int32 accumulators is that of them
                     if (has_logits) {
                         double *d = P.emul_logits + img * ncls;
@@ -669,6 +696,24 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                             else P.lab_dst[d][P.row0 + img] = pos;
                         }
                     }
+                }
+            }
+            if constexpr (kFixed) {
+                fence_proxy_async_smem();   // the bulk copies (async proxy) read what these generic-proxy stores wrote
+                __syncwarp();
+                const size_t img0 = (size_t)tile * kTileM + half * 64 + wq * 16;
+                if (lane == 0 && img0 < P.n) {
+                    // the valid rows' bytes: bulk copies move multiples of 16 bytes, word stores the rest of the last tile's
+                    // block (8 bytes of logits, up to 12 of labels)
+                    auto flush = [](uint32_t *dst, uint32_t src, uint32_t bytes) {
+                        if (bytes >= 16) bulk_store_1d_a(dst, src, bytes & ~15u);
+#pragma unroll 1
+                        for (uint32_t o = bytes & ~15u; o < bytes; o += 4) dst[o / 4] = ld_shared_u32(src + o);
+                    };
+                    const uint32_t rows = (uint32_t)min((size_t)16, P.n - img0);
+                    if (has_logits) flush(reinterpret_cast<uint32_t *>(P.logits + img0 * ncls), out_buf, rows * ncls * 4);
+                    if (P.labels) flush(P.labels + img0, out_buf + kFixedOutLabels, rows * 4);
+                    bulk_commit();
                 }
             }
         };
@@ -842,6 +887,8 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                 }
             }
             wgmma_wait<0>();
+            if constexpr (kFixed)
+                if (lane == 0) bulk_wait_all<0>();   // the last logits and labels have reached global memory
         }
         BNM_TRACE_END();
         BNM_TRACE_STAMP(1);
@@ -1012,10 +1059,11 @@ struct ChainKernel {
     const char *name;
     void (*fn)(CUtensorMap, ChainParams);
     int threads;
+    uint32_t out_bytes;   // shared memory of the epilogue's staging buffers (the fixed-shape row), else 0
 };
 template <int kN, int kPipes = 1, bool kFloatIn = false, int kSlots = 1>
-static constexpr ChainKernel row(const char *name, void (*fn)(CUtensorMap, ChainParams)) {
-    return {name, fn, chain_threads<kN, kPipes, kFloatIn, kSlots>()};
+static constexpr ChainKernel row(const char *name, void (*fn)(CUtensorMap, ChainParams), uint32_t out_bytes = 0) {
+    return {name, fn, chain_threads<kN, kPipes, kFloatIn, kSlots>(), out_bytes};
 }
 
 // The launch forms, indexed by FcForm.  A launch takes everything but its buffers from its form's entry.
@@ -1052,11 +1100,11 @@ static const FormSpec kForms[kFcForms] = {
       row<192>("fc_topk_kernel<192,1,emul,topk>", fc_topk_kernel<192, true>), row<256>("fc_topk_kernel<256,1,emul,topk>", fc_topk_kernel<256, true>)}},
 };
 // kFormInt8's two-pipe two-slot rows: the last layer at full width, 16 wide (kLastN, for heads of at most 16 classes), or the
-// fixed-shape kernel
+// fixed-shape kernel with its logits staging buffers
 static const ChainKernel kTwoPipeRows[3] = {
     row<64, 2, false, 2>("fc_chain_kernel<64,2,2,64>", fc_chain_kernel<64, 2, false, 2>),
     row<64, 2, false, 2>("fc_chain_kernel<64,2,2,16>", fc_chain_kernel<64, 2, false, 2, 16>),
-    row<64, 2, false, 2>("fc_chain_kernel<64,2,2,16,fixed>", fc_chain_kernel<64, 2, false, 2, 16, true>),
+    row<64, 2, false, 2>("fc_chain_kernel<64,2,2,16,fixed>", fc_chain_kernel<64, 2, false, 2, 16, true>, kFixedOutBytes),
 };
 
 FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
@@ -1106,24 +1154,31 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     // rows of at most 256 elements and at most 16 classes
     const uint32_t fring = kFloatQuantWarps * 2 * kFloatGroupRows * 1024;
     const bool float_fits = in_bytes <= 256 && p.n_classes <= 16 && w_fixed + fring + 2 * p.stage_bytes <= smem_limit;
+    // the layout of a form's row: np rings of stages in what the weight image and `extra` bytes (the float rings, or the
+    // fixed-shape row's staging buffers) leave, at most kMaxStages over the pipes (>= 2 per pipe with two: two tile slots need
+    // it), then the weights, then the extra bytes.  The fixed-shape row's 17 kB of staging leave two stages per pipe, not three.
+    auto layout = [&](const FormSpec &s, const ChainKernel *k, uint32_t np) {
+        FormLayout l;
+        const uint32_t extra = s.float_in ? fring : k->out_bytes;
+        l.kernel = k;
+        l.n_stages = std::min({s.stage_cap, kMaxStages / np, (smem_limit - w_fixed - extra) / p.stage_bytes / np});
+        l.off_w = np * l.n_stages * p.stage_bytes;
+        l.off_fring = s.float_in ? l.off_w + w_fixed : 0;
+        l.off_out = k->out_bytes ? l.off_w + w_fixed : 0;
+        // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared
+        // memory enforces it once a CTA asks for more than half of the SM's 227 kB.
+        l.smem_bytes = std::max<size_t>((size_t)l.off_w + w_fixed + extra + 1024, 116 * 1024);
+        return l;
+    };
     FormLayout *forms = plan->forms;
     for (int f = 0; f < kFcForms; f++) {
         const FormSpec &s = kForms[f];
         const uint32_t np = f == kFormInt8 ? pipes : 1;
         const ChainKernel *k = np == 2 ? &kTwoPipeRows[fixed ? 2 : last16 ? 1 : 0] : &s.rows[max_n / 64 - 1];
         if (!k->fn || (s.float_in && !float_fits)) continue;
-        // the layout: np rings of stages in what the weight image and `extra` bytes (the float rings) leave, at most kMaxStages
-        // over the pipes (>= 2 per pipe with two: two tile slots need it), then the weights, then the extra bytes
-        FormLayout &l = forms[f];
-        const uint32_t extra = s.float_in ? fring : 0;
-        l.kernel = k;
-        l.n_stages = std::min({s.stage_cap, kMaxStages / np, (smem_limit - w_fixed - extra) / p.stage_bytes / np});
-        l.off_w = np * l.n_stages * p.stage_bytes;
-        l.off_fring = extra ? l.off_w + w_fixed : 0;
-        // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared
-        // memory enforces it once a CTA asks for more than half of the SM's 227 kB.
-        l.smem_bytes = std::max<size_t>((size_t)l.off_w + w_fixed + extra + 1024, 116 * 1024);
+        forms[f] = layout(s, k, np);
     }
+    if (fixed) plan->int8_general = layout(kForms[kFormInt8], &kTwoPipeRows[1], pipes);
     if (getenv("BNM_VERBOSE")) {   // diagnostics: the shapes this plan launches
         const bool has_float = forms[kFormFloat].kernel;
         auto args = [&](FcForm f) { return has_float ? strchr(forms[f].kernel->name, '<') : ""; };   // the template arguments
@@ -1162,11 +1217,14 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     if (cudaDeviceSynchronize() != cudaSuccess) { fc_chain_plan_destroy(plan); return fail("weight image kernel failed"); }
     p.w_image = plan->d_w_image;
     p.err = plan->d_err;
+    bool smem_ok = true;
     for (const FormLayout &f : plan->forms)
-        if (f.kernel && !raise_smem_limit((const void *)f.kernel->fn, f.smem_bytes)) {
-            fc_chain_plan_destroy(plan);
-            return fail("cannot opt in to the required dynamic shared memory");
-        }
+        smem_ok = smem_ok && (!f.kernel || raise_smem_limit((const void *)f.kernel->fn, f.smem_bytes));
+    const FormLayout &g = plan->int8_general;
+    if (!smem_ok || (g.kernel && !raise_smem_limit((const void *)g.kernel->fn, g.smem_bytes))) {
+        fc_chain_plan_destroy(plan);
+        return fail("cannot opt in to the required dynamic shared memory");
+    }
     return plan;
 }
 
@@ -1214,8 +1272,13 @@ static const CUtensorMap kNoTensorMap{};   // the float-input forms' tensor map:
 int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
-    const FormLayout &form = plan->forms[f];
-    if (!form.kernel) return -6;
+    if (!plan->forms[f].kernel) return -6;
+    // the fixed-shape row writes every warp's logits and labels with bulk copies, which need 16-byte aligned buffers and rows
+    // of whole 64-bit pairs (an even class count), and has no result exchange: other launches of its form take the plan's
+    // general row
+    auto aligned16 = [](const void *q) { return ((uintptr_t)q & 15) == 0; };
+    const bool bulk_out = !out.gather && plan->p.n_classes % 2 == 0 && aligned16(out.logits) && aligned16(out.labels);
+    const FormLayout &form = plan->forms[f].kernel->out_bytes && !bulk_out ? plan->int8_general : plan->forms[f];
     const FormSpec &s = kForms[f];
     // the C engine on int8 rows: the one form with result-exchange destinations and overlapping launches
     const bool engine_i8 = !s.float_in && s.rule == kRuleC && s.out == kOutLogits;
@@ -1228,6 +1291,7 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
     p.n_stages = form.n_stages;
     p.off_w = form.off_w;
     p.off_fring = form.off_fring;
+    p.off_out = form.off_out;
     if (s.rule == kRuleEmul) {
         p.emul_logits = static_cast<double *>(out.logits);
         p.scores_f64 = static_cast<double *>(t.scores);

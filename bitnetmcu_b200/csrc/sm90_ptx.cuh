@@ -98,6 +98,19 @@ __device__ __forceinline__ void mbar_arrive_a(uint32_t bar_addr) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_addr) : "memory");
 }
 
+// ---------------------------------------------------------------- shared memory at 32-bit addresses
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, uint32_t v0, uint32_t v1) {
+    asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(addr), "r"(v0), "r"(v1) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+
 // ---------------------------------------------------------------- fences / barriers
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
@@ -136,6 +149,11 @@ __device__ __forceinline__ uint64_t policy_evict_first() {
 __device__ __forceinline__ void bulk_store_1d(void *gmem_dst, const void *smem_src, uint32_t bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
                  ::"l"(reinterpret_cast<uint64_t>(gmem_dst)), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
+}
+// same, from a 32-bit shared-memory address held in a register
+__device__ __forceinline__ void bulk_store_1d_a(void *gmem_dst, uint32_t smem_src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                 ::"l"(reinterpret_cast<uint64_t>(gmem_dst)), "r"(smem_src), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
