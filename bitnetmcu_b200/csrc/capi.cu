@@ -689,38 +689,6 @@ extern "C" int bnm_infer_launch_count(const bnm_model *m, size_t n) {
     return (int)((n + r.pass - 1) / r.pass * per);
 }
 
-// a call must produce something: logits, labels or (gather) a destination in another buffer
-static bool has_output(const int32_t *logits, const uint32_t *labels, const GatherDst *gather) {
-    return logits || labels || (gather && (gather->n_labels_dst || gather->n_logits_dst));
-}
-
-static int infer_device_impl(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, const GatherDst *gather, void *stream) {
-    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch_device: null argument");
-    if (n && !has_output(logits, labels, gather)) return fail(BNM_E_ARG, "bnm_infer_batch_device: no output (logits, labels and gather destinations all absent)");
-    if (n == 0) return 0;
-    if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned (TMA)");
-    if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
-    CU_TRY(cudaSetDevice(m->device));
-    if (gather && bnm_model_active_path(m) != BNM_PATH_TCGEN05)
-        return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
-    return run_route(m, choose_route(m, kEngineC, false, false), images, n, FcOutputs{logits, labels, gather}, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
-    return infer_device_impl(m, images, n, logits, labels, nullptr, stream);
-}
-
-extern "C" int bnm_infer_batch_device_gather(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels,
-                                             const bnm_gather *gather, void *stream) {
-    static_assert(sizeof(bnm_gather) == sizeof(GatherDst), "bnm_gather and GatherDst must share their layout");
-    if (gather && (gather->n_labels_dst > BNM_MAX_GATHER_DST || gather->n_logits_dst > BNM_MAX_GATHER_DST))
-        return fail(BNM_E_ARG, "at most %d gather destinations", BNM_MAX_GATHER_DST);
-    if (gather)
-        for (uint32_t d = 0; d < gather->n_logits_dst; d++)
-            if ((uintptr_t)gather->logits_dst[d] & 7) return fail(BNM_E_ARG, "gather logits buffers must be 8-byte aligned");
-    return infer_device_impl(m, images, n, logits, labels, reinterpret_cast<const GatherDst *>(gather), stream);
-}
-
 // -----------------------------------------------------------------------------------------------
 // peer memory plumbing for the fused result exchange: cudaMalloc'd buffers exported / opened through CUDA IPC
 // -----------------------------------------------------------------------------------------------
@@ -919,15 +887,6 @@ static int infer_pipelined(bnm_model *m, const Route &r, const int8_t *images, s
     return 0;
 }
 
-extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
-    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch: null argument");
-    if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_infer_batch: no output (logits and labels both NULL)");
-    if (n == 0) return 0;
-    if (n <= kSmallBatch && n <= m->chunk_images) return infer_small(m, images, n, logits, labels);   // sets the device where it launches
-    CU_TRY(cudaSetDevice(m->device));
-    return infer_pipelined(m, choose_route(m, kEngineC, false, false), images, n, FcOutputs{logits, labels});
-}
-
 extern "C" void *bnm_host_alloc(size_t bytes) {
     void *p = nullptr;
     if (cudaHostAlloc(&p, bytes ? bytes : 1, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); fail(BNM_E_CUDA, "cudaHostAlloc(%zu) failed", bytes); return nullptr; }
@@ -1054,19 +1013,6 @@ extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_
     return launch_status();
 }
 
-// float images -> logits / labels on the device.  FC models on the fused path (rows of <= 256 elements, <= 16 classes): ONE kernel, the
-// input scaling fused into its load stage.  Everything else: per pass of 2^20 images the scaling kernel into the call's scratch,
-// then the int8 route on it.
-extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
-    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_infer_batch_device_f32: null argument");
-    if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_infer_batch_device_f32: no output (logits and labels both NULL)");
-    if (n == 0) return 0;
-    if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
-    if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned (64-bit row stores)");
-    CU_TRY(cudaSetDevice(m->device));
-    return run_route(m, choose_route(m, kEngineC, true, false), images, n, FcOutputs{logits, labels}, static_cast<cudaStream_t>(stream));
-}
-
 extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out) {
     if (int rc = require_device()) return rc;
     if (n == 0 || elems == 0) return 0;
@@ -1095,25 +1041,11 @@ extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems
 // -----------------------------------------------------------------------------------------------
 int bnm::level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
 
-extern "C" int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream) {
-    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_emulate_batch_device: null argument");
-    if (n && !logits && !labels) return fail(BNM_E_ARG, "bnm_emulate_batch_device: no output (logits and labels both NULL)");
-    if (n == 0) return 0;
-    if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
-    if (logits && ((uintptr_t)logits & 7)) return fail(BNM_E_ARG, "the device logits buffer must be 8-byte aligned");
-    CU_TRY(cudaSetDevice(m->device));
-    return run_route(m, choose_route(m, kEngineEmul, true, false), images, n, FcOutputs{logits, labels}, static_cast<cudaStream_t>(stream));
-}
-
-// host buffers: per chunk of the layered emulator's pass, images in -> the emulator's route -> logits out, synchronously
-extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits) {
-    if (!m || (n && (!images || !logits))) return fail(BNM_E_ARG, "bnm_emulate_inference_quantized: null argument");
-    if (n == 0) return 0;
-    CU_TRY(cudaSetDevice(m->device));
+// the emulator's route r on host buffers: per chunk of the layered emulator's pass, images in -> run_route -> logits out, synchronously
+static int emulate_host(bnm_model *m, const Route &r, const float *images, size_t n, double *logits) {
     std::lock_guard<std::mutex> turn(m->host_mu);   // takes turns with the other large host calls, on the pipeline's first stream
     const size_t elems = m->img_bytes, ncls = m->n_classes;
     const size_t chunk = std::min(n, kEmulLayerPass[m->model_class == BNM_MODEL_CNNMNIST]);
-    const Route r = choose_route(m, kEngineEmul, true, false);
     cudaStream_t st = m->slots[0].stream;
     Scratch scratch(m, st);
     float *d_in;      // the device copies of a chunk's images and logits
@@ -1134,43 +1066,127 @@ extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images
 // Both engines in one call (test_inference.py:130-175): the C engine's and the emulator's labels of the same float images, and
 // counts of their agreement and of their accuracy against truth.  The one-pass kernel where both float-input rows exist; every
 // other model runs the C engine's float route and the emulator's route per pass, into the caller's label buffers or the call's
-// scratch, then k_engine_counts.
+// scratch, then k_engine_counts (run_engines).
 // -----------------------------------------------------------------------------------------------
-extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth, uint32_t *labels_c,
-                                          uint32_t *labels_py, bnm_engine_counts *counts, void *stream) {
-    static_assert(sizeof(bnm_engine_counts) == 4 * sizeof(unsigned long long), "bnm_engine_counts: four 64-bit counters");
-    if (!m || (n && !images)) return fail(BNM_E_ARG, "bnm_compare_engines_device: null argument");
-    if (!labels_c && !labels_py && !counts) return fail(BNM_E_ARG, "bnm_compare_engines_device: no output (labels_c, labels_py and counts all NULL)");
-    if (truth && !counts) return fail(BNM_E_ARG, "bnm_compare_engines_device: truth without counts");
-    if (n == 0) return 0;
-    if ((uintptr_t)images & 15) return fail(BNM_E_ARG, "the device image buffer must be 16-byte aligned");
-    if ((uintptr_t)counts & 7) return fail(BNM_E_ARG, "the device counts must be 8-byte aligned");
-    CU_TRY(cudaSetDevice(m->device));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    auto *cnt = reinterpret_cast<unsigned long long *>(counts);
-    const Route r = choose_route(m, kEngineBoth, true, false);
-    if (r.fused) return run_route(m, r, images, n, FcOutputs{nullptr, labels_c, nullptr, {}, {labels_py, truth, cnt}}, st);
+// the two engines' route r without a fused form on n float images on st -> out: labels (the C engine's) and engines
+static int run_engines(bnm_model *m, const Route &r, const float *images, size_t n, const FcOutputs &out, cudaStream_t st) {
+    const EngineOutputs &e = out.engines;
     const Route c_route = choose_route(m, kEngineC, true, false), py_route = choose_route(m, kEngineEmul, true, false);
     const size_t chunk = std::min(n, r.pass), elems = m->img_bytes;
     Scratch scratch(m, st);
     uint32_t *own[2];   // C / emulator labels the caller does not take
-    CU_TRY(scratch.get(&own[0], counts && !labels_c ? chunk : 0));
-    CU_TRY(scratch.get(&own[1], counts && !labels_py ? chunk : 0));
+    CU_TRY(scratch.get(&own[0], e.counts && !out.labels ? chunk : 0));
+    CU_TRY(scratch.get(&own[1], e.counts && !e.labels_py ? chunk : 0));
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         const float *img = images + b * elems;
-        uint32_t *lc = labels_c ? labels_c + b : own[0];
-        uint32_t *lp = labels_py ? labels_py + b : own[1];
+        uint32_t *lc = out.labels ? out.labels + b : own[0];
+        uint32_t *lp = e.labels_py ? e.labels_py + b : own[1];
         if (lc)
             if (int rc = run_route(m, c_route, img, nb, FcOutputs{nullptr, lc}, st)) return rc;
         if (lp)
             if (int rc = run_route(m, py_route, img, nb, FcOutputs{nullptr, lp}, st)) return rc;
-        if (counts) launch_engine_counts(lc, lp, truth ? truth + b : nullptr, nb, m->n_classes, cnt, st);
+        if (e.counts) launch_engine_counts(lc, lp, e.truth ? e.truth + b : nullptr, nb, m->n_classes, e.counts, st);
     }
     return launch_status();
 }
 
 // -----------------------------------------------------------------------------------------------
+// the inference entries: each fills one call record, which run_call checks (check_call) and runs
+// -----------------------------------------------------------------------------------------------
+// One inference entry's call: the arguments of choose_route, the input, the outputs, and the rules in which entries differ.  A top-k
+// call needs classes when n > 0, checks k and its buffers' alignment whatever n, and names its route under BNM_VERBOSE.
+struct Call {
+    const char *name;   // the entry, for messages
+    Engine engine;
+    bool f32, topk;     // float32 images in; the k best classes out
+    const void *images;
+    size_t n;
+    FcOutputs out;      // the two engines' entry: the C engine's labels in labels, the rest in engines
+    struct { size_t images = 1, logits = 1, classes = 1, scores = 1, counts = 1; } align;   // in bytes; labels and truth: any
+    void *stream = nullptr;        // a device entry's stream
+    bool host = false;             // host buffers: a synchronous call through the small-batch path, the host pipeline or emulate_host
+    bool need_logits = false;      // logits must be given when n > 0 (the emulator's host entry)
+    bool no_output_at_0 = false;   // a call without outputs is an error even when n == 0 (the two engines' entry)
+};
+
+// The argument rules, in this order: a null model, or (n > 0) null images, classes or needed logits; no output at all; k out of
+// range; a misaligned buffer.  n == 0 ends the checks before the alignment ones except on a top-k call.
+static int check_call(const bnm_model *m, const Call &c) {
+    const FcOutputs &o = c.out;
+    if (!m || (c.n && (!c.images || (c.topk && !o.topk.classes) || (c.need_logits && !o.logits))))
+        return fail(BNM_E_ARG, "%s: null argument", c.name);
+    const bool output = o.logits || o.labels || (o.gather && (o.gather->n_labels_dst || o.gather->n_logits_dst)) || o.topk.classes ||
+                        o.engines.labels_py || o.engines.counts;
+    if (!output && (c.n || c.no_output_at_0)) return fail(BNM_E_ARG, "%s: no output (every output buffer NULL)", c.name);
+    if (c.topk && (o.topk.k < 1 || o.topk.k > std::min<uint32_t>(m->n_classes, BNM_MAX_TOPK)))
+        return fail(BNM_E_ARG, "%s: k = %u, must be 1 .. min(n_classes = %u, %d)", c.name, o.topk.k, m->n_classes, BNM_MAX_TOPK);
+    if (!c.n && !c.topk) return 0;
+    const struct { const void *p; size_t align; const char *what; } bufs[] = {
+        {c.images, c.align.images, "device image buffer"}, {o.logits, c.align.logits, "device logits buffer"},
+        {o.topk.classes, c.align.classes, "classes buffer"}, {o.topk.scores, c.align.scores, "scores buffer"},
+        {o.engines.counts, c.align.counts, "device counts"}};
+    for (const auto &b : bufs)
+        if ((uintptr_t)b.p & (b.align - 1)) return fail(BNM_E_ARG, "%s: the %s must be %zu-byte aligned", c.name, b.what, b.align);
+    return 0;
+}
+
+// Check call c and run its route: on the device entry's stream; for the two engines without a fused form, run_engines; host calls
+// of up to kSmallBatch images (and chunk) through infer_small, the others through infer_pipelined or emulate_host.
+static int run_call(bnm_model *m, const Call &c) {
+    if (int rc = check_call(m, c)) return rc;
+    if (c.n == 0) return 0;
+    const FcOutputs &o = c.out;
+    if (c.host && c.engine == kEngineC && !c.topk && c.n <= kSmallBatch && c.n <= m->chunk_images)   // sets the device where it launches
+        return infer_small(m, static_cast<const int8_t *>(c.images), c.n, static_cast<int32_t *>(o.logits), o.labels);
+    CU_TRY(cudaSetDevice(m->device));
+    const Route r = choose_route(m, c.engine, c.f32, c.topk);
+    if (c.topk && m->verbose) print_route(m, (std::string("topk route: ") + c.name).c_str(), r);
+    if (o.gather && !r.fused)
+        return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
+    cudaStream_t st = static_cast<cudaStream_t>(c.stream);
+    if (c.host && c.engine == kEngineEmul) return emulate_host(m, r, static_cast<const float *>(c.images), c.n, static_cast<double *>(o.logits));
+    if (c.host) return infer_pipelined(m, r, static_cast<const int8_t *>(c.images), c.n, o);
+    if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, static_cast<const float *>(c.images), c.n, o, st);
+    return run_route(m, r, c.images, c.n, o, st);
+}
+
+extern "C" int bnm_infer_batch_device_gather(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels,
+                                             const bnm_gather *gather, void *stream) {
+    static_assert(sizeof(bnm_gather) == sizeof(GatherDst), "bnm_gather and GatherDst must share their layout");
+    if (gather && (gather->n_labels_dst > BNM_MAX_GATHER_DST || gather->n_logits_dst > BNM_MAX_GATHER_DST))
+        return fail(BNM_E_ARG, "at most %d gather destinations", BNM_MAX_GATHER_DST);
+    if (gather)
+        for (uint32_t d = 0; d < gather->n_logits_dst; d++)
+            if ((uintptr_t)gather->logits_dst[d] & 7) return fail(BNM_E_ARG, "gather logits buffers must be 8-byte aligned");
+    const GatherDst *g = reinterpret_cast<const GatherDst *>(gather);
+    return run_call(m, {"bnm_infer_batch_device", kEngineC, false, false, images, n, {logits, labels, g}, {16, 8}, stream});
+}
+
+extern "C" int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
+    return bnm_infer_batch_device_gather(m, images, n, logits, labels, nullptr, stream);
+}
+
+// float images -> logits / labels on the device.  FC models on the fused path (rows of <= 256 elements, <= 16 classes): ONE kernel, the
+// input scaling fused into its load stage.  Everything else: per pass of 2^20 images the scaling kernel into the call's scratch,
+// then the int8 route on it.
+extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
+    return run_call(m, {"bnm_infer_batch_device_f32", kEngineC, true, false, images, n, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream) {
+    return run_call(m, {"bnm_emulate_batch_device", kEngineEmul, true, false, images, n, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth, uint32_t *labels_c,
+                                          uint32_t *labels_py, bnm_engine_counts *counts, void *stream) {
+    static_assert(sizeof(bnm_engine_counts) == 4 * sizeof(unsigned long long), "bnm_engine_counts: four 64-bit counters");
+    if (truth && !counts) return fail(BNM_E_ARG, "bnm_compare_engines_device: truth without counts");
+    const FcOutputs out{nullptr, labels_c, nullptr, {}, {labels_py, truth, reinterpret_cast<unsigned long long *>(counts)}};
+    return run_call(m, {"bnm_compare_engines_device", kEngineBoth, true, false, images, n, out, {16, 1, 1, 1, 8}, stream, false, false,
+                        true});   // no outputs: an error even at n == 0
+}
+
 // Top-k (section 8): the k best classes of every image and their scores -- the classes ranked by logit, highest first, ties to the
 // lower class, so rank 0 is the label of the matching entry -- and no logits written anywhere.
 //   * FC models on the fused path: one launch of fc_topk_kernel, whose epilogue ranks the classes in registers;
@@ -1179,53 +1195,32 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
 //     logits into a chunk of scratch), then k_topk_rows.
 // The float entry scales each pass of 2^20 images into its own scratch, then runs the int8 route on it; the emulator runs its own
 // front-end (scaling kernel or CNN front-end) into its scratch, then fc_topk_kernel with its rule.  choose_route picks the route.
-// -----------------------------------------------------------------------------------------------
-static int topk_check(const bnm_model *m, const char *fn, const void *images, size_t n, uint32_t k, const uint32_t *classes,
-                      const void *scores, uintptr_t score_align, uintptr_t image_align) {
-    if (!m || (n && (!images || !classes))) return fail(BNM_E_ARG, "%s: null argument", fn);
-    if (k < 1 || k > std::min<uint32_t>(m->n_classes, BNM_MAX_TOPK))
-        return fail(BNM_E_ARG, "%s: k = %u, must be 1 .. min(n_classes = %u, %d)", fn, k, m->n_classes, BNM_MAX_TOPK);
-    if ((uintptr_t)images & (image_align - 1)) return fail(BNM_E_ARG, "%s: the device image buffer must be %zu-byte aligned", fn, (size_t)image_align);
-    if ((uintptr_t)classes & 3) return fail(BNM_E_ARG, "%s: the classes buffer must be 4-byte aligned", fn);
-    if ((uintptr_t)scores & (score_align - 1)) return fail(BNM_E_ARG, "%s: the scores buffer must be %zu-byte aligned", fn, (size_t)score_align);
-    return 0;
-}
-
 extern "C" int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
-    if (int rc = topk_check(m, "bnm_infer_topk_device", images, n, k, classes, scores, 4, 16)) return rc;
-    if (n == 0) return 0;
-    CU_TRY(cudaSetDevice(m->device));
-    const Route r = choose_route(m, kEngineC, false, true);
-    print_route(m, "topk route: bnm_infer_topk_device", r);
-    return run_route(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
+    return run_call(m, {"bnm_infer_topk_device", kEngineC, false, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
 }
 
 extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
-    if (int rc = topk_check(m, "bnm_infer_topk_device_f32", images, n, k, classes, scores, 4, 16)) return rc;
-    if (n == 0) return 0;
-    CU_TRY(cudaSetDevice(m->device));
-    const Route r = choose_route(m, kEngineC, true, true);
-    print_route(m, "topk route: bnm_infer_topk_device_f32", r);
-    return run_route(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
+    return run_call(m, {"bnm_infer_topk_device_f32", kEngineC, true, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
 }
 
 extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, double *scores, void *stream) {
-    if (int rc = topk_check(m, "bnm_emulate_topk_device", images, n, k, classes, scores, 8, 16)) return rc;
-    if (n == 0) return 0;
-    CU_TRY(cudaSetDevice(m->device));
-    const Route r = choose_route(m, kEngineEmul, true, true);
-    print_route(m, "topk route: bnm_emulate_topk_device", r);
-    return run_route(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}}, static_cast<cudaStream_t>(stream));
+    return run_call(m, {"bnm_emulate_topk_device", kEngineEmul, true, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
+}
+
+// host buffers: n <= kSmallBatch images share a launch with concurrent small calls, larger batches run the chunked pipeline
+extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
+    return run_call(m, {"bnm_infer_batch", kEngineC, false, false, images, n, {logits, labels}, {}, nullptr, true});   // host buffers
 }
 
 // host buffers: the chunked pipeline of bnm_infer_batch, k classes (and k scores) per image copied back
 extern "C" int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores) {
-    if (int rc = topk_check(m, "bnm_infer_topk", images, n, k, classes, scores, 1, 1)) return rc;
-    if (n == 0) return 0;
-    CU_TRY(cudaSetDevice(m->device));
-    const Route r = choose_route(m, kEngineC, false, true);
-    print_route(m, "topk route: bnm_infer_topk", r);
-    return infer_pipelined(m, r, images, n, FcOutputs{nullptr, nullptr, nullptr, {k, classes, scores}});
+    return run_call(m, {"bnm_infer_topk", kEngineC, false, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {}, nullptr,
+                        true});   // host buffers
+}
+
+extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits) {
+    return run_call(m, {"bnm_emulate_inference_quantized", kEngineEmul, true, false, images, n, {logits}, {}, nullptr, true,
+                        true});   // host buffers, logits required
 }
 
 // -----------------------------------------------------------------------------------------------

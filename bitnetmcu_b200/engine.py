@@ -25,6 +25,9 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else C.c_void_p(a.ctypes.data)
 
 
+N = "n"   # in the shape of a tensor argument of Engine._device_call: the number of images
+
+
 class Engine:
     """One packed model resident on one GPU."""
 
@@ -97,29 +100,29 @@ class Engine:
         work on the stream (include/bitnetmcu_b200.h): its images must already be complete when the previous call was
         enqueued.  Chains such as ``quantize_images_device`` -> ``infer_device`` on one stream need mode 0 or 1."""
         import torch
-        n = images.shape[0]
+        self._device_call(self.lib.bnm_infer_batch_device, images, torch.int8,
+                          [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)
+
+    def _device_call(self, fn, images, in_dtype, args, stream) -> None:
+        """fn(handle, images, n, *args, stream) on this GPU, images a contiguous in_dtype [n, img_bytes] tensor.  A tensor argument
+        is given as (tensor or None, its dtype or element size, its shape with N for n, or N alone for n elements of any shape):
+        asserted contiguous and of that type and shape, it passes as its pointer, None as NULL.  Other arguments pass as they are.
+        stream: a cudaStream_t as int, None for torch's current stream."""
+        import torch
         if stream is None:
             stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.is_contiguous() and images.dtype == torch.int8 and images.shape[1] == self.img_bytes
-        _lib.check(self.lib.bnm_infer_batch_device(self.handle, C.c_void_p(images.data_ptr()), n, self._logits_ptr(logits, n),
-                                                   self._labels_ptr(labels, n), C.c_void_p(stream)), "bnm_infer_batch_device")
-
-    def _logits_ptr(self, logits, n: int):
-        """a torch.int32 [n, n_classes] device tensor as a pointer argument, None as NULL"""
-        import torch
-        if logits is None:
-            return None
-        assert logits.is_contiguous() and logits.dtype == torch.int32 and tuple(logits.shape) == (n, self.n_classes)
-        return C.c_void_p(logits.data_ptr())
-
-    @staticmethod
-    def _labels_ptr(labels, n: int):
-        """a 4-byte [n] device tensor as a pointer argument, None as NULL"""
-        if labels is None:
-            return None
-        assert labels.is_contiguous() and labels.element_size() == 4 and labels.numel() == n
-        return C.c_void_p(labels.data_ptr())
-
+        assert images.is_contiguous() and images.dtype == in_dtype and images.dim() == 2 and images.shape[1] == self.img_bytes
+        n = images.shape[0]
+        vals = []
+        for a in args:
+            if isinstance(a, tuple):
+                t, kind, shape = a
+                if t is not None:
+                    assert t.is_contiguous() and (t.dtype == kind if isinstance(kind, torch.dtype) else t.element_size() == kind)
+                    assert t.numel() == n if shape is N else tuple(t.shape) == tuple(n if d is N else d for d in shape)
+                a = None if t is None else C.c_void_p(t.data_ptr())
+            vals.append(a)
+        _lib.check(fn(self.handle, C.c_void_p(images.data_ptr()), n, *vals, C.c_void_p(stream)), fn.__name__)
 
     def inference_quantized(self, input_data: np.ndarray) -> np.ndarray:
         """``QuantizedModel.inference_quantized`` (/root/reference/BitNetMCU.py:420-535) on the GPU: float32 images [n, img_bytes]
@@ -135,28 +138,16 @@ class Engine:
         [n, n_classes] or None, labels [n] (4-byte elements: ``np.argmax`` of the logits) or None (not both None).  Asynchronous on
         ``stream`` (a cudaStream_t as int; default: torch's current stream).  FC models up to 64 wide: one kernel."""
         import torch
-        n = images.shape[0]
-        if stream is None:
-            stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.is_contiguous() and images.dtype == torch.float32 and images.shape[1] == self.img_bytes
-        lp = None
-        if logits is not None:
-            assert logits.is_contiguous() and logits.dtype == torch.float64 and tuple(logits.shape) == (n, self.n_classes)
-            lp = C.c_void_p(logits.data_ptr())
-        _lib.check(self.lib.bnm_emulate_batch_device(self.handle, C.c_void_p(images.data_ptr()), n, lp, self._labels_ptr(labels, n),
-                                                     C.c_void_p(stream)), "bnm_emulate_batch_device")
+        self._device_call(self.lib.bnm_emulate_batch_device, images, torch.float32,
+                          [(logits, torch.float64, (N, self.n_classes)), (labels, 4, N)], stream)
 
     def infer_device_f32(self, images, logits, labels=None, stream: Optional[int] = None) -> None:
         """images: torch.float32 [n, img_bytes] on this GPU (un-normalised pixels, as test_inference.py:140 sees them) -> logits
         torch.int32 [n, n_classes] or None, labels [n] or None (not both None).  FC models: one kernel with the input scaling fused
         into its load stage."""
         import torch
-        n = images.shape[0]
-        if stream is None:
-            stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.is_contiguous() and images.dtype == torch.float32 and images.shape[1] == self.img_bytes
-        _lib.check(self.lib.bnm_infer_batch_device_f32(self.handle, C.c_void_p(images.data_ptr()), n, self._logits_ptr(logits, n),
-                                                       self._labels_ptr(labels, n), C.c_void_p(stream)), "bnm_infer_batch_device_f32")
+        self._device_call(self.lib.bnm_infer_batch_device_f32, images, torch.float32,
+                          [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)
 
     def compare_engines_device(self, images, truth=None, labels_c=None, labels_py=None, counts=None, stream: Optional[int] = None) -> None:
         """Both engines on the same float images in one call (test_inference.py:130-175): images torch.float32 [n, img_bytes] on
@@ -166,17 +157,8 @@ class Engine:
         counts may be None, not all three.  Asynchronous on ``stream`` (default: torch's current stream).  FC models up to 64
         wide: one kernel."""
         import torch
-        n = images.shape[0]
-        if stream is None:
-            stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.is_contiguous() and images.dtype == torch.float32 and images.shape[1] == self.img_bytes
-        cp = None
-        if counts is not None:
-            assert counts.is_contiguous() and counts.dtype == torch.int64 and tuple(counts.shape) == (4,)
-            cp = C.c_void_p(counts.data_ptr())
-        _lib.check(self.lib.bnm_compare_engines_device(self.handle, C.c_void_p(images.data_ptr()), n, self._labels_ptr(truth, n),
-                                                       self._labels_ptr(labels_c, n), self._labels_ptr(labels_py, n), cp,
-                                                       C.c_void_p(stream)), "bnm_compare_engines_device")
+        self._device_call(self.lib.bnm_compare_engines_device, images, torch.float32,
+                          [(truth, 4, N), (labels_c, 4, N), (labels_py, 4, N), (counts, torch.int64, (4,))], stream)
 
     # ---- top-k: each image's k best classes and their scores (include/bitnetmcu_b200.h section 8) ------------------------------
     # Classes are ranked by logit, highest first, ties to the lower class: np.argsort(-logits, kind="stable")[:, :k].  Rank 0 is
@@ -191,44 +173,25 @@ class Engine:
         _lib.check(self.lib.bnm_infer_topk(self.handle, _ptr(imgs), n, int(k), _ptr(classes), _ptr(scores)), "bnm_infer_topk")
         return classes, scores
 
-    @staticmethod
-    def _topk_ptrs(images, k: int, classes, scores, score_dtype):
-        """the pointer arguments of a top-k device call: classes [n, k] (4-byte elements), scores [n, k] of score_dtype or None"""
-        n = images.shape[0]
-        assert images.is_contiguous() and images.dim() == 2
-        assert classes.is_contiguous() and classes.element_size() == 4 and tuple(classes.shape) == (n, k)
-        sp = None
-        if scores is not None:
-            assert scores.is_contiguous() and scores.dtype == score_dtype and tuple(scores.shape) == (n, k)
-            sp = C.c_void_p(scores.data_ptr())
-        return C.c_void_p(images.data_ptr()), n, C.c_void_p(classes.data_ptr()), sp
-
-    def _topk_device(self, fn, what, images, in_dtype, k, classes, scores, score_dtype, stream):
-        import torch
-        if stream is None:
-            stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.dtype == in_dtype and images.shape[1] == self.img_bytes
-        ip, n, cp, sp = self._topk_ptrs(images, k, classes, scores, score_dtype)
-        _lib.check(fn(self.handle, ip, n, int(k), cp, sp, C.c_void_p(stream)), what)
-
     def topk_device(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
         """images torch.int8 [n, img_bytes] on this GPU -> classes [n, k] (torch.int32 / uint32) and scores torch.int32 [n, k] or
         None.  Asynchronous on ``stream`` (a cudaStream_t as int; default: torch's current stream)."""
         import torch
-        self._topk_device(self.lib.bnm_infer_topk_device, "bnm_infer_topk_device", images, torch.int8, k, classes, scores, torch.int32, stream)
+        self._device_call(self.lib.bnm_infer_topk_device, images, torch.int8,
+                          [int(k), (classes, 4, (N, k)), (scores, torch.int32, (N, k))], stream)
 
     def topk_device_f32(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
         """``topk_device`` on torch.float32 [n, img_bytes] images, scaled to int8 as ``infer_device_f32`` does."""
         import torch
-        self._topk_device(self.lib.bnm_infer_topk_device_f32, "bnm_infer_topk_device_f32", images, torch.float32, k, classes, scores,
-                          torch.int32, stream)
+        self._device_call(self.lib.bnm_infer_topk_device_f32, images, torch.float32,
+                          [int(k), (classes, 4, (N, k)), (scores, torch.int32, (N, k))], stream)
 
     def emulate_topk_device(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
         """The emulator's top-k: images torch.float32 [n, img_bytes] -> classes [n, k] and scores torch.float64 [n, k] (the
         logits ``inference_quantized_device`` writes, at those classes) or None."""
         import torch
-        self._topk_device(self.lib.bnm_emulate_topk_device, "bnm_emulate_topk_device", images, torch.float32, k, classes, scores,
-                          torch.float64, stream)
+        self._device_call(self.lib.bnm_emulate_topk_device, images, torch.float32,
+                          [int(k), (classes, 4, (N, k)), (scores, torch.float64, (N, k))], stream)
 
     def infer_tensor(self, images, want_logits: bool = True):
         """images: torch.int8 [n, img_bytes] on this engine's GPU -> (logits torch.int32 [n, n_classes], labels torch.int32 [n]) on

@@ -20,6 +20,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import _lib
+from .engine import N
 
 
 class _DevArray:
@@ -117,10 +118,10 @@ def infer_gather(eng, images, logits, labels, buffers: PeerGatherBuffers, labels
     """``Engine.infer_device`` whose epilogue also stores this rank's rows into the gather buffers of the ranks listed in
     ``labels_to`` / ``logits_to`` (pass this rank's own slice of its buffer as ``logits`` / ``labels`` and leave it out of the lists).
     ``logits`` / ``labels`` may be None: no local copy of that output (the call still needs one output or destination)."""
+    import torch
     g = buffers.spec(labels_to, logits_to, labels_u8)
-    n = images.shape[0]
-    _lib.check(eng.lib.bnm_infer_batch_device_gather(eng.handle, C.c_void_p(images.data_ptr()), n, eng._logits_ptr(logits, n),
-                                                     eng._labels_ptr(labels, n), C.byref(g), C.c_void_p(stream)), "bnm_infer_batch_device_gather")
+    eng._device_call(eng.lib.bnm_infer_batch_device_gather, images, torch.int8,
+                     [(logits, torch.int32, (N, eng.n_classes)), (labels, 4, N), C.byref(g)], stream)
 
 
 def bench_gathers(ctx, eng, db, ms_compute: float) -> dict:
