@@ -47,6 +47,30 @@ static int launch_status() {
 
 static uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
+// For its scope, the calling thread may make the calls a stream capture in cudaStreamCaptureModeGlobal forbids to every other
+// thread (allocation, stream synchronisation): the host paths' synchronous work runs under it, so that a host call next to
+// another thread's capture neither fails nor invalidates that capture.  The thread's own mode comes back at the end of the scope
+// (cudaThreadExchangeStreamCaptureMode, as PyTorch's allocator does).  None of that work touches a capturing stream.
+struct RelaxedCaptureMode {
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    RelaxedCaptureMode() { cudaThreadExchangeStreamCaptureMode(&mode); }
+    ~RelaxedCaptureMode() { cudaThreadExchangeStreamCaptureMode(&mode); }
+    RelaxedCaptureMode(const RelaxedCaptureMode &) = delete;
+    RelaxedCaptureMode &operator=(const RelaxedCaptureMode &) = delete;
+};
+
+// the capture state of stream st (an eager stream when it cannot be read: a launch on it then reports the error)
+static StreamCapture capture_of(cudaStream_t st) {
+    StreamCapture c;
+    cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
+    if (cudaStreamGetCaptureInfo(st, &s, &c.id) != cudaSuccess) {
+        cudaGetLastError();
+        return StreamCapture{};
+    }
+    c.active = s != cudaStreamCaptureStatusNone;   // an invalidated capture too: its launches must not enter the eager record
+    return c;
+}
+
 // One allocation of T and its only owner, which frees it: device memory, or mapped pinned host memory (kPinned).  grow(need) makes
 // it at least `need` bytes large: a larger request discards the contents and allocates anew (zeroed on request); one it already
 // meets makes no CUDA call.
@@ -184,8 +208,9 @@ static void free_fc_layer(FcLayerDev &L) {
 }
 
 // one FC layer's packed weights (device, zero padded past the end) decoded into its int8 planes, the residual ones only where they
-// are needed.  On failure nothing stays allocated.
-static cudaError_t decode_fc_layer(const void *d_packed, int32_t enc, uint32_t n_in, uint32_t n_out, int nf4_ext, FcLayerDev &L) {
+// are needed, decoded on st and synchronised with it.  On failure nothing stays allocated.
+static cudaError_t decode_fc_layer(const void *d_packed, int32_t enc, uint32_t n_in, uint32_t n_out, int nf4_ext, FcLayerDev &L,
+                                   cudaStream_t st) {
     L.enc = enc;
     L.n_in = n_in;
     L.n_out = n_out;
@@ -198,11 +223,13 @@ static cudaError_t decode_fc_layer(const void *d_packed, int32_t enc, uint32_t n
     if (e == cudaSuccess) e = cudaMalloc(&L.dense_b, plane);
     if (e == cudaSuccess) e = cudaMalloc(&L.quad_a, plane);
     if (e == cudaSuccess) e = cudaMalloc(&L.quad_b, plane);
-    if (e == cudaSuccess) e = d_flag.grow(sizeof(int), true);
+    if (e == cudaSuccess) e = d_flag.grow(sizeof(int));
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_flag.p, 0, sizeof(int), st);
     if (e == cudaSuccess) {
-        launch_decode_fc(d_packed, enc, n_in, n_out, L.k_pad, L.n_pad, L.dense_a, L.dense_b, L.quad_a, L.quad_b, nf4_ext, d_flag.p, 0);
-        e = cudaMemcpy(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost);
+        launch_decode_fc(d_packed, enc, n_in, n_out, L.k_pad, L.n_pad, L.dense_a, L.dense_b, L.quad_a, L.quad_b, nf4_ext, d_flag.p, st);
+        e = cudaMemcpyAsync(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st);
     }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) {
         free_fc_layer(L);
     } else if (!flag) {   // no residual plane needed (everything but FP130 layers that contain +128)
@@ -233,7 +260,7 @@ static int build_fc_dev(bnm_model *m) {
     m->max_nout = 0;
     for (auto &H : m->fc_host) {
         FcLayerDev L;
-        if (cudaError_t e = decode_fc_layer(H.d_packed, H.enc, H.n_in, H.n_out, m->nf4_ext, L)) {   // nothing half-built stays behind
+        if (cudaError_t e = decode_fc_layer(H.d_packed, H.enc, H.n_in, H.n_out, m->nf4_ext, L, 0)) {   // nothing half-built stays behind
             free_fc_dev(m);
             return fail(BNM_E_CUDA, "weight decode of an FC layer failed: %s", cudaGetErrorString(e));
         }
@@ -610,10 +637,12 @@ static FcOutputs outputs_from(const FcOutputs &o, size_t b, uint32_t n_classes, 
                      {o.topk.k, o.topk.classes ? o.topk.classes + b * o.topk.k : nullptr, at(o.topk.scores, o.topk.k)}, o.engines};
 }
 
-// Route r (not the two engines' one) on n images on st, arguments checked -> out: logits (int32 [n][n_classes], float64 for the
-// emulator), labels and gather; or with topk.k > 0 the k best classes of every image and their scores.  A route of one pass and
-// one launch allocates nothing; every other one runs through scratch of this call's own, for one pass.
-static int run_route(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out, cudaStream_t st) {
+// Route r (not the two engines' one) on n images on st, whose capture state is cap, arguments checked -> out: logits (int32
+// [n][n_classes], float64 for the emulator), labels and gather; or with topk.k > 0 the k best classes of every image and their
+// scores.  A route of one pass and one launch allocates nothing; every other one runs through scratch of this call's own, for one
+// pass (in a capture: graph-owned allocations, freed inside the graph).
+static int run_route(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out, cudaStream_t st,
+                     const StreamCapture &cap) {
     const size_t pass = r.pass ? std::min(n, r.pass) : n, inner = r.inner ? std::min(pass, r.inner) : pass;
     const bool emul = r.engine == kEngineEmul;
     const uint32_t elems = m->img_bytes, C = m->channels, k = out.topk.k;
@@ -668,7 +697,7 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
             }
             const FcOutputs o = outputs_from(out, b + c, m->n_classes, emul, g);
             if (r.fused) {
-                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st)))
+                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap)))
                     return fail(BNM_E_CUDA, "fused launch of %s failed (%d): %s", fc_chain_form_name(m->plan, r.form), rc,
                                 cudaGetErrorString(cudaGetLastError()));
                 continue;
@@ -696,11 +725,15 @@ extern "C" int bnm_device_alloc(int device, size_t bytes, void **out) {
     if (!out) return fail(BNM_E_ARG, "bnm_device_alloc: null argument");
     *out = nullptr;
     if (int rc = require_device_index(device)) return rc;
+    RelaxedCaptureMode relaxed;
     CU_TRY(cudaSetDevice(device));
     CU_TRY(cudaMalloc(out, bytes ? bytes : 16));
     return 0;
 }
-extern "C" void bnm_device_free(void *p) { if (p) cudaFree(p); }
+extern "C" void bnm_device_free(void *p) {
+    RelaxedCaptureMode relaxed;
+    if (p) cudaFree(p);
+}
 extern "C" int bnm_ipc_export(const void *dev_ptr, void *handle64) {
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handles are 64 bytes");
     if (!dev_ptr || !handle64) return fail(BNM_E_ARG, "bnm_ipc_export: null argument");
@@ -773,7 +806,7 @@ static int small_launch(bnm_model *m, SmallGen &g) {
     const size_t n_log = g.logits ? n * (size_t)m->n_classes : 0;   // labels-only batches: the labels start the staging buffer
     uint32_t *d_lab = reinterpret_cast<uint32_t *>(d_out + n_log);
     const FcOutputs out{g.logits ? d_out : nullptr, g.labels ? d_lab : nullptr};
-    if (int rc = run_route(m, choose_route(m, kEngineC, false, false), d_in, n, out, st)) return rc;
+    if (int rc = run_route(m, choose_route(m, kEngineC, false, false), d_in, n, out, st, StreamCapture{})) return rc;
     if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(g.h_out.p, g.d_out.p, (n_log + (g.labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
     return 0;
@@ -796,8 +829,10 @@ template <class Ready> static void small_wait(std::unique_lock<std::mutex> &lk, 
 // caller (its leader) launches it for all of them as soon as the other generation's launch has completed, so calls that arrive
 // while a launch is in flight share the next one.  Then every caller copies its own rows out.  A caller alone on the model makes
 // one copy, one launch and one synchronisation, as a plain call would; there is no timer.  Only the leader calls CUDA: a caller
-// that joins a generation must never wait on the runtime while the launch in flight is being synchronised.
+// that joins a generation must never wait on the runtime while the launch in flight is being synchronised.  Like every host path
+// it runs on the model's own streams, which are never captured (StreamCapture{}), in relaxed capture mode.
 static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
+    RelaxedCaptureMode relaxed;
     SmallBatcher &B = m->small;
     std::unique_lock<std::mutex> lk(B.mu);
     if (int rc = small_buffers(m)) return rc;
@@ -851,6 +886,7 @@ static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *lo
 // the C engine's int8 route r on host buffers in chunks of chunk_images, each through one slot's buffers: images in, run_route,
 // out's arrays back.  Synchronous.
 static int infer_pipelined(bnm_model *m, const Route &r, const int8_t *images, size_t n, const FcOutputs &out) {
+    RelaxedCaptureMode relaxed;
     std::lock_guard<std::mutex> turn(m->host_mu);   // large host calls take turns: each one keeps the copy engines busy alone
     const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
     // per image, in 4-byte words: d_logits holds the logits or the top-k scores (bnm_infer_batch sizes it and d_labels whether or
@@ -878,7 +914,7 @@ static int infer_pipelined(bnm_model *m, const Route &r, const int8_t *images, s
         CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
         const FcOutputs d{out.logits ? s.d_logits.p : nullptr, out.labels ? s.d_labels.p : nullptr, nullptr,
                          {(uint32_t)k, s.d_classes.p, out.topk.scores ? s.d_logits.p : nullptr}};
-        if (int rc = run_route(m, r, s.d_images.p, nb, d, s.stream)) return rc;
+        if (int rc = run_route(m, r, s.d_images.p, nb, d, s.stream, StreamCapture{})) return rc;
         if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, s.d_classes.p, nb * k * 4, cudaMemcpyDeviceToHost, s.stream));
         if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * n_logits, s.d_logits.p, nb * n_logits * 4, cudaMemcpyDeviceToHost, s.stream));
         if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, s.d_labels.p, nb * 4, cudaMemcpyDeviceToHost, s.stream));
@@ -888,11 +924,15 @@ static int infer_pipelined(bnm_model *m, const Route &r, const int8_t *images, s
 }
 
 extern "C" void *bnm_host_alloc(size_t bytes) {
+    RelaxedCaptureMode relaxed;
     void *p = nullptr;
     if (cudaHostAlloc(&p, bytes ? bytes : 1, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); fail(BNM_E_CUDA, "cudaHostAlloc(%zu) failed", bytes); return nullptr; }
     return p;
 }
-extern "C" void bnm_host_free(void *p) { if (p) cudaFreeHost(p); }
+extern "C" void bnm_host_free(void *p) {
+    RelaxedCaptureMode relaxed;
+    if (p) cudaFreeHost(p);
+}
 
 // -----------------------------------------------------------------------------------------------
 // the four kernels, batched over host buffers
@@ -908,24 +948,42 @@ static int require_device_index(int device) {
     return 0;
 }
 
+// The stream of the entries without a model (the four kernels' batched forms, bnm_quantize_images) on the current device: one
+// non-blocking stream per device, created by the first such call and kept for the process.  Their copies and kernels run on it
+// and they wait for it alone, so they neither wait for nor hold up the legacy stream or a capture on another stream.
+static int host_stream(cudaStream_t *st) {
+    static std::mutex mu;
+    static std::vector<cudaStream_t> streams;
+    int dev = 0;
+    CU_TRY(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(mu);
+    if ((size_t)dev >= streams.size()) streams.resize(dev + 1, nullptr);
+    if (!streams[dev]) CU_TRY(cudaStreamCreateWithFlags(&streams[dev], cudaStreamNonBlocking));
+    *st = streams[dev];
+    return 0;
+}
+
 extern "C" int bnm_processfclayer_batch(const int8_t *activations, const uint32_t *weights, int32_t enc, uint32_t n_input,
                                         uint32_t n_output, int32_t *output, size_t n, int nf4_extension) {
+    RelaxedCaptureMode relaxed;   // outlives the buffers below: their frees run under it
     if (int rc = require_device()) return rc;
     if (n == 0 || n_output == 0) return 0;
     if (!activations || !weights || !output) return fail(BNM_E_ARG, "bnm_processfclayer_batch: null argument");
+    cudaStream_t st;
+    if (int rc = host_stream(&st)) return rc;
     const size_t need = packed_weight_bytes(enc, n_input, n_output);
     DevBuf<uint8_t> packed;
     if (packed.grow(need + 16)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemset(packed.p, 0, need + 16));
-    if (need) CU_TRY(cudaMemcpy(packed.p, weights, need, cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemsetAsync(packed.p, 0, need + 16, st));
+    if (need) CU_TRY(cudaMemcpyAsync(packed.p, weights, need, cudaMemcpyHostToDevice, st));
     FcLayerDev L;
-    if (cudaError_t e = decode_fc_layer(packed.p, enc, n_input, n_output, nf4_extension, L))
+    if (cudaError_t e = decode_fc_layer(packed.p, enc, n_input, n_output, nf4_extension, L, st))
         return fail(BNM_E_CUDA, "weight decode of an FC layer failed: %s", cudaGetErrorString(e));
     struct Planes { FcLayerDev &L; ~Planes() { free_fc_layer(L); } } planes{L};   // L's planes are freed on every return below
     DevBuf<int8_t> act;
     DevBuf<int32_t> out;
     if (act.grow(n * (size_t)L.k_pad) || out.grow(n * (size_t)n_output * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemset(act.p, 0, n * (size_t)L.k_pad));
+    CU_TRY(cudaMemsetAsync(act.p, 0, n * (size_t)L.k_pad, st));
     // Ternary layers declare n_input padded to a multiple of 10 with zero trits (exportquant.py:132-137,166) and the
     // reference never reads the activations under a zero trit (inference.c:128): a caller may hand in a 256-byte row for
     // n_input = 260.  Read exactly what the reference can read: up to the last non-zero trit of any row.
@@ -945,15 +1003,17 @@ extern "C" int bnm_processfclayer_batch(const int8_t *activations, const uint32_
                 }
             }
     }
-    if (valid_in) CU_TRY(cudaMemcpy2D(act.p, L.k_pad, activations, n_input, valid_in, n, cudaMemcpyHostToDevice));
-    if (!launch_fc_dp4a(act.p, L.k_pad, L, out.p, n, 0))
+    if (valid_in) CU_TRY(cudaMemcpy2DAsync(act.p, L.k_pad, activations, n_input, valid_in, n, cudaMemcpyHostToDevice, st));
+    if (!launch_fc_dp4a(act.p, L.k_pad, L, out.p, n, st))
         return fail(BNM_E_UNSUPPORTED, "processfclayer: n_input %u needs more shared memory than an SM has (layer kernel stages 128 rows)", n_input);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpy(output, out.p, n * (size_t)n_output * 4, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpyAsync(output, out.p, n * (size_t)n_output * 4, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
 extern "C" int bnm_relunorm_batch(const int32_t *input, int8_t *output, uint32_t *argmax, uint32_t n_input, size_t n) {
+    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0) return 0;
     if (n_input == 0) {   // inference.c:24-37: nothing is scanned, position stays 255
@@ -961,47 +1021,57 @@ extern "C" int bnm_relunorm_batch(const int32_t *input, int8_t *output, uint32_t
         return 0;
     }
     if (!input) return fail(BNM_E_ARG, "bnm_relunorm_batch: null input");
+    cudaStream_t st;
+    if (int rc = host_stream(&st)) return rc;
     DevBuf<int32_t> in;
     DevBuf<int8_t> out;
     DevBuf<uint32_t> am;
     if (in.grow(n * (size_t)n_input * 4) || out.grow(n * (size_t)n_input) || am.grow(n * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpy(in.p, input, n * (size_t)n_input * 4, cudaMemcpyHostToDevice));   // copied first: output may alias input
-    launch_relunorm(in.p, n_input, output ? out.p : nullptr, n_input, am.p, n, 0);
+    CU_TRY(cudaMemcpyAsync(in.p, input, n * (size_t)n_input * 4, cudaMemcpyHostToDevice, st));   // copied first: output may alias input
+    launch_relunorm(in.p, n_input, output ? out.p : nullptr, n_input, am.p, n, st);
     CU_TRY(cudaGetLastError());
-    if (argmax) CU_TRY(cudaMemcpy(argmax, am.p, n * 4, cudaMemcpyDeviceToHost));
-    else CU_TRY(cudaDeviceSynchronize());
-    if (output) CU_TRY(cudaMemcpy(output, out.p, n * (size_t)n_input, cudaMemcpyDeviceToHost));
+    if (argmax) CU_TRY(cudaMemcpyAsync(argmax, am.p, n * 4, cudaMemcpyDeviceToHost, st));
+    if (output) CU_TRY(cudaMemcpyAsync(output, out.p, n * (size_t)n_input, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
 extern "C" int bnm_conv33relu_batch(const int32_t *activations, const int8_t *weights, uint32_t n_w, uint32_t xy, uint32_t n_shift,
                                     int32_t *output, size_t n) {
+    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0 || xy < 3) return 0;
     if (!activations || !weights || !output || n_w == 0) return fail(BNM_E_ARG, "bnm_conv33relu_batch: null argument");
+    cudaStream_t st;
+    if (int rc = host_stream(&st)) return rc;
     const size_t in_el = n * (size_t)xy * xy, out_el = n * (size_t)(xy - 2) * (xy - 2);
     DevBuf<int32_t> in, out;
     DevBuf<int8_t> w;
     if (in.grow(in_el * 4) || w.grow((size_t)n_w * 9) || out.grow(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpy(in.p, activations, in_el * 4, cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemcpy(w.p, weights, (size_t)n_w * 9, cudaMemcpyHostToDevice));
-    launch_conv33relu(in.p, w.p, n_w, xy, n_shift, out.p, n, 0);
+    CU_TRY(cudaMemcpyAsync(in.p, activations, in_el * 4, cudaMemcpyHostToDevice, st));
+    CU_TRY(cudaMemcpyAsync(w.p, weights, (size_t)n_w * 9, cudaMemcpyHostToDevice, st));
+    launch_conv33relu(in.p, w.p, n_w, xy, n_shift, out.p, n, st);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpy(output, out.p, out_el * 4, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpyAsync(output, out.p, out_el * 4, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
 extern "C" int bnm_maxpool22_batch(const int32_t *activations, uint32_t xy, int32_t *output, size_t n) {
+    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0 || xy < 2) return 0;
     if (!activations || !output) return fail(BNM_E_ARG, "bnm_maxpool22_batch: null argument");
+    cudaStream_t st;
+    if (int rc = host_stream(&st)) return rc;
     const size_t in_el = n * (size_t)xy * xy, out_el = n * (size_t)(xy / 2) * (xy / 2);
     DevBuf<int32_t> in, out;
     if (in.grow(in_el * 4) || out.grow(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpy(in.p, activations, in_el * 4, cudaMemcpyHostToDevice));
-    launch_maxpool22(in.p, xy, out.p, n, 0);
+    CU_TRY(cudaMemcpyAsync(in.p, activations, in_el * 4, cudaMemcpyHostToDevice, st));
+    launch_maxpool22(in.p, xy, out.p, n, st);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpy(output, out.p, out_el * 4, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpyAsync(output, out.p, out_el * 4, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
@@ -1014,16 +1084,20 @@ extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_
 }
 
 extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out) {
+    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0 || elems == 0) return 0;
     if (!images || !out) return fail(BNM_E_ARG, "bnm_quantize_images: null argument");
+    cudaStream_t st;
+    if (int rc = host_stream(&st)) return rc;
     DevBuf<float> in;
     DevBuf<int8_t> q;
     if (in.grow(n * (size_t)elems * 4) || q.grow(n * (size_t)elems)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpy(in.p, images, n * (size_t)elems * 4, cudaMemcpyHostToDevice));
-    launch_quantize_images(in.p, elems, q.p, n, 0);
+    CU_TRY(cudaMemcpyAsync(in.p, images, n * (size_t)elems * 4, cudaMemcpyHostToDevice, st));
+    launch_quantize_images(in.p, elems, q.p, n, st);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpy(out, q.p, n * (size_t)elems, cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpyAsync(out, q.p, n * (size_t)elems, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
@@ -1043,6 +1117,7 @@ int bnm::level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == 
 
 // the emulator's route r on host buffers: per chunk of the layered emulator's pass, images in -> run_route -> logits out, synchronously
 static int emulate_host(bnm_model *m, const Route &r, const float *images, size_t n, double *logits) {
+    RelaxedCaptureMode relaxed;
     std::lock_guard<std::mutex> turn(m->host_mu);   // takes turns with the other large host calls, on the pipeline's first stream
     const size_t elems = m->img_bytes, ncls = m->n_classes;
     const size_t chunk = std::min(n, kEmulLayerPass[m->model_class == BNM_MODEL_CNNMNIST]);
@@ -1055,7 +1130,7 @@ static int emulate_host(bnm_model *m, const Route &r, const float *images, size_
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
         CU_TRY(cudaMemcpyAsync(d_in, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
-        if (int rc = run_route(m, r, d_in, nb, FcOutputs{d_out, nullptr}, st)) return rc;
+        if (int rc = run_route(m, r, d_in, nb, FcOutputs{d_out, nullptr}, st, StreamCapture{})) return rc;
         CU_TRY(cudaMemcpyAsync(logits + b * ncls, d_out, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
     }
@@ -1068,8 +1143,10 @@ static int emulate_host(bnm_model *m, const Route &r, const float *images, size_
 // other model runs the C engine's float route and the emulator's route per pass, into the caller's label buffers or the call's
 // scratch, then k_engine_counts (run_engines).
 // -----------------------------------------------------------------------------------------------
-// the two engines' route r without a fused form on n float images on st -> out: labels (the C engine's) and engines
-static int run_engines(bnm_model *m, const Route &r, const float *images, size_t n, const FcOutputs &out, cudaStream_t st) {
+// the two engines' route r without a fused form on n float images on st (capture state cap) -> out: labels (the C engine's) and
+// engines
+static int run_engines(bnm_model *m, const Route &r, const float *images, size_t n, const FcOutputs &out, cudaStream_t st,
+                       const StreamCapture &cap) {
     const EngineOutputs &e = out.engines;
     const Route c_route = choose_route(m, kEngineC, true, false), py_route = choose_route(m, kEngineEmul, true, false);
     const size_t chunk = std::min(n, r.pass), elems = m->img_bytes;
@@ -1083,9 +1160,9 @@ static int run_engines(bnm_model *m, const Route &r, const float *images, size_t
         uint32_t *lc = out.labels ? out.labels + b : own[0];
         uint32_t *lp = e.labels_py ? e.labels_py + b : own[1];
         if (lc)
-            if (int rc = run_route(m, c_route, img, nb, FcOutputs{nullptr, lc}, st)) return rc;
+            if (int rc = run_route(m, c_route, img, nb, FcOutputs{nullptr, lc}, st, cap)) return rc;
         if (lp)
-            if (int rc = run_route(m, py_route, img, nb, FcOutputs{nullptr, lp}, st)) return rc;
+            if (int rc = run_route(m, py_route, img, nb, FcOutputs{nullptr, lp}, st, cap)) return rc;
         if (e.counts) launch_engine_counts(lc, lp, e.truth ? e.truth + b : nullptr, nb, m->n_classes, e.counts, st);
     }
     return launch_status();
@@ -1131,8 +1208,9 @@ static int check_call(const bnm_model *m, const Call &c) {
     return 0;
 }
 
-// Check call c and run its route: on the device entry's stream; for the two engines without a fused form, run_engines; host calls
-// of up to kSmallBatch images (and chunk) through infer_small, the others through infer_pipelined or emulate_host.
+// Check call c and run its route: on the device entry's stream, whose capture state it reads once; for the two engines without a
+// fused form, run_engines; host calls of up to kSmallBatch images (and chunk) through infer_small, the others through
+// infer_pipelined or emulate_host.
 static int run_call(bnm_model *m, const Call &c) {
     if (int rc = check_call(m, c)) return rc;
     if (c.n == 0) return 0;
@@ -1147,8 +1225,9 @@ static int run_call(bnm_model *m, const Call &c) {
     cudaStream_t st = static_cast<cudaStream_t>(c.stream);
     if (c.host && c.engine == kEngineEmul) return emulate_host(m, r, static_cast<const float *>(c.images), c.n, static_cast<double *>(o.logits));
     if (c.host) return infer_pipelined(m, r, static_cast<const int8_t *>(c.images), c.n, o);
-    if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, static_cast<const float *>(c.images), c.n, o, st);
-    return run_route(m, r, c.images, c.n, o, st);
+    const StreamCapture cap = capture_of(st);
+    if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, static_cast<const float *>(c.images), c.n, o, st, cap);
+    return run_route(m, r, c.images, c.n, o, st, cap);
 }
 
 extern "C" int bnm_infer_batch_device_gather(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels,

@@ -149,10 +149,16 @@ struct FcChainPlan {
     TmapSlot tmaps[4];                // tensor maps of the most recent (pointer, n) pairs: double/triple-buffered callers hit every time
     unsigned tmap_next = 0;
     // mode 2 bookkeeping: the buffers of the previous launch on this plan (the promise "consecutive launches are independent" is
-    // checked as far as the library can see it: a launch that touches a buffer of the one before keeps the grid-dependency wait)
-    LaunchBuffers prev;
-    cudaStream_t prev_stream = nullptr;
-    bool prev_valid = false;
+    // checked as far as the library can see it: a launch that touches a buffer of the one before keeps the grid-dependency wait).
+    // Eager launches read and write `eager` alone; launches captured into a graph read and write `captured` alone, the record of
+    // the last captured launch and the capture sequence it belongs to.
+    struct LaunchRecord {
+        LaunchBuffers bufs;
+        cudaStream_t stream = nullptr;
+        unsigned long long capture_id = 0;   // 0 for eager launches
+        bool valid = false;
+    };
+    LaunchRecord eager, captured;
     bool verbose = false;             // BNM_VERBOSE at plan creation: every int8-form launch names its wait decision
     // guards the tensor-map cache and the bookkeeping above together with the launch they describe: launches from several host
     // threads enqueue in the order the bookkeeping records
@@ -1232,7 +1238,7 @@ void fc_chain_plan_set_overlap(FcChainPlan *p, int mode) {
     if (!p) return;
     std::lock_guard<std::mutex> lock(p->mu);
     p->overlap = mode;
-    p->prev_valid = false;
+    p->eager.valid = p->captured.valid = false;
 }
 
 void fc_chain_plan_destroy(FcChainPlan *p) {
@@ -1269,7 +1275,17 @@ const char *fc_chain_form_name(const FcChainPlan *plan, FcForm f) { return plan-
 
 static const CUtensorMap kNoTensorMap{};   // the float-input forms' tensor map: not used (no TMA image loads)
 
-int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st) {
+// Whether the driver captures a programmatic dependent launch into a graph as a programmatic edge (CUDA 12.3 and later): decided
+// once per process from the driver's version, never from a failed launch
+static bool programmatic_capture() {
+    static const bool ok = [] {
+        int v = 0;
+        return cudaDriverGetVersion(&v) == cudaSuccess && v >= 12030;
+    }();
+    return ok;
+}
+
+int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
     if (!plan->forms[f].kernel) return -6;
@@ -1343,6 +1359,10 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
     // broken: first launch on this plan / another stream / a buffer of the previous launch touched again, in any role (one
     // launch's logits the next one's images, say) / a launch of another form in between.  A null output is no buffer: it
     // neither reuses nor differs from one.
+    // A launch captured into a graph follows the same rules against the previous captured launch of its capture sequence: the
+    // first captured launch of a sequence keeps its wait, and the eager record is neither read nor written, so an eager launch
+    // compares itself with the eager launch before it whatever was captured in between.  Where the driver cannot capture a
+    // programmatic launch, a captured launch is a plain launch and keeps its (then immediate) wait.
     LaunchBuffers bufs;
     bufs.io[0] = in; bufs.io[1] = out.logits; bufs.io[2] = out.labels;
     if (out.gather) {
@@ -1350,19 +1370,23 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
         for (uint32_t d = 0; d < p.n_log_dst; d++) bufs.dst[bufs.n_dst++] = p.log_dst[d];
         bufs.row0 = p.row0;
     }
-    const bool independent = engine_i8 && plan->overlap == 2 && plan->prev_valid && plan->prev_stream == st && !shares_buffer(plan->prev, bufs);
+    const bool programmatic = engine_i8 && (!cap.active || programmatic_capture());
+    FcChainPlan::LaunchRecord &rec = cap.active ? plan->captured : plan->eager;
+    const bool independent = programmatic && plan->overlap == 2 && rec.valid && rec.capture_id == cap.id && rec.stream == st &&
+                             !shares_buffer(rec.bufs, bufs);
     p.wait_prior_grid = !independent;
     p.early_trigger = engine_i8 && cfg.gridDim.x == (unsigned)plan->sm_count;
-    plan->prev = bufs; plan->prev_stream = st; plan->prev_valid = engine_i8;
-    if (engine_i8 && plan->verbose) fprintf(stderr, "bitnetmcu_b200: fused launch: %s\n", independent ? "independent" : "wait");
+    rec.bufs = bufs; rec.stream = st; rec.capture_id = cap.id; rec.valid = engine_i8;
+    if (engine_i8 && plan->verbose)
+        fprintf(stderr, "bitnetmcu_b200: fused launch: %s%s\n", independent ? "independent" : "wait", cap.active ? " (captured)" : "");
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = engine_i8 ? 1 : 0;
-    trace_before(st);
+    cfg.numAttrs = programmatic ? 1 : 0;
+    if (!cap.active) trace_before(st);   // the trace hooks synchronise: never inside a capture
     if (cudaLaunchKernelEx(&cfg, form.kernel->fn, *tmap_p, p) != cudaSuccess) return -4;
-    trace_after(st);
+    if (!cap.active) trace_after(st);
     return cudaGetLastError() == cudaSuccess ? 0 : -4;
 }
 

@@ -152,9 +152,16 @@ struct FcOutputs {
     TopKOutputs topk;
     EngineOutputs engines;
 };
-// one launch of form f on n images `in` -> out.  0, or a negative code (-5: an output the form does not take, or a missing one;
-// -6: the plan has no form f)
-int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st);
+// The capture state of a call's stream, read once per call (cudaStreamGetCaptureInfo): active while the stream is capturing into
+// a graph, with the capture sequence's id (unique in the process).  A captured launch keeps its launch-overlap bookkeeping apart
+// from the eager launches'.
+struct StreamCapture {
+    bool active = false;
+    unsigned long long id = 0;
+};
+// one launch of form f on n images `in` -> out on st, whose capture state is cap.  0, or a negative code (-5: an output the form
+// does not take, or a missing one; -6: the plan has no form f)
+int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap);
 // the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
 // [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
 constexpr uint32_t kCnnEmulMaxChannels = 128;

@@ -98,7 +98,10 @@ class Engine:
 
         With ``OPT_LAUNCH_OVERLAP`` = 2 a launch whose buffers differ from the previous call's is NOT ordered against earlier
         work on the stream (include/bitnetmcu_b200.h): its images must already be complete when the previous call was
-        enqueued.  Chains such as ``quantize_images_device`` -> ``infer_device`` on one stream need mode 0 or 1."""
+        enqueued.  Chains such as ``quantize_images_device`` -> ``infer_device`` on one stream need mode 0 or 1.
+
+        Inside ``torch.cuda.graph`` the current stream is the capture stream, so the call is captured, and every replay gives what
+        the same call would give on the buffers' contents at replay time (INTEGRATION.md section 4)."""
         import torch
         self._device_call(self.lib.bnm_infer_batch_device, images, torch.int8,
                           [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)

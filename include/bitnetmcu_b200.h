@@ -32,6 +32,29 @@
  * the large host calls (bnm_infer_batch above 1024 images, bnm_infer_topk, bnm_emulate_inference_quantized) take turns.
  * The fused kernel's launch-overlap bookkeeping (BNM_OPT_LAUNCH_OVERLAP) counts launches in the order they are enqueued on the
  * model, from whichever thread.
+ *
+ * Graphs.  Every device entry (bnm_infer_batch_device, _gather, _f32, bnm_emulate_batch_device, bnm_compare_engines_device, the
+ * three top-k device entries and bnm_quantize_images_device) may be captured into a CUDA graph on its stream, in any capture mode,
+ * in any combination and from any thread.  Each replay gives exactly the results of the same call made eagerly on the buffers'
+ * contents at replay time; bnm_compare_engines_device adds to `counts` on every replay.  A graph keeps what its capture decided:
+ * the route, the routing options (BNM_OPT_PATH, BNM_OPT_CHUNK_IMAGES, BNM_OPT_CNN_FRONTEND, BNM_OPT_LAUNCH_OVERLAP) and the
+ * launch-overlap decisions.  Setting one of these four options after the capture changes later calls, not the graph.
+ * BNM_OPT_NF4_EXTENSION is different: changing it rebuilds the model's device weights (the decoded layers and the fused plan's
+ * weight image), which the graph's kernels read, so every graph of the model must be destroyed before it changes, as before
+ * bnm_model_destroy.  BNM_VERBOSE lines are printed at capture, not at replay.  An int8 launch's programmatic-dependent attribute
+ * becomes a programmatic edge in the graph (on drivers that capture it, CUDA 12.3 and later; elsewhere the captured launch is a
+ * plain launch that waits).  Mode 2 applies its rules inside a capture sequence: a captured launch is compared with the captured
+ * launch before it in the same sequence, the first one keeps its wait, and eager launches are compared with eager ones only.
+ * A graph replay is not a launch of that bookkeeping: an eager launch after a replay is compared with the eager launch before
+ * the replay, so a replay that writes the next eager call's images is, like any producer kernel, the caller's promise (mode 0
+ * or 1 for such chains).
+ * A call's scratch becomes graph-owned memory (graph allocation nodes): it is held from the graph's first launch until the
+ * graph is destroyed or cudaDeviceGraphMemTrim releases it, per graph -- 256 MB for a 2^20-image CNN pass.  Graphs must be
+ * destroyed before their model.  Host entries and the reference-named symbols work while another thread captures, in any
+ * mode, and leave that capture valid: their allocations and synchronisations run in relaxed capture mode on the library's own
+ * non-blocking streams.  bnm_model_create, bnm_model_load_blob, bnm_model_destroy and bnm_model_set_option with
+ * BNM_OPT_NF4_EXTENSION synchronise the device and must not overlap a capture; the other options only set fields of the model
+ * and take effect for the calls, eager or captured, made after them.
  */
 #ifndef BITNETMCU_B200_H
 #define BITNETMCU_B200_H
@@ -122,7 +145,8 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      offset (a slice of the previous call's logits as images, destination rows of two offsets that overlap) stay the
  *      caller's promise.  Producer -> inference chains on one stream (bnm_quantize_images_device then
  *      bnm_infer_batch_device) belong to mode 0 or 1.  With BNM_VERBOSE set at model creation every such launch prints
- *      "bitnetmcu_b200: fused launch: wait" or "... independent".
+ *      "bitnetmcu_b200: fused launch: wait" or "... independent", followed by " (captured)" for a launch captured into a
+ *      graph (see "Graphs" above).
  *      Only launches that fill the GPU (>= one 128-image tile per SM) trigger early, and every launch occupies its SM
  *      exclusively (more than half of the shared memory): at most two consecutive launches are ever in flight together.
  *      CNN models are held at mode 1 (the front-end kernel really feeds the FC kernel). */
