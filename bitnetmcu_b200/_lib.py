@@ -23,6 +23,7 @@ EXPORTED = [
     "bnm_enable_peer_access", "bnm_emulate_inference_quantized", "bnm_infer_batch_device_f32", "bnm_emulate_batch_device",
     "bnm_compare_engines_device",
     "bnm_infer_topk", "bnm_infer_topk_device", "bnm_infer_topk_device_f32", "bnm_emulate_topk_device",
+    "bnm_infer_windows_device_f32",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
@@ -88,6 +89,7 @@ def load() -> C.CDLL:
         "bnm_infer_topk_device": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
         "bnm_infer_topk_device_f32": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
         "bnm_emulate_topk_device": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
+        "bnm_infer_windows_device_f32": (C.c_int, [vp, vp, u32, u32, sz, u32, u32, vp, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

@@ -330,26 +330,28 @@ enum Engine { kEngineC, kEngineEmul, kEngineBoth };
 enum Front { kFrontNone, kFrontCnn, kFrontCnnEmul, kFrontCnnEmulLayers };
 
 // A route: which kernels one call runs, chosen once per call (choose_route), named (print_route) and run (run_route) from this
-// record alone.  Per pass of `pass` images (0: one pass), k_quantize_images into scratch when `scale`, then per `inner` images of
+// record alone.  Per pass of `pass` images (0: one pass), k_quantize_images into scratch when `scale` (k_quantize_windows on the
+// window scan's windows when `windows`), then per `inner` images of
 // that pass (0: all of it) the front-end, the FC stage and for a layered top-k k_topk_rows.  The FC stage is one launch of `form`,
 // or the layer-by-layer chain with the engine's rule.  The two engines' route runs each engine's own route per pass instead.
 struct Route {
     Engine engine;
     bool f32, topk;   // float32 images in; the k best classes out
-    bool scale;
+    bool scale, windows;
     Front front;
     bool fused;
     FcForm form;
     size_t pass, inner;
 };
 
-// the route of an entry of `engine` on float32 (f32) or int8 images, top-k or not, on this model with its options
-static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk) {
+// the route of an entry of `engine` on float32 (f32) or int8 images, top-k or not, on this model with its options; windows: the
+// float images are the windows of a plane (the C engine's window scan: the float route with k_quantize_windows as its scale step)
+static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk, bool windows = false) {
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05, cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    Route r{engine, f32, topk, false, kFrontNone, fused, kFormInt8, 0, 0};
-    // FC models whose plan has the engine's float-input form: one launch with the input scaling fused (no such top-k form)
+    Route r{engine, f32, topk, false, windows, kFrontNone, fused, kFormInt8, 0, 0};
+    // FC models whose plan has the engine's float-input form: one launch with the input scaling fused (no such top-k or window form)
     const FcForm float_form = engine == kEngineC ? kFormFloat : engine == kEngineEmul ? kFormEmulFloat : kFormEngines;
-    if (f32 && !topk && fused && !cnn && fc_chain_has_form(m->plan, float_form)) {
+    if (f32 && !topk && !windows && fused && !cnn && fc_chain_has_form(m->plan, float_form)) {
         r.form = float_form;
         return r;
     }
@@ -392,7 +394,7 @@ static void print_route(const bnm_model *m, const char *what, const Route &r) {
     } else if (r.engine == kEngineEmul && !r.fused) {
         s = r.topk ? "layer by layer + k_topk_rows<double>" : "layer by layer";
     } else {
-        if (r.scale) s = "k_quantize_images + ";
+        if (r.scale) s = r.windows ? "k_quantize_windows + " : "k_quantize_images + ";
         if (r.front == kFrontCnn)
             s += cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
         if (r.front == kFrontCnnEmul) s += "k_cnn_emul_frontend + ";
@@ -640,9 +642,10 @@ static FcOutputs outputs_from(const FcOutputs &o, size_t b, uint32_t n_classes, 
 // Route r (not the two engines' one) on n images on st, whose capture state is cap, arguments checked -> out: logits (int32
 // [n][n_classes], float64 for the emulator), labels and gather; or with topk.k > 0 the k best classes of every image and their
 // scores.  A route of one pass and one launch allocates nothing; every other one runs through scratch of this call's own, for one
-// pass (in a capture: graph-owned allocations, freed inside the graph).
+// pass (in a capture: graph-owned allocations, freed inside the graph).  A window route's images are the n windows of grid `win`
+// in window order; its scale step reads them from the plane.
 static int run_route(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out, cudaStream_t st,
-                     const StreamCapture &cap) {
+                     const StreamCapture &cap, const WindowGrid *win = nullptr) {
     const size_t pass = r.pass ? std::min(n, r.pass) : n, inner = r.inner ? std::min(pass, r.inner) : pass;
     const bool emul = r.engine == kEngineEmul;
     const uint32_t elems = m->img_bytes, C = m->channels, k = out.topk.k;
@@ -660,9 +663,14 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
     GatherDst g;
     for (size_t b = 0; b < n; b += pass) {
         const size_t nb = std::min(pass, n - b);
-        const char *in = static_cast<const char *>(images) + b * in_bytes;
+        const char *in = r.windows ? nullptr : static_cast<const char *>(images) + b * in_bytes;
         size_t row_bytes = in_bytes;
-        if (r.scale) {   // test_inference.py:140-141, BitNetMCU.py:435-436
+        if (r.windows) {   // windows b .. b + nb - 1 of the plane, scaled as below
+            if (!launch_quantize_windows(*win, b, nb, q, st))
+                return fail(BNM_E_CUDA, "k_quantize_windows: cannot opt in to its dynamic shared memory");
+            in = reinterpret_cast<const char *>(q);
+            row_bytes = elems;
+        } else if (r.scale) {   // test_inference.py:140-141, BitNetMCU.py:435-436
             launch_quantize_images(reinterpret_cast<const float *>(in), elems, q, nb, st);
             in = reinterpret_cast<const char *>(q);
             row_bytes = elems;
@@ -697,7 +705,7 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
             }
             const FcOutputs o = outputs_from(out, b + c, m->n_classes, emul, g);
             if (r.fused) {
-                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap)))
+                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap, r.windows)))
                     return fail(BNM_E_CUDA, "fused launch of %s failed (%d): %s", fc_chain_form_name(m->plan, r.form), rc,
                                 cudaGetErrorString(cudaGetLastError()));
                 continue;
@@ -1185,6 +1193,7 @@ struct Call {
     bool host = false;             // host buffers: a synchronous call through the small-batch path, the host pipeline or emulate_host
     bool need_logits = false;      // logits must be given when n > 0 (the emulator's host entry)
     bool no_output_at_0 = false;   // a call without outputs is an error even when n == 0 (the two engines' entry)
+    const WindowGrid *windows = nullptr;   // the window scan: the images are the n windows of this grid, `images` its plane
 };
 
 // The argument rules, in this order: a null model, or (n > 0) null images, classes or needed logits; no output at all; k out of
@@ -1218,8 +1227,8 @@ static int run_call(bnm_model *m, const Call &c) {
     if (c.host && c.engine == kEngineC && !c.topk && c.n <= kSmallBatch && c.n <= m->chunk_images)   // sets the device where it launches
         return infer_small(m, static_cast<const int8_t *>(c.images), c.n, static_cast<int32_t *>(o.logits), o.labels);
     CU_TRY(cudaSetDevice(m->device));
-    const Route r = choose_route(m, c.engine, c.f32, c.topk);
-    if (c.topk && m->verbose) print_route(m, (std::string("topk route: ") + c.name).c_str(), r);
+    const Route r = choose_route(m, c.engine, c.f32, c.topk, c.windows);
+    if ((c.topk || c.windows) && m->verbose) print_route(m, (std::string(c.topk ? "topk route: " : "windows route: ") + c.name).c_str(), r);
     if (o.gather && !r.fused)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     cudaStream_t st = static_cast<cudaStream_t>(c.stream);
@@ -1227,7 +1236,7 @@ static int run_call(bnm_model *m, const Call &c) {
     if (c.host) return infer_pipelined(m, r, static_cast<const int8_t *>(c.images), c.n, o);
     const StreamCapture cap = capture_of(st);
     if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, static_cast<const float *>(c.images), c.n, o, st, cap);
-    return run_route(m, r, c.images, c.n, o, st, cap);
+    return run_route(m, r, c.images, c.n, o, st, cap, c.windows);
 }
 
 extern "C" int bnm_infer_batch_device_gather(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels,
@@ -1284,6 +1293,25 @@ extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size
 
 extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, double *scores, void *stream) {
     return run_call(m, {"bnm_emulate_topk_device", kEngineEmul, true, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
+}
+
+// Window scan (section 9): every 16x16 window of a float plane on a stride grid, classified as bnm_infer_batch_device_f32 classifies
+// the extracted windows.  Per pass of 2^20 windows, k_quantize_windows scales them from the plane into the call's scratch, then the
+// int8 route runs on that pass; the fused FC launch after it keeps its wait and counts as a launch of another kind.
+extern "C" int bnm_infer_windows_device_f32(bnm_model *m, const float *image, uint32_t height, uint32_t width, size_t pitch,
+                                            uint32_t stride_y, uint32_t stride_x, int32_t *logits, uint32_t *labels, void *stream) {
+    static const char *name = "bnm_infer_windows_device_f32";
+    if (int rc = require_device()) return rc;
+    if (!stride_y || !stride_x) return fail(BNM_E_ARG, "%s: zero stride (%u, %u)", name, stride_y, stride_x);
+    if (pitch < width || pitch % 4)
+        return fail(BNM_E_ARG, "%s: pitch %zu must be >= width %u and a multiple of 4 elements (16-byte rows)", name, pitch, width);
+    if (m && m->img_bytes != 256)
+        return fail(BNM_E_UNSUPPORTED, "%s: windows are 16x16 images, the model takes %u-element images", name, m->img_bytes);
+    const uint32_t out_h = height < 16 ? 0 : (height - 16) / stride_y + 1, out_w = width < 16 ? 0 : (width - 16) / stride_x + 1;
+    const WindowGrid g{image, height, width, pitch, stride_y, stride_x, out_h, out_w};
+    Call c{name, kEngineC, true, false, image, (size_t)out_h * out_w, {logits, labels}, {16, 8}, stream};
+    c.windows = &g;
+    return run_call(m, c);
 }
 
 // host buffers: n <= kSmallBatch images share a launch with concurrent small calls, larger batches run the chunked pipeline

@@ -1285,7 +1285,8 @@ static bool programmatic_capture() {
     return ok;
 }
 
-int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap) {
+int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap,
+                    bool fed) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
     if (!plan->forms[f].kernel) return -6;
@@ -1363,6 +1364,8 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
     // first captured launch of a sequence keeps its wait, and the eager record is neither read nor written, so an eager launch
     // compares itself with the eager launch before it whatever was captured in between.  Where the driver cannot capture a
     // programmatic launch, a captured launch is a plain launch and keeps its (then immediate) wait.
+    // A fed launch (its images written by the call's own scaling kernel just before) keeps its wait and counts as a launch of
+    // another kind: it leaves the record empty.
     LaunchBuffers bufs;
     bufs.io[0] = in; bufs.io[1] = out.logits; bufs.io[2] = out.labels;
     if (out.gather) {
@@ -1372,11 +1375,11 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
     }
     const bool programmatic = engine_i8 && (!cap.active || programmatic_capture());
     FcChainPlan::LaunchRecord &rec = cap.active ? plan->captured : plan->eager;
-    const bool independent = programmatic && plan->overlap == 2 && rec.valid && rec.capture_id == cap.id && rec.stream == st &&
+    const bool independent = !fed && programmatic && plan->overlap == 2 && rec.valid && rec.capture_id == cap.id && rec.stream == st &&
                              !shares_buffer(rec.bufs, bufs);
     p.wait_prior_grid = !independent;
     p.early_trigger = engine_i8 && cfg.gridDim.x == (unsigned)plan->sm_count;
-    rec.bufs = bufs; rec.stream = st; rec.capture_id = cap.id; rec.valid = engine_i8;
+    rec.bufs = bufs; rec.stream = st; rec.capture_id = cap.id; rec.valid = engine_i8 && !fed;
     if (engine_i8 && plan->verbose)
         fprintf(stderr, "bitnetmcu_b200: fused launch: %s%s\n", independent ? "independent" : "wait", cap.active ? " (captured)" : "");
     cudaLaunchAttribute attr[1];

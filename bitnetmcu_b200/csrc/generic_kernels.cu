@@ -4,6 +4,7 @@
 //   * ReLUNorm           : warp-per-row, shuffle max/argmax reduction             (inference.c:23-72)
 //   * processconv33ReLU / processmaxpool22 batched                                (inference.c:238-277, 300-322)
 //   * fused CNN front-end: conv,conv,pool,conv,pool per channel + ReLUNorm        (BitNetMCU_MNIST_dll.c:64-80)
+//   * input scaling      : float rows, or the 16x16 windows of a float plane (shared band), to int8 rows (test_inference.py:140-141)
 // These are the layer-by-layer path (BNM_PATH_LAYERS) and the front half of every CNN model; the fused
 // wgmma FC chain lives in fc_wgmma.cu.
 #include <algorithm>
@@ -260,6 +261,102 @@ __global__ void __launch_bounds__(256) k_quantize_images(const float *__restrict
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st) {
     if (n == 0 || elems == 0) return;
     k_quantize_images<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(in, elems, out, n);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Window scan (bnm_infer_windows_device_f32): the 16x16 windows of one float32 plane, each scaled as k_quantize_images scales an
+// image, into int8 rows [n][256].  A CTA takes a run of up to kWinCta windows of one window row.  They share their 16 pixel rows,
+// and the columns they span (at most kWinBox) are loaded ONCE into shared memory as a band, row by row with coalesced loads:
+// each pixel of the band comes from L2 / HBM once per band, not once per window covering it.  From the band: every column's
+// max |x| over the 16 rows, then per window (one thread each) the max of its 16 columns -- a 16-wide sliding max -- the scale,
+// and its 256 pixels into a staging row padded to 272 bytes (16-byte stores of one quarter-warp then hit distinct banks).  The
+// CTA's rows are consecutive windows, so they leave as one contiguous run of coalesced 16-byte stores.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kWinCta = 128, kWinBox = 256, kWinStage = 272;
+constexpr size_t kWinSmem = 16 * kWinBox * 4 + kWinBox * 4 + kWinCta * kWinStage;   // band, column maxima, staging
+
+struct WindowRun {
+    const float *image;
+    size_t pitch;
+    uint32_t width, stride_y, stride_x, out_w;
+    uint32_t per_cta, chunks;   // windows per CTA (per_cta columns of the grid, one box); CTAs per window row
+    uint32_t box_w;             // band width in pixels
+    size_t run0;                // the pass's first run of windows: run g covers row g / chunks, columns (g % chunks) * per_cta ..
+    size_t w0, n;               // the pass: windows w0 .. w0 + n - 1
+    int8_t *out;                // [n][256]
+};
+
+__global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    float *band = reinterpret_cast<float *>(smem);        // [16][box_w]
+    float *colmax = band + 16 * kWinBox;                  // [box_w]
+    uint8_t *stage = reinterpret_cast<uint8_t *>(colmax + kWinBox);   // [per_cta][kWinStage]
+    const size_t g = a.run0 + blockIdx.x;   // CTAs cover the runs the pass touches, and no others
+    const uint32_t r = (uint32_t)(g / a.chunks), c0 = (uint32_t)(g % a.chunks) * a.per_cta;
+    const size_t first = (size_t)r * a.out_w + c0;   // the CTA's windows first .. first + per_cta - 1, clipped to the row and the pass
+    const size_t lo = max(first, a.w0), hi = min(first + min(a.per_cta, a.out_w - c0), a.w0 + a.n);
+    if (lo >= hi) return;
+    // the band: rows r * stride_y .. + 15, columns x0 .. x0 + box_w - 1 (zeros past the plane's width, never read by a window)
+    const uint32_t x0 = c0 * a.stride_x, cols = min(a.box_w, a.width - x0);
+    const float *src = a.image + (size_t)r * a.stride_y * a.pitch + x0;
+    for (uint32_t x = threadIdx.x; x < a.box_w; x += blockDim.x) {
+#pragma unroll
+        for (int y = 0; y < 16; y++) band[y * a.box_w + x] = x < cols ? __ldg(src + (size_t)y * a.pitch + x) : 0.0f;
+    }
+    __syncthreads();
+    for (uint32_t x = threadIdx.x; x < a.box_w; x += blockDim.x) {
+        float m = 0.0f;
+#pragma unroll
+        for (int y = 0; y < 16; y++) m = fmaxf(m, fabsf(band[y * a.box_w + x]));
+        colmax[x] = m;
+    }
+    __syncthreads();
+    const uint32_t j = threadIdx.x;   // this thread's window: first + j
+    if (first + j >= lo && first + j < hi) {
+        const uint32_t xj = j * a.stride_x;
+        float m = 0.0f;
+#pragma unroll
+        for (int k = 0; k < 16; k++) m = fmaxf(m, colmax[xj + k]);
+        const float scale = quant_scale(m);
+#pragma unroll 4
+        for (int y = 0; y < 16; y++) {
+            const float *px = band + y * a.box_w + xj;
+            uint32_t v[4];
+#pragma unroll
+            for (int q = 0; q < 4; q++)
+                v[q] = (uint32_t)(quant_pixel(px[4 * q], scale) & 0xff) | (uint32_t)(quant_pixel(px[4 * q + 1], scale) & 0xff) << 8 |
+                       (uint32_t)(quant_pixel(px[4 * q + 2], scale) & 0xff) << 16 | (uint32_t)(quant_pixel(px[4 * q + 3], scale) & 0xff) << 24;
+            *reinterpret_cast<uint4 *>(stage + j * kWinStage + 16 * y) = make_uint4(v[0], v[1], v[2], v[3]);
+        }
+    }
+    __syncthreads();
+    const uint32_t s0 = (uint32_t)(lo - first), chunks = (uint32_t)(hi - lo) * 16;   // 16-byte chunks of the CTA's rows
+    uint4 *dst = reinterpret_cast<uint4 *>(a.out + (lo - a.w0) * 256);
+    for (uint32_t e = threadIdx.x; e < chunks; e += blockDim.x)
+        dst[e] = *reinterpret_cast<const uint4 *>(stage + (s0 + e / 16) * kWinStage + (e % 16) * 16);
+}
+
+bool launch_quantize_windows(const WindowGrid &g, size_t w0, size_t n, int8_t *out, cudaStream_t st) {
+    if (n == 0) return true;
+    WindowRun a;
+    a.image = g.image;
+    a.pitch = g.pitch;
+    a.width = g.width;
+    a.stride_y = g.stride_y;
+    a.stride_x = g.stride_x;
+    a.out_w = g.out_w;
+    a.per_cta = std::min<uint32_t>({kWinCta, (kWinBox - 16) / g.stride_x + 1, g.out_w});
+    a.chunks = (g.out_w + a.per_cta - 1) / a.per_cta;
+    a.box_w = (a.per_cta - 1) * g.stride_x + 16;
+    auto run_of = [&](size_t w) { return w / g.out_w * a.chunks + w % g.out_w / a.per_cta; };
+    a.run0 = run_of(w0);
+    a.w0 = w0;
+    a.n = n;
+    a.out = out;
+    const size_t runs = run_of(w0 + n - 1) - a.run0 + 1;
+    if (!raise_smem_limit((const void *)k_quantize_windows, kWinSmem)) return false;
+    k_quantize_windows<<<(unsigned)runs, kWinCta, kWinSmem, st>>>(a);
+    return true;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -86,6 +86,18 @@ void launch_topk_rows(const double *rows, uint32_t n_cls, uint32_t k, uint32_t *
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 
+// The 16x16 windows of one float32 plane (bnm_infer_windows_device_f32): image [height][pitch] on the device (16-byte aligned,
+// pitch a multiple of 4), windows on an (stride_y, stride_x) grid of out_h x out_w without padding, numbered row-major.
+struct WindowGrid {
+    const float *image;
+    uint32_t height, width;
+    size_t pitch;
+    uint32_t stride_y, stride_x, out_h, out_w;
+};
+// windows w0 .. w0 + n - 1 of g, each flattened row-major and scaled as launch_quantize_images scales an image -> int8 [n][256]
+// (16-byte aligned).  false when the kernel cannot get its shared memory.
+bool launch_quantize_windows(const WindowGrid &g, size_t w0, size_t n, int8_t *out, cudaStream_t st);
+
 // ---- scoring both engines (bnm_compare_engines_device): counts = uint64 {images, correct_c, correct_py, mismatches}, the layout of
 // bnm_engine_counts.  A warp's counters: every lane of the warp calls add() with the row it holds (row = false: none); the flags
 // are counted by ballot, kept in registers across the warp's rows, and flush() adds them with one 64-bit atomic per non-zero
@@ -160,8 +172,11 @@ struct StreamCapture {
     unsigned long long id = 0;
 };
 // one launch of form f on n images `in` -> out on st, whose capture state is cap.  0, or a negative code (-5: an output the form
-// does not take, or a missing one; -6: the plan has no form f)
-int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap);
+// does not take, or a missing one; -6: the plan has no form f).  fed: `in` was written by a kernel of another kind that the same
+// call launched just before (the window scan's scaling kernel); the launch keeps its grid-dependency wait and, as a launch of
+// another kind, leaves the launch-overlap record empty, so the next int8 launch keeps its wait too.
+int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap,
+                    bool fed = false);
 // the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
 // [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
 constexpr uint32_t kCnnEmulMaxChannels = 128;

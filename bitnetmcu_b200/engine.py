@@ -28,6 +28,17 @@ def _ptr(a: Optional[np.ndarray]):
 N = "n"   # in the shape of a tensor argument of Engine._device_call: the number of images
 
 
+def window_grid(height: int, width: int, stride) -> Tuple[int, int]:
+    """(out_h, out_w) of the 16x16 windows of a height x width image on a stride grid without padding (include/bitnetmcu_b200.h
+    section 9); stride is an int or (stride_y, stride_x), each >= 1.  (0, 0)-sized when the image is under 16 pixels either way."""
+    sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
+    if sy < 1 or sx < 1:
+        raise ValueError(f"window_grid: strides must be >= 1, got {(sy, sx)}")
+    if height < 16 or width < 16:
+        return 0, 0
+    return (height - 16) // sy + 1, (width - 16) // sx + 1
+
+
 class Engine:
     """One packed model resident on one GPU."""
 
@@ -106,16 +117,18 @@ class Engine:
         self._device_call(self.lib.bnm_infer_batch_device, images, torch.int8,
                           [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)
 
-    def _device_call(self, fn, images, in_dtype, args, stream) -> None:
+    def _device_call(self, fn, images, in_dtype, args, stream, lead=None) -> None:
         """fn(handle, images, n, *args, stream) on this GPU, images a contiguous in_dtype [n, img_bytes] tensor.  A tensor argument
         is given as (tensor or None, its dtype or element size, its shape with N for n, or N alone for n elements of any shape):
         asserted contiguous and of that type and shape, it passes as its pointer, None as NULL.  Other arguments pass as they are.
-        stream: a cudaStream_t as int, None for torch's current stream."""
+        stream: a cudaStream_t as int, None for torch's current stream.  lead: instead of images and n, these arguments
+        (images is then a 2-D in_dtype tensor of any shape, N counts its elements)."""
         import torch
         if stream is None:
             stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.is_contiguous() and images.dtype == in_dtype and images.dim() == 2 and images.shape[1] == self.img_bytes
-        n = images.shape[0]
+        assert images.dtype == in_dtype and images.dim() == 2
+        assert lead is not None or (images.is_contiguous() and images.shape[1] == self.img_bytes)
+        n = images.shape[0] if lead is None else images.numel()
         vals = []
         for a in args:
             if isinstance(a, tuple):
@@ -125,7 +138,8 @@ class Engine:
                     assert t.numel() == n if shape is N else tuple(t.shape) == tuple(n if d is N else d for d in shape)
                 a = None if t is None else C.c_void_p(t.data_ptr())
             vals.append(a)
-        _lib.check(fn(self.handle, C.c_void_p(images.data_ptr()), n, *vals, C.c_void_p(stream)), fn.__name__)
+        head = [C.c_void_p(images.data_ptr()), n] if lead is None else list(lead)
+        _lib.check(fn(self.handle, *head, *vals, C.c_void_p(stream)), fn.__name__)
 
     def inference_quantized(self, input_data: np.ndarray) -> np.ndarray:
         """``QuantizedModel.inference_quantized`` (/root/reference/BitNetMCU.py:420-535) on the GPU: float32 images [n, img_bytes]
@@ -151,6 +165,22 @@ class Engine:
         import torch
         self._device_call(self.lib.bnm_infer_batch_device_f32, images, torch.float32,
                           [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)
+
+    def infer_windows_device(self, image, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
+        """Window scan (include/bitnetmcu_b200.h section 9): every 16x16 window of image, a torch.float32 [height, width] plane on
+        this GPU with unit column stride (its row stride is the pitch, a multiple of 4), on a stride grid (an int or (sy, sx)) ->
+        logits torch.int32 [out_h, out_w, n_classes] or None, labels [out_h, out_w] (4-byte elements) or None (not both None), where
+        (out_h, out_w) = window_grid(height, width, stride).  Window (r, c) covers image[r*sy : r*sy+16, c*sx : c*sx+16]; its
+        results are what ``infer_device_f32`` returns for that window flattened.  Asynchronous on ``stream`` (default: torch's
+        current stream)."""
+        import torch
+        assert image.dim() == 2 and image.stride(1) == 1
+        sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
+        h, w = image.shape
+        out_h, out_w = window_grid(h, w, (sy, sx))
+        lead = (C.c_void_p(image.data_ptr()), h, w, image.stride(0), sy, sx)
+        self._device_call(self.lib.bnm_infer_windows_device_f32, image, torch.float32,
+                          [(logits, torch.int32, (out_h, out_w, self.n_classes)), (labels, 4, (out_h, out_w))], stream, lead=lead)
 
     def compare_engines_device(self, images, truth=None, labels_c=None, labels_py=None, counts=None, stream: Optional[int] = None) -> None:
         """Both engines on the same float images in one call (test_inference.py:130-175): images torch.float32 [n, img_bytes] on

@@ -17,6 +17,7 @@
  * Section 4 exposes the four kernels batched, for parity tests and partial integration.
  * Sections 5 to 7 take float images: the C engine (5), the reference's Python emulator (6), and both at once, scored (7).
  * Section 8 returns each image's k best classes and their scores (top-k) from either engine.
+ * Section 9 classifies every 16x16 window of a larger float image on a stride grid (window scan).
  *
  * Pointers are plain host (or, where the name says _device, CUDA device) pointers; sizes are element
  * counts unless named *_bytes.  All-integer arithmetic: results are bit-exact with the reference.
@@ -34,8 +35,8 @@
  * model, from whichever thread.
  *
  * Graphs.  Every device entry (bnm_infer_batch_device, _gather, _f32, bnm_emulate_batch_device, bnm_compare_engines_device, the
- * three top-k device entries and bnm_quantize_images_device) may be captured into a CUDA graph on its stream, in any capture mode,
- * in any combination and from any thread.  Each replay gives exactly the results of the same call made eagerly on the buffers'
+ * three top-k device entries, bnm_infer_windows_device_f32 and bnm_quantize_images_device) may be captured into a CUDA graph on
+ * its stream, in any capture mode, in any combination and from any thread.  Each replay gives exactly the results of the same call made eagerly on the buffers'
  * contents at replay time; bnm_compare_engines_device adds to `counts` on every replay.  A graph keeps what its capture decided:
  * the route, the routing options (BNM_OPT_PATH, BNM_OPT_CHUNK_IMAGES, BNM_OPT_CNN_FRONTEND, BNM_OPT_LAUNCH_OVERLAP) and the
  * launch-overlap decisions.  Setting one of these four options after the capture changes later calls, not the graph.
@@ -137,7 +138,7 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      call k must therefore be complete before call k-1 was enqueued (resident inputs, or produced on another stream and
  *      joined by an event before call k-1).  The library keeps ordinary stream semantics (the wait) for every launch where it
  *      can see the promise broken: the first launch after the option is set, a launch on another stream than the one before,
- *      a launch right after a launch of another kind (float input, emulator, top-k, ...), and a launch that touches a buffer
+ *      a launch right after a launch of another kind (float input, emulator, top-k, window scan, ...), and a launch that touches a buffer
  *      of the one before.  That is: one of its images, logits, labels or gather destination pointers equals one of the
  *      previous launch's, whatever the roles (the logits of call k-1 passed as the images of call k count), except that a
  *      gather destination both write counts only at the same row_offset.  A NULL pointer is no buffer: two labels-only
@@ -331,6 +332,25 @@ BNM_API int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint32_
 BNM_API int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream);
 BNM_API int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream);
 BNM_API int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, double *scores, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 9. Window scan: the classifier run over a larger image, one 16x16 window at every position on a stride grid (a page scanned
+ *    for characters, say).  The windows are never materialised as float rows: each one is scaled as section 5 scales an image,
+ *    straight from the plane, and neighbouring windows share the pixel reads.
+ * ------------------------------------------------------------------------------------------- */
+/* image: one float32 plane of height x width pixels, device memory on the model's GPU, 16-byte aligned, rows `pitch` elements
+ * apart (pitch >= width, a multiple of 4).  The window grid is out_h = (height - 16) / stride_y + 1 by out_w = (width - 16) /
+ * stride_x + 1, without padding; window w = r * out_w + c covers rows r * stride_y .. + 15 and columns c * stride_x .. + 15,
+ * flattened row-major.  labels: uint32 [out_h * out_w], logits: int32 [out_h * out_w][n_classes] (8-byte aligned); either may be
+ * NULL, not both.  Results are bit for bit those of bnm_infer_batch_device_f32 on the extracted windows in that order.
+ * BNM_E_ARG: a zero stride, pitch < width, pitch not a multiple of 4, a misaligned image or logits buffer, no output.
+ * BNM_E_UNSUPPORTED: a model whose images are not 256 elements.  height or width < 16: no windows, returns 0 and writes nothing.
+ * Per pass of 2^20 windows a scaling kernel loads each run of windows' 16-row band once and writes their int8 rows into the
+ * call's scratch (256 B per window), then the int8 route of bnm_infer_batch_device runs on that pass.  For BNM_OPT_LAUNCH_OVERLAP mode 2 a window call is a launch
+ * of another kind: its own fused launch and the next int8 launch keep their wait.  Asynchronous on `stream`, no host
+ * synchronisation. */
+BNM_API int bnm_infer_windows_device_f32(bnm_model *m, const float *image, uint32_t height, uint32_t width, size_t pitch,
+                                         uint32_t stride_y, uint32_t stride_x, int32_t *logits, uint32_t *labels, void *stream);
 
 #ifdef __cplusplus
 }
