@@ -112,20 +112,19 @@ struct FcLayerHost {
     size_t packed_bytes;
 };
 
+// one stream of the host pipeline (infer_pipelined) and its chunk's device copies, in bytes: images, logits or top-k scores,
+// labels, top-k classes
 struct PipeSlot {
     cudaStream_t stream = nullptr;
-    DevBuf<int8_t> d_images;
-    DevBuf<int32_t> d_logits;
-    DevBuf<uint32_t> d_labels;
-    DevBuf<uint32_t> d_classes;   // bnm_infer_topk: the chunk's classes (its scores go to d_logits)
+    DevBuf<char> d_images, d_logits, d_labels, d_classes;
 };
 
 // One staging generation of the small-batch path (infer_small): the rows of every call that joined it, in arrival order.
 struct SmallGen {
     PinnedBuf<int8_t> h_in;     // [kSmallBatch][img_bytes]
-    PinnedBuf<int32_t> h_out;   // logits [rows][n_classes] when a member asks for them, then labels [rows]
-    DevBuf<int8_t> d_in;        // their device counterparts
-    DevBuf<int32_t> d_out;
+    PinnedBuf<int32_t> h_out;   // logits [rows][n_classes] when a member asks for them, then labels [rows]: the kernels write
+                                // them straight into this mapped memory
+    DevBuf<int8_t> d_in;        // the device copy of h_in
     enum State { kOpen, kLaunched, kDone };
     // written under the batcher's lock; atomic so that a waiting caller may poll them without it (small_wait)
     std::atomic<int> state{kOpen};
@@ -171,7 +170,7 @@ struct bnm_model {
     FcChainPlan *plan = nullptr;
     std::string plan_err;
     uint32_t max_kpad = 0, max_nout = 0;   // the layer-by-layer path's scratch per image (LayerScratch)
-    // every call's device scratch comes from this pool, stream-ordered on the call's stream (Scratch)
+    // the decoded FC planes and every call's device scratch come from this pool, stream-ordered (Scratch: on the call's stream)
     cudaMemPool_t pool = nullptr;
     // host pipeline: the large host calls take turns on host_mu
     std::mutex host_mu;
@@ -180,8 +179,6 @@ struct bnm_model {
     // test_inference.py:146-150): pinned staging buffers, one stream, one synchronisation per shared launch
     SmallBatcher small;
     bool verbose = false;           // BNM_VERBOSE at model creation: the top-k entries name their route on every call
-    int small_zero_copy = 1;   // 0: H2D + D2H copies; 1 (default): the kernel writes results
-                               // straight into mapped pinned host memory; 2: ... and reads the images from it (TMA over PCIe)
 };
 static const size_t kSmallBatch = 1024;
 
@@ -198,51 +195,52 @@ static size_t packed_weight_bytes(int32_t enc, uint32_t n_in, uint32_t n_out) {
     }
 }
 
-static void free_fc_layer(FcLayerDev &L) {
-    cudaFree(L.dense_a);
-    cudaFree(L.dense_b);
-    cudaFree(L.quad_a);
-    cudaFree(L.quad_b);
+// an FC layer's decoded planes handed back to their pool on st, once the work enqueued on st before has used them
+static void free_fc_layer(FcLayerDev &L, cudaStream_t st) {
+    for (void *p : {(void *)L.dense_a, (void *)L.dense_b, (void *)L.quad_a, (void *)L.quad_b})
+        if (p) cudaFreeAsync(p, st);
     L.dense_a = L.dense_b = nullptr;
     L.quad_a = L.quad_b = nullptr;
 }
 
 // one FC layer's packed weights (device, zero padded past the end) decoded into its int8 planes, the residual ones only where they
-// are needed, decoded on st and synchronised with it.  On failure nothing stays allocated.
+// are needed: stream-ordered allocations from `pool`, decoded on st and synchronised with it.  On failure nothing stays allocated.
 static cudaError_t decode_fc_layer(const void *d_packed, int32_t enc, uint32_t n_in, uint32_t n_out, int nf4_ext, FcLayerDev &L,
-                                   cudaStream_t st) {
+                                   cudaMemPool_t pool, cudaStream_t st) {
     L.enc = enc;
     L.n_in = n_in;
     L.n_out = n_out;
     L.k_pad = round_up(std::max(n_in, 1u), 32);
     L.n_pad = round_up(n_out, 16);
     const size_t plane = (size_t)L.k_pad * L.n_pad;
-    DevBuf<int> d_flag;
+    int *d_flag = nullptr;
     int flag = 0;
-    cudaError_t e = cudaMalloc(&L.dense_a, plane);
-    if (e == cudaSuccess) e = cudaMalloc(&L.dense_b, plane);
-    if (e == cudaSuccess) e = cudaMalloc(&L.quad_a, plane);
-    if (e == cudaSuccess) e = cudaMalloc(&L.quad_b, plane);
-    if (e == cudaSuccess) e = d_flag.grow(sizeof(int));
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_flag.p, 0, sizeof(int), st);
+    cudaError_t e = cudaMallocFromPoolAsync(&L.dense_a, plane, pool, st);
+    if (e == cudaSuccess) e = cudaMallocFromPoolAsync(&L.dense_b, plane, pool, st);
+    if (e == cudaSuccess) e = cudaMallocFromPoolAsync(&L.quad_a, plane, pool, st);
+    if (e == cudaSuccess) e = cudaMallocFromPoolAsync(&L.quad_b, plane, pool, st);
+    if (e == cudaSuccess) e = cudaMallocFromPoolAsync(&d_flag, sizeof(int), pool, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_flag, 0, sizeof(int), st);
     if (e == cudaSuccess) {
-        launch_decode_fc(d_packed, enc, n_in, n_out, L.k_pad, L.n_pad, L.dense_a, L.dense_b, L.quad_a, L.quad_b, nf4_ext, d_flag.p, st);
-        e = cudaMemcpyAsync(&flag, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st);
+        launch_decode_fc(d_packed, enc, n_in, n_out, L.k_pad, L.n_pad, L.dense_a, L.dense_b, L.quad_a, L.quad_b, nf4_ext, d_flag, st);
+        e = cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st);
     }
+    if (d_flag) cudaFreeAsync(d_flag, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) {
-        free_fc_layer(L);
+        free_fc_layer(L, st);
     } else if (!flag) {   // no residual plane needed (everything but FP130 layers that contain +128)
-        cudaFree(L.dense_b);
-        cudaFree(L.quad_b);
+        cudaFreeAsync(L.dense_b, st);
+        cudaFreeAsync(L.quad_b, st);
         L.dense_b = nullptr;
         L.quad_b = nullptr;
     }
     return e;
 }
 
+// the model's decoded layers (on the legacy stream: every caller has synchronised the device) and fused plan
 static void free_fc_dev(bnm_model *m) {
-    for (auto &L : m->fc) free_fc_layer(L);
+    for (auto &L : m->fc) free_fc_layer(L, 0);
     m->fc.clear();
     if (m->plan) fc_chain_plan_destroy(m->plan);
     m->plan = nullptr;
@@ -260,7 +258,7 @@ static int build_fc_dev(bnm_model *m) {
     m->max_nout = 0;
     for (auto &H : m->fc_host) {
         FcLayerDev L;
-        if (cudaError_t e = decode_fc_layer(H.d_packed, H.enc, H.n_in, H.n_out, m->nf4_ext, L, 0)) {   // nothing half-built stays behind
+        if (cudaError_t e = decode_fc_layer(H.d_packed, H.enc, H.n_in, H.n_out, m->nf4_ext, L, m->pool, 0)) {   // nothing half-built stays behind
             free_fc_dev(m);
             return fail(BNM_E_CUDA, "weight decode of an FC layer failed: %s", cudaGetErrorString(e));
         }
@@ -278,15 +276,16 @@ static int build_fc_dev(bnm_model *m) {
     return 0;
 }
 
-// One call's device scratch: stream-ordered allocations from the model's pool on the call's stream, handed back on that stream
-// once the call has enqueued the work that uses them (the destructor).  Two calls in flight never share a byte of it, whatever
-// their threads and streams, and no call waits on the host for another.  The pool keeps what it has (its release threshold
-// is unbounded), so in steady state an allocation neither reaches the driver nor synchronises.
+// One call's device scratch: stream-ordered allocations from a pool (a model's, or the device's default one for the entries
+// without a model) on the call's stream, handed back on that stream once the call has enqueued the work that uses them (the
+// destructor).  Two calls in flight never share a byte of it, whatever their threads and streams, and no call waits on the host
+// for another.  A model's pool keeps what it has (its release threshold is unbounded), so in steady state an allocation neither
+// reaches the driver nor synchronises.
 struct Scratch {
     cudaMemPool_t pool;
     cudaStream_t st;
     std::vector<void *> held;
-    Scratch(const bnm_model *m, cudaStream_t s) : pool(m->pool), st(s) {}
+    Scratch(cudaMemPool_t p, cudaStream_t s) : pool(p), st(s) {}
     Scratch(const Scratch &) = delete;
     Scratch &operator=(const Scratch &) = delete;
     ~Scratch() { for (void *p : held) cudaFreeAsync(p, st); }
@@ -475,8 +474,6 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         }
     }
     if (rc == 0 && model_class == BNM_MODEL_FCMNIST && !front.empty()) rc = fail(BNM_E_ARG, "MODEL_FCMNIST with conv/pool layers");
-    if (rc == 0) rc = build_fc_dev(m);
-    if (rc == 0 && m->d_err.grow(sizeof(int), true) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaMalloc failed");
     if (rc == 0) {
         cudaMemPoolProps props = {};
         props.allocType = cudaMemAllocationTypePinned;
@@ -486,8 +483,9 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         if (cudaMemPoolCreate(&m->pool, &props) != cudaSuccess || cudaMemPoolSetAttribute(m->pool, cudaMemPoolAttrReleaseThreshold, &keep) != cudaSuccess)
             rc = fail(BNM_E_CUDA, "scratch memory pool: %s", cudaGetErrorString(cudaGetLastError()));
     }
+    if (rc == 0) rc = build_fc_dev(m);
+    if (rc == 0 && m->d_err.grow(sizeof(int), true) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaMalloc failed");
     if (rc == 0) {
-        if (const char *e = getenv("BNM_SMALL_ZC")) m->small_zero_copy = std::max(0, std::min(2, atoi(e)));   // development knob, read once per model
         for (auto &s : m->slots)
             if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(BNM_E_CUDA, "cudaStreamCreate failed"); break; }
         if (rc == 0 && cudaStreamCreateWithFlags(&m->small.stream, cudaStreamNonBlocking) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaStreamCreate failed");
@@ -533,7 +531,9 @@ extern "C" void bnm_model_destroy(bnm_model *m) {
     for (auto &s : m->slots)
         if (s.stream) cudaStreamDestroy(s.stream);
     if (m->small.stream) cudaStreamDestroy(m->small.stream);
-    if (m->pool) cudaMemPoolDestroy(m->pool);   // every call's scratch went back to it before the synchronisation above
+    // every call's scratch went back to it before the synchronisation above; the driver releases the pool once the planes'
+    // frees enqueued by free_fc_dev have run
+    if (m->pool) cudaMemPoolDestroy(m->pool);
     delete m;   // and with it the buffers it owns as members
 }
 
@@ -650,7 +650,7 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
     const bool emul = r.engine == kEngineEmul;
     const uint32_t elems = m->img_bytes, C = m->channels, k = out.topk.k;
     const size_t in_bytes = r.f32 ? elems * sizeof(float) : elems;   // per input image
-    Scratch s(m, st);
+    Scratch s(m->pool, st);
     int8_t *q, *feat;     // a pass's scaled images; an inner pass's CNN features for the fused FC stage
     LayerScratch ls;      // the layer-by-layer chain's accumulators and activations
     double *lg;           // the layered emulator's top-k: its float64 logits
@@ -786,7 +786,7 @@ extern "C" int bnm_enable_peer_access(int device, int peer) {
 // Both generations' staging buffers, allocated by the first small call (under the batcher's lock): all of them or none.
 static int small_buffers(bnm_model *m) {
     SmallGen *g = m->small.gen;
-    if (g[1].d_out.p) return 0;
+    if (g[1].d_in.p) return 0;
     CU_TRY(cudaSetDevice(m->device));
     const size_t in_bytes = kSmallBatch * (size_t)m->img_bytes, out_bytes = kSmallBatch * ((size_t)m->n_classes + 1) * 4;
     cudaError_t e = cudaSuccess;
@@ -794,28 +794,25 @@ static int small_buffers(bnm_model *m) {
         e = g[i].h_in.grow(in_bytes);
         if (e == cudaSuccess) e = g[i].h_out.grow(out_bytes);
         if (e == cudaSuccess) e = g[i].d_in.grow(in_bytes);
-        if (e == cudaSuccess) e = g[i].d_out.grow(out_bytes);
     }
     if (e == cudaSuccess) return 0;
-    for (int i = 0; i < 2; i++) { g[i].h_in.release(); g[i].h_out.release(); g[i].d_in.release(); g[i].d_out.release(); }
+    for (int i = 0; i < 2; i++) { g[i].h_in.release(); g[i].h_out.release(); g[i].d_in.release(); }
     return fail(-100 - (int)e, "small-batch staging buffers: %s", cudaGetErrorString(e));
 }
 
-// One generation's rows through the GPU: one copy in, one launch, one copy out (or zero-copy), one synchronisation.
+// One generation's rows through the GPU: one copy in, one launch that writes the results into the mapped h_out, one
+// synchronisation.
 static int small_launch(bnm_model *m, SmallGen &g) {
     CU_TRY(cudaSetDevice(m->device));
     cudaStream_t st = m->small.stream;
     const size_t n = g.rows;
-    const int8_t *d_in = g.d_in.p;
-    int32_t *d_out = g.d_out.p;
-    if (m->small_zero_copy >= 2) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(const_cast<int8_t **>(&d_in)), g.h_in.p, 0));
-    else CU_TRY(cudaMemcpyAsync(g.d_in.p, g.h_in.p, n * (size_t)m->img_bytes, cudaMemcpyHostToDevice, st));
-    if (m->small_zero_copy >= 1) CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), g.h_out.p, 0));
+    int32_t *d_out;
+    CU_TRY(cudaMemcpyAsync(g.d_in.p, g.h_in.p, n * (size_t)m->img_bytes, cudaMemcpyHostToDevice, st));
+    CU_TRY(cudaHostGetDevicePointer(reinterpret_cast<void **>(&d_out), g.h_out.p, 0));
     const size_t n_log = g.logits ? n * (size_t)m->n_classes : 0;   // labels-only batches: the labels start the staging buffer
     uint32_t *d_lab = reinterpret_cast<uint32_t *>(d_out + n_log);
     const FcOutputs out{g.logits ? d_out : nullptr, g.labels ? d_lab : nullptr};
-    if (int rc = run_route(m, choose_route(m, kEngineC, false, false), d_in, n, out, st, StreamCapture{})) return rc;
-    if (m->small_zero_copy == 0) CU_TRY(cudaMemcpyAsync(g.h_out.p, g.d_out.p, (n_log + (g.labels ? n : 0)) * 4, cudaMemcpyDeviceToHost, st));
+    if (int rc = run_route(m, choose_route(m, kEngineC, false, false), g.d_in.p, n, out, st, StreamCapture{})) return rc;
     CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
@@ -891,41 +888,43 @@ static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *lo
     return rc;
 }
 
-// the C engine's int8 route r on host buffers in chunks of chunk_images, each through one slot's buffers: images in, run_route,
-// out's arrays back.  Synchronous.
-static int infer_pipelined(bnm_model *m, const Route &r, const int8_t *images, size_t n, const FcOutputs &out) {
+// Route r (not the two engines' one) on host buffers in chunks of chunk_images, each through one slot's buffers: images in,
+// run_route, out's arrays back.  Synchronous.
+static int infer_pipelined(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out) {
     RelaxedCaptureMode relaxed;
     std::lock_guard<std::mutex> turn(m->host_mu);   // large host calls take turns: each one keeps the copy engines busy alone
     const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
-    // per image, in 4-byte words: d_logits holds the logits or the top-k scores (bnm_infer_batch sizes it and d_labels whether or
-    // not it takes them), d_classes the top-k classes
-    const size_t n_logits = k ? (out.topk.scores ? k : 0) : m->n_classes, n_labels = k ? 0 : 1;
+    // per image, in bytes: the images (float32 or int8), d_logits the logits or the top-k scores (float64 for the emulator, else
+    // int32; bnm_infer_batch sizes it and d_labels whether or not it takes them), d_labels the label, d_classes the top-k classes
+    const size_t in_bytes = r.f32 ? 4 * m->img_bytes : m->img_bytes, el = r.engine == kEngineEmul ? 8 : 4;
+    const size_t logit_bytes = (k ? (out.topk.scores ? k : 0) : m->n_classes) * el, label_bytes = k ? 0 : 4, class_bytes = k * 4;
     bool small = false;
     for (auto &s : m->slots)
-        small = small || s.d_images.bytes < chunk * m->img_bytes || s.d_classes.bytes < chunk * k * 4 ||
-                s.d_logits.bytes < chunk * n_logits * 4 || s.d_labels.bytes < chunk * n_labels * 4;
+        small = small || s.d_images.bytes < chunk * in_bytes || s.d_classes.bytes < chunk * class_bytes ||
+                s.d_logits.bytes < chunk * logit_bytes || s.d_labels.bytes < chunk * label_bytes;
     if (small) {
         for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));   // no chunk of an earlier call may still use a buffer that is reallocated
         for (auto &s : m->slots) {
-            CU_TRY(s.d_images.grow(chunk * (size_t)m->img_bytes));
-            CU_TRY(s.d_classes.grow(chunk * k * 4));
-            CU_TRY(s.d_logits.grow(chunk * n_logits * 4));
-            CU_TRY(s.d_labels.grow(chunk * n_labels * 4));
+            CU_TRY(s.d_images.grow(chunk * in_bytes));
+            CU_TRY(s.d_classes.grow(chunk * class_bytes));
+            CU_TRY(s.d_logits.grow(chunk * logit_bytes));
+            CU_TRY(s.d_labels.grow(chunk * label_bytes));
         }
     }
     // every chunk's scratch is its own (run_route): the chunks of every path overlap in time on all three streams
-    int32_t *h_logits = static_cast<int32_t *>(k ? out.topk.scores : out.logits);   // where d_logits goes
+    char *h_logits = static_cast<char *>(k ? out.topk.scores : out.logits);   // where d_logits goes
     size_t c = 0;
     for (size_t b = 0; b < n; b += chunk, c++) {
         const size_t nb = std::min(chunk, n - b);
         PipeSlot &s = m->slots[c % 3];
-        CU_TRY(cudaMemcpyAsync(s.d_images.p, images + b * m->img_bytes, nb * (size_t)m->img_bytes, cudaMemcpyHostToDevice, s.stream));
-        const FcOutputs d{out.logits ? s.d_logits.p : nullptr, out.labels ? s.d_labels.p : nullptr, nullptr,
-                         {(uint32_t)k, s.d_classes.p, out.topk.scores ? s.d_logits.p : nullptr}};
+        CU_TRY(cudaMemcpyAsync(s.d_images.p, static_cast<const char *>(images) + b * in_bytes, nb * in_bytes, cudaMemcpyHostToDevice, s.stream));
+        uint32_t *d_labels = reinterpret_cast<uint32_t *>(s.d_labels.p), *d_classes = reinterpret_cast<uint32_t *>(s.d_classes.p);
+        const FcOutputs d{out.logits ? s.d_logits.p : nullptr, out.labels ? d_labels : nullptr, nullptr,
+                         {(uint32_t)k, d_classes, out.topk.scores ? s.d_logits.p : nullptr}};
         if (int rc = run_route(m, r, s.d_images.p, nb, d, s.stream, StreamCapture{})) return rc;
-        if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, s.d_classes.p, nb * k * 4, cudaMemcpyDeviceToHost, s.stream));
-        if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * n_logits, s.d_logits.p, nb * n_logits * 4, cudaMemcpyDeviceToHost, s.stream));
-        if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, s.d_labels.p, nb * 4, cudaMemcpyDeviceToHost, s.stream));
+        if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, d_classes, nb * class_bytes, cudaMemcpyDeviceToHost, s.stream));
+        if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * logit_bytes, s.d_logits.p, nb * logit_bytes, cudaMemcpyDeviceToHost, s.stream));
+        if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, d_labels, nb * 4, cudaMemcpyDeviceToHost, s.stream));
     }
     for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
     return 0;
@@ -971,27 +970,48 @@ static int host_stream(cudaStream_t *st) {
     return 0;
 }
 
+// The device side of a host call without a model: Scratch from the device's default memory pool on its host stream, each buffer
+// copied from host memory (in) or, once the entry's kernels have run, to it (out).
+struct HostStaging : Scratch {
+    struct Copy { void *host; const void *dev; size_t bytes; };
+    std::vector<Copy> outs;
+    using Scratch::Scratch;
+    template <class T> cudaError_t in(T **d, const T *h, size_t count) {   // count elements of h
+        cudaError_t e = get(d, count);
+        return e != cudaSuccess || !count ? e : cudaMemcpyAsync(*d, h, count * sizeof(T), cudaMemcpyHostToDevice, st);
+    }
+    template <class T> cudaError_t out(T **d, T *h, size_t count) {   // count elements for h; null h: a buffer nothing copies out
+        cudaError_t e = get(d, count);
+        if (e == cudaSuccess && h && count) outs.push_back({h, *d, count * sizeof(T)});
+        return e;
+    }
+};
+
+// A host call without a model, its arguments checked, on the current device in relaxed capture mode: body(s) stages its inputs
+// in s and enqueues its kernels on s.st (the device's host stream); then the launch status, the copies out and one
+// synchronisation of that stream.  Every temporary is stream-ordered, so the call waits for its own stream and never for the
+// device.
+template <class Body> static int host_call(Body body) {
+    RelaxedCaptureMode relaxed;   // outlives the staging: its frees run under it
+    int dev = 0;
+    cudaStream_t st;
+    cudaMemPool_t pool;
+    CU_TRY(cudaGetDevice(&dev));
+    CU_TRY(cudaDeviceGetDefaultMemPool(&pool, dev));
+    if (int rc = host_stream(&st)) return rc;
+    HostStaging s(pool, st);
+    if (int rc = body(s)) return rc;
+    CU_TRY(cudaGetLastError());
+    for (const auto &c : s.outs) CU_TRY(cudaMemcpyAsync(c.host, c.dev, c.bytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
 extern "C" int bnm_processfclayer_batch(const int8_t *activations, const uint32_t *weights, int32_t enc, uint32_t n_input,
                                         uint32_t n_output, int32_t *output, size_t n, int nf4_extension) {
-    RelaxedCaptureMode relaxed;   // outlives the buffers below: their frees run under it
     if (int rc = require_device()) return rc;
     if (n == 0 || n_output == 0) return 0;
     if (!activations || !weights || !output) return fail(BNM_E_ARG, "bnm_processfclayer_batch: null argument");
-    cudaStream_t st;
-    if (int rc = host_stream(&st)) return rc;
-    const size_t need = packed_weight_bytes(enc, n_input, n_output);
-    DevBuf<uint8_t> packed;
-    if (packed.grow(need + 16)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemsetAsync(packed.p, 0, need + 16, st));
-    if (need) CU_TRY(cudaMemcpyAsync(packed.p, weights, need, cudaMemcpyHostToDevice, st));
-    FcLayerDev L;
-    if (cudaError_t e = decode_fc_layer(packed.p, enc, n_input, n_output, nf4_extension, L, st))
-        return fail(BNM_E_CUDA, "weight decode of an FC layer failed: %s", cudaGetErrorString(e));
-    struct Planes { FcLayerDev &L; ~Planes() { free_fc_layer(L); } } planes{L};   // L's planes are freed on every return below
-    DevBuf<int8_t> act;
-    DevBuf<int32_t> out;
-    if (act.grow(n * (size_t)L.k_pad) || out.grow(n * (size_t)n_output * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemsetAsync(act.p, 0, n * (size_t)L.k_pad, st));
     // Ternary layers declare n_input padded to a multiple of 10 with zero trits (exportquant.py:132-137,166) and the
     // reference never reads the activations under a zero trit (inference.c:128): a caller may hand in a 256-byte row for
     // n_input = 260.  Read exactly what the reference can read: up to the last non-zero trit of any row.
@@ -1011,17 +1031,29 @@ extern "C" int bnm_processfclayer_batch(const int8_t *activations, const uint32_
                 }
             }
     }
-    if (valid_in) CU_TRY(cudaMemcpy2DAsync(act.p, L.k_pad, activations, n_input, valid_in, n, cudaMemcpyHostToDevice, st));
-    if (!launch_fc_dp4a(act.p, L.k_pad, L, out.p, n, st))
-        return fail(BNM_E_UNSUPPORTED, "processfclayer: n_input %u needs more shared memory than an SM has (layer kernel stages 128 rows)", n_input);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(output, out.p, n * (size_t)n_output * 4, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    return 0;
+    return host_call([&](HostStaging &s) {
+        const size_t need = packed_weight_bytes(enc, n_input, n_output);
+        uint8_t *packed;
+        CU_TRY(s.get(&packed, need + 16));
+        CU_TRY(cudaMemsetAsync(packed, 0, need + 16, s.st));
+        if (need) CU_TRY(cudaMemcpyAsync(packed, weights, need, cudaMemcpyHostToDevice, s.st));
+        FcLayerDev L;
+        if (cudaError_t e = decode_fc_layer(packed, enc, n_input, n_output, nf4_extension, L, s.pool, s.st))
+            return fail(BNM_E_CUDA, "weight decode of an FC layer failed: %s", cudaGetErrorString(e));
+        struct Planes { FcLayerDev &L; cudaStream_t st; ~Planes() { free_fc_layer(L, st); } } planes{L, s.st};   // on every return below
+        int8_t *act;
+        int32_t *out;
+        CU_TRY(s.get(&act, n * (size_t)L.k_pad));
+        CU_TRY(s.out(&out, output, n * (size_t)n_output));
+        CU_TRY(cudaMemsetAsync(act, 0, n * (size_t)L.k_pad, s.st));
+        if (valid_in) CU_TRY(cudaMemcpy2DAsync(act, L.k_pad, activations, n_input, valid_in, n, cudaMemcpyHostToDevice, s.st));
+        if (!launch_fc_dp4a(act, L.k_pad, L, out, n, s.st))
+            return fail(BNM_E_UNSUPPORTED, "processfclayer: n_input %u needs more shared memory than an SM has (layer kernel stages 128 rows)", n_input);
+        return 0;
+    });
 }
 
 extern "C" int bnm_relunorm_batch(const int32_t *input, int8_t *output, uint32_t *argmax, uint32_t n_input, size_t n) {
-    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0) return 0;
     if (n_input == 0) {   // inference.c:24-37: nothing is scanned, position stays 255
@@ -1029,58 +1061,45 @@ extern "C" int bnm_relunorm_batch(const int32_t *input, int8_t *output, uint32_t
         return 0;
     }
     if (!input) return fail(BNM_E_ARG, "bnm_relunorm_batch: null input");
-    cudaStream_t st;
-    if (int rc = host_stream(&st)) return rc;
-    DevBuf<int32_t> in;
-    DevBuf<int8_t> out;
-    DevBuf<uint32_t> am;
-    if (in.grow(n * (size_t)n_input * 4) || out.grow(n * (size_t)n_input) || am.grow(n * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpyAsync(in.p, input, n * (size_t)n_input * 4, cudaMemcpyHostToDevice, st));   // copied first: output may alias input
-    launch_relunorm(in.p, n_input, output ? out.p : nullptr, n_input, am.p, n, st);
-    CU_TRY(cudaGetLastError());
-    if (argmax) CU_TRY(cudaMemcpyAsync(argmax, am.p, n * 4, cudaMemcpyDeviceToHost, st));
-    if (output) CU_TRY(cudaMemcpyAsync(output, out.p, n * (size_t)n_input, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    return 0;
+    return host_call([&](HostStaging &s) {
+        int32_t *in;
+        uint32_t *am;
+        int8_t *out;
+        CU_TRY(s.in(&in, input, n * (size_t)n_input));   // copied in before anything is copied out: output may alias input
+        CU_TRY(s.out(&am, argmax, n));
+        CU_TRY(s.out(&out, output, output ? n * (size_t)n_input : 0));
+        launch_relunorm(in, n_input, out, n_input, am, n, s.st);
+        return 0;
+    });
 }
 
 extern "C" int bnm_conv33relu_batch(const int32_t *activations, const int8_t *weights, uint32_t n_w, uint32_t xy, uint32_t n_shift,
                                     int32_t *output, size_t n) {
-    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0 || xy < 3) return 0;
     if (!activations || !weights || !output || n_w == 0) return fail(BNM_E_ARG, "bnm_conv33relu_batch: null argument");
-    cudaStream_t st;
-    if (int rc = host_stream(&st)) return rc;
-    const size_t in_el = n * (size_t)xy * xy, out_el = n * (size_t)(xy - 2) * (xy - 2);
-    DevBuf<int32_t> in, out;
-    DevBuf<int8_t> w;
-    if (in.grow(in_el * 4) || w.grow((size_t)n_w * 9) || out.grow(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpyAsync(in.p, activations, in_el * 4, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaMemcpyAsync(w.p, weights, (size_t)n_w * 9, cudaMemcpyHostToDevice, st));
-    launch_conv33relu(in.p, w.p, n_w, xy, n_shift, out.p, n, st);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(output, out.p, out_el * 4, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    return 0;
+    return host_call([&](HostStaging &s) {
+        int32_t *in, *out;
+        int8_t *w;
+        CU_TRY(s.in(&in, activations, n * (size_t)xy * xy));
+        CU_TRY(s.in(&w, weights, (size_t)n_w * 9));
+        CU_TRY(s.out(&out, output, n * (size_t)(xy - 2) * (xy - 2)));
+        launch_conv33relu(in, w, n_w, xy, n_shift, out, n, s.st);
+        return 0;
+    });
 }
 
 extern "C" int bnm_maxpool22_batch(const int32_t *activations, uint32_t xy, int32_t *output, size_t n) {
-    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0 || xy < 2) return 0;
     if (!activations || !output) return fail(BNM_E_ARG, "bnm_maxpool22_batch: null argument");
-    cudaStream_t st;
-    if (int rc = host_stream(&st)) return rc;
-    const size_t in_el = n * (size_t)xy * xy, out_el = n * (size_t)(xy / 2) * (xy / 2);
-    DevBuf<int32_t> in, out;
-    if (in.grow(in_el * 4) || out.grow(out_el * 4)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpyAsync(in.p, activations, in_el * 4, cudaMemcpyHostToDevice, st));
-    launch_maxpool22(in.p, xy, out.p, n, st);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(output, out.p, out_el * 4, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    return 0;
+    return host_call([&](HostStaging &s) {
+        int32_t *in, *out;
+        CU_TRY(s.in(&in, activations, n * (size_t)xy * xy));
+        CU_TRY(s.out(&out, output, n * (size_t)(xy / 2) * (xy / 2)));
+        launch_maxpool22(in, xy, out, n, s.st);
+        return 0;
+    });
 }
 
 extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_t elems, int8_t *out, void *stream) {
@@ -1092,21 +1111,17 @@ extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_
 }
 
 extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out) {
-    RelaxedCaptureMode relaxed;
     if (int rc = require_device()) return rc;
     if (n == 0 || elems == 0) return 0;
     if (!images || !out) return fail(BNM_E_ARG, "bnm_quantize_images: null argument");
-    cudaStream_t st;
-    if (int rc = host_stream(&st)) return rc;
-    DevBuf<float> in;
-    DevBuf<int8_t> q;
-    if (in.grow(n * (size_t)elems * 4) || q.grow(n * (size_t)elems)) return fail(BNM_E_CUDA, "cudaMalloc failed");
-    CU_TRY(cudaMemcpyAsync(in.p, images, n * (size_t)elems * 4, cudaMemcpyHostToDevice, st));
-    launch_quantize_images(in.p, elems, q.p, n, st);
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(out, q.p, n * (size_t)elems, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    return 0;
+    return host_call([&](HostStaging &s) {
+        float *in;
+        int8_t *q;
+        CU_TRY(s.in(&in, images, n * (size_t)elems));
+        CU_TRY(s.out(&q, out, n * (size_t)elems));
+        launch_quantize_images(in, elems, q, n, s.st);
+        return 0;
+    });
 }
 
 // -----------------------------------------------------------------------------------------------
@@ -1123,28 +1138,6 @@ extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems
 // -----------------------------------------------------------------------------------------------
 int bnm::level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
 
-// the emulator's route r on host buffers: per chunk of the layered emulator's pass, images in -> run_route -> logits out, synchronously
-static int emulate_host(bnm_model *m, const Route &r, const float *images, size_t n, double *logits) {
-    RelaxedCaptureMode relaxed;
-    std::lock_guard<std::mutex> turn(m->host_mu);   // takes turns with the other large host calls, on the pipeline's first stream
-    const size_t elems = m->img_bytes, ncls = m->n_classes;
-    const size_t chunk = std::min(n, kEmulLayerPass[m->model_class == BNM_MODEL_CNNMNIST]);
-    cudaStream_t st = m->slots[0].stream;
-    Scratch scratch(m, st);
-    float *d_in;      // the device copies of a chunk's images and logits
-    double *d_out;
-    CU_TRY(scratch.get(&d_in, chunk * elems));
-    CU_TRY(scratch.get(&d_out, chunk * ncls));
-    for (size_t b = 0; b < n; b += chunk) {
-        const size_t nb = std::min(chunk, n - b);
-        CU_TRY(cudaMemcpyAsync(d_in, images + b * elems, nb * elems * sizeof(float), cudaMemcpyHostToDevice, st));
-        if (int rc = run_route(m, r, d_in, nb, FcOutputs{d_out, nullptr}, st, StreamCapture{})) return rc;
-        CU_TRY(cudaMemcpyAsync(logits + b * ncls, d_out, nb * ncls * sizeof(double), cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaStreamSynchronize(st));
-    }
-    return 0;
-}
-
 // -----------------------------------------------------------------------------------------------
 // Both engines in one call (test_inference.py:130-175): the C engine's and the emulator's labels of the same float images, and
 // counts of their agreement and of their accuracy against truth.  The one-pass kernel where both float-input rows exist; every
@@ -1158,7 +1151,7 @@ static int run_engines(bnm_model *m, const Route &r, const float *images, size_t
     const EngineOutputs &e = out.engines;
     const Route c_route = choose_route(m, kEngineC, true, false), py_route = choose_route(m, kEngineEmul, true, false);
     const size_t chunk = std::min(n, r.pass), elems = m->img_bytes;
-    Scratch scratch(m, st);
+    Scratch scratch(m->pool, st);
     uint32_t *own[2];   // C / emulator labels the caller does not take
     CU_TRY(scratch.get(&own[0], e.counts && !out.labels ? chunk : 0));
     CU_TRY(scratch.get(&own[1], e.counts && !e.labels_py ? chunk : 0));
@@ -1190,7 +1183,7 @@ struct Call {
     FcOutputs out;      // the two engines' entry: the C engine's labels in labels, the rest in engines
     struct { size_t images = 1, logits = 1, classes = 1, scores = 1, counts = 1; } align;   // in bytes; labels and truth: any
     void *stream = nullptr;        // a device entry's stream
-    bool host = false;             // host buffers: a synchronous call through the small-batch path, the host pipeline or emulate_host
+    bool host = false;             // host buffers: a synchronous call through the small-batch path or the host pipeline
     bool need_logits = false;      // logits must be given when n > 0 (the emulator's host entry)
     bool no_output_at_0 = false;   // a call without outputs is an error even when n == 0 (the two engines' entry)
     const WindowGrid *windows = nullptr;   // the window scan: the images are the n windows of this grid, `images` its plane
@@ -1218,8 +1211,8 @@ static int check_call(const bnm_model *m, const Call &c) {
 }
 
 // Check call c and run its route: on the device entry's stream, whose capture state it reads once; for the two engines without a
-// fused form, run_engines; host calls of up to kSmallBatch images (and chunk) through infer_small, the others through
-// infer_pipelined or emulate_host.
+// fused form, run_engines; the C engine's int8 host calls of up to kSmallBatch images (and chunk) through infer_small, every other
+// host call through infer_pipelined.
 static int run_call(bnm_model *m, const Call &c) {
     if (int rc = check_call(m, c)) return rc;
     if (c.n == 0) return 0;
@@ -1232,8 +1225,7 @@ static int run_call(bnm_model *m, const Call &c) {
     if (o.gather && !r.fused)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     cudaStream_t st = static_cast<cudaStream_t>(c.stream);
-    if (c.host && c.engine == kEngineEmul) return emulate_host(m, r, static_cast<const float *>(c.images), c.n, static_cast<double *>(o.logits));
-    if (c.host) return infer_pipelined(m, r, static_cast<const int8_t *>(c.images), c.n, o);
+    if (c.host) return infer_pipelined(m, r, c.images, c.n, o);
     const StreamCapture cap = capture_of(st);
     if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, static_cast<const float *>(c.images), c.n, o, st, cap);
     return run_route(m, r, c.images, c.n, o, st, cap, c.windows);

@@ -30,7 +30,10 @@
  * call in flight holds its own chunk's scratch -- for example 256 MB of CNN features per 2^20-image chunk -- and the pool holds
  * the most that was ever in flight at once until the model is destroyed.  No call synchronises the host with another.
  * Small host calls (bnm_infer_batch with n <= 1024) that arrive while another one's launch is in flight share the next launch;
- * the large host calls (bnm_infer_batch above 1024 images, bnm_infer_topk, bnm_emulate_inference_quantized) take turns.
+ * the large host calls (bnm_infer_batch above 1024 images, bnm_infer_topk, bnm_emulate_inference_quantized) take turns.  They
+ * all run one pipeline in chunks of BNM_OPT_CHUNK_IMAGES images, and the model keeps that pipeline's device buffers for the
+ * largest chunk it has run: after bnm_emulate_inference_quantized three chunks of float images, 3 x chunk x 1 KiB (192 MB at
+ * the default chunk).
  * The fused kernel's launch-overlap bookkeeping (BNM_OPT_LAUNCH_OVERLAP) counts launches in the order they are enqueued on the
  * model, from whichever thread.
  *
@@ -122,6 +125,9 @@ enum {
     BNM_PATH_TCGEN05 = 2   /* fused persistent kernel: TMA -> wgmma s8 -> in-register ReLUNorm             */
 };
 enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BNM_OPT_LAUNCH_OVERLAP = 4, BNM_OPT_CNN_FRONTEND = 5 };
+/* BNM_OPT_CHUNK_IMAGES (>= 128, default 65536): images per chunk of the host pipeline, which runs bnm_infer_batch above 1024
+ * images (or above the chunk), bnm_infer_topk and bnm_emulate_inference_quantized.  Chunks go round-robin over three streams,
+ * so one chunk's copies overlap another's kernels.  Results do not depend on it. */
 /* BNM_OPT_CNN_FRONTEND (CNN models, the conv/pool loop of BitNetMCU_MNIST_dll.c:64-80): 0 (default) conv1 on the tensor cores
  * (wgmma, depthwise tail fed from shared memory) when the channel count is a multiple of 16 and <= 128, else the CUDA-core kernel;
  * 1 CUDA-core kernel; 2 tensor-core kernel or fail.  Results are identical. */
