@@ -102,6 +102,9 @@ void launch_decode_fc(const void *d_packed, int32_t enc, uint32_t n_in, uint32_t
 // ------------------------------------------------------------------------------------------------
 // processfclayer on CUDA cores: 128 images per CTA (one per thread), activations staged in smem with an
 // odd word stride (conflict-free), weights read as warp-uniform 128-bit loads, 4 outputs per pass (dp4a).
+// A row holds act_valid bytes, then zeros up to k_pad (the reference's memset layer_in).  Rows of 4-aligned
+// address and stride (act_valid is then a multiple of 4) stage as words; any other row -- a first layer on
+// images of img_bytes % 4 != 0, e.g. a 130-byte Ternary row -- byte by byte, never past its own last byte.
 // ------------------------------------------------------------------------------------------------
 template <bool HAS_B>
 __global__ void __launch_bounds__(128) k_fc_dp4a(const int8_t *__restrict__ act, uint32_t act_stride, uint32_t act_valid,
@@ -111,10 +114,20 @@ __global__ void __launch_bounds__(128) k_fc_dp4a(const int8_t *__restrict__ act,
     const uint32_t tid = threadIdx.x;
     const size_t img0 = (size_t)blockIdx.x * 128;
     const uint32_t stride = k4n + 1;
+    const bool words = (((uintptr_t)act | act_stride) & 3) == 0;
     for (uint32_t idx = tid; idx < 128 * k4n; idx += 128) {
         uint32_t im = idx / k4n, k4 = idx % k4n;
         uint32_t v = 0;
-        if (img0 + im < n && k4 * 4 < act_valid) v = *reinterpret_cast<const uint32_t *>(act + (img0 + im) * act_stride + k4 * 4);
+        if (img0 + im < n && k4 * 4 < act_valid) {
+            const int8_t *p = act + (img0 + im) * act_stride + k4 * 4;
+            if (words) {
+                v = *reinterpret_cast<const uint32_t *>(p);
+            } else {
+#pragma unroll
+                for (uint32_t j = 0; j < 4; j++)
+                    if (k4 * 4 + j < act_valid) v |= (uint32_t)(uint8_t)p[j] << (8 * j);
+            }
+        }
         s_act[im * stride + k4] = v;
     }
     __syncthreads();

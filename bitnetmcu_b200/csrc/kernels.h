@@ -41,8 +41,9 @@ void launch_decode_fc(const void *d_packed, int32_t enc, uint32_t n_in, uint32_t
                       cudaStream_t st);
 
 // ---- layer-by-layer CUDA-core path (any shape)
-// act int8 [n][act_stride] (zero padded to >= k_pad) -> out int32 [n][n_out]
-// false: the layer needs more shared memory than an SM has (n_in above ~1.8k)
+// act int8 [n][act_stride] -> out int32 [n][n_out]; any stride and any byte alignment (rows that are not 4-byte aligned stage
+// byte by byte), bytes of a row past act_stride read as zero
+// false: the layer needs more shared memory than an SM has (k_pad > 1792: 128 staged rows of k_pad + 4 bytes in 227 kB)
 bool launch_fc_dp4a(const int8_t *act, uint32_t act_stride, const FcLayerDev &L, int32_t *out, size_t n, cudaStream_t st);
 // in int32 [n][n_in] -> out int8 [n][out_stride] (zero padded), argmax uint32 [n]; out / argmax may be null
 void launch_relunorm(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t out_stride, uint32_t *argmax, size_t n,

@@ -121,9 +121,14 @@ typedef struct bnm_model bnm_model;   /* opaque; weights decoded and resident on
 /* execution path of the FC chain */
 enum {
     BNM_PATH_AUTO = 0,     /* fused wgmma kernel when the model shape is supported, else BNM_PATH_LAYERS   */
-    BNM_PATH_LAYERS = 1,   /* one CUDA-core (dp4a) kernel per layer + ReLUNorm kernel; any shape          */
+    BNM_PATH_LAYERS = 1,   /* one CUDA-core (dp4a) kernel per layer + ReLUNorm kernel; any shape (below)  */
     BNM_PATH_TCGEN05 = 2   /* fused persistent kernel: TMA -> wgmma s8 -> in-register ReLUNorm             */
 };
+/* The fused path takes image rows of a multiple of 16 bytes up to 1024, layers up to 256 outputs and weights that fit in shared
+ * memory; every other FC model runs BNM_PATH_LAYERS.  That path takes image rows of any length (img_bytes need not be a multiple of
+ * 4 or 16: a 130-byte Ternary row is fine) and bytes a layer reads past the image are zero, as in the reference driver.  Its one
+ * limit: an FC layer of more than 1792 inputs (rounded up to 32) needs more shared memory than an SM has.  Such a model loads, and
+ * every inference call on it with n > 0 returns BNM_E_UNSUPPORTED with "FC layer <l>: <n> inputs need more shared memory than an SM has". */
 enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BNM_OPT_LAUNCH_OVERLAP = 4, BNM_OPT_CNN_FRONTEND = 5 };
 /* BNM_OPT_CHUNK_IMAGES (>= 128, default 65536): images per chunk of the host pipeline, which runs bnm_infer_batch above 1024
  * images (or above the chunk), bnm_infer_topk and bnm_emulate_inference_quantized.  Chunks go round-robin over three streams,
