@@ -705,7 +705,9 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
             }
             const FcOutputs o = outputs_from(out, b + c, m->n_classes, emul, g);
             if (r.fused) {
-                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap, r.windows)))
+                // fed: the FC stage reads what this call's own scaling kernel or CNN front-end just wrote into its scratch
+                const bool fed = r.windows || r.scale || r.front != kFrontNone;
+                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap, fed)))
                     return fail(BNM_E_CUDA, "fused launch of %s failed (%d): %s", fc_chain_form_name(m->plan, r.form), rc,
                                 cudaGetErrorString(cudaGetLastError()));
                 continue;

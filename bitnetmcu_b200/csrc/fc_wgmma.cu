@@ -1364,8 +1364,10 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
     // first captured launch of a sequence keeps its wait, and the eager record is neither read nor written, so an eager launch
     // compares itself with the eager launch before it whatever was captured in between.  Where the driver cannot capture a
     // programmatic launch, a captured launch is a plain launch and keeps its (then immediate) wait.
-    // A fed launch (its images written by the call's own scaling kernel just before) keeps its wait and counts as a launch of
-    // another kind: it leaves the record empty.
+    // A fed launch (its images written into the call's own scratch just before, by k_quantize_windows, k_quantize_images or a CNN
+    // front-end: the window scan, float input on a plan without a float-input form, every CNN call) keeps its wait and counts as
+    // a launch of another kind: it leaves the record empty.  The caller's mode-2 promise covers the caller's buffers, never the
+    // producer kernels the library itself enqueues.
     LaunchBuffers bufs;
     bufs.io[0] = in; bufs.io[1] = out.logits; bufs.io[2] = out.labels;
     if (out.gather) {

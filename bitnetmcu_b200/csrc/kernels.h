@@ -174,7 +174,7 @@ struct StreamCapture {
 };
 // one launch of form f on n images `in` -> out on st, whose capture state is cap.  0, or a negative code (-5: an output the form
 // does not take, or a missing one; -6: the plan has no form f).  fed: `in` was written by a kernel of another kind that the same
-// call launched just before (the window scan's scaling kernel); the launch keeps its grid-dependency wait and, as a launch of
+// call launched just before into its scratch (k_quantize_windows, k_quantize_images, a CNN front-end); the launch keeps its grid-dependency wait and, as a launch of
 // another kind, leaves the launch-overlap record empty, so the next int8 launch keeps its wait too.
 int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap,
                     bool fed = false);

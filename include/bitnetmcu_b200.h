@@ -149,7 +149,7 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      call k must therefore be complete before call k-1 was enqueued (resident inputs, or produced on another stream and
  *      joined by an event before call k-1).  The library keeps ordinary stream semantics (the wait) for every launch where it
  *      can see the promise broken: the first launch after the option is set, a launch on another stream than the one before,
- *      a launch right after a launch of another kind (float input, emulator, top-k, window scan, ...), and a launch that touches a buffer
+ *      a launch right after a launch of another kind (float input, emulator, top-k, window scan, CNN, ...), and a launch that touches a buffer
  *      of the one before.  That is: one of its images, logits, labels or gather destination pointers equals one of the
  *      previous launch's, whatever the roles (the logits of call k-1 passed as the images of call k count), except that a
  *      gather destination both write counts only at the same row_offset.  A NULL pointer is no buffer: two labels-only
@@ -161,7 +161,11 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      graph (see "Graphs" above).
  *      Only launches that fill the GPU (>= one 128-image tile per SM) trigger early, and every launch occupies its SM
  *      exclusively (more than half of the shared memory): at most two consecutive launches are ever in flight together.
- *      CNN models are held at mode 1 (the front-end kernel really feeds the FC kernel). */
+ *      A call whose fused FC launch reads rows the call itself produced just before, into its own scratch, is such a launch of
+ *      another kind, and keeps the wait: float input on a model without a fused float-input kernel (scaled by
+ *      k_quantize_images), the window scan (k_quantize_windows) and every CNN call (the front-end's features).  The caller's
+ *      promise covers the caller's buffers only, never these producer kernels; the int8 launch right after such a call keeps
+ *      its wait too.  CNN models are held at mode 1 besides (the front-end kernel really feeds the FC kernel). */
 BNM_API int bnm_version(void);
 BNM_API const char *bnm_last_error(void);           /* thread-local text of the last failure */
 BNM_API int bnm_device_count(void);                 /* 0 when no CUDA device is usable        */
