@@ -24,6 +24,7 @@ EXPORTED = [
     "bnm_compare_engines_device",
     "bnm_infer_topk", "bnm_infer_topk_device", "bnm_infer_topk_device_f32", "bnm_emulate_topk_device",
     "bnm_infer_windows_device_f32",
+    "bnm_scan_windows_device", "bnm_scan_windows_topk_device", "bnm_emulate_windows_device", "bnm_emulate_windows_topk_device",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
@@ -44,6 +45,12 @@ class BnmGather(C.Structure):
     """bnm_gather (include/bitnetmcu_b200.h): destinations of the fused result exchange."""
     _fields_ = [("n_labels_dst", C.c_uint32), ("n_logits_dst", C.c_uint32), ("labels_dst", C.c_void_p * MAX_GATHER_DST),
                 ("logits_dst", C.c_void_p * MAX_GATHER_DST), ("row_offset", C.c_size_t), ("labels_u8", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class BnmWindows(C.Structure):
+    """bnm_windows (include/bitnetmcu_b200.h section 10): a stack of equally sized float planes and the window strides."""
+    _fields_ = [("image", C.c_void_p), ("planes", C.c_uint32), ("height", C.c_uint32), ("width", C.c_uint32), ("pitch", C.c_size_t),
+                ("plane_pitch", C.c_size_t), ("stride_y", C.c_uint32), ("stride_x", C.c_uint32)]
 
 
 _lib = None
@@ -90,6 +97,10 @@ def load() -> C.CDLL:
         "bnm_infer_topk_device_f32": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
         "bnm_emulate_topk_device": (C.c_int, [vp, vp, sz, u32, vp, vp, vp]),
         "bnm_infer_windows_device_f32": (C.c_int, [vp, vp, u32, u32, sz, u32, u32, vp, vp, vp]),
+        "bnm_scan_windows_device": (C.c_int, [vp, C.POINTER(BnmWindows), vp, vp, vp]),
+        "bnm_scan_windows_topk_device": (C.c_int, [vp, C.POINTER(BnmWindows), u32, vp, vp, vp]),
+        "bnm_emulate_windows_device": (C.c_int, [vp, C.POINTER(BnmWindows), vp, vp, vp]),
+        "bnm_emulate_windows_topk_device": (C.c_int, [vp, C.POINTER(BnmWindows), u32, vp, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

@@ -325,12 +325,13 @@ static const size_t kPass = 1 << 20, kLayerPass = 1 << 17, kEmulLayerPass[2] = {
 
 enum Engine { kEngineC, kEngineEmul, kEngineBoth };
 // the stage that turns a pass of (scaled) images into the FC stage's int8 rows: none, the C engine's CNN front-end (the kernel
-// cnn_frontend_kernel picks), k_cnn_emul_frontend, or the layered emulator's expand / conv / renorm / pool / k_i32_to_i8
+// cnn_frontend_kernel picks), the emulator's fused CNN front-end (k_cnn_emul_frontend on the float images, k_cnn_emul_frontend_i8
+// on the scaled rows of a route that scales), or the layered emulator's expand / conv / renorm / pool / k_i32_to_i8
 enum Front { kFrontNone, kFrontCnn, kFrontCnnEmul, kFrontCnnEmulLayers };
 
 // A route: which kernels one call runs, chosen once per call (choose_route), named (print_route) and run (run_route) from this
 // record alone.  Per pass of `pass` images (0: one pass), k_quantize_images into scratch when `scale` (k_quantize_windows on the
-// window scan's windows when `windows`), then per `inner` images of
+// window scan's windows when `windows`: such a route always scales), then per `inner` images of
 // that pass (0: all of it) the front-end, the FC stage and for a layered top-k k_topk_rows.  The FC stage is one launch of `form`,
 // or the layer-by-layer chain with the engine's rule.  The two engines' route runs each engine's own route per pass instead.
 struct Route {
@@ -344,7 +345,8 @@ struct Route {
 };
 
 // the route of an entry of `engine` on float32 (f32) or int8 images, top-k or not, on this model with its options; windows: the
-// float images are the windows of a plane (the C engine's window scan: the float route with k_quantize_windows as its scale step)
+// float images are the windows of a stack of planes (the window scan: the engine's float route with k_quantize_windows as its
+// scale step, never a fused float form; the emulator's fused CNN route then runs its front-end on the scaled rows)
 static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk, bool windows = false) {
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05, cnn = m->model_class == BNM_MODEL_CNNMNIST;
     Route r{engine, f32, topk, false, windows, kFrontNone, fused, kFormInt8, 0, 0};
@@ -367,7 +369,7 @@ static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk
             r.pass = kEmulLayerPass[cnn];
         } else {
             r.form = topk ? kFormEmulTopK : kFormEmulInt8;
-            r.scale = !cnn;
+            r.scale = !cnn || windows;
             r.front = cnn ? kFrontCnnEmul : kFrontNone;
             r.pass = kPass;
         }
@@ -391,12 +393,12 @@ static void print_route(const bnm_model *m, const char *what, const Route &r) {
     if (r.engine == kEngineBoth && !r.fused) {
         s = "bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts";
     } else if (r.engine == kEngineEmul && !r.fused) {
-        s = r.topk ? "layer by layer + k_topk_rows<double>" : "layer by layer";
+        s = std::string(r.windows ? "k_quantize_windows + " : "") + (r.topk ? "layer by layer + k_topk_rows<double>" : "layer by layer");
     } else {
         if (r.scale) s = r.windows ? "k_quantize_windows + " : "k_quantize_images + ";
         if (r.front == kFrontCnn)
             s += cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
-        if (r.front == kFrontCnnEmul) s += "k_cnn_emul_frontend + ";
+        if (r.front == kFrontCnnEmul) s += r.scale ? "k_cnn_emul_frontend_i8 + " : "k_cnn_emul_frontend + ";
         s += r.fused ? fc_chain_form_name(m->plan, r.form) : r.topk ? "layer by layer + k_topk_rows<int32>" : "layer by layer";
     }
     fprintf(stderr, "bitnetmcu_b200: %s: %s\n", what, s.c_str());
@@ -643,7 +645,7 @@ static FcOutputs outputs_from(const FcOutputs &o, size_t b, uint32_t n_classes, 
 // [n][n_classes], float64 for the emulator), labels and gather; or with topk.k > 0 the k best classes of every image and their
 // scores.  A route of one pass and one launch allocates nothing; every other one runs through scratch of this call's own, for one
 // pass (in a capture: graph-owned allocations, freed inside the graph).  A window route's images are the n windows of grid `win`
-// in window order; its scale step reads them from the plane.
+// in window order; its scale step reads them from the planes.
 static int run_route(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out, cudaStream_t st,
                      const StreamCapture &cap, const WindowGrid *win = nullptr) {
     const size_t pass = r.pass ? std::min(n, r.pass) : n, inner = r.inner ? std::min(pass, r.inner) : pass;
@@ -665,7 +667,7 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
         const size_t nb = std::min(pass, n - b);
         const char *in = r.windows ? nullptr : static_cast<const char *>(images) + b * in_bytes;
         size_t row_bytes = in_bytes;
-        if (r.windows) {   // windows b .. b + nb - 1 of the plane, scaled as below
+        if (r.windows) {   // windows b .. b + nb - 1 of the stack, scaled as below
             if (!launch_quantize_windows(*win, b, nb, q, st))
                 return fail(BNM_E_CUDA, "k_quantize_windows: cannot opt in to its dynamic shared memory");
             in = reinterpret_cast<const char *>(q);
@@ -683,8 +685,9 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
             if (r.front == kFrontCnn) {
                 if ((rc = run_cnn_front(m, static_cast<const int8_t *>(rows), nc, feat, st))) return rc;
             } else if (r.front == kFrontCnnEmul) {
-                if (!launch_cnn_emul_frontend(static_cast<const float *>(rows), m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, feat, m->feat_stride, nc, st))
-                    return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
+                const bool ok = r.scale ? launch_cnn_emul_frontend_i8(static_cast<const int8_t *>(rows), m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, feat, m->feat_stride, nc, st)
+                                        : launch_cnn_emul_frontend(static_cast<const float *>(rows), m->d_conv[0].p, m->d_conv[1].p, m->d_conv[2].p, C, feat, m->feat_stride, nc, st);
+                if (!ok) return fail(BNM_E_CUDA, "emulator CNN front-end: cannot opt in to its dynamic shared memory");
             } else if (r.front == kFrontCnnEmulLayers) {
                 // conv (ReLU, no shift) -> per-image renormalisation, pools in between (BitNetMCU.py:459-526)
                 int32_t *p0 = planes[0], *p1 = planes[1];
@@ -1135,7 +1138,8 @@ extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems
 // On the fused path (fc_wgmma.cu):
 //   * FC models whose rows have <= 256 elements, up to 64 wide with <= 16 classes: one kernel, fc_emul_kernel;
 //   * other FC models: the scaling kernel (k_quantize_images), then fc_emul_i8_kernel at the plan's width;
-//   * CNN models up to kCnnEmulMaxChannels channels: the front-end kernel k_cnn_emul_frontend, then fc_emul_i8_kernel on its features.
+//   * CNN models up to kCnnEmulMaxChannels channels: the front-end kernel k_cnn_emul_frontend, then fc_emul_i8_kernel on its features;
+//     the window scan runs k_quantize_windows, then the same front-end on the scaled rows (k_cnn_emul_frontend_i8).
 // BNM_PATH_LAYERS, models without a fused plan and wider CNN models run the emulation kernels layer by layer (choose_route).
 // -----------------------------------------------------------------------------------------------
 int bnm::level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == BNM_ENC_4BITSYM) ? 1 : 0; }
@@ -1188,7 +1192,7 @@ struct Call {
     bool host = false;             // host buffers: a synchronous call through the small-batch path or the host pipeline
     bool need_logits = false;      // logits must be given when n > 0 (the emulator's host entry)
     bool no_output_at_0 = false;   // a call without outputs is an error even when n == 0 (the two engines' entry)
-    const WindowGrid *windows = nullptr;   // the window scan: the images are the n windows of this grid, `images` its plane
+    const WindowGrid *windows = nullptr;   // the window scan: the images are the n windows of this grid, `images` its first plane
 };
 
 // The argument rules, in this order: a null model, or (n > 0) null images, classes or needed logits; no output at all; k out of
@@ -1223,7 +1227,7 @@ static int run_call(bnm_model *m, const Call &c) {
         return infer_small(m, static_cast<const int8_t *>(c.images), c.n, static_cast<int32_t *>(o.logits), o.labels);
     CU_TRY(cudaSetDevice(m->device));
     const Route r = choose_route(m, c.engine, c.f32, c.topk, c.windows);
-    if ((c.topk || c.windows) && m->verbose) print_route(m, (std::string(c.topk ? "topk route: " : "windows route: ") + c.name).c_str(), r);
+    if ((c.topk || c.windows) && m->verbose) print_route(m, (std::string(c.windows ? "windows route: " : "topk route: ") + c.name).c_str(), r);
     if (o.gather && !r.fused)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     cudaStream_t st = static_cast<cudaStream_t>(c.stream);
@@ -1289,23 +1293,56 @@ extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t
     return run_call(m, {"bnm_emulate_topk_device", kEngineEmul, true, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
 }
 
-// Window scan (section 9): every 16x16 window of a float plane on a stride grid, classified as bnm_infer_batch_device_f32 classifies
-// the extracted windows.  Per pass of 2^20 windows, k_quantize_windows scales them from the plane into the call's scratch, then the
-// int8 route runs on that pass; the fused FC launch after it keeps its wait and counts as a launch of another kind.
-extern "C" int bnm_infer_windows_device_f32(bnm_model *m, const float *image, uint32_t height, uint32_t width, size_t pitch,
-                                            uint32_t stride_y, uint32_t stride_x, int32_t *logits, uint32_t *labels, void *stream) {
-    static const char *name = "bnm_infer_windows_device_f32";
+// Window scan (sections 9 and 10): every 16x16 window of a stack of float planes on a stride grid, classified as the entry named
+// in the header classifies the extracted windows.  Per pass of 2^20 windows (the layered emulator: of its own pass), k_quantize_windows
+// scales them from the planes into the call's scratch, then that entry's route runs on the scaled rows; a fused FC launch after it
+// keeps its wait and counts as a launch of another kind.  w's checks, then call c (name, engine, top-k, outputs, alignment,
+// stream) on its windows.
+static int run_windows(bnm_model *m, const bnm_windows *w, Call c) {
     if (int rc = require_device()) return rc;
-    if (!stride_y || !stride_x) return fail(BNM_E_ARG, "%s: zero stride (%u, %u)", name, stride_y, stride_x);
-    if (pitch < width || pitch % 4)
-        return fail(BNM_E_ARG, "%s: pitch %zu must be >= width %u and a multiple of 4 elements (16-byte rows)", name, pitch, width);
+    if (!w) return fail(BNM_E_ARG, "%s: null window descriptor", c.name);
+    if (!w->stride_y || !w->stride_x) return fail(BNM_E_ARG, "%s: zero stride (%u, %u)", c.name, w->stride_y, w->stride_x);
+    if (w->pitch < w->width || w->pitch % 4)
+        return fail(BNM_E_ARG, "%s: pitch %zu must be >= width %u and a multiple of 4 elements (16-byte rows)", c.name, w->pitch, w->width);
+    if (w->planes > 1 && w->plane_pitch % 4)
+        return fail(BNM_E_ARG, "%s: plane pitch %zu must be a multiple of 4 elements (16-byte aligned planes)", c.name, w->plane_pitch);
     if (m && m->img_bytes != 256)
-        return fail(BNM_E_UNSUPPORTED, "%s: windows are 16x16 images, the model takes %u-element images", name, m->img_bytes);
-    const uint32_t out_h = height < 16 ? 0 : (height - 16) / stride_y + 1, out_w = width < 16 ? 0 : (width - 16) / stride_x + 1;
-    const WindowGrid g{image, height, width, pitch, stride_y, stride_x, out_h, out_w};
-    Call c{name, kEngineC, true, false, image, (size_t)out_h * out_w, {logits, labels}, {16, 8}, stream};
+        return fail(BNM_E_UNSUPPORTED, "%s: windows are 16x16 images, the model takes %u-element images", c.name, m->img_bytes);
+    const uint32_t out_h = w->height < 16 ? 0 : (w->height - 16) / w->stride_y + 1;
+    const uint32_t out_w = w->width < 16 ? 0 : (w->width - 16) / w->stride_x + 1;
+    const WindowGrid g{w->image, w->planes, w->height, w->width, w->pitch, w->planes > 1 ? w->plane_pitch : 0,
+                       w->stride_y, w->stride_x, out_h, out_w};
+    c.f32 = true;
+    c.images = w->image;
+    c.n = (size_t)w->planes * out_h * out_w;
     c.windows = &g;
     return run_call(m, c);
+}
+
+extern "C" int bnm_infer_windows_device_f32(bnm_model *m, const float *image, uint32_t height, uint32_t width, size_t pitch,
+                                            uint32_t stride_y, uint32_t stride_x, int32_t *logits, uint32_t *labels, void *stream) {
+    const bnm_windows w{image, 1, height, width, pitch, 0, stride_y, stride_x};
+    return run_windows(m, &w, {"bnm_infer_windows_device_f32", kEngineC, true, false, image, 0, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_scan_windows_device(bnm_model *m, const bnm_windows *w, int32_t *logits, uint32_t *labels, void *stream) {
+    return run_windows(m, w, {"bnm_scan_windows_device", kEngineC, true, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_scan_windows_topk_device(bnm_model *m, const bnm_windows *w, uint32_t k, uint32_t *classes, int32_t *scores,
+                                            void *stream) {
+    return run_windows(m, w, {"bnm_scan_windows_topk_device", kEngineC, true, true, nullptr, 0, {nullptr, nullptr, nullptr, {k, classes, scores}},
+                              {16, 1, 4, 4}, stream});
+}
+
+extern "C" int bnm_emulate_windows_device(bnm_model *m, const bnm_windows *w, double *logits, uint32_t *labels, void *stream) {
+    return run_windows(m, w, {"bnm_emulate_windows_device", kEngineEmul, true, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_emulate_windows_topk_device(bnm_model *m, const bnm_windows *w, uint32_t k, uint32_t *classes, double *scores,
+                                               void *stream) {
+    return run_windows(m, w, {"bnm_emulate_windows_topk_device", kEngineEmul, true, true, nullptr, 0,
+                              {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
 }
 
 // host buffers: n <= kSmallBatch images share a launch with concurrent small calls, larger batches run the chunked pipeline

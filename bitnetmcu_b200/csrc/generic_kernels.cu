@@ -277,8 +277,9 @@ void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t
 }
 
 // ------------------------------------------------------------------------------------------------
-// Window scan (bnm_infer_windows_device_f32): the 16x16 windows of one float32 plane, each scaled as k_quantize_images scales an
-// image, into int8 rows [n][256].  A CTA takes a run of up to kWinCta windows of one window row.  They share their 16 pixel rows,
+// Window scan (bnm_infer_windows_device_f32, bnm_scan_windows_device and the other stacked entries): the 16x16 windows of a stack
+// of float32 planes, each scaled as k_quantize_images scales an image, into int8 rows [n][256].  The window rows of the stack are
+// numbered plane by plane, and a CTA takes a run of up to kWinCta windows of one window row.  They share their 16 pixel rows,
 // and the columns they span (at most kWinBox) are loaded ONCE into shared memory as a band, row by row with coalesced loads:
 // each pixel of the band comes from L2 / HBM once per band, not once per window covering it.  From the band: every column's
 // max |x| over the 16 rows, then per window (one thread each) the max of its 16 columns -- a 16-wide sliding max -- the scale,
@@ -290,11 +291,12 @@ constexpr size_t kWinSmem = 16 * kWinBox * 4 + kWinBox * 4 + kWinCta * kWinStage
 
 struct WindowRun {
     const float *image;
-    size_t pitch;
-    uint32_t width, stride_y, stride_x, out_w;
+    size_t pitch, plane_pitch;  // elements between rows, between planes
+    uint32_t width, stride_y, stride_x, out_h, out_w;
     uint32_t per_cta, chunks;   // windows per CTA (per_cta columns of the grid, one box); CTAs per window row
     uint32_t box_w;             // band width in pixels
-    size_t run0;                // the pass's first run of windows: run g covers row g / chunks, columns (g % chunks) * per_cta ..
+    size_t run0;                // the pass's first run of windows: run g covers window row g / chunks of the stack (row
+                                // g / chunks % out_h of plane g / chunks / out_h), columns (g % chunks) * per_cta ..
     size_t w0, n;               // the pass: windows w0 .. w0 + n - 1
     int8_t *out;                // [n][256]
 };
@@ -305,13 +307,15 @@ __global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a)
     float *colmax = band + 16 * kWinBox;                  // [box_w]
     uint8_t *stage = reinterpret_cast<uint8_t *>(colmax + kWinBox);   // [per_cta][kWinStage]
     const size_t g = a.run0 + blockIdx.x;   // CTAs cover the runs the pass touches, and no others
-    const uint32_t r = (uint32_t)(g / a.chunks), c0 = (uint32_t)(g % a.chunks) * a.per_cta;
-    const size_t first = (size_t)r * a.out_w + c0;   // the CTA's windows first .. first + per_cta - 1, clipped to the row and the pass
+    const size_t row = g / a.chunks, p = row / a.out_h;   // the window row in the stack, its plane
+    const uint32_t r = (uint32_t)(row - p * a.out_h), c0 = (uint32_t)(g % a.chunks) * a.per_cta;
+    const size_t first = row * a.out_w + c0;   // the CTA's windows first .. first + per_cta - 1, clipped to the row and the pass
     const size_t lo = max(first, a.w0), hi = min(first + min(a.per_cta, a.out_w - c0), a.w0 + a.n);
     if (lo >= hi) return;
-    // the band: rows r * stride_y .. + 15, columns x0 .. x0 + box_w - 1 (zeros past the plane's width, never read by a window)
+    // the band: rows r * stride_y .. + 15 of plane p, columns x0 .. x0 + box_w - 1 (zeros past the plane's width, never read by a
+    // window); the plane's offset is 64-bit, past 2^31 elements in a stack of large pages
     const uint32_t x0 = c0 * a.stride_x, cols = min(a.box_w, a.width - x0);
-    const float *src = a.image + (size_t)r * a.stride_y * a.pitch + x0;
+    const float *src = a.image + p * a.plane_pitch + (size_t)r * a.stride_y * a.pitch + x0;
     for (uint32_t x = threadIdx.x; x < a.box_w; x += blockDim.x) {
 #pragma unroll
         for (int y = 0; y < 16; y++) band[y * a.box_w + x] = x < cols ? __ldg(src + (size_t)y * a.pitch + x) : 0.0f;
@@ -354,9 +358,11 @@ bool launch_quantize_windows(const WindowGrid &g, size_t w0, size_t n, int8_t *o
     WindowRun a;
     a.image = g.image;
     a.pitch = g.pitch;
+    a.plane_pitch = g.plane_pitch;
     a.width = g.width;
     a.stride_y = g.stride_y;
     a.stride_x = g.stride_x;
+    a.out_h = g.out_h;
     a.out_w = g.out_w;
     a.per_cta = std::min<uint32_t>({kWinCta, (kWinBox - 16) / g.stride_x + 1, g.out_w});
     a.chunks = (g.out_w + a.per_cta - 1) / a.per_cta;
@@ -663,36 +669,16 @@ __device__ __forceinline__ int emul_conv2(const uint32_t *c1, const int (&k)[3],
     return m;
 }
 
-__global__ void __launch_bounds__(kCnnEmulThreads, 2)
-k_cnn_emul_frontend(const float *__restrict__ images, const int8_t *__restrict__ w1, const int8_t *__restrict__ w2,
-                    const int8_t *__restrict__ w3, uint32_t C, uint32_t ipb, int8_t *__restrict__ feats, uint32_t feat_stride, size_t n) {
-    extern __shared__ __align__(16) uint32_t s_emul[];
+// The front-end of a CTA's images img0 .. img0 + ipb - 1 from their scaled rows on, which the calling kernel has stored into s_img
+// (shared memory after s_max: [ipb][kEmulImgStride / 4] words, bytes 4w .. 4w + 3 of a row in its word w; zeros for images past n)
+// without a barrier since: the three convolutions with their renormalisations and pools, then the features.
+__device__ __forceinline__ void cnn_emul_convs(uint32_t *s_emul, const int8_t *__restrict__ w1, const int8_t *__restrict__ w2,
+                                               const int8_t *__restrict__ w3, uint32_t C, uint32_t ipb, int8_t *__restrict__ feats,
+                                               uint32_t feat_stride, size_t n, size_t img0) {
     int *s_max = reinterpret_cast<int *>(s_emul);                  // [3][ipb]: the image maxima of conv1, conv2, conv3
     uint32_t *s_img = s_emul + 3 * ipb;                             // [ipb][kEmulImgStride / 4]
     uint32_t *s_c1 = s_img + ipb * (kEmulImgStride / 4);            // [ipb * C][kEmulC1Words]
-    const uint32_t t = threadIdx.x, lane = t & 31;
-    const size_t img0 = (size_t)blockIdx.x * ipb;
-
-    // input scaling (BitNetMCU.py:435-436): warp w scales images w, w + 8, ...; lane l holds elements 4l .. 4l+3 and 128 + 4l ..
-    for (uint32_t il = t >> 5; il < ipb; il += kCnnEmulThreads / 32) {
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-        if (img0 + il < n) {
-            const float4 *x = reinterpret_cast<const float4 *>(images + (img0 + il) * 256);
-            a = x[lane];
-            b = x[lane + 32];
-        }
-        float m = fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))),
-                        fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w))));
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
-        const float sc = quant_scale(m);
-        auto pack = [&](float4 v) {
-            return (uint32_t)(quant_pixel(v.x, sc) & 255) | (uint32_t)(quant_pixel(v.y, sc) & 255) << 8 |
-                   (uint32_t)(quant_pixel(v.z, sc) & 255) << 16 | (uint32_t)(quant_pixel(v.w, sc) & 255) << 24;
-        };
-        s_img[il * (kEmulImgStride / 4) + lane] = pack(a);
-        s_img[il * (kEmulImgStride / 4) + 32 + lane] = pack(b);
-    }
+    const uint32_t t = threadIdx.x;
     if (t < 3 * ipb) s_max[t] = 0;
     __syncthreads();
 
@@ -734,18 +720,84 @@ k_cnn_emul_frontend(const float *__restrict__ images, const int8_t *__restrict__
     }
 }
 
+__global__ void __launch_bounds__(kCnnEmulThreads, 2)
+k_cnn_emul_frontend(const float *__restrict__ images, const int8_t *__restrict__ w1, const int8_t *__restrict__ w2,
+                    const int8_t *__restrict__ w3, uint32_t C, uint32_t ipb, int8_t *__restrict__ feats, uint32_t feat_stride, size_t n) {
+    extern __shared__ __align__(16) uint32_t s_emul[];
+    uint32_t *s_img = s_emul + 3 * ipb;                             // [ipb][kEmulImgStride / 4]
+    const uint32_t t = threadIdx.x, lane = t & 31;
+    const size_t img0 = (size_t)blockIdx.x * ipb;
+
+    // input scaling (BitNetMCU.py:435-436): warp w scales images w, w + 8, ...; lane l holds elements 4l .. 4l+3 and 128 + 4l ..
+    for (uint32_t il = t >> 5; il < ipb; il += kCnnEmulThreads / 32) {
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+        if (img0 + il < n) {
+            const float4 *x = reinterpret_cast<const float4 *>(images + (img0 + il) * 256);
+            a = x[lane];
+            b = x[lane + 32];
+        }
+        float m = fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))),
+                        fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w))));
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+        const float sc = quant_scale(m);
+        auto pack = [&](float4 v) {
+            return (uint32_t)(quant_pixel(v.x, sc) & 255) | (uint32_t)(quant_pixel(v.y, sc) & 255) << 8 |
+                   (uint32_t)(quant_pixel(v.z, sc) & 255) << 16 | (uint32_t)(quant_pixel(v.w, sc) & 255) << 24;
+        };
+        s_img[il * (kEmulImgStride / 4) + lane] = pack(a);
+        s_img[il * (kEmulImgStride / 4) + 32 + lane] = pack(b);
+    }
+    cnn_emul_convs(s_emul, w1, w2, w3, C, ipb, feats, feat_stride, n, img0);
+}
+
+// the same front-end on rows already scaled (k_quantize_windows' output): warp w copies rows w, w + 8, ... into s_img, lane l
+// words l and 32 + l of its row; the scaling rule is the float kernel's, so the features are too
+__global__ void __launch_bounds__(kCnnEmulThreads, 2)
+k_cnn_emul_frontend_i8(const int8_t *__restrict__ images, const int8_t *__restrict__ w1, const int8_t *__restrict__ w2,
+                       const int8_t *__restrict__ w3, uint32_t C, uint32_t ipb, int8_t *__restrict__ feats, uint32_t feat_stride, size_t n) {
+    extern __shared__ __align__(16) uint32_t s_emul[];
+    uint32_t *s_img = s_emul + 3 * ipb;                             // [ipb][kEmulImgStride / 4]
+    const uint32_t t = threadIdx.x, lane = t & 31;
+    const size_t img0 = (size_t)blockIdx.x * ipb;
+    for (uint32_t il = t >> 5; il < ipb; il += kCnnEmulThreads / 32) {
+        uint32_t a = 0u, b = 0u;
+        if (img0 + il < n) {
+            const uint32_t *x = reinterpret_cast<const uint32_t *>(images + (img0 + il) * 256);
+            a = x[lane];
+            b = x[lane + 32];
+        }
+        s_img[il * (kEmulImgStride / 4) + lane] = a;
+        s_img[il * (kEmulImgStride / 4) + 32 + lane] = b;
+    }
+    cnn_emul_convs(s_emul, w1, w2, w3, C, ipb, feats, feat_stride, n, img0);
+}
+
 static uint32_t cnn_emul_ipb(uint32_t C) { return std::min(kCnnEmulMaxImages, kCnnEmulThreads / C); }
 
-bool launch_cnn_emul_frontend(const float *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
-                              int8_t *features, uint32_t feat_stride, size_t n, cudaStream_t st) {
+// kernel (k_cnn_emul_frontend or k_cnn_emul_frontend_i8) on n images: a CTA per ipb images
+template <class In>
+static bool launch_cnn_emul(void (*kernel)(const In *, const int8_t *, const int8_t *, const int8_t *, uint32_t, uint32_t, int8_t *,
+                                           uint32_t, size_t),
+                            const In *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels, int8_t *features,
+                            uint32_t feat_stride, size_t n, cudaStream_t st) {
     if (channels == 0 || channels > kCnnEmulMaxChannels) return false;
     if (n == 0) return true;
     const uint32_t ipb = cnn_emul_ipb(channels);
     const size_t smem = 4 * ((size_t)3 * ipb + ipb * (kEmulImgStride / 4) + (size_t)ipb * channels * kEmulC1Words);
-    if (!raise_smem_limit((const void *)k_cnn_emul_frontend, smem)) return false;
-    k_cnn_emul_frontend<<<(unsigned)((n + ipb - 1) / ipb), kCnnEmulThreads, smem, st>>>(images, w1, w2, w3, channels, ipb, features,
-                                                                                       feat_stride, n);
+    if (!raise_smem_limit((const void *)kernel, smem)) return false;
+    kernel<<<(unsigned)((n + ipb - 1) / ipb), kCnnEmulThreads, smem, st>>>(images, w1, w2, w3, channels, ipb, features, feat_stride, n);
     return true;
+}
+
+bool launch_cnn_emul_frontend(const float *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
+                              int8_t *features, uint32_t feat_stride, size_t n, cudaStream_t st) {
+    return launch_cnn_emul(k_cnn_emul_frontend, images, w1, w2, w3, channels, features, feat_stride, n, st);
+}
+
+bool launch_cnn_emul_frontend_i8(const int8_t *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
+                                 int8_t *features, uint32_t feat_stride, size_t n, cudaStream_t st) {
+    return launch_cnn_emul(k_cnn_emul_frontend_i8, images, w1, w2, w3, channels, features, feat_stride, n, st);
 }
 
 // ------------------------------------------------------------------------------------------------

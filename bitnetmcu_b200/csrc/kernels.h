@@ -87,12 +87,13 @@ void launch_topk_rows(const double *rows, uint32_t n_cls, uint32_t k, uint32_t *
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 
-// The 16x16 windows of one float32 plane (bnm_infer_windows_device_f32): image [height][pitch] on the device (16-byte aligned,
-// pitch a multiple of 4), windows on an (stride_y, stride_x) grid of out_h x out_w without padding, numbered row-major.
+// The 16x16 windows of a stack of float32 planes (sections 9 and 10 of the header): plane p is image + p * plane_pitch, [height][pitch]
+// on the device (16-byte aligned, pitch and plane_pitch multiples of 4), its windows on an (stride_y, stride_x) grid of out_h x
+// out_w without padding.  Windows are numbered plane by plane, row-major within a plane: w = (p * out_h + r) * out_w + c.
 struct WindowGrid {
     const float *image;
-    uint32_t height, width;
-    size_t pitch;
+    uint32_t planes, height, width;
+    size_t pitch, plane_pitch;
     uint32_t stride_y, stride_x, out_h, out_w;
 };
 // windows w0 .. w0 + n - 1 of g, each flattened row-major and scaled as launch_quantize_images scales an image -> int8 [n][256]
@@ -183,5 +184,9 @@ int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const Fc
 constexpr uint32_t kCnnEmulMaxChannels = 128;
 bool launch_cnn_emul_frontend(const float *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
                               int8_t *features, uint32_t feat_stride, size_t n, cudaStream_t st);
+// the same front-end on images already scaled to int8 [n][256] (16-byte aligned rows, k_quantize_windows' output):
+// k_cnn_emul_frontend_i8, the same features as the float kernel gives on the float images those rows were scaled from
+bool launch_cnn_emul_frontend_i8(const int8_t *images, const int8_t *w1, const int8_t *w2, const int8_t *w3, uint32_t channels,
+                                 int8_t *features, uint32_t feat_stride, size_t n, cudaStream_t st);
 
 }  // namespace bnm

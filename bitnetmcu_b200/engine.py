@@ -122,11 +122,11 @@ class Engine:
         is given as (tensor or None, its dtype or element size, its shape with N for n, or N alone for n elements of any shape):
         asserted contiguous and of that type and shape, it passes as its pointer, None as NULL.  Other arguments pass as they are.
         stream: a cudaStream_t as int, None for torch's current stream.  lead: instead of images and n, these arguments
-        (images is then a 2-D in_dtype tensor of any shape, N counts its elements)."""
+        (images is then an in_dtype tensor of any shape, N counts its elements)."""
         import torch
         if stream is None:
             stream = torch.cuda.current_stream(images.device).cuda_stream
-        assert images.dtype == in_dtype and images.dim() == 2
+        assert images.dtype == in_dtype and (lead is not None or images.dim() == 2)
         assert lead is not None or (images.is_contiguous() and images.shape[1] == self.img_bytes)
         n = images.shape[0] if lead is None else images.numel()
         vals = []
@@ -181,6 +181,53 @@ class Engine:
         lead = (C.c_void_p(image.data_ptr()), h, w, image.stride(0), sy, sx)
         self._device_call(self.lib.bnm_infer_windows_device_f32, image, torch.float32,
                           [(logits, torch.int32, (out_h, out_w, self.n_classes)), (labels, 4, (out_h, out_w))], stream, lead=lead)
+
+    # ---- window scan of a stack of pages (include/bitnetmcu_b200.h section 10) -------------------------------------------------
+    # pages: a torch.float32 [P, H, W] stack on this GPU ([H, W]: one page) with unit column stride; its row stride is the pitch
+    # and its plane stride the plane pitch (multiples of 4).  stride: an int or (sy, sx).  Every output is [P, out_h, out_w, ...]
+    # with (out_h, out_w) = window_grid(H, W, stride); window (p, r, c) covers pages[p, r*sy : r*sy+16, c*sx : c*sx+16], and its
+    # results are those of the matching entry on that window flattened.  Asynchronous on ``stream`` (default: torch's current
+    # stream).
+    def _windows_call(self, fn, pages, stride, args, stream) -> None:
+        """fn(handle, the stack's bnm_windows, *args, stream) as _device_call passes args, a tensor argument's shape given past
+        the window grid [P, out_h, out_w]"""
+        import torch
+        p = pages if pages.dim() == 3 else pages.unsqueeze(0)
+        assert p.dim() == 3 and p.stride(2) == 1
+        sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
+        n_p, h, w = p.shape
+        desc = _lib.BnmWindows(p.data_ptr(), n_p, h, w, p.stride(1), p.stride(0), sy, sx)
+        grid = (n_p,) + window_grid(h, w, (sy, sx))
+        args = [(a[0], a[1], grid + a[2]) if isinstance(a, tuple) else a for a in args]
+        self._device_call(fn, p, torch.float32, args, stream, lead=(C.byref(desc),))
+
+    def scan_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
+        """The C engine on every window of a stack of pages: logits torch.int32 [P, out_h, out_w, n_classes] or None, labels
+        [P, out_h, out_w] (4-byte elements) or None (not both None); ``infer_device_f32`` on each window."""
+        import torch
+        self._windows_call(self.lib.bnm_scan_windows_device, pages, stride,
+                           [(logits, torch.int32, (self.n_classes,)), (labels, 4, ())], stream)
+
+    def scan_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
+        """The C engine's top-k of every window: classes [P, out_h, out_w, k] (4-byte elements), scores torch.int32
+        [P, out_h, out_w, k] or None; ``topk_device_f32`` on each window."""
+        import torch
+        self._windows_call(self.lib.bnm_scan_windows_topk_device, pages, stride,
+                           [int(k), (classes, 4, (k,)), (scores, torch.int32, (k,))], stream)
+
+    def emulate_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
+        """The emulator on every window: logits torch.float64 [P, out_h, out_w, n_classes] or None, labels [P, out_h, out_w]
+        or None (not both None); ``inference_quantized_device`` on each window."""
+        import torch
+        self._windows_call(self.lib.bnm_emulate_windows_device, pages, stride,
+                           [(logits, torch.float64, (self.n_classes,)), (labels, 4, ())], stream)
+
+    def emulate_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
+        """The emulator's top-k of every window: classes [P, out_h, out_w, k], scores torch.float64 [P, out_h, out_w, k] or
+        None; ``emulate_topk_device`` on each window."""
+        import torch
+        self._windows_call(self.lib.bnm_emulate_windows_topk_device, pages, stride,
+                           [int(k), (classes, 4, (k,)), (scores, torch.float64, (k,))], stream)
 
     def compare_engines_device(self, images, truth=None, labels_c=None, labels_py=None, counts=None, stream: Optional[int] = None) -> None:
         """Both engines on the same float images in one call (test_inference.py:130-175): images torch.float32 [n, img_bytes] on

@@ -18,6 +18,7 @@
  * Sections 5 to 7 take float images: the C engine (5), the reference's Python emulator (6), and both at once, scored (7).
  * Section 8 returns each image's k best classes and their scores (top-k) from either engine.
  * Section 9 classifies every 16x16 window of a larger float image on a stride grid (window scan).
+ * Section 10 scans a stack of such images in one call, on either engine, with labels, logits or top-k.
  *
  * Pointers are plain host (or, where the name says _device, CUDA device) pointers; sizes are element
  * counts unless named *_bytes.  All-integer arithmetic: results are bit-exact with the reference.
@@ -25,7 +26,8 @@
  * Threads.  Every entry point may be called concurrently from any number of host threads on one model, on the same stream or
  * on different streams, and each call's results are exactly those of the same call made alone.  The exceptions are
  * bnm_model_set_option and bnm_model_destroy: like any handle's, they must not overlap other calls on that model.  A call's
- * device scratch (CNN features, the layer-by-layer path's buffers, scaled images, the emulator's planes) is its own, allocated
+ * device scratch (CNN features, the layer-by-layer path's buffers, scaled images and windows, the emulator's planes) is its own,
+ * the window entries' of sections 9 and 10 included, allocated
  * stream-ordered on the call's stream from a memory pool of the model that keeps what it has: concurrency costs memory, as each
  * call in flight holds its own chunk's scratch -- for example 256 MB of CNN features per 2^20-image chunk -- and the pool holds
  * the most that was ever in flight at once until the model is destroyed.  No call synchronises the host with another.
@@ -38,7 +40,8 @@
  * model, from whichever thread.
  *
  * Graphs.  Every device entry (bnm_infer_batch_device, _gather, _f32, bnm_emulate_batch_device, bnm_compare_engines_device, the
- * three top-k device entries, bnm_infer_windows_device_f32 and bnm_quantize_images_device) may be captured into a CUDA graph on
+ * three top-k device entries, bnm_infer_windows_device_f32, the four stacked window entries bnm_scan_windows_device,
+ * bnm_scan_windows_topk_device, bnm_emulate_windows_device and bnm_emulate_windows_topk_device, and bnm_quantize_images_device) may be captured into a CUDA graph on
  * its stream, in any capture mode, in any combination and from any thread.  Each replay gives exactly the results of the same call made eagerly on the buffers'
  * contents at replay time; bnm_compare_engines_device adds to `counts` on every replay.  A graph keeps what its capture decided:
  * the route, the routing options (BNM_OPT_PATH, BNM_OPT_CHUNK_IMAGES, BNM_OPT_CNN_FRONTEND, BNM_OPT_LAUNCH_OVERLAP) and the
@@ -163,7 +166,8 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      exclusively (more than half of the shared memory): at most two consecutive launches are ever in flight together.
  *      A call whose fused FC launch reads rows the call itself produced just before, into its own scratch, is such a launch of
  *      another kind, and keeps the wait: float input on a model without a fused float-input kernel (scaled by
- *      k_quantize_images), the window scan (k_quantize_windows) and every CNN call (the front-end's features).  The caller's
+ *      k_quantize_images), the window scans of sections 9 and 10 (k_quantize_windows) and every CNN call (the front-end's
+ *      features).  The caller's
  *      promise covers the caller's buffers only, never these producer kernels; the int8 launch right after such a call keeps
  *      its wait too.  CNN models are held at mode 1 besides (the front-end kernel really feeds the FC kernel). */
 BNM_API int bnm_version(void);
@@ -366,6 +370,45 @@ BNM_API int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n,
  * synchronisation. */
 BNM_API int bnm_infer_windows_device_f32(bnm_model *m, const float *image, uint32_t height, uint32_t width, size_t pitch,
                                          uint32_t stride_y, uint32_t stride_x, int32_t *logits, uint32_t *labels, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 10. Window scan of a stack of pages: the windows of every plane of a stack in one call (a document's pages, say), on the C
+ *     engine or the Python emulator, with labels and logits or with each window's top-k (section 8).  One call spreads its fixed
+ *     cost (launches, scratch) over the whole stack.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct bnm_windows {
+    const float *image;       /* plane p starts at image + p * plane_pitch; device memory on the model's GPU, 16-byte aligned */
+    uint32_t planes;          /* >= 0; 0 = no windows                                                                        */
+    uint32_t height, width;   /* of every plane                                                                              */
+    size_t pitch;             /* elements between rows: >= width, a multiple of 4                                            */
+    size_t plane_pitch;       /* elements between planes: a multiple of 4 (ignored when planes <= 1)                         */
+    uint32_t stride_y, stride_x;
+} bnm_windows;
+/* Each plane has out_h x out_w windows as in section 9.  Window w = (p * out_h + r) * out_w + c covers rows r * stride_y .. + 15
+ * and columns c * stride_x .. + 15 of plane p, flattened row-major; every output is in that order, [planes][out_h][out_w]...
+ * Each entry's results are bit for bit those of the entry named beside it on the extracted windows in that order:
+ *   bnm_scan_windows_device           bnm_infer_batch_device_f32   labels uint32 [n], logits int32 [n][n_classes] (8-byte aligned)
+ *   bnm_scan_windows_topk_device      bnm_infer_topk_device_f32    classes uint32 [n][k] (4-byte aligned), scores int32 [n][k]
+ *   bnm_emulate_windows_device        bnm_emulate_batch_device     labels uint32 [n], logits float64 [n][n_classes] (8-byte aligned)
+ *   bnm_emulate_windows_topk_device   bnm_emulate_topk_device      classes uint32 [n][k], scores float64 [n][k] (8-byte aligned)
+ * Labels and logits may each be NULL, not both; classes are required, scores may be NULL; 1 <= k <= min(n_classes, BNM_MAX_TOPK).
+ * BNM_E_ARG: a NULL descriptor, a zero stride, pitch < width or not a multiple of 4, a plane pitch not a multiple of 4 (planes > 1),
+ * a misaligned image, logits or scores buffer, no output, a bad k.  BNM_E_UNSUPPORTED: a model whose images are not 256 elements.
+ * No windows (planes == 0, or height or width < 16): returns 0 and writes nothing; a top-k call still checks k and alignment.
+ * Routes: per pass of 2^20 windows a scaling kernel reads each run of windows' 16-row band once and writes their int8 rows into
+ * the call's scratch (planes are 64-bit offsets apart: a stack may pass 2^31 elements); then the C engine runs the int8 route of
+ * bnm_infer_batch_device or bnm_infer_topk_device on them; the emulator its int8-input FC kernel (FC models), its CNN front-end on
+ * the scaled rows, then that kernel (CNN models up to 128 channels), or its layer-by-layer route (BNM_PATH_LAYERS, models without
+ * a fused plan, wider CNN models, in passes of 65 536 (FC) or 2 048 (CNN) windows).  No fused float-input kernel serves windows.
+ * With BNM_VERBOSE set at model creation every call prints "bitnetmcu_b200: windows route: <entry>: k_quantize_windows + ...".
+ * For BNM_OPT_LAUNCH_OVERLAP mode 2 a window call is a launch of another kind (section 9).  Asynchronous on `stream`, no host
+ * synchronisation. */
+BNM_API int bnm_scan_windows_device(bnm_model *m, const bnm_windows *windows, int32_t *logits, uint32_t *labels, void *stream);
+BNM_API int bnm_scan_windows_topk_device(bnm_model *m, const bnm_windows *windows, uint32_t k, uint32_t *classes, int32_t *scores,
+                                         void *stream);
+BNM_API int bnm_emulate_windows_device(bnm_model *m, const bnm_windows *windows, double *logits, uint32_t *labels, void *stream);
+BNM_API int bnm_emulate_windows_topk_device(bnm_model *m, const bnm_windows *windows, uint32_t k, uint32_t *classes, double *scores,
+                                            void *stream);
 
 #ifdef __cplusplus
 }
