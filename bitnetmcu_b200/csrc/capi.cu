@@ -320,8 +320,9 @@ static int require_device_index(int device);
 // -----------------------------------------------------------------------------------------------
 // Images per pass, each bounding the scratch of a call: 2^20 where a pass stages rows in scratch (scaled images, CNN features, the
 // two-engine entry's labels), 2^17 for the C engine layer by layer, 65 536 (FC) / 2 048 (CNN: 2 x C kB of conv planes per image)
-// for the emulator layer by layer
-static const size_t kPass = 1 << 20, kLayerPass = 1 << 17, kEmulLayerPass[2] = {65536, 2048};
+// for the emulator layer by layer.  A fused FC route that stages nothing runs one launch per pass of kFusedPass images: a launch
+// takes at most 0x7fffff00 (its TMA row coordinate is an int32), and 2^28 costs one more launch per 64 GiB of 256-byte rows.
+static const size_t kPass = 1 << 20, kLayerPass = 1 << 17, kEmulLayerPass[2] = {65536, 2048}, kFusedPass = 1 << 28;
 
 enum Engine { kEngineC, kEngineEmul, kEngineBoth };
 // the stage that turns a pass of (scaled) images into the FC stage's int8 rows: none, the C engine's CNN front-end (the kernel
@@ -330,7 +331,7 @@ enum Engine { kEngineC, kEngineEmul, kEngineBoth };
 enum Front { kFrontNone, kFrontCnn, kFrontCnnEmul, kFrontCnnEmulLayers };
 
 // A route: which kernels one call runs, chosen once per call (choose_route), named (print_route) and run (run_route) from this
-// record alone.  Per pass of `pass` images (0: one pass), k_quantize_images into scratch when `scale` (k_quantize_windows on the
+// record alone.  Per pass of `pass` images, k_quantize_images into scratch when `scale` (k_quantize_windows on the
 // window scan's windows when `windows`: such a route always scales), then per `inner` images of
 // that pass (0: all of it) the front-end, the FC stage and for a layered top-k k_topk_rows.  The FC stage is one launch of `form`,
 // or the layer-by-layer chain with the engine's rule.  The two engines' route runs each engine's own route per pass instead.
@@ -354,6 +355,7 @@ static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk
     const FcForm float_form = engine == kEngineC ? kFormFloat : engine == kEngineEmul ? kFormEmulFloat : kFormEngines;
     if (f32 && !topk && !windows && fused && !cnn && fc_chain_has_form(m->plan, float_form)) {
         r.form = float_form;
+        r.pass = kFusedPass;
         return r;
     }
     if (engine == kEngineBoth) {
@@ -377,7 +379,7 @@ static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk
     }
     r.form = topk ? kFormTopK : kFormInt8;
     r.front = cnn ? kFrontCnn : kFrontNone;
-    r.pass = !fused ? kLayerPass : cnn ? kPass : 0;
+    r.pass = !fused ? kLayerPass : cnn ? kPass : kFusedPass;
     if (f32) {   // the int8 route on each pass of scaled images
         r.scale = true;
         r.inner = r.pass;
@@ -643,12 +645,12 @@ static FcOutputs outputs_from(const FcOutputs &o, size_t b, uint32_t n_classes, 
 
 // Route r (not the two engines' one) on n images on st, whose capture state is cap, arguments checked -> out: logits (int32
 // [n][n_classes], float64 for the emulator), labels and gather; or with topk.k > 0 the k best classes of every image and their
-// scores.  A route of one pass and one launch allocates nothing; every other one runs through scratch of this call's own, for one
-// pass (in a capture: graph-owned allocations, freed inside the graph).  A window route's images are the n windows of grid `win`
+// scores.  A fused route without a scale step or front-end allocates nothing; every other one runs through scratch of this
+// call's own, for one pass (in a capture: graph-owned allocations, freed inside the graph).  A window route's images are the n windows of grid `win`
 // in window order; its scale step reads them from the planes.
 static int run_route(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out, cudaStream_t st,
                      const StreamCapture &cap, const WindowGrid *win = nullptr) {
-    const size_t pass = r.pass ? std::min(n, r.pass) : n, inner = r.inner ? std::min(pass, r.inner) : pass;
+    const size_t pass = std::min(n, r.pass), inner = r.inner ? std::min(pass, r.inner) : pass;
     const bool emul = r.engine == kEngineEmul;
     const uint32_t elems = m->img_bytes, C = m->channels, k = out.topk.k;
     const size_t in_bytes = r.f32 ? elems * sizeof(float) : elems;   // per input image
@@ -708,8 +710,11 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
             }
             const FcOutputs o = outputs_from(out, b + c, m->n_classes, emul, g);
             if (r.fused) {
-                // fed: the FC stage reads what this call's own scaling kernel or CNN front-end just wrote into its scratch
-                const bool fed = r.windows || r.scale || r.front != kFrontNone;
+                // fed: the FC stage reads what this call's own scaling kernel or CNN front-end just wrote into its scratch.  Every
+                // pass after a call's first is treated alike and keeps its wait: it reads and writes the same caller buffers as
+                // the pass before it, and the mode-2 promise covers the call before this one, not the producer of these images
+                // that the first pass may have waited for
+                const bool fed = r.windows || r.scale || r.front != kFrontNone || b + c > 0;
                 if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap, fed)))
                     return fail(BNM_E_CUDA, "fused launch of %s failed (%d): %s", fc_chain_form_name(m->plan, r.form), rc,
                                 cudaGetErrorString(cudaGetLastError()));
@@ -726,7 +731,6 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
 extern "C" int bnm_infer_launch_count(const bnm_model *m, size_t n) {
     if (!m || n == 0) return 0;
     const Route r = choose_route(m, kEngineC, false, false);
-    if (!r.pass) return 1;
     const int per = (r.front != kFrontNone) + (r.fused ? 1 : (int)(2 * m->fc.size()));   // front-end, fc + relunorm per layer
     return (int)((n + r.pass - 1) / r.pass * per);
 }

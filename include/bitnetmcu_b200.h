@@ -212,7 +212,10 @@ BNM_API int bnm_model_active_path(const bnm_model *m);
 BNM_API int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels);
 
 /* Device version: pointers are device memory on the model's GPU (images 16-byte, logits 8-byte aligned); asynchronous on `stream`
- * (a cudaStream_t, NULL = default stream).  No host synchronisation. */
+ * (a cudaStream_t, NULL = default stream).  No host synchronisation.  On the fused path one launch of an FC model takes at most
+ * 2^28 images (the kernel's limit is 0x7fffff00): a larger batch runs as several launches of up to 2^28 images, in order on
+ * `stream` (bnm_infer_launch_count counts them; the same holds for bnm_infer_batch_device_gather and bnm_infer_topk_device).
+ * For BNM_OPT_LAUNCH_OVERLAP mode 2, every launch of a call after its first keeps its wait. */
 BNM_API int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels,
                                    void *stream);
 /* Fused result exchange (SURVEY.md 8e; the reference has none -- its caller collects one label per call,
