@@ -25,11 +25,14 @@ EXPORTED = [
     "bnm_infer_topk", "bnm_infer_topk_device", "bnm_infer_topk_device_f32", "bnm_emulate_topk_device",
     "bnm_infer_windows_device_f32",
     "bnm_scan_windows_device", "bnm_scan_windows_topk_device", "bnm_emulate_windows_device", "bnm_emulate_windows_topk_device",
+    "bnm_infer_batch_device_f16", "bnm_emulate_batch_device_f16", "bnm_compare_engines_device_f16", "bnm_infer_topk_device_f16",
+    "bnm_emulate_topk_device_f16", "bnm_quantize_images_device_f16",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
 OPT_PATH, OPT_NF4_EXTENSION, OPT_CHUNK_IMAGES, OPT_LAUNCH_OVERLAP, OPT_CNN_FRONTEND = 1, 2, 3, 4, 5
 CNN_AUTO, CNN_CUDA_CORES, CNN_TENSOR_CORES = 0, 1, 2
+FLOAT16, BFLOAT16 = 1, 2   # BNM_FLOAT16, BNM_BFLOAT16 (section 11)
 
 
 class BnmLayer(C.Structure):
@@ -101,6 +104,12 @@ def load() -> C.CDLL:
         "bnm_scan_windows_topk_device": (C.c_int, [vp, C.POINTER(BnmWindows), u32, vp, vp, vp]),
         "bnm_emulate_windows_device": (C.c_int, [vp, C.POINTER(BnmWindows), vp, vp, vp]),
         "bnm_emulate_windows_topk_device": (C.c_int, [vp, C.POINTER(BnmWindows), u32, vp, vp, vp]),
+        "bnm_infer_batch_device_f16": (C.c_int, [vp, vp, C.c_int, sz, vp, vp, vp]),
+        "bnm_emulate_batch_device_f16": (C.c_int, [vp, vp, C.c_int, sz, vp, vp, vp]),
+        "bnm_compare_engines_device_f16": (C.c_int, [vp, vp, C.c_int, sz, vp, vp, vp, vp, vp]),
+        "bnm_infer_topk_device_f16": (C.c_int, [vp, vp, C.c_int, sz, u32, vp, vp, vp]),
+        "bnm_emulate_topk_device_f16": (C.c_int, [vp, vp, C.c_int, sz, u32, vp, vp, vp]),
+        "bnm_quantize_images_device_f16": (C.c_int, [vp, C.c_int, sz, u32, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

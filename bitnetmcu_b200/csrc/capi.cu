@@ -325,19 +325,26 @@ static int require_device_index(int device);
 static const size_t kPass = 1 << 20, kLayerPass = 1 << 17, kEmulLayerPass[2] = {65536, 2048}, kFusedPass = 1 << 28;
 
 enum Engine { kEngineC, kEngineEmul, kEngineBoth };
+// the element type of a call's images: int8 (already scaled), float32, or 16-bit floats (section 11) of either format
+enum InKind { kInI8, kInF32, kInF16, kInBF16 };
+static_assert(kHalfFloat16 == BNM_FLOAT16 && kHalfBFloat16 == BNM_BFLOAT16, "HalfFormat follows the header's formats");
+static size_t in_elem_bytes(InKind in) { return in == kInI8 ? 1 : in == kInF32 ? 4 : 2; }
+static bool half_in(InKind in) { return in == kInF16 || in == kInBF16; }
+static HalfFormat half_format(InKind in) { return in == kInBF16 ? kHalfBFloat16 : kHalfFloat16; }
 // the stage that turns a pass of (scaled) images into the FC stage's int8 rows: none, the C engine's CNN front-end (the kernel
 // cnn_frontend_kernel picks), the emulator's fused CNN front-end (k_cnn_emul_frontend on the float images, k_cnn_emul_frontend_i8
 // on the scaled rows of a route that scales), or the layered emulator's expand / conv / renorm / pool / k_i32_to_i8
 enum Front { kFrontNone, kFrontCnn, kFrontCnnEmul, kFrontCnnEmulLayers };
 
 // A route: which kernels one call runs, chosen once per call (choose_route), named (print_route) and run (run_route) from this
-// record alone.  Per pass of `pass` images, k_quantize_images into scratch when `scale` (k_quantize_windows on the
+// record alone.  Per pass of `pass` images, k_quantize_images (for its input kind) into scratch when `scale` (k_quantize_windows on the
 // window scan's windows when `windows`: such a route always scales), then per `inner` images of
 // that pass (0: all of it) the front-end, the FC stage and for a layered top-k k_topk_rows.  The FC stage is one launch of `form`,
 // or the layer-by-layer chain with the engine's rule.  The two engines' route runs each engine's own route per pass instead.
 struct Route {
     Engine engine;
-    bool f32, topk;   // float32 images in; the k best classes out
+    InKind in;
+    bool topk;        // the k best classes out
     bool scale, windows;
     Front front;
     bool fused;
@@ -345,14 +352,17 @@ struct Route {
     size_t pass, inner;
 };
 
-// the route of an entry of `engine` on float32 (f32) or int8 images, top-k or not, on this model with its options; windows: the
-// float images are the windows of a stack of planes (the window scan: the engine's float route with k_quantize_windows as its
-// scale step, never a fused float form; the emulator's fused CNN route then runs its front-end on the scaled rows)
-static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk, bool windows = false) {
+// the route of an entry of `engine` on images of kind `in`, top-k or not, on this model with its options; windows: the float
+// images are the windows of a stack of planes (the window scan: the engine's float route with k_quantize_windows as its scale
+// step, never a fused float form; the emulator's fused CNN route then runs its front-end on the scaled rows).  16-bit images take
+// the route of float32 ones, with the 16-bit float-input forms, or the 16-bit scaling kernel as the scale step.
+static Route choose_route(const bnm_model *m, Engine engine, InKind in, bool topk, bool windows = false) {
     const bool fused = bnm_model_active_path(m) == BNM_PATH_TCGEN05, cnn = m->model_class == BNM_MODEL_CNNMNIST;
-    Route r{engine, f32, topk, false, windows, kFrontNone, fused, kFormInt8, 0, 0};
+    const bool f32 = in != kInI8, half = half_in(in);
+    Route r{engine, in, topk, false, windows, kFrontNone, fused, kFormInt8, 0, 0};
     // FC models whose plan has the engine's float-input form: one launch with the input scaling fused (no such top-k or window form)
-    const FcForm float_form = engine == kEngineC ? kFormFloat : engine == kEngineEmul ? kFormEmulFloat : kFormEngines;
+    const FcForm float_form = engine == kEngineC ? (half ? kFormFloat16 : kFormFloat)
+                              : engine == kEngineEmul ? (half ? kFormEmulFloat16 : kFormEmulFloat) : (half ? kFormEngines16 : kFormEngines);
     if (f32 && !topk && !windows && fused && !cnn && fc_chain_has_form(m->plan, float_form)) {
         r.form = float_form;
         r.pass = kFusedPass;
@@ -363,7 +373,7 @@ static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk
         r.pass = kPass;
         return r;
     }
-    if (engine == kEngineEmul) {   // float32 images only
+    if (engine == kEngineEmul) {   // float images only
         if (!fused || (cnn && m->channels > kCnnEmulMaxChannels)) {
             r.fused = false;
             r.scale = true;
@@ -371,7 +381,7 @@ static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk
             r.pass = kEmulLayerPass[cnn];
         } else {
             r.form = topk ? kFormEmulTopK : kFormEmulInt8;
-            r.scale = !cnn || windows;
+            r.scale = !cnn || windows || half;   // 16-bit CNN images: k_cnn_emul_frontend_i8 on the scaled rows
             r.front = cnn ? kFrontCnnEmul : kFrontNone;
             r.pass = kPass;
         }
@@ -392,12 +402,14 @@ static Route choose_route(const bnm_model *m, Engine engine, bool f32, bool topk
 static void print_route(const bnm_model *m, const char *what, const Route &r) {
     if (!m->verbose) return;
     std::string s;
+    const char *scale = r.in == kInF16 ? "k_quantize_images<float16> + " : r.in == kInBF16 ? "k_quantize_images<bfloat16> + " : "k_quantize_images + ";
     if (r.engine == kEngineBoth && !r.fused) {
-        s = "bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts";
+        s = half_in(r.in) ? "bnm_infer_batch_device_f16 + bnm_emulate_batch_device_f16 + k_engine_counts"
+                          : "bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts";
     } else if (r.engine == kEngineEmul && !r.fused) {
         s = std::string(r.windows ? "k_quantize_windows + " : "") + (r.topk ? "layer by layer + k_topk_rows<double>" : "layer by layer");
     } else {
-        if (r.scale) s = r.windows ? "k_quantize_windows + " : "k_quantize_images + ";
+        if (r.scale) s = r.windows ? "k_quantize_windows + " : scale;
         if (r.front == kFrontCnn)
             s += cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
         if (r.front == kFrontCnnEmul) s += r.scale ? "k_cnn_emul_frontend_i8 + " : "k_cnn_emul_frontend + ";
@@ -497,8 +509,8 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
     if (rc != 0) { std::string keep = g_err; bnm_model_destroy(m); g_err = keep; return rc; }
     m->verbose = getenv("BNM_VERBOSE") != nullptr;
     if (m->verbose) {   // diagnostics: the routes of bnm_emulate_batch_device and bnm_compare_engines_device on the default path
-        print_route(m, "emulator route", choose_route(m, kEngineEmul, true, false));
-        print_route(m, "engines route", choose_route(m, kEngineBoth, true, false));
+        print_route(m, "emulator route", choose_route(m, kEngineEmul, kInF32, false));
+        print_route(m, "engines route", choose_route(m, kEngineBoth, kInF32, false));
         // and which conv3 the tensor-core CNN front-end runs
         if (m->model_class == BNM_MODEL_CNNMNIST)
             fprintf(stderr, "bitnetmcu_b200: cnn front-end: conv3 bound %lld, conv3 on %s\n", m->conv3_bound,
@@ -653,7 +665,7 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
     const size_t pass = std::min(n, r.pass), inner = r.inner ? std::min(pass, r.inner) : pass;
     const bool emul = r.engine == kEngineEmul;
     const uint32_t elems = m->img_bytes, C = m->channels, k = out.topk.k;
-    const size_t in_bytes = r.f32 ? elems * sizeof(float) : elems;   // per input image
+    const size_t in_bytes = elems * in_elem_bytes(r.in);   // per input image
     Scratch s(m->pool, st);
     int8_t *q, *feat;     // a pass's scaled images; an inner pass's CNN features for the fused FC stage
     LayerScratch ls;      // the layer-by-layer chain's accumulators and activations
@@ -675,7 +687,8 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
             in = reinterpret_cast<const char *>(q);
             row_bytes = elems;
         } else if (r.scale) {   // test_inference.py:140-141, BitNetMCU.py:435-436
-            launch_quantize_images(reinterpret_cast<const float *>(in), elems, q, nb, st);
+            if (half_in(r.in)) launch_quantize_images(reinterpret_cast<const uint16_t *>(in), half_format(r.in), elems, q, nb, st);
+            else launch_quantize_images(reinterpret_cast<const float *>(in), elems, q, nb, st);
             in = reinterpret_cast<const char *>(q);
             row_bytes = elems;
         }
@@ -715,7 +728,7 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
                 // the pass before it, and the mode-2 promise covers the call before this one, not the producer of these images
                 // that the first pass may have waited for
                 const bool fed = r.windows || r.scale || r.front != kFrontNone || b + c > 0;
-                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap, fed)))
+                if ((rc = fc_chain_launch(m->plan, r.form, rows, nc, o, st, cap, fed, half_in(r.in) && !r.scale ? half_format(r.in) : 0)))
                     return fail(BNM_E_CUDA, "fused launch of %s failed (%d): %s", fc_chain_form_name(m->plan, r.form), rc,
                                 cudaGetErrorString(cudaGetLastError()));
                 continue;
@@ -730,7 +743,7 @@ static int run_route(bnm_model *m, const Route &r, const void *images, size_t n,
 
 extern "C" int bnm_infer_launch_count(const bnm_model *m, size_t n) {
     if (!m || n == 0) return 0;
-    const Route r = choose_route(m, kEngineC, false, false);
+    const Route r = choose_route(m, kEngineC, kInI8, false);
     const int per = (r.front != kFrontNone) + (r.fused ? 1 : (int)(2 * m->fc.size()));   // front-end, fc + relunorm per layer
     return (int)((n + r.pass - 1) / r.pass * per);
 }
@@ -821,7 +834,7 @@ static int small_launch(bnm_model *m, SmallGen &g) {
     const size_t n_log = g.logits ? n * (size_t)m->n_classes : 0;   // labels-only batches: the labels start the staging buffer
     uint32_t *d_lab = reinterpret_cast<uint32_t *>(d_out + n_log);
     const FcOutputs out{g.logits ? d_out : nullptr, g.labels ? d_lab : nullptr};
-    if (int rc = run_route(m, choose_route(m, kEngineC, false, false), g.d_in.p, n, out, st, StreamCapture{})) return rc;
+    if (int rc = run_route(m, choose_route(m, kEngineC, kInI8, false), g.d_in.p, n, out, st, StreamCapture{})) return rc;
     CU_TRY(cudaStreamSynchronize(st));
     return 0;
 }
@@ -905,7 +918,7 @@ static int infer_pipelined(bnm_model *m, const Route &r, const void *images, siz
     const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
     // per image, in bytes: the images (float32 or int8), d_logits the logits or the top-k scores (float64 for the emulator, else
     // int32; bnm_infer_batch sizes it and d_labels whether or not it takes them), d_labels the label, d_classes the top-k classes
-    const size_t in_bytes = r.f32 ? 4 * m->img_bytes : m->img_bytes, el = r.engine == kEngineEmul ? 8 : 4;
+    const size_t in_bytes = in_elem_bytes(r.in) * m->img_bytes, el = r.engine == kEngineEmul ? 8 : 4;
     const size_t logit_bytes = (k ? (out.topk.scores ? k : 0) : m->n_classes) * el, label_bytes = k ? 0 : 4, class_bytes = k * 4;
     bool small = false;
     for (auto &s : m->slots)
@@ -1119,6 +1132,16 @@ extern "C" int bnm_quantize_images_device(const float *images, size_t n, uint32_
     return launch_status();
 }
 
+extern "C" int bnm_quantize_images_device_f16(const uint16_t *images, int format, size_t n, uint32_t elems, int8_t *out, void *stream) {
+    if (int rc = require_device()) return rc;
+    if (format != BNM_FLOAT16 && format != BNM_BFLOAT16)
+        return fail(BNM_E_ARG, "bnm_quantize_images_device_f16: format %d, must be BNM_FLOAT16 (1) or BNM_BFLOAT16 (2)", format);
+    if (n == 0 || elems == 0) return 0;
+    if (!images || !out) return fail(BNM_E_ARG, "bnm_quantize_images_device_f16: null argument");
+    launch_quantize_images(images, static_cast<HalfFormat>(format), elems, out, n, static_cast<cudaStream_t>(stream));
+    return launch_status();
+}
+
 extern "C" int bnm_quantize_images(const float *images, size_t n, uint32_t elems, int8_t *out) {
     if (int rc = require_device()) return rc;
     if (n == 0 || elems == 0) return 0;
@@ -1154,20 +1177,20 @@ int bnm::level_shift_of(int32_t enc) { return (enc == BNM_ENC_2BITSYM || enc == 
 // other model runs the C engine's float route and the emulator's route per pass, into the caller's label buffers or the call's
 // scratch, then k_engine_counts (run_engines).
 // -----------------------------------------------------------------------------------------------
-// the two engines' route r without a fused form on n float images on st (capture state cap) -> out: labels (the C engine's) and
-// engines
-static int run_engines(bnm_model *m, const Route &r, const float *images, size_t n, const FcOutputs &out, cudaStream_t st,
+// the two engines' route r without a fused form on n float images (of r's input kind) on st (capture state cap) -> out: labels
+// (the C engine's) and engines
+static int run_engines(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out, cudaStream_t st,
                        const StreamCapture &cap) {
     const EngineOutputs &e = out.engines;
-    const Route c_route = choose_route(m, kEngineC, true, false), py_route = choose_route(m, kEngineEmul, true, false);
-    const size_t chunk = std::min(n, r.pass), elems = m->img_bytes;
+    const Route c_route = choose_route(m, kEngineC, r.in, false), py_route = choose_route(m, kEngineEmul, r.in, false);
+    const size_t chunk = std::min(n, r.pass), row_bytes = m->img_bytes * in_elem_bytes(r.in);
     Scratch scratch(m->pool, st);
     uint32_t *own[2];   // C / emulator labels the caller does not take
     CU_TRY(scratch.get(&own[0], e.counts && !out.labels ? chunk : 0));
     CU_TRY(scratch.get(&own[1], e.counts && !e.labels_py ? chunk : 0));
     for (size_t b = 0; b < n; b += chunk) {
         const size_t nb = std::min(chunk, n - b);
-        const float *img = images + b * elems;
+        const void *img = static_cast<const char *>(images) + b * row_bytes;
         uint32_t *lc = out.labels ? out.labels + b : own[0];
         uint32_t *lp = e.labels_py ? e.labels_py + b : own[1];
         if (lc)
@@ -1187,7 +1210,8 @@ static int run_engines(bnm_model *m, const Route &r, const float *images, size_t
 struct Call {
     const char *name;   // the entry, for messages
     Engine engine;
-    bool f32, topk;     // float32 images in; the k best classes out
+    InKind in;
+    bool topk;          // the k best classes out
     const void *images;
     size_t n;
     FcOutputs out;      // the two engines' entry: the C engine's labels in labels, the rest in engines
@@ -1230,14 +1254,14 @@ static int run_call(bnm_model *m, const Call &c) {
     if (c.host && c.engine == kEngineC && !c.topk && c.n <= kSmallBatch && c.n <= m->chunk_images)   // sets the device where it launches
         return infer_small(m, static_cast<const int8_t *>(c.images), c.n, static_cast<int32_t *>(o.logits), o.labels);
     CU_TRY(cudaSetDevice(m->device));
-    const Route r = choose_route(m, c.engine, c.f32, c.topk, c.windows);
+    const Route r = choose_route(m, c.engine, c.in, c.topk, c.windows);
     if ((c.topk || c.windows) && m->verbose) print_route(m, (std::string(c.windows ? "windows route: " : "topk route: ") + c.name).c_str(), r);
     if (o.gather && !r.fused)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     cudaStream_t st = static_cast<cudaStream_t>(c.stream);
     if (c.host) return infer_pipelined(m, r, c.images, c.n, o);
     const StreamCapture cap = capture_of(st);
-    if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, static_cast<const float *>(c.images), c.n, o, st, cap);
+    if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, c.images, c.n, o, st, cap);
     return run_route(m, r, c.images, c.n, o, st, cap, c.windows);
 }
 
@@ -1250,7 +1274,7 @@ extern "C" int bnm_infer_batch_device_gather(bnm_model *m, const int8_t *images,
         for (uint32_t d = 0; d < gather->n_logits_dst; d++)
             if ((uintptr_t)gather->logits_dst[d] & 7) return fail(BNM_E_ARG, "gather logits buffers must be 8-byte aligned");
     const GatherDst *g = reinterpret_cast<const GatherDst *>(gather);
-    return run_call(m, {"bnm_infer_batch_device", kEngineC, false, false, images, n, {logits, labels, g}, {16, 8}, stream});
+    return run_call(m, {"bnm_infer_batch_device", kEngineC, kInI8, false, images, n, {logits, labels, g}, {16, 8}, stream});
 }
 
 extern "C" int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
@@ -1261,11 +1285,11 @@ extern "C" int bnm_infer_batch_device(bnm_model *m, const int8_t *images, size_t
 // input scaling fused into its load stage.  Everything else: per pass of 2^20 images the scaling kernel into the call's scratch,
 // then the int8 route on it.
 extern "C" int bnm_infer_batch_device_f32(bnm_model *m, const float *images, size_t n, int32_t *logits, uint32_t *labels, void *stream) {
-    return run_call(m, {"bnm_infer_batch_device_f32", kEngineC, true, false, images, n, {logits, labels}, {16, 8}, stream});
+    return run_call(m, {"bnm_infer_batch_device_f32", kEngineC, kInF32, false, images, n, {logits, labels}, {16, 8}, stream});
 }
 
 extern "C" int bnm_emulate_batch_device(bnm_model *m, const float *images, size_t n, double *logits, uint32_t *labels, void *stream) {
-    return run_call(m, {"bnm_emulate_batch_device", kEngineEmul, true, false, images, n, {logits, labels}, {16, 8}, stream});
+    return run_call(m, {"bnm_emulate_batch_device", kEngineEmul, kInF32, false, images, n, {logits, labels}, {16, 8}, stream});
 }
 
 extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, size_t n, const uint32_t *truth, uint32_t *labels_c,
@@ -1273,7 +1297,7 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
     static_assert(sizeof(bnm_engine_counts) == 4 * sizeof(unsigned long long), "bnm_engine_counts: four 64-bit counters");
     if (truth && !counts) return fail(BNM_E_ARG, "bnm_compare_engines_device: truth without counts");
     const FcOutputs out{nullptr, labels_c, nullptr, {}, {labels_py, truth, reinterpret_cast<unsigned long long *>(counts)}};
-    return run_call(m, {"bnm_compare_engines_device", kEngineBoth, true, false, images, n, out, {16, 1, 1, 1, 8}, stream, false, false,
+    return run_call(m, {"bnm_compare_engines_device", kEngineBoth, kInF32, false, images, n, out, {16, 1, 1, 1, 8}, stream, false, false,
                         true});   // no outputs: an error even at n == 0
 }
 
@@ -1286,15 +1310,15 @@ extern "C" int bnm_compare_engines_device(bnm_model *m, const float *images, siz
 // The float entry scales each pass of 2^20 images into its own scratch, then runs the int8 route on it; the emulator runs its own
 // front-end (scaling kernel or CNN front-end) into its scratch, then fc_topk_kernel with its rule.  choose_route picks the route.
 extern "C" int bnm_infer_topk_device(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
-    return run_call(m, {"bnm_infer_topk_device", kEngineC, false, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
+    return run_call(m, {"bnm_infer_topk_device", kEngineC, kInI8, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
 }
 
 extern "C" int bnm_infer_topk_device_f32(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
-    return run_call(m, {"bnm_infer_topk_device_f32", kEngineC, true, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
+    return run_call(m, {"bnm_infer_topk_device_f32", kEngineC, kInF32, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
 }
 
 extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n, uint32_t k, uint32_t *classes, double *scores, void *stream) {
-    return run_call(m, {"bnm_emulate_topk_device", kEngineEmul, true, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
+    return run_call(m, {"bnm_emulate_topk_device", kEngineEmul, kInF32, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
 }
 
 // Window scan (sections 9 and 10): every 16x16 window of a stack of float planes on a stride grid, classified as the entry named
@@ -1316,7 +1340,7 @@ static int run_windows(bnm_model *m, const bnm_windows *w, Call c) {
     const uint32_t out_w = w->width < 16 ? 0 : (w->width - 16) / w->stride_x + 1;
     const WindowGrid g{w->image, w->planes, w->height, w->width, w->pitch, w->planes > 1 ? w->plane_pitch : 0,
                        w->stride_y, w->stride_x, out_h, out_w};
-    c.f32 = true;
+    c.in = kInF32;
     c.images = w->image;
     c.n = (size_t)w->planes * out_h * out_w;
     c.windows = &g;
@@ -1326,42 +1350,81 @@ static int run_windows(bnm_model *m, const bnm_windows *w, Call c) {
 extern "C" int bnm_infer_windows_device_f32(bnm_model *m, const float *image, uint32_t height, uint32_t width, size_t pitch,
                                             uint32_t stride_y, uint32_t stride_x, int32_t *logits, uint32_t *labels, void *stream) {
     const bnm_windows w{image, 1, height, width, pitch, 0, stride_y, stride_x};
-    return run_windows(m, &w, {"bnm_infer_windows_device_f32", kEngineC, true, false, image, 0, {logits, labels}, {16, 8}, stream});
+    return run_windows(m, &w, {"bnm_infer_windows_device_f32", kEngineC, kInF32, false, image, 0, {logits, labels}, {16, 8}, stream});
 }
 
 extern "C" int bnm_scan_windows_device(bnm_model *m, const bnm_windows *w, int32_t *logits, uint32_t *labels, void *stream) {
-    return run_windows(m, w, {"bnm_scan_windows_device", kEngineC, true, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
+    return run_windows(m, w, {"bnm_scan_windows_device", kEngineC, kInF32, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
 }
 
 extern "C" int bnm_scan_windows_topk_device(bnm_model *m, const bnm_windows *w, uint32_t k, uint32_t *classes, int32_t *scores,
                                             void *stream) {
-    return run_windows(m, w, {"bnm_scan_windows_topk_device", kEngineC, true, true, nullptr, 0, {nullptr, nullptr, nullptr, {k, classes, scores}},
+    return run_windows(m, w, {"bnm_scan_windows_topk_device", kEngineC, kInF32, true, nullptr, 0, {nullptr, nullptr, nullptr, {k, classes, scores}},
                               {16, 1, 4, 4}, stream});
 }
 
 extern "C" int bnm_emulate_windows_device(bnm_model *m, const bnm_windows *w, double *logits, uint32_t *labels, void *stream) {
-    return run_windows(m, w, {"bnm_emulate_windows_device", kEngineEmul, true, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
+    return run_windows(m, w, {"bnm_emulate_windows_device", kEngineEmul, kInF32, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
 }
 
 extern "C" int bnm_emulate_windows_topk_device(bnm_model *m, const bnm_windows *w, uint32_t k, uint32_t *classes, double *scores,
                                                void *stream) {
-    return run_windows(m, w, {"bnm_emulate_windows_topk_device", kEngineEmul, true, true, nullptr, 0,
+    return run_windows(m, w, {"bnm_emulate_windows_topk_device", kEngineEmul, kInF32, true, nullptr, 0,
                               {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
+}
+
+// 16-bit float images (section 11): call c of the float32 sibling, its input kind the one of `format` (BNM_E_ARG for any other
+// value, whatever n).  Its route is the sibling's (choose_route) and every output is the sibling's on the images widened to float32.
+static int run_half(bnm_model *m, int format, Call c) {
+    if (format != BNM_FLOAT16 && format != BNM_BFLOAT16)
+        return fail(BNM_E_ARG, "%s: format %d, must be BNM_FLOAT16 (1) or BNM_BFLOAT16 (2)", c.name, format);
+    c.in = format == BNM_BFLOAT16 ? kInBF16 : kInF16;
+    return run_call(m, c);
+}
+
+extern "C" int bnm_infer_batch_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, int32_t *logits, uint32_t *labels,
+                                          void *stream) {
+    return run_half(m, format, {"bnm_infer_batch_device_f16", kEngineC, kInF16, false, images, n, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_emulate_batch_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, double *logits, uint32_t *labels,
+                                            void *stream) {
+    return run_half(m, format, {"bnm_emulate_batch_device_f16", kEngineEmul, kInF16, false, images, n, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_compare_engines_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, const uint32_t *truth,
+                                              uint32_t *labels_c, uint32_t *labels_py, bnm_engine_counts *counts, void *stream) {
+    if (truth && !counts) return fail(BNM_E_ARG, "bnm_compare_engines_device_f16: truth without counts");
+    const FcOutputs out{nullptr, labels_c, nullptr, {}, {labels_py, truth, reinterpret_cast<unsigned long long *>(counts)}};
+    return run_half(m, format, {"bnm_compare_engines_device_f16", kEngineBoth, kInF16, false, images, n, out, {16, 1, 1, 1, 8}, stream,
+                                false, false, true});   // no outputs: an error even at n == 0
+}
+
+extern "C" int bnm_infer_topk_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, uint32_t k, uint32_t *classes,
+                                         int32_t *scores, void *stream) {
+    return run_half(m, format, {"bnm_infer_topk_device_f16", kEngineC, kInF16, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}},
+                                {16, 1, 4, 4}, stream});
+}
+
+extern "C" int bnm_emulate_topk_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, uint32_t k, uint32_t *classes,
+                                           double *scores, void *stream) {
+    return run_half(m, format, {"bnm_emulate_topk_device_f16", kEngineEmul, kInF16, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}},
+                                {16, 1, 4, 8}, stream});
 }
 
 // host buffers: n <= kSmallBatch images share a launch with concurrent small calls, larger batches run the chunked pipeline
 extern "C" int bnm_infer_batch(bnm_model *m, const int8_t *images, size_t n, int32_t *logits, uint32_t *labels) {
-    return run_call(m, {"bnm_infer_batch", kEngineC, false, false, images, n, {logits, labels}, {}, nullptr, true});   // host buffers
+    return run_call(m, {"bnm_infer_batch", kEngineC, kInI8, false, images, n, {logits, labels}, {}, nullptr, true});   // host buffers
 }
 
 // host buffers: the chunked pipeline of bnm_infer_batch, k classes (and k scores) per image copied back
 extern "C" int bnm_infer_topk(bnm_model *m, const int8_t *images, size_t n, uint32_t k, uint32_t *classes, int32_t *scores) {
-    return run_call(m, {"bnm_infer_topk", kEngineC, false, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {}, nullptr,
+    return run_call(m, {"bnm_infer_topk", kEngineC, kInI8, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {}, nullptr,
                         true});   // host buffers
 }
 
 extern "C" int bnm_emulate_inference_quantized(bnm_model *m, const float *images, size_t n, double *logits) {
-    return run_call(m, {"bnm_emulate_inference_quantized", kEngineEmul, true, false, images, n, {logits}, {}, nullptr, true,
+    return run_call(m, {"bnm_emulate_inference_quantized", kEngineEmul, kInF32, false, images, n, {logits}, {}, nullptr, true,
                         true});   // host buffers, logits required
 }
 

@@ -94,6 +94,8 @@ struct ChainParams {
     int32_t *scores_i32;
     double *scores_f64;
     uint32_t off_out;                 // fixed-shape launches: smem offset of the consumer warps' logits / labels staging buffers
+    // 16-bit float-input launches: fimages holds uint16 [n][in_elems], each element kHalfFloat16 (IEEE binary16) or kHalfBFloat16
+    uint32_t in_format;
 };
 
 struct ChainKernel;
@@ -243,6 +245,18 @@ __device__ __forceinline__ uint32_t norm_pack4(uint32_t x0, uint32_t x1, uint32_
     return __byte_perm(__byte_perm(emul_q(x0, c), emul_q(x1, c), 0x0040), __byte_perm(emul_q(x2, c), emul_q(x3, c), 0x0040), 0x5410);
 }
 
+// four 16-bit input elements (one 8-byte group of a row) widened exactly to float32: bfloat16 is the top half of a float32;
+// float16 converts with cvt.f32.f16, which is exact for every value (subnormals, infinities and NaN included)
+__device__ __forceinline__ float widen16(uint32_t h, bool bf16) {
+    if (bf16) return __uint_as_float(h << 16);
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"((unsigned short)h));
+    return f;
+}
+__device__ __forceinline__ float4 widen4(uint2 g, bool bf16) {
+    return make_float4(widen16(g.x & 0xffffu, bf16), widen16(g.x >> 16, bf16), widen16(g.y & 0xffffu, bf16), widen16(g.y >> 16, bf16));
+}
+
 // ---------------------------------------------------------------------------------------------------
 // phase trace (diagnostics build only: make -C bitnetmcu_b200/csrc EXTRA=-DBNM_FC_TRACE; tools/fc_phase_trace.py reads it).
 // In the first kTraceCtas CTAs, lane 0 of warp 0 of every consumer warpgroup (writer cw) and the producer warp (writer
@@ -284,7 +298,7 @@ __device__ __forceinline__ unsigned long long globaltimer() {
 //     of its pipe at once (slots A and B, each with its own accumulators and fragments) and alternates between them, so that the
 //     MMAs of one slot are in flight while the warpgroup runs the ReLUNorm or the epilogue of the other.
 //   * one producer warp: barrier setup, the weight copy, and (int8 input) the TMA image loads of every pipe in tile order.
-//   * kFloatIn: eight quantiser warps in place of the TMA loads (see below).
+//   * float input (kInBytes 4 or 2): eight quantiser warps in place of the TMA loads (see below).
 // Barriers: full[stage] (tile landed: TMA bytes, or the eight quantiser warps), empty[stage] (the eight consumer warps of the pipe
 // have finished reading the stage).  Every consumer and the producer visit the stages of their pipe in order, so every parity
 // wait starts after the barrier's previous phase has completed: one full and one empty barrier per stage suffice.  Two slots keep
@@ -344,8 +358,11 @@ struct RingPos {
 // one unrolled run of MMAs at compile-time descriptor offsets, ReLUNorm without predicates.
 // kRule, kOut: the rule and the outputs of the launch form (the form table, host side below).
 // The body of the kernels below; tmap_in and P are their __grid_constant__ parameters (TMA reads the tensor map by address).
-template <int kN, int kPipes, bool kFloatIn, int kSlots, int kLastN, bool kFixed, FcRule kRule, FcOut kOut>
+// kInBytes: bytes per input element -- 1: int8 rows over TMA; 4: float32 rows, 2: float16 or bfloat16 rows (P.in_format), both
+// through the quantiser warps.
+template <int kN, int kPipes, int kInBytes, int kSlots, int kLastN, bool kFixed, FcRule kRule, FcOut kOut>
 __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const ChainParams &P) {
+    constexpr bool kFloatIn = kInBytes > 1;
     static_assert(kSlots == 1 || (kSlots == 2 && kN == 64 && kPipes == 2 && !kFloatIn), "two slots: 64-wide int8 two-pipe launches");
     static_assert((kRule == kRuleC && kOut == kOutLogits) || (kPipes == 1 && kSlots == 1 && kLastN == kN && !kFixed),
                   "the emulator, both engines and top-k: one-pipe one-slot launches at full width");
@@ -909,9 +926,12 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
         // its SWIZZLE_128B layout -- the place of the TMA load.
         if (P.wait_prior_grid) asm volatile("griddepcontrol.wait;" ::: "memory");
         const uint32_t qw = warp - prod_warp - 1;
+        const bool bf16 = kInBytes == 2 && P.in_format == kHalfBFloat16;
         const uint32_t elems = P.in_elems, n_f4 = elems >> 2, row_words = P.in_atoms * 32;   // float4 per float row, 4-byte words per int8 row
-        const float *src = P.fimages;
-        uint8_t *ring = smem + P.off_fring + qw * (2 * kFloatGroupRows * 1024);
+        using InElem = std::conditional_t<kInBytes == 4, float, uint16_t>;
+        constexpr uint32_t kSlotBytes = kFloatGroupRows * 256 * kInBytes;   // a ring slot: four rows of up to 256 elements
+        const InElem *src = reinterpret_cast<const InElem *>(P.fimages);
+        uint8_t *ring = smem + P.off_fring + qw * (2 * kSlotBytes);
         uint64_t *fbar = &bar_fload[qw][0];
         constexpr uint32_t kGroupsPerTile = kFloatRowsPerWarp / kFloatGroupRows;
         const uint32_t n_groups = my_tiles * kGroupsPerTile;   // groups of rows of this warp, in order
@@ -924,8 +944,8 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
             size_t row;
             const uint32_t valid = group_rows(gi, row);
             if (lane == 0 && valid) {
-                mbar_arrive_expect_tx(&fbar[gi & 1], valid * elems * 4);
-                bulk_load_1d(ring + (gi & 1) * (kFloatGroupRows * 1024), src + row * elems, valid * elems * 4, &fbar[gi & 1]);
+                mbar_arrive_expect_tx(&fbar[gi & 1], valid * elems * kInBytes);
+                bulk_load_1d(ring + (gi & 1) * kSlotBytes, src + row * elems, valid * elems * kInBytes, &fbar[gi & 1]);
             }
         };
         const uint32_t u = lane >> 3, sub = lane & 7;   // row of the pass, position inside the row's eight-lane team
@@ -945,14 +965,17 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                 mbar_wait(&fbar[slot], (fphase >> slot) & 1, P.err, 9);
                 fphase ^= 1u << slot;
             }
-            const float4 *fr = reinterpret_cast<const float4 *>(ring + slot * (kFloatGroupRows * 1024)) + u * n_f4;
+            // a lane's element group c: four floats (one float4), or four 16-bit elements (one uint2) widened exactly to float32
+            const float4 *fr = reinterpret_cast<const float4 *>(ring + slot * kSlotBytes) + u * n_f4;
+            const uint2 *hr = reinterpret_cast<const uint2 *>(ring + slot * kSlotBytes) + u * n_f4;
             const uint32_t r = qw * kFloatRowsPerWarp + k * kFloatGroupRows + u;   // this lane's row inside the tile
             float4 v[8];
             float m = 0.f;
 #pragma unroll
             for (int j = 0; j < 8; j++) {
                 const uint32_t c = sub + 8 * ((j + u) & 7);
-                v[j] = (u < valid && c < n_f4) ? fr[c] : make_float4(0.f, 0.f, 0.f, 0.f);
+                if constexpr (kInBytes == 4) v[j] = (u < valid && c < n_f4) ? fr[c] : make_float4(0.f, 0.f, 0.f, 0.f);
+                else v[j] = widen4((u < valid && c < n_f4) ? hr[c] : make_uint2(0u, 0u), bf16);
                 m = fmaxf(m, fmaxf(fmaxf(fabsf(v[j].x), fabsf(v[j].y)), fmaxf(fabsf(v[j].z), fabsf(v[j].w))));
             }
             m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
@@ -984,14 +1007,29 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
 template <int kN, int kPipes, bool kFloatIn, int kSlots = 1, int kLastN = kN, bool kFixed = false>
 __global__ void __launch_bounds__(chain_threads<kN, kPipes, kFloatIn, kSlots>(), 1)
 fc_chain_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<kN, kPipes, kFloatIn, kSlots, kLastN, kFixed, kRuleC, kOutLogits>(tmap_in, P);
+    fc_chain_body<kN, kPipes, kFloatIn ? 4 : 1, kSlots, kLastN, kFixed, kRuleC, kOutLogits>(tmap_in, P);
+}
+
+// The three float-input launches on 16-bit rows (float16 or bfloat16, P.in_format): the C engine, the emulator and both engines,
+// each what its float32 kernel computes on the rows widened to float32.  Half the bytes per row of the float32 kernels.
+__global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
+fc_chain_h16_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<64, 1, 2, 1, 64, false, kRuleC, kOutLogits>(tmap_in, P);
+}
+__global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
+fc_emul_h16_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<64, 1, 2, 1, 64, false, kRuleEmul, kOutLogits>(tmap_in, P);
+}
+__global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
+fc_engines_h16_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
+    fc_chain_body<64, 1, 2, 1, 64, false, kRuleBoth, kOutEngines>(tmap_in, P);
 }
 
 // QuantizedModel.inference_quantized (BitNetMCU.py:420-535) of FC models: the float-input launch <64,1,float> with the emulator's
 // hidden-layer rule and float64 logits.  The input scaling of BitNetMCU.py:435-436 is the quantiser warps' (test_inference.py:140-141).
 __global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
 fc_emul_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<64, 1, true, 1, 64, false, kRuleEmul, kOutLogits>(tmap_in, P);
+    fc_chain_body<64, 1, 4, 1, 64, false, kRuleEmul, kOutLogits>(tmap_in, P);
 }
 
 // The same emulator on int8 rows that are already scaled (k_quantize_images, or the features of k_cnn_emul_frontend): TMA
@@ -999,14 +1037,14 @@ fc_emul_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constan
 template <int kN>
 __global__ void __launch_bounds__(chain_threads<kN, 1, false, 1>(), 1)
 fc_emul_i8_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<kN, 1, false, 1, kN, false, kRuleEmul, kOutLogits>(tmap_in, P);
+    fc_chain_body<kN, 1, 1, 1, kN, false, kRuleEmul, kOutLogits>(tmap_in, P);
 }
 
 // The reference's check of its two engines (test_inference.py:130-175) in one pass: the float-input launch <64,1,float> that
 // runs the C engine's chain and the emulator's after one shared layer 1, and writes both labels and their counts.
 __global__ void __launch_bounds__(chain_threads<64, 1, true, 1>(), 1)
 fc_engines_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<64, 1, true, 1, 64, false, kRuleBoth, kOutEngines>(tmap_in, P);
+    fc_chain_body<64, 1, 4, 1, 64, false, kRuleBoth, kOutEngines>(tmap_in, P);
 }
 
 // Top-k on int8 rows: the chain of fc_chain_kernel (kEmul false) or of fc_emul_i8_kernel (true) on one pipe and one slot at the
@@ -1014,7 +1052,7 @@ fc_engines_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
 template <int kN, bool kEmul>
 __global__ void __launch_bounds__(chain_threads<kN, 1, false, 1>(), 1)
 fc_topk_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ ChainParams P) {
-    fc_chain_body<kN, 1, false, 1, kN, false, kEmul ? kRuleEmul : kRuleC, kOutTopK>(tmap_in, P);
+    fc_chain_body<kN, 1, 1, 1, kN, false, kEmul ? kRuleEmul : kRuleC, kOutTopK>(tmap_in, P);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1074,36 +1112,42 @@ static constexpr ChainKernel row(const char *name, void (*fn)(CUtensorMap, Chain
 
 // The launch forms, indexed by FcForm.  A launch takes everything but its buffers from its form's entry.
 struct FormSpec {
-    bool float_in;           // float32 rows through the quantiser warps, else int8 rows over TMA
+    uint32_t in_bytes;       // bytes per input element: 1 int8 rows over TMA; 4 float32, 2 float16 / bfloat16 rows through the
+                             // quantiser warps
     FcRule rule;
     FcOut out;               // kOutLogits: the C engine on int8 rows alone also takes result-exchange destinations
     uint32_t stage_cap;      // stages per pipe at most
     ChainKernel rows[4];     // by accumulator width 64, 128, 192, 256; fn null: the form has no row at that width
 };
-// The float-input forms have a 64-wide row only: the eight quantiser warps make 17 warps, so at most 96 registers per thread.
+// The float-input forms (float32 and 16-bit) have a 64-wide row only: the eight quantiser warps make 17 warps, so at most 96
+// registers per thread.
 static const FormSpec kForms[kFcForms] = {
     // kFormInt8; a 64-wide plan with room for two pipes takes one of kTwoPipeRows instead of the one-pipe row
-    {false, kRuleC, kOutLogits, 6,
+    {1, kRuleC, kOutLogits, 6,
      {row<64>("fc_chain_kernel<64,1>", fc_chain_kernel<64, 1, false>), row<128>("fc_chain_kernel<128,1>", fc_chain_kernel<128, 1, false>),
       row<192>("fc_chain_kernel<192,1>", fc_chain_kernel<192, 1, false>), row<256>("fc_chain_kernel<256,1>", fc_chain_kernel<256, 1, false>)}},
     // kFormFloat
-    {true, kRuleC, kOutLogits, 4, {row<64, 1, true>("fc_chain_kernel<64,1,float>", fc_chain_kernel<64, 1, true>)}},
+    {4, kRuleC, kOutLogits, 4, {row<64, 1, true>("fc_chain_kernel<64,1,float>", fc_chain_kernel<64, 1, true>)}},
     // kFormEmulFloat
-    {true, kRuleEmul, kOutLogits, 4, {row<64, 1, true>("fc_emul_kernel<64,1,float,emul>", fc_emul_kernel)}},
+    {4, kRuleEmul, kOutLogits, 4, {row<64, 1, true>("fc_emul_kernel<64,1,float,emul>", fc_emul_kernel)}},
     // kFormEmulInt8
-    {false, kRuleEmul, kOutLogits, 6,
+    {1, kRuleEmul, kOutLogits, 6,
      {row<64>("fc_emul_i8_kernel<64,1,emul>", fc_emul_i8_kernel<64>), row<128>("fc_emul_i8_kernel<128,1,emul>", fc_emul_i8_kernel<128>),
       row<192>("fc_emul_i8_kernel<192,1,emul>", fc_emul_i8_kernel<192>), row<256>("fc_emul_i8_kernel<256,1,emul>", fc_emul_i8_kernel<256>)}},
     // kFormEngines
-    {true, kRuleBoth, kOutEngines, 4, {row<64, 1, true>("fc_engines_kernel<64,1,float,engines>", fc_engines_kernel)}},
+    {4, kRuleBoth, kOutEngines, 4, {row<64, 1, true>("fc_engines_kernel<64,1,float,engines>", fc_engines_kernel)}},
     // kFormTopK
-    {false, kRuleC, kOutTopK, 6,
+    {1, kRuleC, kOutTopK, 6,
      {row<64>("fc_topk_kernel<64,1,topk>", fc_topk_kernel<64, false>), row<128>("fc_topk_kernel<128,1,topk>", fc_topk_kernel<128, false>),
       row<192>("fc_topk_kernel<192,1,topk>", fc_topk_kernel<192, false>), row<256>("fc_topk_kernel<256,1,topk>", fc_topk_kernel<256, false>)}},
     // kFormEmulTopK
-    {false, kRuleEmul, kOutTopK, 6,
+    {1, kRuleEmul, kOutTopK, 6,
      {row<64>("fc_topk_kernel<64,1,emul,topk>", fc_topk_kernel<64, true>), row<128>("fc_topk_kernel<128,1,emul,topk>", fc_topk_kernel<128, true>),
       row<192>("fc_topk_kernel<192,1,emul,topk>", fc_topk_kernel<192, true>), row<256>("fc_topk_kernel<256,1,emul,topk>", fc_topk_kernel<256, true>)}},
+    // kFormFloat16, kFormEmulFloat16, kFormEngines16: the three float-input forms on 16-bit rows
+    {2, kRuleC, kOutLogits, 4, {row<64, 1, true>("fc_chain_h16_kernel<64,1,16bit>", fc_chain_h16_kernel)}},
+    {2, kRuleEmul, kOutLogits, 4, {row<64, 1, true>("fc_emul_h16_kernel<64,1,16bit,emul>", fc_emul_h16_kernel)}},
+    {2, kRuleBoth, kOutEngines, 4, {row<64, 1, true>("fc_engines_h16_kernel<64,1,16bit,engines>", fc_engines_h16_kernel)}},
 };
 // kFormInt8's two-pipe two-slot rows: the last layer at full width, 16 wide (kLastN, for heads of at most 16 classes), or the
 // fixed-shape kernel with its logits staging buffers
@@ -1156,20 +1200,21 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
     bool fixed = pipes == 2 && last16 && n_layers == kFixedLayers && p.in_atoms == kFixedInAtoms;
     for (int l = 0; l < n_layers && fixed; l++)
         fixed = p.planes[l] == 1 && p.n_pad[l] == fixed_n_pad(l) && p.k_steps[l] == fixed_k_steps(l) && p.b_off[l] == fixed_b_off(l);
-    // the float-input forms (one pipe, fewer int8 stages) hold the quantiser warps' float rings in the shared memory they free:
-    // rows of at most 256 elements and at most 16 classes
-    const uint32_t fring = kFloatQuantWarps * 2 * kFloatGroupRows * 1024;
-    const bool float_fits = in_bytes <= 256 && p.n_classes <= 16 && w_fixed + fring + 2 * p.stage_bytes <= smem_limit;
+    // the float-input forms (one pipe, fewer int8 stages) hold the quantiser warps' rings in the shared memory they free: rows of
+    // at most 256 elements and at most 16 classes.  A plan has the 16-bit forms exactly where it has the float32 ones (whose
+    // rings, twice as large, decide), so a 16-bit call always takes its float32 sibling's route.
+    auto fring = [](const FormSpec &s) { return kFloatQuantWarps * 2 * kFloatGroupRows * 256 * s.in_bytes; };
+    const bool float_fits = in_bytes <= 256 && p.n_classes <= 16 && w_fixed + fring(kForms[kFormFloat]) + 2 * p.stage_bytes <= smem_limit;
     // the layout of a form's row: np rings of stages in what the weight image and `extra` bytes (the float rings, or the
     // fixed-shape row's staging buffers) leave, at most kMaxStages over the pipes (>= 2 per pipe with two: two tile slots need
     // it), then the weights, then the extra bytes.  The fixed-shape row's 17 kB of staging leave two stages per pipe, not three.
     auto layout = [&](const FormSpec &s, const ChainKernel *k, uint32_t np) {
         FormLayout l;
-        const uint32_t extra = s.float_in ? fring : k->out_bytes;
+        const uint32_t extra = s.in_bytes > 1 ? fring(s) : k->out_bytes;
         l.kernel = k;
         l.n_stages = std::min({s.stage_cap, kMaxStages / np, (smem_limit - w_fixed - extra) / p.stage_bytes / np});
         l.off_w = np * l.n_stages * p.stage_bytes;
-        l.off_fring = s.float_in ? l.off_w + w_fixed : 0;
+        l.off_fring = s.in_bytes > 1 ? l.off_w + w_fixed : 0;
         l.off_out = k->out_bytes ? l.off_w + w_fixed : 0;
         // One CTA per SM is part of the launch-overlap contract (launch k+2 must never run next to launch k on an SM): shared
         // memory enforces it once a CTA asks for more than half of the SM's 227 kB.
@@ -1181,7 +1226,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
         const FormSpec &s = kForms[f];
         const uint32_t np = f == kFormInt8 ? pipes : 1;
         const ChainKernel *k = np == 2 ? &kTwoPipeRows[fixed ? 2 : last16 ? 1 : 0] : &s.rows[max_n / 64 - 1];
-        if (!k->fn || (s.float_in && !float_fits)) continue;
+        if (!k->fn || (s.in_bytes > 1 && !float_fits)) continue;
         forms[f] = layout(s, k, np);
     }
     if (fixed) plan->int8_general = layout(kForms[kFormInt8], &kTwoPipeRows[1], pipes);
@@ -1286,7 +1331,7 @@ static bool programmatic_capture() {
 }
 
 int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap,
-                    bool fed) {
+                    bool fed, uint32_t in_format) {
     if (n == 0) return 0;
     if (n > 0x7fffff00ull) return -2;
     if (!plan->forms[f].kernel) return -6;
@@ -1298,12 +1343,13 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
     const FormLayout &form = plan->forms[f].kernel->out_bytes && !bulk_out ? plan->int8_general : plan->forms[f];
     const FormSpec &s = kForms[f];
     // the C engine on int8 rows: the one form with result-exchange destinations and overlapping launches
-    const bool engine_i8 = !s.float_in && s.rule == kRuleC && s.out == kOutLogits;
+    const bool engine_i8 = s.in_bytes == 1 && s.rule == kRuleC && s.out == kOutLogits;
     const EngineOutputs &e = out.engines;
     const TopKOutputs &t = out.topk;
     if ((out.logits && s.out != kOutLogits) || (out.gather && !engine_i8) || ((e.labels_py || e.truth || e.counts) && s.out != kOutEngines) ||
         (s.out == kOutTopK) != (t.k != 0) || (t.k && (out.labels || !t.classes || t.k > plan->p.n_classes)))
         return -5;
+    if ((s.in_bytes == 2) != (in_format == kHalfFloat16 || in_format == kHalfBFloat16)) return -5;
     ChainParams p = plan->p;   // the model's shapes and the emulator's logit scale; null outputs, no result exchange
     p.n_stages = form.n_stages;
     p.off_w = form.off_w;
@@ -1338,9 +1384,10 @@ int fc_chain_launch(FcChainPlan *plan, FcForm f, const void *in, size_t n, const
     // launch has copied it, and "the previous launch" of mode 2 is the previous launch enqueued on this plan, from any thread.
     std::lock_guard<std::mutex> lock(plan->mu);
     const CUtensorMap *tmap_p = &kNoTensorMap;
-    if (s.float_in) {
-        p.fimages = static_cast<const float *>(in);
+    if (s.in_bytes > 1) {
+        p.fimages = static_cast<const float *>(in);   // 16-bit forms: the kernel reads uint16 elements (in_format)
         p.in_elems = plan->in_bytes;
+        p.in_format = in_format;
     } else if (!(tmap_p = plan_tensor_map(plan, static_cast<const int8_t *>(in), n))) {
         return -3;
     }

@@ -276,6 +276,35 @@ void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t
     k_quantize_images<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(in, elems, out, n);
 }
 
+// The same scaling on 16-bit elements of format kFmt: each element widened exactly to float32 (bfloat16: the top half of a
+// float32; float16: cvt.f32.f16), then the float32 kernel's steps, row maximum in float32 included.  Any row length.
+template <HalfFormat kFmt> __device__ __forceinline__ float widen_half(uint16_t h) {
+    if (kFmt == kHalfBFloat16) return __uint_as_float((uint32_t)h << 16);
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
+    return f;
+}
+template <HalfFormat kFmt>
+__global__ void __launch_bounds__(256) k_quantize_images(const uint16_t *__restrict__ in, uint32_t elems, int8_t *__restrict__ out, size_t n) {
+    const uint32_t lane = threadIdx.x & 31;
+    const size_t img = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (img >= n) return;
+    const uint16_t *x = in + img * elems;
+    float m = 0.0f;
+    for (uint32_t i = lane; i < elems; i += 32) m = fmaxf(m, fabsf(widen_half<kFmt>(x[i])));
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+    const float scale = quant_scale(m);
+    int8_t *q = out + img * elems;
+    for (uint32_t i = lane; i < elems; i += 32) q[i] = (int8_t)quant_pixel(widen_half<kFmt>(x[i]), scale);
+}
+
+void launch_quantize_images(const uint16_t *in, HalfFormat fmt, uint32_t elems, int8_t *out, size_t n, cudaStream_t st) {
+    if (n == 0 || elems == 0) return;
+    if (fmt == kHalfBFloat16) k_quantize_images<kHalfBFloat16><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(in, elems, out, n);
+    else k_quantize_images<kHalfFloat16><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(in, elems, out, n);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Window scan (bnm_infer_windows_device_f32, bnm_scan_windows_device and the other stacked entries): the 16x16 windows of a stack
 // of float32 planes, each scaled as k_quantize_images scales an image, into int8 rows [n][256].  The window rows of the stack are

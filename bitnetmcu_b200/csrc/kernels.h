@@ -84,8 +84,13 @@ void launch_emul_logits(const int32_t *acc, uint32_t n_cls, int level_shift, dou
 void launch_topk_rows(const int32_t *rows, uint32_t n_cls, uint32_t k, uint32_t *classes, int32_t *scores, size_t n, cudaStream_t st);
 void launch_topk_rows(const double *rows, uint32_t n_cls, uint32_t k, uint32_t *classes, double *scores, size_t n, cudaStream_t st);
 
+// 16-bit float image elements (BNM_FLOAT16 / BNM_BFLOAT16 of the header)
+enum HalfFormat : uint32_t { kHalfFloat16 = 1, kHalfBFloat16 = 2 };
+
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
+// the same on 16-bit elements of format fmt [n][elems]: what the float32 kernel gives on them widened to float32
+void launch_quantize_images(const uint16_t *in, HalfFormat fmt, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 
 // The 16x16 windows of a stack of float32 planes (sections 9 and 10 of the header): plane p is image + p * plane_pitch, [height][pitch]
 // on the device (16-byte aligned, pitch and plane_pitch multiples of 4), its windows on an (stride_y, stride_x) grid of out_h x
@@ -136,7 +141,10 @@ void fc_chain_plan_set_overlap(FcChainPlan *p, int mode);
 // into the load stage), its rule (the C engine's, the reference's Python emulator's, or both), its outputs and its kernel rows.
 // A plan has every int8 form; the float-input forms only for models up to 64 wide with rows of up to 256 elements and up to
 // 16 classes.  The emulator's logits are the last layer's accumulators x 2^-level_shift_of(its encoding), in float64.
-enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFormEngines, kFormTopK, kFormEmulTopK, kFcForms };
+// kFormFloat16, kFormEmulFloat16 and kFormEngines16 are kFormFloat, kFormEmulFloat and kFormEngines on 16-bit rows (HalfFormat):
+// a plan has them exactly where it has those, and each gives what its float32 form gives on the rows widened to float32.
+enum FcForm { kFormInt8, kFormFloat, kFormEmulFloat, kFormEmulInt8, kFormEngines, kFormTopK, kFormEmulTopK,
+              kFormFloat16, kFormEmulFloat16, kFormEngines16, kFcForms };
 bool fc_chain_has_form(const FcChainPlan *p, FcForm f);
 // the kernel of a form the plan has, e.g. "fc_emul_i8_kernel<192,1,emul>"
 const char *fc_chain_form_name(const FcChainPlan *p, FcForm f);
@@ -176,9 +184,10 @@ struct StreamCapture {
 // one launch of form f on n images `in` -> out on st, whose capture state is cap.  0, or a negative code (-5: an output the form
 // does not take, or a missing one; -6: the plan has no form f).  fed: `in` was written by a kernel of another kind that the same
 // call launched just before into its scratch (k_quantize_windows, k_quantize_images, a CNN front-end); the launch keeps its grid-dependency wait and, as a launch of
-// another kind, leaves the launch-overlap record empty, so the next int8 launch keeps its wait too.
+// another kind, leaves the launch-overlap record empty, so the next int8 launch keeps its wait too.  in_format: the HalfFormat of
+// a 16-bit form's rows, 0 for every other form.
 int fc_chain_launch(FcChainPlan *p, FcForm f, const void *in, size_t n, const FcOutputs &out, cudaStream_t st, const StreamCapture &cap,
-                    bool fed = false);
+                    bool fed = false, uint32_t in_format = 0);
 // the emulator's CNN front-end (BitNetMCU.py:435-445, 459-526) in one kernel: float32 images [n][256] -> int8 features
 // [n][feat_stride], the (C, 2, 2) flatten; false when channels is 0 or more than kCnnEmulMaxChannels
 constexpr uint32_t kCnnEmulMaxChannels = 128;

@@ -28,6 +28,12 @@ def _ptr(a: Optional[np.ndarray]):
 N = "n"   # in the shape of a tensor argument of Engine._device_call: the number of images
 
 
+def _half_format(dtype) -> Optional[int]:
+    """The 16-bit format (include/bitnetmcu_b200.h section 11) of a torch dtype: FLOAT16, BFLOAT16, or None for float32"""
+    import torch
+    return {torch.float32: None, torch.float16: _lib.FLOAT16, torch.bfloat16: _lib.BFLOAT16}[dtype]
+
+
 def window_grid(height: int, width: int, stride) -> Tuple[int, int]:
     """(out_h, out_w) of the 16x16 windows of a height x width image on a stride grid without padding (include/bitnetmcu_b200.h
     section 9); stride is an int or (stride_y, stride_x), each >= 1.  (0, 0)-sized when the image is under 16 pixels either way."""
@@ -117,12 +123,18 @@ class Engine:
         self._device_call(self.lib.bnm_infer_batch_device, images, torch.int8,
                           [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)
 
-    def _device_call(self, fn, images, in_dtype, args, stream, lead=None) -> None:
+    def _float_call(self, fn, fn16, images, args, stream) -> None:
+        """fn on torch.float32 images, or its 16-bit sibling fn16 (section 11) with the tensor's format on torch.float16 or
+        torch.bfloat16 images: bit for bit what fn gives on ``images.float()``."""
+        fmt = _half_format(images.dtype)
+        self._device_call(fn if fmt is None else fn16, images, images.dtype, args, stream, fmt=fmt)
+
+    def _device_call(self, fn, images, in_dtype, args, stream, lead=None, fmt=None) -> None:
         """fn(handle, images, n, *args, stream) on this GPU, images a contiguous in_dtype [n, img_bytes] tensor.  A tensor argument
         is given as (tensor or None, its dtype or element size, its shape with N for n, or N alone for n elements of any shape):
         asserted contiguous and of that type and shape, it passes as its pointer, None as NULL.  Other arguments pass as they are.
         stream: a cudaStream_t as int, None for torch's current stream.  lead: instead of images and n, these arguments
-        (images is then an in_dtype tensor of any shape, N counts its elements)."""
+        (images is then an in_dtype tensor of any shape, N counts its elements).  fmt: a 16-bit entry's format, passed after images."""
         import torch
         if stream is None:
             stream = torch.cuda.current_stream(images.device).cuda_stream
@@ -138,7 +150,7 @@ class Engine:
                     assert t.numel() == n if shape is N else tuple(t.shape) == tuple(n if d is N else d for d in shape)
                 a = None if t is None else C.c_void_p(t.data_ptr())
             vals.append(a)
-        head = [C.c_void_p(images.data_ptr()), n] if lead is None else list(lead)
+        head = ([C.c_void_p(images.data_ptr()), n] if fmt is None else [C.c_void_p(images.data_ptr()), fmt, n]) if lead is None else list(lead)
         _lib.check(fn(self.handle, *head, *vals, C.c_void_p(stream)), fn.__name__)
 
     def inference_quantized(self, input_data: np.ndarray) -> np.ndarray:
@@ -153,18 +165,20 @@ class Engine:
     def inference_quantized_device(self, images, logits=None, labels=None, stream: Optional[int] = None) -> None:
         """``inference_quantized`` on device buffers: images torch.float32 [n, img_bytes] on this GPU -> logits torch.float64
         [n, n_classes] or None, labels [n] (4-byte elements: ``np.argmax`` of the logits) or None (not both None).  Asynchronous on
-        ``stream`` (a cudaStream_t as int; default: torch's current stream).  FC models up to 64 wide: one kernel."""
+        ``stream`` (a cudaStream_t as int; default: torch's current stream).  FC models up to 64 wide: one kernel.
+        torch.float16 / torch.bfloat16 images: what float32 gives on ``images.float()``, reading 2 bytes per pixel."""
         import torch
-        self._device_call(self.lib.bnm_emulate_batch_device, images, torch.float32,
-                          [(logits, torch.float64, (N, self.n_classes)), (labels, 4, N)], stream)
+        self._float_call(self.lib.bnm_emulate_batch_device, self.lib.bnm_emulate_batch_device_f16, images,
+                         [(logits, torch.float64, (N, self.n_classes)), (labels, 4, N)], stream)
 
     def infer_device_f32(self, images, logits, labels=None, stream: Optional[int] = None) -> None:
         """images: torch.float32 [n, img_bytes] on this GPU (un-normalised pixels, as test_inference.py:140 sees them) -> logits
         torch.int32 [n, n_classes] or None, labels [n] or None (not both None).  FC models: one kernel with the input scaling fused
-        into its load stage."""
+        into its load stage.  torch.float16 / torch.bfloat16 images: what float32 gives on ``images.float()``, reading 2 bytes per
+        pixel."""
         import torch
-        self._device_call(self.lib.bnm_infer_batch_device_f32, images, torch.float32,
-                          [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)
+        self._float_call(self.lib.bnm_infer_batch_device_f32, self.lib.bnm_infer_batch_device_f16, images,
+                         [(logits, torch.int32, (N, self.n_classes)), (labels, 4, N)], stream)
 
     def infer_windows_device(self, image, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
         """Window scan (include/bitnetmcu_b200.h section 9): every 16x16 window of image, a torch.float32 [height, width] plane on
@@ -235,10 +249,10 @@ class Engine:
         and counts, a torch.int64 [4] tensor (images, correct_c, correct_py, mismatches) that the call ADDS to.  truth: [n] true
         classes (4-byte elements), counted into correct_c / correct_py, and only with counts.  Any of labels_c, labels_py and
         counts may be None, not all three.  Asynchronous on ``stream`` (default: torch's current stream).  FC models up to 64
-        wide: one kernel."""
+        wide: one kernel.  torch.float16 / torch.bfloat16 images: what float32 gives on ``images.float()``."""
         import torch
-        self._device_call(self.lib.bnm_compare_engines_device, images, torch.float32,
-                          [(truth, 4, N), (labels_c, 4, N), (labels_py, 4, N), (counts, torch.int64, (4,))], stream)
+        self._float_call(self.lib.bnm_compare_engines_device, self.lib.bnm_compare_engines_device_f16, images,
+                         [(truth, 4, N), (labels_c, 4, N), (labels_py, 4, N), (counts, torch.int64, (4,))], stream)
 
     # ---- top-k: each image's k best classes and their scores (include/bitnetmcu_b200.h section 8) ------------------------------
     # Classes are ranked by logit, highest first, ties to the lower class: np.argsort(-logits, kind="stable")[:, :k].  Rank 0 is
@@ -261,17 +275,19 @@ class Engine:
                           [int(k), (classes, 4, (N, k)), (scores, torch.int32, (N, k))], stream)
 
     def topk_device_f32(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
-        """``topk_device`` on torch.float32 [n, img_bytes] images, scaled to int8 as ``infer_device_f32`` does."""
+        """``topk_device`` on torch.float32 [n, img_bytes] images, scaled to int8 as ``infer_device_f32`` does (torch.float16 /
+        torch.bfloat16 images: what float32 gives on ``images.float()``)."""
         import torch
-        self._device_call(self.lib.bnm_infer_topk_device_f32, images, torch.float32,
-                          [int(k), (classes, 4, (N, k)), (scores, torch.int32, (N, k))], stream)
+        self._float_call(self.lib.bnm_infer_topk_device_f32, self.lib.bnm_infer_topk_device_f16, images,
+                         [int(k), (classes, 4, (N, k)), (scores, torch.int32, (N, k))], stream)
 
     def emulate_topk_device(self, images, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
         """The emulator's top-k: images torch.float32 [n, img_bytes] -> classes [n, k] and scores torch.float64 [n, k] (the
-        logits ``inference_quantized_device`` writes, at those classes) or None."""
+        logits ``inference_quantized_device`` writes, at those classes) or None.  torch.float16 / torch.bfloat16 images: what
+        float32 gives on ``images.float()``."""
         import torch
-        self._device_call(self.lib.bnm_emulate_topk_device, images, torch.float32,
-                          [int(k), (classes, 4, (N, k)), (scores, torch.float64, (N, k))], stream)
+        self._float_call(self.lib.bnm_emulate_topk_device, self.lib.bnm_emulate_topk_device_f16, images,
+                         [int(k), (classes, 4, (N, k)), (scores, torch.float64, (N, k))], stream)
 
     def infer_tensor(self, images, want_logits: bool = True):
         """images: torch.int8 [n, img_bytes] on this engine's GPU -> (logits torch.int32 [n, n_classes], labels torch.int32 [n]) on
@@ -343,12 +359,15 @@ def quantize_images(images: np.ndarray) -> np.ndarray:
 
 def quantize_images_device(images, out, stream: Optional[int] = None) -> None:
     """Device-buffer form: images torch.float32 [n, elems] -> out torch.int8 [n, elems] on the same GPU, asynchronous on
-    ``stream`` (default: torch's current stream), so it chains with ``Engine.infer_device`` without a host pass."""
+    ``stream`` (default: torch's current stream), so it chains with ``Engine.infer_device`` without a host pass.
+    torch.float16 / torch.bfloat16 images: what float32 gives on ``images.float()``."""
     import torch
     lib = _lib.load()
-    assert images.is_contiguous() and out.is_contiguous() and images.dtype == torch.float32 and out.dtype == torch.int8
+    fmt = _half_format(images.dtype)
+    assert images.is_contiguous() and out.is_contiguous() and out.dtype == torch.int8
     assert images.dim() == 2 and tuple(out.shape) == tuple(images.shape)
     if stream is None:
         stream = torch.cuda.current_stream(images.device).cuda_stream
-    _lib.check(lib.bnm_quantize_images_device(C.c_void_p(images.data_ptr()), images.shape[0], images.shape[1],
-                                              C.c_void_p(out.data_ptr()), C.c_void_p(stream)), "bnm_quantize_images_device")
+    head = [C.c_void_p(images.data_ptr())] if fmt is None else [C.c_void_p(images.data_ptr()), fmt]
+    fn = lib.bnm_quantize_images_device if fmt is None else lib.bnm_quantize_images_device_f16
+    _lib.check(fn(*head, images.shape[0], images.shape[1], C.c_void_p(out.data_ptr()), C.c_void_p(stream)), fn.__name__)

@@ -19,6 +19,7 @@
  * Section 8 returns each image's k best classes and their scores (top-k) from either engine.
  * Section 9 classifies every 16x16 window of a larger float image on a stride grid (window scan).
  * Section 10 scans a stack of such images in one call, on either engine, with labels, logits or top-k.
+ * Section 11 takes float16 and bfloat16 images on the float device entries.
  *
  * Pointers are plain host (or, where the name says _device, CUDA device) pointers; sizes are element
  * counts unless named *_bytes.  All-integer arithmetic: results are bit-exact with the reference.
@@ -41,7 +42,9 @@
  *
  * Graphs.  Every device entry (bnm_infer_batch_device, _gather, _f32, bnm_emulate_batch_device, bnm_compare_engines_device, the
  * three top-k device entries, bnm_infer_windows_device_f32, the four stacked window entries bnm_scan_windows_device,
- * bnm_scan_windows_topk_device, bnm_emulate_windows_device and bnm_emulate_windows_topk_device, and bnm_quantize_images_device) may be captured into a CUDA graph on
+ * bnm_scan_windows_topk_device, bnm_emulate_windows_device and bnm_emulate_windows_topk_device, bnm_quantize_images_device, and the six
+ * 16-bit entries of section 11: bnm_infer_batch_device_f16, bnm_emulate_batch_device_f16, bnm_compare_engines_device_f16,
+ * bnm_infer_topk_device_f16, bnm_emulate_topk_device_f16 and bnm_quantize_images_device_f16) may be captured into a CUDA graph on
  * its stream, in any capture mode, in any combination and from any thread.  Each replay gives exactly the results of the same call made eagerly on the buffers'
  * contents at replay time; bnm_compare_engines_device adds to `counts` on every replay.  A graph keeps what its capture decided:
  * the route, the routing options (BNM_OPT_PATH, BNM_OPT_CHUNK_IMAGES, BNM_OPT_CNN_FRONTEND, BNM_OPT_LAUNCH_OVERLAP) and the
@@ -412,6 +415,41 @@ BNM_API int bnm_scan_windows_topk_device(bnm_model *m, const bnm_windows *window
 BNM_API int bnm_emulate_windows_device(bnm_model *m, const bnm_windows *windows, double *logits, uint32_t *labels, void *stream);
 BNM_API int bnm_emulate_windows_topk_device(bnm_model *m, const bnm_windows *windows, uint32_t k, uint32_t *classes, double *scores,
                                             void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 11. 16-bit float images: float16 or bfloat16 images, as torch.float16 / torch.bfloat16 tensors hold them, on the float device
+ *     entries, without a float32 copy.  The row is read at 2 bytes per element instead of 4.
+ * ------------------------------------------------------------------------------------------- */
+#define BNM_FLOAT16 1    /* IEEE 754 binary16                            */
+#define BNM_BFLOAT16 2   /* bfloat16: the top 16 bits of an IEEE float32 */
+/* Each entry below is the sibling named beside it, with `const uint16_t *images, int format` in place of `const float *images`:
+ *   bnm_infer_batch_device_f16        bnm_infer_batch_device_f32
+ *   bnm_emulate_batch_device_f16      bnm_emulate_batch_device
+ *   bnm_compare_engines_device_f16    bnm_compare_engines_device
+ *   bnm_infer_topk_device_f16         bnm_infer_topk_device_f32
+ *   bnm_emulate_topk_device_f16       bnm_emulate_topk_device
+ *   bnm_quantize_images_device_f16    bnm_quantize_images_device
+ * images: [n][img_bytes] (bnm_quantize_images_device_f16: [n][elems]) 16-bit elements of `format`, device memory.  Every output
+ * is bit for bit the sibling's output on the images widened to float32 (a conversion that is exact for every value: subnormals,
+ * infinities and NaN included).  A format other than BNM_FLOAT16 or BNM_BFLOAT16 returns BNM_E_ARG, whatever n.  Everything
+ * else is the sibling's: argument checks (NULL combinations, k), the 16-byte alignment of images and the other buffers'
+ * alignment, counts adding up across calls, per-call scratch and concurrency ("Threads"), capture into a CUDA graph ("Graphs"),
+ * and for BNM_OPT_LAUNCH_OVERLAP mode 2 a 16-bit call is a launch of another kind, like a float call.
+ * Routes: a 16-bit call takes its sibling's route.  Where that is one kernel with the input scaling fused (FC models on the fused
+ * path with rows of up to 256 elements, up to 64 wide and at most 16 classes), that kernel's 16-bit form reads the 16-bit rows;
+ * every other route scales each pass of 16-bit images into the call's scratch (k_quantize_images<float16> or <bfloat16>), then
+ * runs its int8 route on them.  Asynchronous on `stream`, no host synchronisation. */
+BNM_API int bnm_infer_batch_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, int32_t *logits, uint32_t *labels,
+                                       void *stream);
+BNM_API int bnm_emulate_batch_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, double *logits, uint32_t *labels,
+                                         void *stream);
+BNM_API int bnm_compare_engines_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, const uint32_t *truth,
+                                           uint32_t *labels_c, uint32_t *labels_py, bnm_engine_counts *counts, void *stream);
+BNM_API int bnm_infer_topk_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, uint32_t k, uint32_t *classes,
+                                      int32_t *scores, void *stream);
+BNM_API int bnm_emulate_topk_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, uint32_t k, uint32_t *classes,
+                                        double *scores, void *stream);
+BNM_API int bnm_quantize_images_device_f16(const uint16_t *images, int format, size_t n, uint32_t elems, int8_t *out, void *stream);
 
 #ifdef __cplusplus
 }
