@@ -136,6 +136,137 @@ def c_frontend(model, images):
     return Frontend(c1, c2, c3, raw, relunorm(raw))
 
 
+# ---- the fused FC plan (fc_chain_plan_create, fc_wgmma.cu) ------------------------------------------------------------------
+# The constants, each from the line of fc_wgmma.cu named beside it.  A wrong one shows on the GPU, where
+# test_plan_shapes.test_plan_line compares the restated plan line with the library's.
+
+SMEM_LIMIT = 227 * 1024 - 1024 - 1024          # :1192 an SM's 227 kB less the alignment slack and the static barriers
+MAX_STAGES = 8                                  # :36 kMaxStages, ring stages over all pipes of a CTA
+FLOAT_RING_BYTES = 8 * 2 * 4 * 256              # :1206 fring / element byte: kFloatQuantWarps (:38) x 2 slots x kFloatGroupRows (:40) x 256
+FIXED_OUT_BYTES = 2 * 8 * (16 * 16 * 4 + 16 * 4)  # :334-336 kFixedOutBytes, the fixed-shape row's logits staging
+MIN_SMEM = 116 * 1024                           # :1221 every form asks for more than half the SM: one CTA per SM
+FIXED_SHAPE = dict(in_atoms=2, n_pad=[64, 64, 64, 16], k_steps=[8, 2, 2, 2], b_off=[0, 16384, 20480, 24576])   # :327-331
+TWO_PIPE_ROWS = {"full": "fc_chain_kernel<64,2,2,64>", "last16": "fc_chain_kernel<64,2,2,16>",
+                 "fixed": "fc_chain_kernel<64,2,2,16,fixed>"}                                                   # :1154-1158
+
+
+class FormSpec(NamedTuple):
+    in_bytes: int           # bytes per input element: 1 int8 rows, 4 float32, 2 float16 / bfloat16
+    stage_cap: int          # stages per pipe at most
+    rows: dict              # accumulator width -> kernel row name (the float-input forms: 64 only)
+
+
+def _rows(fmt, widths=(64, 128, 192, 256)):
+    return {n: fmt % n for n in widths}
+
+
+FORMS = {   # :1124-1151 kForms, in FcForm order
+    "int8": FormSpec(1, 6, _rows("fc_chain_kernel<%d,1>")),
+    "float": FormSpec(4, 4, _rows("fc_chain_kernel<%d,1,float>", (64,))),
+    "emul_float": FormSpec(4, 4, _rows("fc_emul_kernel<%d,1,float,emul>", (64,))),
+    "emul_i8": FormSpec(1, 6, _rows("fc_emul_i8_kernel<%d,1,emul>")),
+    "engines": FormSpec(4, 4, _rows("fc_engines_kernel<%d,1,float,engines>", (64,))),
+    "topk": FormSpec(1, 6, _rows("fc_topk_kernel<%d,1,topk>")),
+    "emul_topk": FormSpec(1, 6, _rows("fc_topk_kernel<%d,1,emul,topk>")),
+    "float16": FormSpec(2, 4, _rows("fc_chain_h16_kernel<%d,1,16bit>", (64,))),
+    "emul_float16": FormSpec(2, 4, _rows("fc_emul_h16_kernel<%d,1,16bit,emul>", (64,))),
+    "engines16": FormSpec(2, 4, _rows("fc_engines_h16_kernel<%d,1,16bit,engines>", (64,))),
+}
+REFUSE_LAYERS = "fused path: 1..8 FC layers"
+REFUSE_ROW = "fused path: input row must be a multiple of 16 bytes, <= 1024"
+REFUSE_WIDE = "fused path: layer wider than 256 outputs"
+REFUSE_SMEM = "fused path: weights do not fit in shared memory"
+
+
+class Form(NamedTuple):
+    row: str                # the kernel row's name
+    stages: int             # per pipe
+    smem: int               # dynamic shared memory of a launch
+
+
+class Plan(NamedTuple):
+    in_atoms: int           # the input row in 128-byte atoms
+    n_pad: list             # per layer: outputs rounded up to 16
+    k_steps: list           # per layer: K-steps of 32 in the weight image
+    planes: list            # per layer: 2 where the layer holds a +128 weight (FP130), else 1
+    b_off: list             # per layer: byte offset of its first plane in the weight image
+    w_bytes: int            # the weight image, the zero tile behind the layers included
+    max_n: int              # the accumulator width: 64, 128, 192 or 256
+    pipes: int              # of the int8 C-engine form
+    two_pipe_row: str       # "fixed", "last16" or "full" with two pipes, else ""
+    float_fits: bool        # rows, classes and shared memory admit the float-input forms' rings
+    forms: dict             # form name -> Form, for the forms the plan has
+    logit_scale: float      # the emulator's logits: the last layer's accumulators times this
+
+    @property
+    def row(self):
+        """the int8 C-engine form's row, its template arguments only ("<64,2,2,16>")"""
+        return self.forms["int8"].row[self.forms["int8"].row.index("<"):]
+
+    @property
+    def float_forms(self):
+        return "float" in self.forms
+
+
+def _up(x, m):
+    return -(-x // m) * m
+
+
+def plan_of(model, nf4_extension=False):
+    """fc_chain_plan_create's shape rules on an FC model (img_bytes-byte rows): the Plan, or the refusal message"""
+    fc = model.fc_layers
+    in_bytes = model.img_bytes
+    if not 1 <= len(fc) <= 8:
+        return REFUSE_LAYERS
+    if in_bytes % 16 or in_bytes == 0 or in_bytes > 1024:
+        return REFUSE_ROW
+    n_pad = [_up(l.n_out, 16) for l in fc]
+    k_pad = [_up(max(l.n_in, 1), 32) for l in fc]
+    if max(n_pad) > 256:
+        return REFUSE_WIDE
+    in_atoms = -(-in_bytes // 128)
+    stage = in_atoms * 16384
+    # K of layer l > 0 stops at the previous layer's padded width: the activations past it are zero
+    k_steps = [4 * in_atoms] + [_up(min(k_pad[l], n_pad[l - 1]), 32) // 32 for l in range(1, len(fc))]
+    planes = [1 + int((P.decode_int_weights(l, nf4_extension) == 128).any()) for l in fc]
+    sizes = [p * k * n * 32 for p, k, n in zip(planes, k_steps, n_pad)]
+    b_off = [int(s) for s in np.cumsum([0] + sizes[:-1])]
+    max_n = _up(max(n_pad), 64)
+    w_bytes = sum(sizes) + max_n * 32
+    w_fixed = _up(w_bytes, 128)
+    if w_fixed + 2 * stage > SMEM_LIMIT:
+        return REFUSE_SMEM
+    pipes = 2 if max_n == 64 and (SMEM_LIMIT - w_fixed) // stage >= 4 else 1
+    last16 = n_pad[-1] <= 16
+    fixed = pipes == 2 and last16 and planes == [1] * len(fc) and \
+        dict(in_atoms=in_atoms, n_pad=n_pad, k_steps=k_steps, b_off=b_off) == FIXED_SHAPE
+    two_pipe_row = ("fixed" if fixed else "last16" if last16 else "full") if pipes == 2 else ""
+    float_fits = in_bytes <= 256 and fc[-1].n_out <= 16 and w_fixed + 4 * FLOAT_RING_BYTES + 2 * stage <= SMEM_LIMIT
+    forms = {}
+    for name, s in FORMS.items():
+        np_ = pipes if name == "int8" else 1
+        row = TWO_PIPE_ROWS[two_pipe_row] if np_ == 2 else s.rows.get(max_n)
+        if row is None or (s.in_bytes > 1 and not float_fits):
+            continue
+        extra = s.in_bytes * FLOAT_RING_BYTES if s.in_bytes > 1 else FIXED_OUT_BYTES if fixed and name == "int8" else 0
+        stages = min(s.stage_cap, MAX_STAGES // np_, (SMEM_LIMIT - w_fixed - extra) // stage // np_)
+        forms[name] = Form(row, stages, max(np_ * stages * stage + w_fixed + extra + 1024, MIN_SMEM))
+    return Plan(in_atoms, n_pad, k_steps, planes, b_off, w_bytes, max_n, pipes, two_pipe_row, float_fits, forms,
+                2.0 ** -LEVEL_SHIFT.get(fc[-1].bitperweight, 0))
+
+
+def plan_lines(plan):
+    """the two lines fc_chain_plan_create prints under BNM_VERBOSE (fc_wgmma.cu:1233-1246) for a Plan"""
+    f = plan.forms
+    i8 = f["int8"]
+    fl = (f", float input {f['float'].row[f['float'].row.index('<'):]}, emulator {f['emul_float'].row[f['emul_float'].row.index('<'):]}"
+          f", float input stages {f['float'].stages}") if plan.float_forms else ""
+    return (f"bitnetmcu_b200: fused FC plan: {plan.max_n} accumulator columns, {plan.pipes} pipes x {i8.stages} stages, "
+            f"{plan.w_bytes} weight bytes, {i8.smem} B smem, {i8.row}{fl}, int8 emulator {f['emul_i8'].row} x {f['emul_i8'].stages} stages",
+            f"bitnetmcu_b200: fused FC top-k forms: {f['topk'].row} x {f['topk'].stages} stages, emulator {f['emul_topk'].row} x "
+            f"{f['emul_topk'].stages} stages, {f['topk'].smem} B smem")
+
+
 # ---- the fused FC kernels' tile schedule (tests/test_fc_ring_rounds.py) -----------------------------------------------------
 
 class Schedule(NamedTuple):

@@ -152,6 +152,40 @@ def random_fc(enc, widths, seed):
     return m
 
 
+def with_plus128(codes, l):
+    """FP130 codes with +128 (code 7) in every third row: row o at column (5 o + l) % n_in"""
+    c = codes.copy()
+    o = np.arange(0, c.shape[0], 3)
+    c[o, (5 * o + l) % c.shape[1]] = 7
+    return c
+
+
+def fp130_codes(rng, n_out, n_in):
+    """random FP130 codes without +128; -128 (code 15) stays, it fits an int8 plane"""
+    c = rng.integers(0, 16, size=(n_out, n_in), dtype=np.uint32)
+    c[c == 7] = 15
+    return c
+
+
+def chain(img_bytes, layers, seed):
+    """a random FC model of img_bytes-byte rows; layers: (encoding, outputs), or (FP130, outputs, True) for +128 weights"""
+    from bitnetmcu_b200 import model as M, pack as P
+    rng = np.random.default_rng(seed)
+    out, n_in = [], img_bytes
+    for i, (enc, n_out, *plus) in enumerate(layers):
+        name = f"L{i + 1}"
+        if enc == M.ENC_TERNARY:
+            out.append(P.fc_layer_from_trits(name, rng.integers(-1, 2, size=(n_out, n_in))))
+        else:
+            codes = fp130_codes(rng, n_out, n_in) if enc == M.ENC_FP130 else \
+                rng.integers(0, 1 << P.CODE_BITS[enc], size=(n_out, n_in), dtype=np.uint32)
+            out.append(P.fc_layer_from_codes(name, enc, with_plus128(codes, i) if plus else codes))
+        n_in = n_out
+    m = M.Model(model_class=M.MODEL_FCMNIST, layers=out, img_bytes=img_bytes)
+    m.validate()
+    return m
+
+
 # every row of kChainKernels (fc_wgmma.cu), with a model that selects it (checked against the plan's BNM_VERBOSE line)
 CHAIN_ROWS = [
     ("<64,1>", lambda: random_fc(4, (512, 64, 64, 10), 1)),           # 512-byte rows: room for three 64 kB stages, one pipe
@@ -194,6 +228,16 @@ def cnn_model(channels, n_classes, seed, w=(None, None, None), hidden=(64,)):
 
 
 # ---- inputs -------------------------------------------------------------------------------------------------------------------
+
+def int8_images(n, d, seed):
+    """n int8 rows of d bytes: rows at the int8 rails, all zero, one value, then random rows"""
+    rng = np.random.default_rng(seed)
+    q = rng.integers(-128, 128, size=(n, d)).astype(np.int8)
+    rails = [np.full(d, 127), np.full(d, -128), np.zeros(d), np.where(np.arange(d) % 2, -128, 127),
+             np.where(rng.random(d) < 0.5, 127, -128), np.full(d, 1)]
+    q[:len(rails)] = np.stack(rails)
+    return q
+
 
 def normal_images(n, seed, elems=256):
     """normal float32 rows, the first 40 of them MNIST-normalised"""
@@ -266,6 +310,70 @@ def gather_call(lib, e, d_img, d_log, d_lab, g, stream):
                                                Ct.c_void_p(stream.cuda_stream))
         stream.synchronize()
     return rc
+
+
+# ---- device checks of one case's rows ------------------------------------------------------------------------------------
+# d: the case on the device -- d.name, d.C (classes), d.idx(n) (the rows of a batch of n) and d.check(n, got, want, sentinel,
+# what), which compares rows :n of an (n + 128)-row buffer with want[d.idx(n)] and the rows past n with the sentinel.
+
+def to_device(a):
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+
+def out(shape, dtype, sentinel):
+    """a device buffer of shape with 128 rows more, all sentinel"""
+    import torch
+    return torch.full((shape[0] + 128,) + tuple(shape[1:]), sentinel, dtype=dtype, device="cuda")
+
+
+def top_k(logits, k):
+    """the k best classes of each row and their scores: a stable sort, highest first, ties to the lower class"""
+    cls = np.argsort(-logits, axis=1, kind="stable")[:, :k]
+    return cls.astype(np.int32), np.take_along_axis(logits, cls, axis=1)
+
+
+
+def c_float(e, d, n, x, want_lo, want_la, what):
+    """the C engine's float entry (float32 or 16-bit rows x): logits and labels, then labels alone"""
+    import torch
+    lo, la = out((n, d.C), torch.int32, -5), out((n,), torch.int32, -7)
+    e.infer_device_f32(x, lo[:n], la[:n])
+    torch.cuda.synchronize()
+    d.check(n, lo, want_lo, -5, f"{what} logits")
+    d.check(n, la, want_la, -7, f"{what} labels")
+    la.fill_(-7)
+    e.infer_device_f32(x, None, la[:n])
+    torch.cuda.synchronize()
+    d.check(n, la, want_la, -7, f"{what} labels only")
+
+
+def emulator(e, d, n, x, want_lo, want_la, what):
+    """the emulator's entry: float64 logits and labels"""
+    import torch
+    lo, la = out((n, d.C), torch.float64, -12345.5), out((n,), torch.int32, -7)
+    e.inference_quantized_device(x, lo[:n], la[:n])
+    torch.cuda.synchronize()
+    d.check(n, lo, want_lo, -12345.5, f"{what} emulator logits")
+    d.check(n, la, want_la, -7, f"{what} emulator labels")
+
+
+def both_engines(e, d, n, x, want_la, want_py_la, what):
+    """bnm_compare_engines_device: the C labels, the emulator's labels where it is exact, and the counts"""
+    import torch
+    truth = ((torch.arange(n, device="cuda") * 7) % (d.C + 1)).to(torch.int32)
+    lc, lp = out((n,), torch.int32, -7), out((n,), torch.int32, -7)
+    counts = torch.zeros(4, dtype=torch.int64, device="cuda")
+    e.compare_engines_device(x, truth, lc[:n], lp[:n], counts)
+    torch.cuda.synchronize()
+    d.check(n, lc, want_la, -7, f"{what} engines: C labels")
+    wc = want_la[d.idx(n)]
+    got = counts.cpu().tolist()
+    assert got[:2] == [n, int((wc == truth).sum())], (d.name, n, what, "engines: counts", got)
+    if want_py_la is not None:
+        d.check(n, lp, want_py_la, -7, f"{what} engines: emulator labels")
+        wp = want_py_la[d.idx(n)]
+        assert got[2:] == [int((wp == truth).sum()), int((wc != wp).sum())], (d.name, n, what, "engines: counts", got)
 
 
 # ---- kernel neighbours of a launch -------------------------------------------------------------------------------------------

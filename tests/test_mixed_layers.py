@@ -13,7 +13,7 @@ FP130 models with +128 in the first or in the last layer on every one-pipe row; 
 first, a hidden and a last layer, both emulator logit scales after a first layer of the other scale, and a mixed chain of the
 fixed shape.
 
-CPU: the plan's weight layout and rows restated in NumPy (plan_layout), the coverage of the cases, and the oracle and the
+CPU: the plan's weight layout and rows restated in NumPy (restate.plan_of), the coverage of the cases, and the oracle and the
 emulator restatement against the unmodified reference where it is present.  GPU (tolerance 0): the plan line against the
 restatement, then every entry the plan serves at 1, 129 and a size past two trips round the ring of every form it launches, and
 the layer-by-layer path."""
@@ -28,8 +28,9 @@ import pytest
 
 from bitnetmcu_b200 import model as M, pack as P
 from conftest import load_model
-from restate import LEVEL_SHIFT, emulate, scale_images
-from support import Sweep, lib, plan_line, plan_ring, scattered_edge_images, verbose_engine  # noqa: F401  (lib: fixture)
+from restate import LEVEL_SHIFT, Plan, emulate, plan_of, scale_images
+from support import (Sweep, both_engines, c_float, chain, emulator, fp130_codes, int8_images, lib, out, plan_line, plan_ring,  # noqa: F401
+                     scattered_edge_images, to_device as t, top_k, verbose_engine, with_plus128)                     # (lib: fixture)
 
 REF_PY = "/root/reference"
 N_UNIQUE = 389          # distinct images per model; batches repeat them (row i is image i % N_UNIQUE)
@@ -39,94 +40,10 @@ PLUS = True             # an FP130 layer with +128 weights
 MAX_TOPK = 16           # the top-k entries take k <= min(n_classes, 16)
 
 
-# ---- the fused plan's weight layout and rows (fc_chain_plan_create, fc_wgmma.cu) ------------------------------------------------
-
-SMEM_LIMIT = 227 * 1024 - 2048      # an SM's shared memory less the alignment slack and the static barriers
-FLOAT_RINGS = 8 * 2 * 4 * 256 * 4   # the float32 quantiser warps' rings: 8 warps x 2 slots x 4 rows x 256 elements x 4 bytes
 FIXED_ROW = "<64,2,2,16,fixed>"
-FIXED_SHAPE = dict(in_atoms=2, n_pad=[64, 64, 64, 16], k_steps=[8, 2, 2, 2], b_off=[0, 16384, 20480, 24576])
-
-
-class Layout(NamedTuple):
-    in_atoms: int
-    n_pad: list             # per layer: outputs rounded up to 16
-    k_steps: list           # per layer: K-steps of 32 in the weight image
-    planes: list            # per layer: 2 where the layer holds a +128 weight (FP130), else 1
-    b_off: list             # per layer: byte offset of its first plane in the weight image
-    w_bytes: int            # the weight image, the zero tile behind the layers included
-    pipes: int              # of the int8 C-engine form
-    row: str                # that form's kernel row
-    float_forms: bool       # the one-kernel float-input forms (float32, 16-bit, emulator, both engines) exist
-    logit_scale: float      # the emulator's logits: the last layer's accumulators times this
-
-
-def _up(x, m):
-    return -(-x // m) * m
-
-
-def plan_layout(model, nf4_extension=False):
-    """the fused plan of an FC model (img_bytes-byte rows) or None where it has none: the weight image and the launch rows"""
-    fc = model.fc_layers
-    in_bytes = model.img_bytes
-    n_pad = [_up(l.n_out, 16) for l in fc]
-    k_pad = [_up(max(l.n_in, 1), 32) for l in fc]
-    if not (1 <= len(fc) <= 8 and in_bytes % 16 == 0 and 0 < in_bytes <= 1024 and max(n_pad) <= 256):
-        return None
-    in_atoms = -(-in_bytes // 128)
-    # K of layer l > 0 stops at the previous layer's padded width: the activations past it are zero
-    k_steps = [4 * in_atoms] + [-(-min(k_pad[l], n_pad[l - 1]) // 32) for l in range(1, len(fc))]
-    planes = [1 + int((P.decode_int_weights(l, nf4_extension) == 128).any()) for l in fc]
-    sizes = [p * k * n * 32 for p, k, n in zip(planes, k_steps, n_pad)]
-    b_off = [int(s) for s in np.cumsum([0] + sizes[:-1])]
-    max_n = _up(max(n_pad), 64)
-    w_bytes = sum(sizes) + max_n * 32
-    w_fixed, stage = _up(w_bytes, 128), in_atoms * 16384
-    if w_fixed + 2 * stage > SMEM_LIMIT:
-        return None
-    pipes = 2 if max_n == 64 and (SMEM_LIMIT - w_fixed) // stage >= 4 else 1
-    last16 = n_pad[-1] <= 16
-    fixed = pipes == 2 and last16 and planes == [1] * len(fc) and \
-        dict(in_atoms=in_atoms, n_pad=n_pad, k_steps=k_steps, b_off=b_off) == FIXED_SHAPE
-    row = FIXED_ROW if fixed else ("<64,2,2,16>" if last16 else "<64,2,2,64>") if pipes == 2 else f"<{max_n},1>"
-    float_forms = max_n == 64 and in_bytes <= 256 and fc[-1].n_out <= 16 and w_fixed + FLOAT_RINGS + 2 * stage <= SMEM_LIMIT
-    return Layout(in_atoms, n_pad, k_steps, planes, b_off, w_bytes, pipes, row, float_forms,
-                  2.0 ** -LEVEL_SHIFT.get(fc[-1].bitperweight, 0))
 
 
 # ---- the models --------------------------------------------------------------------------------------------------------------
-
-def with_plus128(codes, l):
-    """FP130 codes with +128 (code 7) in every third row: row o at column (5 o + l) % n_in"""
-    c = codes.copy()
-    o = np.arange(0, c.shape[0], 3)
-    c[o, (5 * o + l) % c.shape[1]] = 7
-    return c
-
-
-def fp130_codes(rng, n_out, n_in):
-    """random FP130 codes without +128; -128 (code 15) stays, it fits an int8 plane"""
-    c = rng.integers(0, 16, size=(n_out, n_in), dtype=np.uint32)
-    c[c == 7] = 15
-    return c
-
-
-def chain(img_bytes, layers, seed):
-    """a random FC model of img_bytes-byte rows; layers: (encoding, outputs) or (FP130, outputs, PLUS) per layer"""
-    rng = np.random.default_rng(seed)
-    out, n_in = [], img_bytes
-    for i, (enc, n_out, *plus) in enumerate(layers):
-        name = f"L{i + 1}"
-        if enc == T:
-            out.append(P.fc_layer_from_trits(name, rng.integers(-1, 2, size=(n_out, n_in))))
-        else:
-            codes = fp130_codes(rng, n_out, n_in) if enc == F else \
-                rng.integers(0, 1 << P.CODE_BITS[enc], size=(n_out, n_in), dtype=np.uint32)
-            out.append(P.fc_layer_from_codes(name, enc, with_plus128(codes, i) if plus else codes))
-        n_in = n_out
-    m = M.Model(model_class=M.MODEL_FCMNIST, layers=out, img_bytes=img_bytes)
-    m.validate()
-    return m
-
 
 def fp130_subset(subset, classes):
     """12k_FP130 with +128 in the layers of `subset`; classes != 10: its first three layers and a random FP130 head"""
@@ -202,7 +119,7 @@ def model(name):
 
 @functools.lru_cache(maxsize=None)
 def layout(name):
-    return plan_layout(model(name), BY_NAME[name].nf4_ext)
+    return plan_of(model(name), BY_NAME[name].nf4_ext)
 
 
 def exact(m):
@@ -217,7 +134,7 @@ def test_restated_layout(name):
     """each model's restated plan: its stated row, the plane pattern its construction gives, offsets that sum the planes and
     K-steps of every earlier layer, and a weight image that fits"""
     c, m, lay = BY_NAME[name], model(name), layout(name)
-    assert lay is not None and lay.row == c.row, (name, lay)
+    assert isinstance(lay, Plan) and lay.row == c.row, (name, lay)
     fc = m.fc_layers
     assert lay.planes == [1 + int(l.bitperweight == F and (P.decode_int_weights(l) == 128).any()) for l in fc]
     for l in range(1, len(fc)):
@@ -232,14 +149,14 @@ def test_restated_layout(name):
 def test_layout_restatement_edges():
     """the rules on known models: the fixture rows, the fixed shape with residual planes (general row), 512-byte rows (one pipe),
     and a Ternary layer after a 32-wide one (32 inputs padded to 40, K padded to 64: one K-step, from the previous width)"""
-    fixed = plan_layout(load_model("fc"))
+    fixed = plan_of(load_model("fc"))
     assert fixed.row == FIXED_ROW and fixed.w_bytes == 27648 and fixed.b_off == [0, 16384, 20480, 24576] and fixed.logit_scale == 0.5
-    res = plan_layout(load_model("rand_fp130_64"))
+    res = plan_of(load_model("rand_fp130_64"))
     assert res.row == "<64,2,2,16>" and res.planes == [2] * 4 and res.b_off == [0, 32768, 40960, 49152] and res.w_bytes == 53248
     assert res.float_forms and res.logit_scale == 1.0
-    wide = plan_layout(model("fp130-512-64-64-10-first"))
+    wide = plan_of(model("fp130-512-64-64-10-first"))
     assert wide.row == "<64,1>" and wide.k_steps == [16, 2, 2] and wide.planes == [2, 1, 1] and not wide.float_forms
-    t = plan_layout(chain(256, ((I8, 32), (T, 64), (I8, 10)), 0))
+    t = plan_of(chain(256, ((I8, 32), (T, 64), (I8, 10)), 0))
     assert t.k_steps == [8, 1, 2] and t.n_pad == [32, 64, 16] and t.b_off == [0, 8192, 10240]
 
 
@@ -282,16 +199,6 @@ def test_cases_cover_every_layout():
 
 # ---- CPU: the models against the unmodified reference -------------------------------------------------------------------------
 
-def int8_images(n, d, seed):
-    """n int8 rows of d bytes: rows at the int8 rails, all zero, one value, then random rows"""
-    rng = np.random.default_rng(seed)
-    q = rng.integers(-128, 128, size=(n, d)).astype(np.int8)
-    rails = [np.full(d, 127), np.full(d, -128), np.zeros(d), np.where(np.arange(d) % 2, -128, 127),
-             np.where(rng.random(d) < 0.5, 127, -128), np.full(d, 1)]
-    q[:len(rails)] = np.stack(rails)
-    return q
-
-
 def quantized_model_list(m):
     """the reference emulator's layer list for FC model m (tests/golden/make_emulator_golden.py): weight levels = the integer
     weights over the encoding's level scale, Ternary's zero pad columns dropped"""
@@ -333,23 +240,6 @@ def test_emulate_matches_reference_emulator(name):
 
 
 # ---- GPU helpers --------------------------------------------------------------------------------------------------------------
-
-def t(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def out(shape, dtype, sentinel):
-    """a device buffer of shape with 128 rows more, all sentinel"""
-    import torch
-    return torch.full((shape[0] + 128,) + tuple(shape[1:]), sentinel, dtype=dtype, device="cuda")
-
-
-def top_k(logits, k):
-    """the k best classes of each row and their scores: a stable sort, highest first, ties to the lower class"""
-    cls = np.argsort(-logits, axis=1, kind="stable")[:, :k]
-    return cls.astype(np.int32), np.take_along_axis(logits, cls, axis=1)
-
 
 class Data:
     """one model's N_UNIQUE images and expectations on the device; row i of a batch of n is image i % N_UNIQUE"""
@@ -439,48 +329,6 @@ def half_results(e, d, fmt):
             assert np.array_equal(r["emu"].cpu().numpy()[fin], emulate(d.m, xw_np[fin])), (d.name, fmt, "emulator on the widened rows")
         d.half[fmt] = r
     return d.half[fmt]
-
-
-def c_float(e, d, n, x, want_lo, want_la, what):
-    """the C engine's float entry (float32 or 16-bit rows x): logits and labels, then labels alone"""
-    import torch
-    lo, la = out((n, d.C), torch.int32, -5), out((n,), torch.int32, -7)
-    e.infer_device_f32(x, lo[:n], la[:n])
-    torch.cuda.synchronize()
-    d.check(n, lo, want_lo, -5, f"{what} logits")
-    d.check(n, la, want_la, -7, f"{what} labels")
-    la.fill_(-7)
-    e.infer_device_f32(x, None, la[:n])
-    torch.cuda.synchronize()
-    d.check(n, la, want_la, -7, f"{what} labels only")
-
-
-def emulator(e, d, n, x, want_lo, want_la, what):
-    """the emulator's entry: float64 logits and labels"""
-    import torch
-    lo, la = out((n, d.C), torch.float64, -12345.5), out((n,), torch.int32, -7)
-    e.inference_quantized_device(x, lo[:n], la[:n])
-    torch.cuda.synchronize()
-    d.check(n, lo, want_lo, -12345.5, f"{what} emulator logits")
-    d.check(n, la, want_la, -7, f"{what} emulator labels")
-
-
-def both_engines(e, d, n, x, want_la, want_py_la, what):
-    """bnm_compare_engines_device: the C labels, the emulator's labels where it is exact, and the counts"""
-    import torch
-    truth = ((torch.arange(n, device="cuda") * 7) % (d.C + 1)).to(torch.int32)
-    lc, lp = out((n,), torch.int32, -7), out((n,), torch.int32, -7)
-    counts = torch.zeros(4, dtype=torch.int64, device="cuda")
-    e.compare_engines_device(x, truth, lc[:n], lp[:n], counts)
-    torch.cuda.synchronize()
-    d.check(n, lc, want_la, -7, f"{what} engines: C labels")
-    wc = want_la[d.idx(n)]
-    got = counts.cpu().tolist()
-    assert got[:2] == [n, int((wc == truth).sum())], (d.name, n, what, "engines: counts", got)
-    if want_py_la is not None:
-        d.check(n, lp, want_py_la, -7, f"{what} engines: emulator labels")
-        wp = want_py_la[d.idx(n)]
-        assert got[2:] == [int((wp == truth).sum()), int((wc != wp).sum())], (d.name, n, what, "engines: counts", got)
 
 
 def top_k_entries(e, d, n, q, x):
