@@ -27,6 +27,8 @@ EXPORTED = [
     "bnm_scan_windows_device", "bnm_scan_windows_topk_device", "bnm_emulate_windows_device", "bnm_emulate_windows_topk_device",
     "bnm_infer_batch_device_f16", "bnm_emulate_batch_device_f16", "bnm_compare_engines_device_f16", "bnm_infer_topk_device_f16",
     "bnm_emulate_topk_device_f16", "bnm_quantize_images_device_f16",
+    "bnm_scan_windows_device_f16", "bnm_scan_windows_topk_device_f16", "bnm_emulate_windows_device_f16",
+    "bnm_emulate_windows_topk_device_f16",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
@@ -51,7 +53,8 @@ class BnmGather(C.Structure):
 
 
 class BnmWindows(C.Structure):
-    """bnm_windows (include/bitnetmcu_b200.h section 10): a stack of equally sized float planes and the window strides."""
+    """bnm_windows (include/bitnetmcu_b200.h section 10): a stack of equally sized float planes and the window strides.  It is
+    also bnm_windows_f16 (section 12), whose fields are laid out alike, the image holding 16-bit elements."""
     _fields_ = [("image", C.c_void_p), ("planes", C.c_uint32), ("height", C.c_uint32), ("width", C.c_uint32), ("pitch", C.c_size_t),
                 ("plane_pitch", C.c_size_t), ("stride_y", C.c_uint32), ("stride_x", C.c_uint32)]
 
@@ -110,6 +113,10 @@ def load() -> C.CDLL:
         "bnm_infer_topk_device_f16": (C.c_int, [vp, vp, C.c_int, sz, u32, vp, vp, vp]),
         "bnm_emulate_topk_device_f16": (C.c_int, [vp, vp, C.c_int, sz, u32, vp, vp, vp]),
         "bnm_quantize_images_device_f16": (C.c_int, [vp, C.c_int, sz, u32, vp, vp]),
+        "bnm_scan_windows_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, vp, vp, vp]),
+        "bnm_scan_windows_topk_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, u32, vp, vp, vp]),
+        "bnm_emulate_windows_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, vp, vp, vp]),
+        "bnm_emulate_windows_topk_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, u32, vp, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

@@ -403,13 +403,14 @@ static void print_route(const bnm_model *m, const char *what, const Route &r) {
     if (!m->verbose) return;
     std::string s;
     const char *scale = r.in == kInF16 ? "k_quantize_images<float16> + " : r.in == kInBF16 ? "k_quantize_images<bfloat16> + " : "k_quantize_images + ";
+    const char *windows = r.in == kInF16 ? "k_quantize_windows<float16> + " : r.in == kInBF16 ? "k_quantize_windows<bfloat16> + " : "k_quantize_windows + ";
     if (r.engine == kEngineBoth && !r.fused) {
         s = half_in(r.in) ? "bnm_infer_batch_device_f16 + bnm_emulate_batch_device_f16 + k_engine_counts"
                           : "bnm_infer_batch_device_f32 + bnm_emulate_batch_device + k_engine_counts";
     } else if (r.engine == kEngineEmul && !r.fused) {
-        s = std::string(r.windows ? "k_quantize_windows + " : "") + (r.topk ? "layer by layer + k_topk_rows<double>" : "layer by layer");
+        s = std::string(r.windows ? windows : "") + (r.topk ? "layer by layer + k_topk_rows<double>" : "layer by layer");
     } else {
-        if (r.scale) s = r.windows ? "k_quantize_windows + " : scale;
+        if (r.scale) s = r.windows ? windows : scale;
         if (r.front == kFrontCnn)
             s += cnn_frontend_kernel(m->channels, m->xy0, m->cnn_frontend) == kCnnFrontendTensorCores ? "k_cnn_frontend16_tc + " : "k_cnn_frontend16 + ";
         if (r.front == kFrontCnnEmul) s += r.scale ? "k_cnn_emul_frontend_i8 + " : "k_cnn_emul_frontend + ";
@@ -1321,26 +1322,29 @@ extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t
     return run_call(m, {"bnm_emulate_topk_device", kEngineEmul, kInF32, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
 }
 
-// Window scan (sections 9 and 10): every 16x16 window of a stack of float planes on a stride grid, classified as the entry named
-// in the header classifies the extracted windows.  Per pass of 2^20 windows (the layered emulator: of its own pass), k_quantize_windows
-// scales them from the planes into the call's scratch, then that entry's route runs on the scaled rows; a fused FC launch after it
-// keeps its wait and counts as a launch of another kind.  w's checks, then call c (name, engine, top-k, outputs, alignment,
-// stream) on its windows.
-static int run_windows(bnm_model *m, const bnm_windows *w, Call c) {
+// Window scan (sections 9, 10 and 12): every 16x16 window of a stack of float32 or 16-bit planes on a stride grid, classified as
+// the entry named in the header classifies the extracted windows (widened to float32).  Per pass of 2^20 windows (the layered
+// emulator: of its own pass), k_quantize_windows scales them from the planes into the call's scratch, then that entry's route runs
+// on the scaled rows; a fused FC launch after it keeps its wait and counts as a launch of another kind.  w's checks, then call c
+// (name, engine, the planes' element kind, top-k, outputs, alignment, stream) on its windows.  Windows: bnm_windows or
+// bnm_windows_f16, whose fields differ in the image's element type only.
+template <class Windows> static int run_windows(bnm_model *m, const Windows *w, Call c) {
     if (int rc = require_device()) return rc;
     if (!w) return fail(BNM_E_ARG, "%s: null window descriptor", c.name);
     if (!w->stride_y || !w->stride_x) return fail(BNM_E_ARG, "%s: zero stride (%u, %u)", c.name, w->stride_y, w->stride_x);
-    if (w->pitch < w->width || w->pitch % 4)
-        return fail(BNM_E_ARG, "%s: pitch %zu must be >= width %u and a multiple of 4 elements (16-byte rows)", c.name, w->pitch, w->width);
-    if (w->planes > 1 && w->plane_pitch % 4)
-        return fail(BNM_E_ARG, "%s: plane pitch %zu must be a multiple of 4 elements (16-byte aligned planes)", c.name, w->plane_pitch);
+    const size_t row_elems = 16 / in_elem_bytes(c.in);   // elements in 16 bytes
+    if (w->pitch < w->width || w->pitch % row_elems)
+        return fail(BNM_E_ARG, "%s: pitch %zu must be >= width %u and a multiple of %zu elements (16-byte rows)", c.name, w->pitch,
+                    w->width, row_elems);
+    if (w->planes > 1 && w->plane_pitch % row_elems)
+        return fail(BNM_E_ARG, "%s: plane pitch %zu must be a multiple of %zu elements (16-byte aligned planes)", c.name,
+                    w->plane_pitch, row_elems);
     if (m && m->img_bytes != 256)
         return fail(BNM_E_UNSUPPORTED, "%s: windows are 16x16 images, the model takes %u-element images", c.name, m->img_bytes);
     const uint32_t out_h = w->height < 16 ? 0 : (w->height - 16) / w->stride_y + 1;
     const uint32_t out_w = w->width < 16 ? 0 : (w->width - 16) / w->stride_x + 1;
-    const WindowGrid g{w->image, w->planes, w->height, w->width, w->pitch, w->planes > 1 ? w->plane_pitch : 0,
-                       w->stride_y, w->stride_x, out_h, out_w};
-    c.in = kInF32;
+    const WindowGrid g{w->image, half_in(c.in) ? (uint32_t)half_format(c.in) : 0u, w->planes, w->height, w->width, w->pitch,
+                       w->planes > 1 ? w->plane_pitch : 0, w->stride_y, w->stride_x, out_h, out_w};
     c.images = w->image;
     c.n = (size_t)w->planes * out_h * out_w;
     c.windows = &g;
@@ -1375,10 +1379,14 @@ extern "C" int bnm_emulate_windows_topk_device(bnm_model *m, const bnm_windows *
 
 // 16-bit float images (section 11): call c of the float32 sibling, its input kind the one of `format` (BNM_E_ARG for any other
 // value, whatever n).  Its route is the sibling's (choose_route) and every output is the sibling's on the images widened to float32.
-static int run_half(bnm_model *m, int format, Call c) {
+static int half_kind(const char *name, int format, InKind &in) {
     if (format != BNM_FLOAT16 && format != BNM_BFLOAT16)
-        return fail(BNM_E_ARG, "%s: format %d, must be BNM_FLOAT16 (1) or BNM_BFLOAT16 (2)", c.name, format);
-    c.in = format == BNM_BFLOAT16 ? kInBF16 : kInF16;
+        return fail(BNM_E_ARG, "%s: format %d, must be BNM_FLOAT16 (1) or BNM_BFLOAT16 (2)", name, format);
+    in = format == BNM_BFLOAT16 ? kInBF16 : kInF16;
+    return 0;
+}
+static int run_half(bnm_model *m, int format, Call c) {
+    if (int rc = half_kind(c.name, format, c.in)) return rc;
     return run_call(m, c);
 }
 
@@ -1410,6 +1418,45 @@ extern "C" int bnm_emulate_topk_device_f16(bnm_model *m, const uint16_t *images,
                                            double *scores, void *stream) {
     return run_half(m, format, {"bnm_emulate_topk_device_f16", kEngineEmul, kInF16, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}},
                                 {16, 1, 4, 8}, stream});
+}
+
+// 16-bit pages (section 12): the stacked window entries of section 10 on a bnm_windows_f16, which one Python structure serves with
+// bnm_windows; the planes' element kind is the one of `format`, and every output is the sibling's on the planes widened to float32
+static_assert(sizeof(bnm_windows_f16) == sizeof(bnm_windows) && offsetof(bnm_windows_f16, image) == offsetof(bnm_windows, image) &&
+                  offsetof(bnm_windows_f16, planes) == offsetof(bnm_windows, planes) &&
+                  offsetof(bnm_windows_f16, height) == offsetof(bnm_windows, height) &&
+                  offsetof(bnm_windows_f16, width) == offsetof(bnm_windows, width) &&
+                  offsetof(bnm_windows_f16, pitch) == offsetof(bnm_windows, pitch) &&
+                  offsetof(bnm_windows_f16, plane_pitch) == offsetof(bnm_windows, plane_pitch) &&
+                  offsetof(bnm_windows_f16, stride_y) == offsetof(bnm_windows, stride_y) &&
+                  offsetof(bnm_windows_f16, stride_x) == offsetof(bnm_windows, stride_x),
+              "bnm_windows_f16 has the field layout of bnm_windows");
+static int run_windows_half(bnm_model *m, const bnm_windows_f16 *w, int format, Call c) {
+    if (int rc = half_kind(c.name, format, c.in)) return rc;
+    return run_windows(m, w, c);
+}
+
+extern "C" int bnm_scan_windows_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format, int32_t *logits, uint32_t *labels,
+                                           void *stream) {
+    return run_windows_half(m, w, format, {"bnm_scan_windows_device_f16", kEngineC, kInF16, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_scan_windows_topk_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format, uint32_t k, uint32_t *classes,
+                                                int32_t *scores, void *stream) {
+    return run_windows_half(m, w, format, {"bnm_scan_windows_topk_device_f16", kEngineC, kInF16, true, nullptr, 0,
+                                           {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
+}
+
+extern "C" int bnm_emulate_windows_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format, double *logits, uint32_t *labels,
+                                              void *stream) {
+    return run_windows_half(m, w, format, {"bnm_emulate_windows_device_f16", kEngineEmul, kInF16, false, nullptr, 0, {logits, labels}, {16, 8},
+                                           stream});
+}
+
+extern "C" int bnm_emulate_windows_topk_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format, uint32_t k, uint32_t *classes,
+                                                   double *scores, void *stream) {
+    return run_windows_half(m, w, format, {"bnm_emulate_windows_topk_device_f16", kEngineEmul, kInF16, true, nullptr, 0,
+                                           {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
 }
 
 // host buffers: n <= kSmallBatch images share a launch with concurrent small calls, larger batches run the chunked pipeline

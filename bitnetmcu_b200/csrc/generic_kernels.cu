@@ -306,11 +306,12 @@ void launch_quantize_images(const uint16_t *in, HalfFormat fmt, uint32_t elems, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Window scan (bnm_infer_windows_device_f32, bnm_scan_windows_device and the other stacked entries): the 16x16 windows of a stack
-// of float32 planes, each scaled as k_quantize_images scales an image, into int8 rows [n][256].  The window rows of the stack are
-// numbered plane by plane, and a CTA takes a run of up to kWinCta windows of one window row.  They share their 16 pixel rows,
-// and the columns they span (at most kWinBox) are loaded ONCE into shared memory as a band, row by row with coalesced loads:
-// each pixel of the band comes from L2 / HBM once per band, not once per window covering it.  From the band: every column's
+// Window scan (bnm_infer_windows_device_f32, bnm_scan_windows_device and the other stacked entries, float32 or 16-bit): the 16x16
+// windows of a stack of planes, each scaled as k_quantize_images scales an image, into int8 rows [n][256].  The window rows of
+// the stack are numbered plane by plane, and a CTA takes a run of up to kWinCta windows of one window row.  They share their 16
+// pixel rows, and the columns they span (at most kWinBox) are loaded ONCE into shared memory as a float32 band, row by row with
+// coalesced loads (16-bit elements widened on the way: the plane's element kind is a runtime field, so one function serves all
+// three): each pixel of the band comes from L2 / HBM once per band, not once per window covering it.  From the band: every column's
 // max |x| over the 16 rows, then per window (one thread each) the max of its 16 columns -- a 16-wide sliding max -- the scale,
 // and its 256 pixels into a staging row padded to 272 bytes (16-byte stores of one quarter-warp then hit distinct banks).  The
 // CTA's rows are consecutive windows, so they leave as one contiguous run of coalesced 16-byte stores.
@@ -319,7 +320,8 @@ constexpr uint32_t kWinCta = 128, kWinBox = 256, kWinStage = 272;
 constexpr size_t kWinSmem = 16 * kWinBox * 4 + kWinBox * 4 + kWinCta * kWinStage;   // band, column maxima, staging
 
 struct WindowRun {
-    const float *image;
+    const void *image;
+    uint32_t half;              // 0: float32 planes; else the HalfFormat of 16-bit planes
     size_t pitch, plane_pitch;  // elements between rows, between planes
     uint32_t width, stride_y, stride_x, out_h, out_w;
     uint32_t per_cta, chunks;   // windows per CTA (per_cta columns of the grid, one box); CTAs per window row
@@ -329,6 +331,28 @@ struct WindowRun {
     size_t w0, n;               // the pass: windows w0 .. w0 + n - 1
     int8_t *out;                // [n][256]
 };
+
+// a band element as float32: float32 as it is, a 16-bit one widened exactly (widen_half)
+template <HalfFormat kFmt> __device__ __forceinline__ float band_elem(float x) { return x; }
+template <HalfFormat kFmt> __device__ __forceinline__ float band_elem(uint16_t h) { return widen_half<kFmt>(h); }
+
+// the band of 16 rows from src (the first row's column x0, rows pitch elements apart) into band [16][box_w], cols columns of
+// pixels and zeros past them (a zero element widens to +0.0); kFmt: the format of 16-bit elements (unused for float32 ones).  A
+// column's rows go in two groups of 8 loads, each issued before its first store (measured on float32 planes: no slower than the
+// float32-only loop this replaced; all 16 at once was 0.4% slower on 4096-wide pages at stride 1)
+template <HalfFormat kFmt = kHalfFloat16, class T>
+__device__ __forceinline__ void load_band(float *band, const T *__restrict__ src, size_t pitch, uint32_t box_w, uint32_t cols) {
+    for (uint32_t x = threadIdx.x; x < box_w; x += blockDim.x) {
+#pragma unroll
+        for (int y0 = 0; y0 < 16; y0 += 8) {
+            T v[8];
+#pragma unroll
+            for (int y = 0; y < 8; y++) v[y] = x < cols ? __ldg(src + (size_t)(y0 + y) * pitch + x) : T(0);
+#pragma unroll
+            for (int y = 0; y < 8; y++) band[(y0 + y) * box_w + x] = band_elem<kFmt>(v[y]);
+        }
+    }
+}
 
 __global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a) {
     extern __shared__ __align__(16) uint8_t smem[];
@@ -342,13 +366,13 @@ __global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a)
     const size_t lo = max(first, a.w0), hi = min(first + min(a.per_cta, a.out_w - c0), a.w0 + a.n);
     if (lo >= hi) return;
     // the band: rows r * stride_y .. + 15 of plane p, columns x0 .. x0 + box_w - 1 (zeros past the plane's width, never read by a
-    // window); the plane's offset is 64-bit, past 2^31 elements in a stack of large pages
+    // window); the plane's offset is 64-bit, past 2^31 elements in a stack of large pages.  16-bit planes are widened to float32
+    // here, so everything after the band load is the float32 kernel's
     const uint32_t x0 = c0 * a.stride_x, cols = min(a.box_w, a.width - x0);
-    const float *src = a.image + p * a.plane_pitch + (size_t)r * a.stride_y * a.pitch + x0;
-    for (uint32_t x = threadIdx.x; x < a.box_w; x += blockDim.x) {
-#pragma unroll
-        for (int y = 0; y < 16; y++) band[y * a.box_w + x] = x < cols ? __ldg(src + (size_t)y * a.pitch + x) : 0.0f;
-    }
+    const size_t at = p * a.plane_pitch + (size_t)r * a.stride_y * a.pitch + x0;   // elements
+    if (a.half == kHalfFloat16) load_band<kHalfFloat16>(band, static_cast<const uint16_t *>(a.image) + at, a.pitch, a.box_w, cols);
+    else if (a.half == kHalfBFloat16) load_band<kHalfBFloat16>(band, static_cast<const uint16_t *>(a.image) + at, a.pitch, a.box_w, cols);
+    else load_band(band, static_cast<const float *>(a.image) + at, a.pitch, a.box_w, cols);
     __syncthreads();
     for (uint32_t x = threadIdx.x; x < a.box_w; x += blockDim.x) {
         float m = 0.0f;
@@ -386,6 +410,7 @@ bool launch_quantize_windows(const WindowGrid &g, size_t w0, size_t n, int8_t *o
     if (n == 0) return true;
     WindowRun a;
     a.image = g.image;
+    a.half = g.half;
     a.pitch = g.pitch;
     a.plane_pitch = g.plane_pitch;
     a.width = g.width;

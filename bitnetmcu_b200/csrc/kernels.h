@@ -92,17 +92,19 @@ void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t
 // the same on 16-bit elements of format fmt [n][elems]: what the float32 kernel gives on them widened to float32
 void launch_quantize_images(const uint16_t *in, HalfFormat fmt, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 
-// The 16x16 windows of a stack of float32 planes (sections 9 and 10 of the header): plane p is image + p * plane_pitch, [height][pitch]
-// on the device (16-byte aligned, pitch and plane_pitch multiples of 4), its windows on an (stride_y, stride_x) grid of out_h x
-// out_w without padding.  Windows are numbered plane by plane, row-major within a plane: w = (p * out_h + r) * out_w + c.
+// The 16x16 windows of a stack of planes (sections 9, 10 and 12 of the header) of float32 elements (half == 0) or 16-bit ones of
+// format half: plane p is image + p * plane_pitch elements, [height][pitch] on the device (16-byte aligned, pitch and plane_pitch
+// multiples of 16 bytes), its windows on an (stride_y, stride_x) grid of out_h x out_w without padding.  Windows are numbered
+// plane by plane, row-major within a plane: w = (p * out_h + r) * out_w + c.
 struct WindowGrid {
-    const float *image;
+    const void *image;
+    uint32_t half;   // 0: float32 elements; kHalfFloat16 / kHalfBFloat16: 16-bit elements of that format
     uint32_t planes, height, width;
     size_t pitch, plane_pitch;
     uint32_t stride_y, stride_x, out_h, out_w;
 };
-// windows w0 .. w0 + n - 1 of g, each flattened row-major and scaled as launch_quantize_images scales an image -> int8 [n][256]
-// (16-byte aligned).  false when the kernel cannot get its shared memory.
+// windows w0 .. w0 + n - 1 of g, each flattened row-major and scaled as launch_quantize_images scales an image (16-bit elements:
+// widened to float32 first) -> int8 [n][256] (16-byte aligned).  false when the kernel cannot get its shared memory.
 bool launch_quantize_windows(const WindowGrid &g, size_t w0, size_t n, int8_t *out, cudaStream_t st);
 
 // ---- scoring both engines (bnm_compare_engines_device): counts = uint64 {images, correct_c, correct_py, mismatches}, the layout of

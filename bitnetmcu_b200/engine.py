@@ -186,9 +186,15 @@ class Engine:
         logits torch.int32 [out_h, out_w, n_classes] or None, labels [out_h, out_w] (4-byte elements) or None (not both None), where
         (out_h, out_w) = window_grid(height, width, stride).  Window (r, c) covers image[r*sy : r*sy+16, c*sx : c*sx+16]; its
         results are what ``infer_device_f32`` returns for that window flattened.  Asynchronous on ``stream`` (default: torch's
-        current stream)."""
+        current stream).  A torch.float16 / torch.bfloat16 plane (pitch a multiple of 8): what float32 gives on ``image.float()``,
+        through ``bnm_scan_windows_device_f16`` with one plane."""
         import torch
         assert image.dim() == 2 and image.stride(1) == 1
+        if _half_format(image.dtype) is not None:
+            one = [None if t is None else t.unsqueeze(0) for t in (logits, labels)]
+            self._windows_call(None, self.lib.bnm_scan_windows_device_f16, image, stride,
+                               [(one[0], torch.int32, (self.n_classes,)), (one[1], 4, ())], stream)
+            return
         sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
         h, w = image.shape
         out_h, out_w = window_grid(h, w, (sy, sx))
@@ -200,47 +206,50 @@ class Engine:
     # pages: a torch.float32 [P, H, W] stack on this GPU ([H, W]: one page) with unit column stride; its row stride is the pitch
     # and its plane stride the plane pitch (multiples of 4).  stride: an int or (sy, sx).  Every output is [P, out_h, out_w, ...]
     # with (out_h, out_w) = window_grid(H, W, stride); window (p, r, c) covers pages[p, r*sy : r*sy+16, c*sx : c*sx+16], and its
-    # results are those of the matching entry on that window flattened.  Asynchronous on ``stream`` (default: torch's current
-    # stream).
-    def _windows_call(self, fn, pages, stride, args, stream) -> None:
-        """fn(handle, the stack's bnm_windows, *args, stream) as _device_call passes args, a tensor argument's shape given past
-        the window grid [P, out_h, out_w]"""
-        import torch
+    # results are those of the matching entry on that window flattened.  torch.float16 / torch.bfloat16 pages (section 12;
+    # pitches multiples of 8): what float32 gives on ``pages.float()``, reading 2 bytes per pixel.  Asynchronous on ``stream``
+    # (default: torch's current stream).
+    def _windows_call(self, fn, fn16, pages, stride, args, stream) -> None:
+        """fn(handle, the stack's bnm_windows, *args, stream) on float32 pages, or fn16(handle, the stack's bnm_windows_f16, format,
+        *args, stream) on 16-bit ones, as _device_call passes args, a tensor argument's shape given past the window grid
+        [P, out_h, out_w]"""
         p = pages if pages.dim() == 3 else pages.unsqueeze(0)
         assert p.dim() == 3 and p.stride(2) == 1
+        fmt = _half_format(p.dtype)
         sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
         n_p, h, w = p.shape
         desc = _lib.BnmWindows(p.data_ptr(), n_p, h, w, p.stride(1), p.stride(0), sy, sx)
         grid = (n_p,) + window_grid(h, w, (sy, sx))
         args = [(a[0], a[1], grid + a[2]) if isinstance(a, tuple) else a for a in args]
-        self._device_call(fn, p, torch.float32, args, stream, lead=(C.byref(desc),))
+        lead = (C.byref(desc),) if fmt is None else (C.byref(desc), fmt)
+        self._device_call(fn if fmt is None else fn16, p, p.dtype, args, stream, lead=lead)
 
     def scan_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
         """The C engine on every window of a stack of pages: logits torch.int32 [P, out_h, out_w, n_classes] or None, labels
         [P, out_h, out_w] (4-byte elements) or None (not both None); ``infer_device_f32`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_scan_windows_device, pages, stride,
+        self._windows_call(self.lib.bnm_scan_windows_device, self.lib.bnm_scan_windows_device_f16, pages, stride,
                            [(logits, torch.int32, (self.n_classes,)), (labels, 4, ())], stream)
 
     def scan_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
         """The C engine's top-k of every window: classes [P, out_h, out_w, k] (4-byte elements), scores torch.int32
         [P, out_h, out_w, k] or None; ``topk_device_f32`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_scan_windows_topk_device, pages, stride,
+        self._windows_call(self.lib.bnm_scan_windows_topk_device, self.lib.bnm_scan_windows_topk_device_f16, pages, stride,
                            [int(k), (classes, 4, (k,)), (scores, torch.int32, (k,))], stream)
 
     def emulate_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
         """The emulator on every window: logits torch.float64 [P, out_h, out_w, n_classes] or None, labels [P, out_h, out_w]
         or None (not both None); ``inference_quantized_device`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_emulate_windows_device, pages, stride,
+        self._windows_call(self.lib.bnm_emulate_windows_device, self.lib.bnm_emulate_windows_device_f16, pages, stride,
                            [(logits, torch.float64, (self.n_classes,)), (labels, 4, ())], stream)
 
     def emulate_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
         """The emulator's top-k of every window: classes [P, out_h, out_w, k], scores torch.float64 [P, out_h, out_w, k] or
         None; ``emulate_topk_device`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_emulate_windows_topk_device, pages, stride,
+        self._windows_call(self.lib.bnm_emulate_windows_topk_device, self.lib.bnm_emulate_windows_topk_device_f16, pages, stride,
                            [int(k), (classes, 4, (k,)), (scores, torch.float64, (k,))], stream)
 
     def compare_engines_device(self, images, truth=None, labels_c=None, labels_py=None, counts=None, stream: Optional[int] = None) -> None:

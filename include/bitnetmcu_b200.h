@@ -44,7 +44,9 @@
  * three top-k device entries, bnm_infer_windows_device_f32, the four stacked window entries bnm_scan_windows_device,
  * bnm_scan_windows_topk_device, bnm_emulate_windows_device and bnm_emulate_windows_topk_device, bnm_quantize_images_device, and the six
  * 16-bit entries of section 11: bnm_infer_batch_device_f16, bnm_emulate_batch_device_f16, bnm_compare_engines_device_f16,
- * bnm_infer_topk_device_f16, bnm_emulate_topk_device_f16 and bnm_quantize_images_device_f16) may be captured into a CUDA graph on
+ * bnm_infer_topk_device_f16, bnm_emulate_topk_device_f16 and bnm_quantize_images_device_f16, and the four 16-bit window entries of
+ * section 12: bnm_scan_windows_device_f16, bnm_scan_windows_topk_device_f16, bnm_emulate_windows_device_f16 and
+ * bnm_emulate_windows_topk_device_f16) may be captured into a CUDA graph on
  * its stream, in any capture mode, in any combination and from any thread.  Each replay gives exactly the results of the same call made eagerly on the buffers'
  * contents at replay time; bnm_compare_engines_device adds to `counts` on every replay.  A graph keeps what its capture decided:
  * the route, the routing options (BNM_OPT_PATH, BNM_OPT_CHUNK_IMAGES, BNM_OPT_CNN_FRONTEND, BNM_OPT_LAUNCH_OVERLAP) and the
@@ -169,7 +171,7 @@ enum { BNM_OPT_PATH = 1, BNM_OPT_NF4_EXTENSION = 2, BNM_OPT_CHUNK_IMAGES = 3, BN
  *      exclusively (more than half of the shared memory): at most two consecutive launches are ever in flight together.
  *      A call whose fused FC launch reads rows the call itself produced just before, into its own scratch, is such a launch of
  *      another kind, and keeps the wait: float input on a model without a fused float-input kernel (scaled by
- *      k_quantize_images), the window scans of sections 9 and 10 (k_quantize_windows) and every CNN call (the front-end's
+ *      k_quantize_images), the window scans of sections 9, 10 and 12 (k_quantize_windows) and every CNN call (the front-end's
  *      features).  The caller's
  *      promise covers the caller's buffers only, never these producer kernels; the int8 launch right after such a call keeps
  *      its wait too.  CNN models are held at mode 1 besides (the front-end kernel really feeds the FC kernel). */
@@ -450,6 +452,42 @@ BNM_API int bnm_infer_topk_device_f16(bnm_model *m, const uint16_t *images, int 
 BNM_API int bnm_emulate_topk_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, uint32_t k, uint32_t *classes,
                                         double *scores, void *stream);
 BNM_API int bnm_quantize_images_device_f16(const uint16_t *images, int format, size_t n, uint32_t elems, int8_t *out, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 12. 16-bit pages: the window scan of a stack of float16 or bfloat16 planes (section 10 on section 11's formats), without a
+ *     float32 copy of the stack.  The planes are read at 2 bytes per pixel and widened to float32 as they are loaded.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct bnm_windows_f16 {
+    const uint16_t *image;    /* plane p starts at image + p * plane_pitch; device memory on the model's GPU, 16-byte aligned */
+    uint32_t planes;          /* >= 0; 0 = no windows                                                                        */
+    uint32_t height, width;   /* of every plane                                                                              */
+    size_t pitch;             /* 16-bit elements between rows: >= width, a multiple of 8                                     */
+    size_t plane_pitch;       /* 16-bit elements between planes: a multiple of 8 (ignored when planes <= 1)                  */
+    uint32_t stride_y, stride_x;
+} bnm_windows_f16;            /* the field layout of bnm_windows */
+/* Each entry below is the section 10 sibling named beside it, with `const bnm_windows_f16 *windows, int format` (BNM_FLOAT16 or
+ * BNM_BFLOAT16) in place of `const bnm_windows *windows`:
+ *   bnm_scan_windows_device_f16           bnm_scan_windows_device
+ *   bnm_scan_windows_topk_device_f16      bnm_scan_windows_topk_device
+ *   bnm_emulate_windows_device_f16        bnm_emulate_windows_device
+ *   bnm_emulate_windows_topk_device_f16   bnm_emulate_windows_topk_device
+ * Every output is bit for bit the sibling's output on the stack widened to float32 (exact for every value, as in section 11):
+ * the same window order, outputs, k rules and NULL combinations.  A format other than BNM_FLOAT16 or BNM_BFLOAT16 returns
+ * BNM_E_ARG, whatever the descriptor holds (planes == 0 or a NULL descriptor included).  The other argument rules are the
+ * sibling's, in 16-bit elements: the image 16-byte aligned, pitch >= width and a multiple of 8, plane_pitch a multiple of 8 when
+ * planes > 1.  One page is planes = 1.  Pixels outside the windows (pitch padding, rows below a page, gaps between planes) are
+ * never read.  Routes: the sibling's, with the 16-bit form of the scaling step, named k_quantize_windows<float16> or
+ * k_quantize_windows<bfloat16> in the "windows route:" line under BNM_VERBOSE.  Threads, graphs ("Graphs") and
+ * BNM_OPT_LAUNCH_OVERLAP mode 2 (a launch of another kind: its fused launch and the int8 launch after it keep their wait) follow
+ * the sibling.  Asynchronous on `stream`, no host synchronisation. */
+BNM_API int bnm_scan_windows_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format, int32_t *logits, uint32_t *labels,
+                                        void *stream);
+BNM_API int bnm_scan_windows_topk_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format, uint32_t k, uint32_t *classes,
+                                             int32_t *scores, void *stream);
+BNM_API int bnm_emulate_windows_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format, double *logits, uint32_t *labels,
+                                           void *stream);
+BNM_API int bnm_emulate_windows_topk_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format, uint32_t k, uint32_t *classes,
+                                                double *scores, void *stream);
 
 #ifdef __cplusplus
 }
