@@ -976,13 +976,14 @@ __device__ __forceinline__ void fc_chain_body(const CUtensorMap &tmap_in, const 
                 const uint32_t c = sub + 8 * ((j + u) & 7);
                 if constexpr (kInBytes == 4) v[j] = (u < valid && c < n_f4) ? fr[c] : make_float4(0.f, 0.f, 0.f, 0.f);
                 else v[j] = widen4((u < valid && c < n_f4) ? hr[c] : make_uint2(0u, 0u), bf16);
-                m = fmaxf(m, fmaxf(fmaxf(fabsf(v[j].x), fabsf(v[j].y)), fmaxf(fabsf(v[j].z), fabsf(v[j].w))));
+                m = fmax_nan(m, fmax_nan(fmax_nan(fabsf(v[j].x), fabsf(v[j].y)), fmax_nan(fabsf(v[j].z), fabsf(v[j].w))));
             }
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-            // test_inference.py:140-141 / BitNetMCU.py:435-436, every step one correctly rounded float32 operation
-            const float scale = __fdiv_rn(127.0f, fmaxf(m, 1e-5f));
+            m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, 4));
+            m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, 1));
+            // test_inference.py:140-141 / BitNetMCU.py:435-436, every step one correctly rounded float32 operation.  The maxima
+            // carry NaN (fmax_nan, kernels.h) and cvt gives 0 for a NaN product: a row with a NaN or an infinity becomes all zeros
+            const float scale = __fdiv_rn(127.0f, fmax_nan(m, 1e-5f));
             auto q = [&](float x) { int d; asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(d) : "f"(__fmul_rn(x, scale))); return (uint32_t)d; };   // round half to even, clip to int8
 #pragma unroll
             for (int j = 0; j < 8; j++) {

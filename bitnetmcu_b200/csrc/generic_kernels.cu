@@ -248,13 +248,14 @@ void launch_relunorm(const int32_t *in, uint32_t n_in, int8_t *out, uint32_t out
 // Input quantisation, the step right before the path (SURVEY.md 8f rank 3): test_inference.py:140-141 /
 // BitNetMCU.py:435-436:  scale = 127 / max(max|x|, 1e-5);  q = round_half_even(x * scale).clip(-128, 127)  in float32.
 // One warp per image; every operation is a single correctly rounded IEEE float32 op (no FMA contraction), so the result
-// is bit-identical to the NumPy expression.
+// is bit-identical to the NumPy expression.  The maxima propagate NaN (fmax_nan, kernels.h) and a NaN product scales to 0, as
+// NumPy's expression followed by .astype(np.int8) does: a row with any NaN or infinity becomes the all-zero row.
 // ------------------------------------------------------------------------------------------------
 // scale of an image whose largest |x| is absmax, and one pixel scaled with it (k_quantize_images, k_cnn_emul_frontend)
-__device__ __forceinline__ float quant_scale(float absmax) { return __fdiv_rn(127.0f, fmaxf(absmax, 1e-5f)); }
+__device__ __forceinline__ float quant_scale(float absmax) { return __fdiv_rn(127.0f, fmax_nan(absmax, 1e-5f)); }
 __device__ __forceinline__ int quant_pixel(float x, float scale) {
-    const float y = rintf(__fmul_rn(x, scale));            // np.round: round half to even
-    return (int)fminf(fmaxf(y, -128.0f), 127.0f);          // .clip(-128, 127)
+    // np.round (half to even) with cvt.rni, which gives 0 for NaN and saturates at the int32 range, then .clip(-128, 127)
+    return min(max(__float2int_rn(__fmul_rn(x, scale)), -128), 127);
 }
 
 __global__ void __launch_bounds__(256) k_quantize_images(const float *__restrict__ in, uint32_t elems, int8_t *__restrict__ out, size_t n) {
@@ -263,9 +264,9 @@ __global__ void __launch_bounds__(256) k_quantize_images(const float *__restrict
     if (img >= n) return;
     const float *x = in + img * elems;
     float m = 0.0f;
-    for (uint32_t i = lane; i < elems; i += 32) m = fmaxf(m, fabsf(x[i]));
+    for (uint32_t i = lane; i < elems; i += 32) m = fmax_nan(m, fabsf(x[i]));
 #pragma unroll
-    for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+    for (int off = 16; off > 0; off >>= 1) m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, off));
     const float scale = quant_scale(m);
     int8_t *q = out + img * elems;
     for (uint32_t i = lane; i < elems; i += 32) q[i] = (int8_t)quant_pixel(x[i], scale);
@@ -291,9 +292,9 @@ __global__ void __launch_bounds__(256) k_quantize_images(const uint16_t *__restr
     if (img >= n) return;
     const uint16_t *x = in + img * elems;
     float m = 0.0f;
-    for (uint32_t i = lane; i < elems; i += 32) m = fmaxf(m, fabsf(widen_half<kFmt>(x[i])));
+    for (uint32_t i = lane; i < elems; i += 32) m = fmax_nan(m, fabsf(widen_half<kFmt>(x[i])));
 #pragma unroll
-    for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+    for (int off = 16; off > 0; off >>= 1) m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, off));
     const float scale = quant_scale(m);
     int8_t *q = out + img * elems;
     for (uint32_t i = lane; i < elems; i += 32) q[i] = (int8_t)quant_pixel(widen_half<kFmt>(x[i]), scale);
@@ -312,7 +313,8 @@ void launch_quantize_images(const uint16_t *in, HalfFormat fmt, uint32_t elems, 
 // pixel rows, and the columns they span (at most kWinBox) are loaded ONCE into shared memory as a float32 band, row by row with
 // coalesced loads (16-bit elements widened on the way: the plane's element kind is a runtime field, so one function serves all
 // three): each pixel of the band comes from L2 / HBM once per band, not once per window covering it.  From the band: every column's
-// max |x| over the 16 rows, then per window (one thread each) the max of its 16 columns -- a 16-wide sliding max -- the scale,
+// max |x| over the 16 rows, then per window (one thread each) the max of its 16 columns -- a 16-wide sliding max; both carry NaN,
+// so a window covering a NaN or infinite pixel is the all-zero row and its neighbours are untouched -- the scale,
 // and its 256 pixels into a staging row padded to 272 bytes (16-byte stores of one quarter-warp then hit distinct banks).  The
 // CTA's rows are consecutive windows, so they leave as one contiguous run of coalesced 16-byte stores.
 // ------------------------------------------------------------------------------------------------
@@ -377,7 +379,7 @@ __global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a)
     for (uint32_t x = threadIdx.x; x < a.box_w; x += blockDim.x) {
         float m = 0.0f;
 #pragma unroll
-        for (int y = 0; y < 16; y++) m = fmaxf(m, fabsf(band[y * a.box_w + x]));
+        for (int y = 0; y < 16; y++) m = fmax_nan(m, fabsf(band[y * a.box_w + x]));
         colmax[x] = m;
     }
     __syncthreads();
@@ -386,7 +388,7 @@ __global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a)
         const uint32_t xj = j * a.stride_x;
         float m = 0.0f;
 #pragma unroll
-        for (int k = 0; k < 16; k++) m = fmaxf(m, colmax[xj + k]);
+        for (int k = 0; k < 16; k++) m = fmax_nan(m, colmax[xj + k]);
         const float scale = quant_scale(m);
 #pragma unroll 4
         for (int y = 0; y < 16; y++) {
@@ -790,10 +792,10 @@ k_cnn_emul_frontend(const float *__restrict__ images, const int8_t *__restrict__
             a = x[lane];
             b = x[lane + 32];
         }
-        float m = fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))),
-                        fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w))));
+        float m = fmax_nan(fmax_nan(fmax_nan(fabsf(a.x), fabsf(a.y)), fmax_nan(fabsf(a.z), fabsf(a.w))),
+                           fmax_nan(fmax_nan(fabsf(b.x), fabsf(b.y)), fmax_nan(fabsf(b.z), fabsf(b.w))));
 #pragma unroll
-        for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+        for (int off = 16; off > 0; off >>= 1) m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, off));
         const float sc = quant_scale(m);
         auto pack = [&](float4 v) {
             return (uint32_t)(quant_pixel(v.x, sc) & 255) | (uint32_t)(quant_pixel(v.y, sc) & 255) << 8 |

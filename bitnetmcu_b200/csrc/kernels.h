@@ -87,6 +87,16 @@ void launch_topk_rows(const double *rows, uint32_t n_cls, uint32_t k, uint32_t *
 // 16-bit float image elements (BNM_FLOAT16 / BNM_BFLOAT16 of the header)
 enum HalfFormat : uint32_t { kHalfFloat16 = 1, kHalfBFloat16 = 2 };
 
+// The maximum of the input scaling's row maxima and of its 1e-5 floor: NaN if either operand is NaN, as NumPy's max and np.maximum
+// are (fmaxf drops NaN).  With it a row holding any NaN gets a NaN scale, and one holding an infinity (and no NaN) a scale of 0;
+// every product is then NaN or +-0, and a NaN product scales to 0 (what NaN.astype(np.int8) gives on x86-64 and AArch64): a row
+// with any non-finite element scales to the all-zero int8 row, on every route.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+    float d;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+    return d;
+}
+
 // input quantisation ahead of the path (test_inference.py:140-141): float [n][elems] -> int8 [n][elems]
 void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 // the same on 16-bit elements of format fmt [n][elems]: what the float32 kernel gives on them widened to float32

@@ -274,7 +274,9 @@ BNM_API int bnm_maxpool22_batch(const int32_t *activations, uint32_t xy_input, i
  * 5. Input quantisation, the step right before the path (the reference does it in Python per image:
  *    /root/reference/test_inference.py:140-141, BitNetMCU.py:435-436):
  *        scale = 127 / max(max|x|, 1e-5);  q = round_half_even(x * scale) clipped to [-128, 127]      (all float32)
- *    images float32 [n][elems] -> int8 [n][elems]; bit-identical to the NumPy expression.
+ *    images float32 [n][elems] -> int8 [n][elems]; bit-identical to the NumPy expression followed by .astype(np.int8), rows
+ *    holding NaN or infinity included: such a row scales to the all-zero int8 row on every entry and route (NumPy's maximum
+ *    carries a NaN into the scale, an infinity makes the scale 0, and NaN casts to 0).
  * ------------------------------------------------------------------------------------------- */
 /* Float images straight to logits / labels (device buffers, asynchronous on `stream`): for FC models on the fused path (image rows of
  * <= 256 elements, <= 16 classes) this is ONE kernel -- four extra warps read the float rows, reduce the row maximum, quantise and write
@@ -363,7 +365,8 @@ BNM_API int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t n,
 /* ---------------------------------------------------------------------------------------------
  * 9. Window scan: the classifier run over a larger image, one 16x16 window at every position on a stride grid (a page scanned
  *    for characters, say).  The windows are never materialised as float rows: each one is scaled as section 5 scales an image,
- *    straight from the plane, and neighbouring windows share the pixel reads.
+ *    straight from the plane, and neighbouring windows share the pixel reads.  So a NaN or infinite pixel makes every window
+ *    that covers it the all-zero row, and leaves every other window as it is.
  * ------------------------------------------------------------------------------------------- */
 /* image: one float32 plane of height x width pixels, device memory on the model's GPU, 16-byte aligned, rows `pitch` elements
  * apart (pitch >= width, a multiple of 4).  The window grid is out_h = (height - 16) / stride_y + 1 by out_w = (width - 16) /
@@ -433,7 +436,7 @@ BNM_API int bnm_emulate_windows_topk_device(bnm_model *m, const bnm_windows *win
  *   bnm_quantize_images_device_f16    bnm_quantize_images_device
  * images: [n][img_bytes] (bnm_quantize_images_device_f16: [n][elems]) 16-bit elements of `format`, device memory.  Every output
  * is bit for bit the sibling's output on the images widened to float32 (a conversion that is exact for every value: subnormals,
- * infinities and NaN included).  A format other than BNM_FLOAT16 or BNM_BFLOAT16 returns BNM_E_ARG, whatever n.  Everything
+ * infinities and NaN included; a float16 value past 65504 is already inf, so its row scales to zeros as in section 5).  A format other than BNM_FLOAT16 or BNM_BFLOAT16 returns BNM_E_ARG, whatever n.  Everything
  * else is the sibling's: argument checks (NULL combinations, k), the 16-byte alignment of images and the other buffers'
  * alignment, counts adding up across calls, per-call scratch and concurrency ("Threads"), capture into a CUDA graph ("Graphs"),
  * and for BNM_OPT_LAUNCH_OVERLAP mode 2 a 16-bit call is a launch of another kind, like a float call.
@@ -471,8 +474,8 @@ typedef struct bnm_windows_f16 {
  *   bnm_scan_windows_topk_device_f16      bnm_scan_windows_topk_device
  *   bnm_emulate_windows_device_f16        bnm_emulate_windows_device
  *   bnm_emulate_windows_topk_device_f16   bnm_emulate_windows_topk_device
- * Every output is bit for bit the sibling's output on the stack widened to float32 (exact for every value, as in section 11):
- * the same window order, outputs, k rules and NULL combinations.  A format other than BNM_FLOAT16 or BNM_BFLOAT16 returns
+ * Every output is bit for bit the sibling's output on the stack widened to float32 (exact for every value, as in section 11; a
+ * window holding NaN or infinity is the all-zero row, section 9): the same window order, outputs, k rules and NULL combinations.  A format other than BNM_FLOAT16 or BNM_BFLOAT16 returns
  * BNM_E_ARG, whatever the descriptor holds (planes == 0 or a NULL descriptor included).  The other argument rules are the
  * sibling's, in 16-bit elements: the image 16-byte aligned, pitch >= width and a multiple of 8, plane_pitch a multiple of 8 when
  * planes > 1.  One page is planes = 1.  Pixels outside the windows (pitch padding, rows below a page, gaps between planes) are

@@ -15,10 +15,15 @@ TILE = 128                          # images per tile (kTileM)
 
 def scale_images(x):
     """float32 images -> int8, test_inference.py:140-141 and BitNetMCU.py:435-436 in float32:
-    round_half_even(x * 127 / max(max|x|, 1e-5)).clip(-128, 127)"""
+    round_half_even(x * 127 / max(max|x|, 1e-5)).clip(-128, 127), then .astype(np.int8).  A row with any NaN or infinity
+    becomes the all-zero row: max and np.maximum carry a NaN into the scale, an infinity makes the scale 0 (inf * 0 is NaN, any
+    finite pixel +-0), and each NaN product casts to 0 -- what .astype(np.int8) gives on x86-64 and AArch64, stated here so the
+    restatement does not depend on the platform's cast."""
     x = np.asarray(x, dtype=np.float32)
-    scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
-    return np.round(x * scale).clip(-128, 127).astype(np.int8)
+    with np.errstate(invalid="ignore", over="ignore"):
+        scale = np.float32(127.0) / np.maximum(np.abs(x).max(axis=-1, keepdims=True), np.float32(1e-5))
+        y = np.round(x * scale).clip(-128, 127)
+    return np.where(np.isnan(y), np.float32(0), y).astype(np.int8)
 
 
 def bitlinear(model, act):

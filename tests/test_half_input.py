@@ -70,7 +70,8 @@ def test_widening_restatement_matches_numpy():
 @pytest.mark.parametrize("fmt", FORMATS)
 def test_scaling_restatement_on_widened_rows(fmt):
     """the 16-bit scaling restated (widen, then restate.scale_images) on the edge rows equals the float32 scaling of the
-    images a torch caller passes today, ``images.float()`` (all-zero rows, subnormals, the 1e-5 floor, 65504, ties, infinities)"""
+    images a torch caller passes today, ``images.float()`` (all-zero rows, subnormals, the 1e-5 floor, 65504, ties, infinities,
+    NaN: the rows holding either scale to zeros)"""
     import torch
     rows = _edge_rows(256, fmt)
     bits = _bits(rows, fmt)
@@ -82,6 +83,8 @@ def test_scaling_restatement_on_widened_rows(fmt):
         if fmt == "float16":
             assert np.array_equal(q, scale_images(bits.view(np.float16).astype(np.float32)))
     assert not q[0].any()                                   # an all-zero row scales to zeros
+    assert not q[5:9].any()                                 # so does every row holding an infinity or a NaN
+    assert q[[1, 2, 3, 9, 11]].any(axis=1).all()            # the finite rows around them do not
     assert np.array_equal(q[4], np.round(rows[4]).clip(-128, 127).astype(np.int8))   # scale 1: ties to even
 
 

@@ -58,18 +58,19 @@ def stacked_windows_np(buf, planes, h, w, pitch, plane_pitch, sy, sx):
 def window_scaling(page, sy, sx):
     """the window scaling kernel's steps on one float32 page [h, w]: every column's max |x| over a window row's 16 rows, the max of
     16 of them per window, scale = 127 / max(that, 1e-5), each pixel round_half_even(x * scale) clipped, all in float32.  Its
-    maxima skip NaN (fmaxf), and a NaN product (a NaN pixel, or inf times a scale of 0) clips to -128 -> int8 [windows, 256]"""
+    maxima carry NaN, as NumPy's do, and a NaN product (a NaN pixel, or inf times a scale of 0) scales to 0: a window holding a
+    NaN or an infinity is the all-zero row -> int8 [windows, 256]"""
     h, w = page.shape
     oh, ow = (h - 16) // sy + 1, (w - 16) // sx + 1
     out = np.empty((oh, ow, 256), dtype=np.int8)
     for r, c in np.ndindex(oh, ow):
         band = page[r * sy:r * sy + 16]
-        col = np.fmax.reduce(np.abs(band), axis=0, initial=np.float32(0))
-        m = np.fmax.reduce(col[c * sx:c * sx + 16], initial=np.float32(0))
+        col = np.abs(band).max(axis=0)
+        m = col[c * sx:c * sx + 16].max()
         scale = np.float32(127.0) / np.maximum(m, np.float32(1e-5))
         with np.errstate(invalid="ignore"):
-            y = np.round(band[:, c * sx:c * sx + 16] * scale).reshape(256)
-        out[r, c] = np.where(np.isnan(y), -128, np.clip(np.nan_to_num(y), -128, 127)).astype(np.int8)
+            y = np.round(band[:, c * sx:c * sx + 16] * scale).clip(-128, 127).reshape(256)
+        out[r, c] = np.where(np.isnan(y), 0, y).astype(np.int8)
     return out.reshape(-1, 256)
 
 
@@ -92,6 +93,12 @@ def edge_page_bits(fmt, h=48, w=64, seed=0):
     bits[40, 30], bits[44, 60] = inf, inf | 0x8000
     bits[25, 45], bits[46, 10] = nan, nan | 0x8000
     return bits
+
+
+def edge_pages_bits(fmt):
+    """edge_page_bits and its mirror image with every sign flipped: two planes [2, 48, 64]"""
+    bits = edge_page_bits(fmt)
+    return np.ascontiguousarray(np.stack([bits, bits[::-1, ::-1] ^ np.uint16(0x8000)]))
 
 
 def widen_inverse(v, fmt):
@@ -185,26 +192,19 @@ def test_widening_restatement_matches_numpy():
 def test_window_scaling_restatement_on_widened_windows(fmt, sy, sx):
     """widening, then the window scaling (column maxima, sliding maximum) equals restate.scale_images on the widened windows
     extracted one by one, on a page with zeros of both signs, subnormals, maxima below 1e-5, the format's largest finite value,
-    infinities and NaN.  Where scale_images' own result is undefined -- a NaN product, which NumPy casts to int8 as it likes --
-    the kernel's rule gives -128, and a window holding NaN scales by the maximum of its other pixels"""
+    infinities and NaN; every window holding a NaN or an infinity is the all-zero row"""
     bits = edge_page_bits(fmt)
     page = widen(bits, fmt)
     got = window_scaling(page, sy, sx)
     wins = stacked_windows_np(page.reshape(-1), 1, *page.shape, page.shape[1], 0, sy, sx)
     assert got.shape == wins.shape and len(got) > 0
-    with np.errstate(invalid="ignore", over="ignore"):
-        want = scale_images(np.where(np.isnan(wins), np.float32(0), wins))   # NaN pixels do not count toward the maximum
-        scale = np.float32(127.0) / np.maximum(np.nanmax(np.abs(wins), axis=1, keepdims=True, initial=0), np.float32(1e-5))
-        undefined = np.isnan(wins * scale)
-    assert undefined.any() and np.isnan(wins).any() and np.isinf(wins).any()
-    assert np.array_equal(got[~undefined], want[~undefined])
-    assert (got[undefined] == -128).all()
-    clean = ~np.isnan(wins).any(axis=1)
-    with np.errstate(invalid="ignore", over="ignore"):
-        whole = scale_images(wins[clean])
-    assert np.array_equal(got[clean][~undefined[clean]], whole[~undefined[clean]])
-    # the cases are there: a window whose maximum is a subnormal, one below 1e-5 but normal, one at the format's largest value
-    m = np.nanmax(np.abs(wins), axis=1, initial=0)
+    assert np.array_equal(got, scale_images(wins))
+    poisoned = ~np.isfinite(wins).all(axis=1)
+    assert poisoned.any() and (~poisoned).any() and np.isnan(wins).any() and np.isinf(wins).any()
+    assert not got[poisoned].any()
+    # the finite cases are there too: a window whose maximum is a subnormal, one below 1e-5 but normal, one at the format's
+    # largest value
+    m = np.abs(wins[~poisoned]).max(axis=1)
     assert (m[m > 0] < np.float32(1.2e-38) if fmt == "bfloat16" else m[m > 0] < np.float32(6.1e-5)).any()
     assert ((m > 0) & (m < np.float32(1e-5))).any()
     assert (m == widen(np.uint16(0x7BFF if fmt == "float16" else 0x7F7F), fmt)).any()
@@ -367,27 +367,42 @@ def test_only_the_window_pixels_count(lib, name, fmt):
 @pytest.mark.parametrize("name", ["fc", "binary160", "cnn_48"])
 def test_scaling_edges(lib, name, fmt):
     """windows whose maximum is a subnormal or below 1e-5, windows holding infinities or NaN, and the format's largest finite
-    value, through every entry: the sibling's results, and the int8 rows restated (the C engine's logits of them)"""
+    value, through every entry: the sibling's results"""
     import torch
-    bits = edge_page_bits(fmt)
-    flip = bits[::-1, ::-1] ^ np.uint16(0x8000)
-    t = torch.from_numpy(np.stack([bits, flip]).view(np.int16)).view(getattr(torch, fmt))
-    pages = stack(t, getattr(torch, fmt))
+    pages = stack(torch.from_numpy(edge_pages_bits(fmt).view(np.int16)).view(getattr(torch, fmt)), getattr(torch, fmt))
     e = _engine(name)
     for stride in [(1, 1), (2, 3), (16, 16)]:
         for entry in ENTRIES:
             assert_sibling(e, entry, pages, stride, (name, fmt, "edges", stride, entry))
     e.close()
-    if name == "fc":   # the rows the GPU scaled: its int8-input logits of the restated rows
-        page = widen(bits, fmt)
-        rows = window_scaling(page, 2, 3)
-        e = _engine("fc")
-        lo, _ = run_stack(e, "scan", pages[:1], (2, 3))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("fmt", FORMATS)
+def test_scaling_edges_follow_numpy(lib, fmt):
+    """the rows the GPU scaled from the edge pages are the NumPy rule's (window_scaling, pinned to the reference expression on
+    the CPU): the C engine's logits of each window equal its int8-input logits of the restated rows, and every window holding a
+    NaN or an infinity has the all-zero row's logits"""
+    import torch
+    bits = edge_pages_bits(fmt)
+    pages = stack(torch.from_numpy(bits.view(np.int16)).view(getattr(torch, fmt)), getattr(torch, fmt))
+    e = _engine("fc")
+    zero = torch.zeros((1, 256), dtype=torch.int8, device="cuda")
+    zlo = torch.empty((1, 10), dtype=torch.int32, device="cuda")
+    e.infer_device(zero, zlo, None)
+    for stride in [(1, 1), (2, 3), (16, 16)]:
+        lo, _ = run_stack(e, "scan", pages, stride)
+        page_rows = [window_scaling(widen(b, fmt), *stride) for b in bits]
+        rows = np.concatenate(page_rows)
         want = torch.empty((len(rows), 10), dtype=torch.int32, device="cuda")
         e.infer_device(torch.from_numpy(rows).cuda(), want, None)
         torch.cuda.synchronize()
-        assert np.array_equal(lo, want.cpu().numpy())
-        e.close()
+        assert np.array_equal(lo, want.cpu().numpy()), (fmt, stride)
+        wins = np.concatenate([stacked_windows_np(widen(b, fmt).reshape(-1), 1, *b.shape, b.shape[1], 0, *stride) for b in bits])
+        poisoned = ~np.isfinite(wins).all(axis=1)
+        assert poisoned.any() and (~poisoned).any(), (fmt, stride)
+        assert (lo[poisoned] == zlo.cpu().numpy()).all(), (fmt, stride)
+    e.close()
 
 
 @pytest.mark.gpu
