@@ -29,12 +29,16 @@ EXPORTED = [
     "bnm_emulate_topk_device_f16", "bnm_quantize_images_device_f16",
     "bnm_scan_windows_device_f16", "bnm_scan_windows_topk_device_f16", "bnm_emulate_windows_device_f16",
     "bnm_emulate_windows_topk_device_f16",
+    "bnm_scan_windows_padded_device", "bnm_scan_windows_topk_padded_device", "bnm_emulate_windows_padded_device",
+    "bnm_emulate_windows_topk_padded_device", "bnm_scan_windows_padded_device_f16", "bnm_scan_windows_topk_padded_device_f16",
+    "bnm_emulate_windows_padded_device_f16", "bnm_emulate_windows_topk_padded_device_f16",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
 OPT_PATH, OPT_NF4_EXTENSION, OPT_CHUNK_IMAGES, OPT_LAUNCH_OVERLAP, OPT_CNN_FRONTEND = 1, 2, 3, 4, 5
 CNN_AUTO, CNN_CUDA_CORES, CNN_TENSOR_CORES = 0, 1, 2
 FLOAT16, BFLOAT16 = 1, 2   # BNM_FLOAT16, BNM_BFLOAT16 (section 11)
+PAD_CONSTANT, PAD_REPLICATE, PAD_REFLECT = 0, 1, 2   # BNM_PAD_* (section 13)
 
 
 class BnmLayer(C.Structure):
@@ -57,6 +61,13 @@ class BnmWindows(C.Structure):
     also bnm_windows_f16 (section 12), whose fields are laid out alike, the image holding 16-bit elements."""
     _fields_ = [("image", C.c_void_p), ("planes", C.c_uint32), ("height", C.c_uint32), ("width", C.c_uint32), ("pitch", C.c_size_t),
                 ("plane_pitch", C.c_size_t), ("stride_y", C.c_uint32), ("stride_x", C.c_uint32)]
+
+
+class BnmWindowPadding(C.Structure):
+    """bnm_window_padding (include/bitnetmcu_b200.h section 13): the border added to every plane of a window scan, in
+    torch.nn.functional.pad's order, its mode (PAD_*) and the constant mode's fill value."""
+    _fields_ = [("left", C.c_uint32), ("right", C.c_uint32), ("top", C.c_uint32), ("bottom", C.c_uint32), ("mode", C.c_uint32),
+                ("value", C.c_float)]
 
 
 _lib = None
@@ -117,6 +128,17 @@ def load() -> C.CDLL:
         "bnm_scan_windows_topk_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, u32, vp, vp, vp]),
         "bnm_emulate_windows_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, vp, vp, vp]),
         "bnm_emulate_windows_topk_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, u32, vp, vp, vp]),
+        "bnm_scan_windows_padded_device": (C.c_int, [vp, C.POINTER(BnmWindows), C.POINTER(BnmWindowPadding), vp, vp, vp]),
+        "bnm_scan_windows_topk_padded_device": (C.c_int, [vp, C.POINTER(BnmWindows), C.POINTER(BnmWindowPadding), u32, vp, vp, vp]),
+        "bnm_emulate_windows_padded_device": (C.c_int, [vp, C.POINTER(BnmWindows), C.POINTER(BnmWindowPadding), vp, vp, vp]),
+        "bnm_emulate_windows_topk_padded_device": (C.c_int, [vp, C.POINTER(BnmWindows), C.POINTER(BnmWindowPadding), u32, vp, vp, vp]),
+        "bnm_scan_windows_padded_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, C.POINTER(BnmWindowPadding), vp, vp, vp]),
+        "bnm_scan_windows_topk_padded_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, C.POINTER(BnmWindowPadding), u32, vp,
+                                                              vp, vp]),
+        "bnm_emulate_windows_padded_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, C.POINTER(BnmWindowPadding), vp, vp,
+                                                            vp]),
+        "bnm_emulate_windows_topk_padded_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, C.POINTER(BnmWindowPadding), u32,
+                                                                 vp, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

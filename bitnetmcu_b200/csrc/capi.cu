@@ -1322,13 +1322,14 @@ extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t
     return run_call(m, {"bnm_emulate_topk_device", kEngineEmul, kInF32, true, images, n, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
 }
 
-// Window scan (sections 9, 10 and 12): every 16x16 window of a stack of float32 or 16-bit planes on a stride grid, classified as
-// the entry named in the header classifies the extracted windows (widened to float32).  Per pass of 2^20 windows (the layered
-// emulator: of its own pass), k_quantize_windows scales them from the planes into the call's scratch, then that entry's route runs
-// on the scaled rows; a fused FC launch after it keeps its wait and counts as a launch of another kind.  w's checks, then call c
+// Window scan (sections 9, 10, 12 and 13): every 16x16 window of a stack of float32 or 16-bit planes, padded or not, on a stride
+// grid, classified as the entry named in the header classifies the extracted windows (widened to float32, padded as
+// torch.nn.functional.pad pads).  Per pass of 2^20 windows (the layered emulator: of its own pass), k_quantize_windows scales them
+// from the planes into the call's scratch, then that entry's route runs on the scaled rows; a fused FC launch after it keeps its
+// wait and counts as a launch of another kind.  w's checks and pad's (NULL: no padding, the grid of sections 9 to 12), then call c
 // (name, engine, the planes' element kind, top-k, outputs, alignment, stream) on its windows.  Windows: bnm_windows or
 // bnm_windows_f16, whose fields differ in the image's element type only.
-template <class Windows> static int run_windows(bnm_model *m, const Windows *w, Call c) {
+template <class Windows> static int run_windows(bnm_model *m, const Windows *w, Call c, const bnm_window_padding *pad = nullptr) {
     if (int rc = require_device()) return rc;
     if (!w) return fail(BNM_E_ARG, "%s: null window descriptor", c.name);
     if (!w->stride_y || !w->stride_x) return fail(BNM_E_ARG, "%s: zero stride (%u, %u)", c.name, w->stride_y, w->stride_x);
@@ -1341,12 +1342,32 @@ template <class Windows> static int run_windows(bnm_model *m, const Windows *w, 
                     w->plane_pitch, row_elems);
     if (m && m->img_bytes != 256)
         return fail(BNM_E_UNSUPPORTED, "%s: windows are 16x16 images, the model takes %u-element images", c.name, m->img_bytes);
-    const uint32_t out_h = w->height < 16 ? 0 : (w->height - 16) / w->stride_y + 1;
-    const uint32_t out_w = w->width < 16 ? 0 : (w->width - 16) / w->stride_x + 1;
+    const bnm_window_padding none{};
+    const bnm_window_padding &pd = pad ? *pad : none;
+    if (pad) {
+        if (pd.left > 15 || pd.right > 15 || pd.top > 15 || pd.bottom > 15)
+            return fail(BNM_E_ARG, "%s: padding (left %u, right %u, top %u, bottom %u): each side must be at most 15", c.name, pd.left,
+                        pd.right, pd.top, pd.bottom);
+        if (pd.mode != BNM_PAD_CONSTANT && pd.mode != BNM_PAD_REPLICATE && pd.mode != BNM_PAD_REFLECT)
+            return fail(BNM_E_ARG, "%s: padding mode %u, must be BNM_PAD_CONSTANT (0), BNM_PAD_REPLICATE (1) or BNM_PAD_REFLECT (2)",
+                        c.name, pd.mode);
+        const bool empty = !w->planes || !w->height || !w->width;   // no windows, whatever the padding
+        if (!empty && pd.mode == BNM_PAD_REFLECT && (pd.top >= w->height || pd.bottom >= w->height || pd.left >= w->width || pd.right >= w->width))
+            return fail(BNM_E_ARG, "%s: reflect padding (left %u, right %u, top %u, bottom %u) must be less than the page's %u x %u on each side",
+                        c.name, pd.left, pd.right, pd.top, pd.bottom, w->height, w->width);
+    }
+    // the grid over the padded planes, sized in 64 bits; a page of no pixels has no windows, padded or not
+    const uint64_t pad_h = (uint64_t)w->height + pd.top + pd.bottom, pad_w = (uint64_t)w->width + pd.left + pd.right;
+    if (pad_h > UINT32_MAX || pad_w > UINT32_MAX)
+        return fail(BNM_E_ARG, "%s: the padded page (%llu x %llu) must be at most 2^32 - 1 pixels either way", c.name,
+                    (unsigned long long)pad_h, (unsigned long long)pad_w);
+    const uint32_t out_h = pad_h < 16 ? 0 : (uint32_t)((pad_h - 16) / w->stride_y + 1);
+    const uint32_t out_w = pad_w < 16 ? 0 : (uint32_t)((pad_w - 16) / w->stride_x + 1);
     const WindowGrid g{w->image, half_in(c.in) ? (uint32_t)half_format(c.in) : 0u, w->planes, w->height, w->width, w->pitch,
-                       w->planes > 1 ? w->plane_pitch : 0, w->stride_y, w->stride_x, out_h, out_w};
+                       w->planes > 1 ? w->plane_pitch : 0, w->stride_y, w->stride_x, out_h, out_w,
+                       pd.top, pd.left, pd.right, pd.mode, pd.value};
     c.images = w->image;
-    c.n = (size_t)w->planes * out_h * out_w;
+    c.n = w->height && w->width ? (size_t)w->planes * out_h * out_w : 0;
     c.windows = &g;
     return run_call(m, c);
 }
@@ -1457,6 +1478,67 @@ extern "C" int bnm_emulate_windows_topk_device_f16(bnm_model *m, const bnm_windo
                                                    double *scores, void *stream) {
     return run_windows_half(m, w, format, {"bnm_emulate_windows_topk_device_f16", kEngineEmul, kInF16, true, nullptr, 0,
                                            {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
+}
+
+// Padded pages (section 13): the stacked window entries of sections 10 and 12 on the planes padded as torch.nn.functional.pad pads
+// them (BNM_E_ARG for a NULL padding); the same Call as the sibling's, and k_quantize_windows makes the border as it loads a band
+static_assert(BNM_PAD_CONSTANT == kPadConstant && BNM_PAD_REPLICATE == kPadReplicate && BNM_PAD_REFLECT == kPadReflect,
+              "BNM_PAD_* are the kernel's PadMode values");
+template <class Windows> static int run_windows_padded(bnm_model *m, const Windows *w, const bnm_window_padding *pad, Call c) {
+    if (!pad) return fail(BNM_E_ARG, "%s: null padding", c.name);
+    return run_windows(m, w, c, pad);
+}
+static int run_windows_padded_half(bnm_model *m, const bnm_windows_f16 *w, int format, const bnm_window_padding *pad, Call c) {
+    if (int rc = half_kind(c.name, format, c.in)) return rc;
+    return run_windows_padded(m, w, pad, c);
+}
+
+extern "C" int bnm_scan_windows_padded_device(bnm_model *m, const bnm_windows *w, const bnm_window_padding *padding, int32_t *logits,
+                                              uint32_t *labels, void *stream) {
+    return run_windows_padded(m, w, padding, {"bnm_scan_windows_padded_device", kEngineC, kInF32, false, nullptr, 0, {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_scan_windows_topk_padded_device(bnm_model *m, const bnm_windows *w, const bnm_window_padding *padding, uint32_t k,
+                                                   uint32_t *classes, int32_t *scores, void *stream) {
+    return run_windows_padded(m, w, padding, {"bnm_scan_windows_topk_padded_device", kEngineC, kInF32, true, nullptr, 0,
+                                              {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
+}
+
+extern "C" int bnm_emulate_windows_padded_device(bnm_model *m, const bnm_windows *w, const bnm_window_padding *padding, double *logits,
+                                                 uint32_t *labels, void *stream) {
+    return run_windows_padded(m, w, padding, {"bnm_emulate_windows_padded_device", kEngineEmul, kInF32, false, nullptr, 0, {logits, labels},
+                                              {16, 8}, stream});
+}
+
+extern "C" int bnm_emulate_windows_topk_padded_device(bnm_model *m, const bnm_windows *w, const bnm_window_padding *padding, uint32_t k,
+                                                      uint32_t *classes, double *scores, void *stream) {
+    return run_windows_padded(m, w, padding, {"bnm_emulate_windows_topk_padded_device", kEngineEmul, kInF32, true, nullptr, 0,
+                                              {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
+}
+
+extern "C" int bnm_scan_windows_padded_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format, const bnm_window_padding *padding,
+                                                  int32_t *logits, uint32_t *labels, void *stream) {
+    return run_windows_padded_half(m, w, format, padding, {"bnm_scan_windows_padded_device_f16", kEngineC, kInF16, false, nullptr, 0,
+                                                           {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_scan_windows_topk_padded_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format, const bnm_window_padding *padding,
+                                                       uint32_t k, uint32_t *classes, int32_t *scores, void *stream) {
+    return run_windows_padded_half(m, w, format, padding, {"bnm_scan_windows_topk_padded_device_f16", kEngineC, kInF16, true, nullptr, 0,
+                                                           {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 4}, stream});
+}
+
+extern "C" int bnm_emulate_windows_padded_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format, const bnm_window_padding *padding,
+                                                     double *logits, uint32_t *labels, void *stream) {
+    return run_windows_padded_half(m, w, format, padding, {"bnm_emulate_windows_padded_device_f16", kEngineEmul, kInF16, false, nullptr, 0,
+                                                           {logits, labels}, {16, 8}, stream});
+}
+
+extern "C" int bnm_emulate_windows_topk_padded_device_f16(bnm_model *m, const bnm_windows_f16 *w, int format,
+                                                          const bnm_window_padding *padding, uint32_t k, uint32_t *classes, double *scores,
+                                                          void *stream) {
+    return run_windows_padded_half(m, w, format, padding, {"bnm_emulate_windows_topk_padded_device_f16", kEngineEmul, kInF16, true, nullptr,
+                                                           0, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
 }
 
 // host buffers: n <= kSmallBatch images share a launch with concurrent small calls, larger batches run the chunked pipeline

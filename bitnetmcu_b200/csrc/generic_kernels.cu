@@ -307,12 +307,15 @@ void launch_quantize_images(const uint16_t *in, HalfFormat fmt, uint32_t elems, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Window scan (bnm_infer_windows_device_f32, bnm_scan_windows_device and the other stacked entries, float32 or 16-bit): the 16x16
-// windows of a stack of planes, each scaled as k_quantize_images scales an image, into int8 rows [n][256].  The window rows of
-// the stack are numbered plane by plane, and a CTA takes a run of up to kWinCta windows of one window row.  They share their 16
-// pixel rows, and the columns they span (at most kWinBox) are loaded ONCE into shared memory as a float32 band, row by row with
-// coalesced loads (16-bit elements widened on the way: the plane's element kind is a runtime field, so one function serves all
-// three): each pixel of the band comes from L2 / HBM once per band, not once per window covering it.  From the band: every column's
+// Window scan (bnm_infer_windows_device_f32, bnm_scan_windows_device and the other stacked entries, float32 or 16-bit, padded or
+// not): the 16x16 windows of a stack of planes, each scaled as k_quantize_images scales an image, into int8 rows [n][256].  The
+// window rows of the stack are numbered plane by plane, and a CTA takes a run of up to kWinCta windows of one window row.  They
+// share their 16 pixel rows, and the columns they span (at most kWinBox) are loaded ONCE into shared memory as a float32 band, row
+// by row with coalesced loads (16-bit elements widened on the way: the plane's element kind is a runtime field, so one function
+// serves all three): each pixel of the band comes from L2 / HBM once per band, not once per window covering it.  Padding (section
+// 13) is runtime fields too, and only changes where a band element comes from: a band wholly on the page takes the plain load,
+// a band reaching into the border maps each of its rows and columns to the page's (clamped or mirrored) or to the fill value.
+// From the band: every column's
 // max |x| over the 16 rows, then per window (one thread each) the max of its 16 columns -- a 16-wide sliding max; both carry NaN,
 // so a window covering a NaN or infinite pixel is the all-zero row and its neighbours are untouched -- the scale,
 // and its 256 pixels into a staging row padded to 272 bytes (16-byte stores of one quarter-warp then hit distinct banks).  The
@@ -325,7 +328,11 @@ struct WindowRun {
     const void *image;
     uint32_t half;              // 0: float32 planes; else the HalfFormat of 16-bit planes
     size_t pitch, plane_pitch;  // elements between rows, between planes
-    uint32_t width, stride_y, stride_x, out_h, out_w;
+    uint32_t height, width;     // of the page
+    uint32_t top, left, pad_w;  // pixels added above and left; the padded width (the page's when unpadded)
+    uint32_t pad_mode;          // a PadMode
+    float pad_value;            // kPadConstant: the border's pixel value
+    uint32_t stride_y, stride_x, out_h, out_w;   // the grid over the padded page
     uint32_t per_cta, chunks;   // windows per CTA (per_cta columns of the grid, one box); CTAs per window row
     uint32_t box_w;             // band width in pixels
     size_t run0;                // the pass's first run of windows: run g covers window row g / chunks of the stack (row
@@ -356,6 +363,33 @@ __device__ __forceinline__ void load_band(float *band, const T *__restrict__ src
     }
 }
 
+// the page index of padded index i (counted from the page's first pixel) on a side of n pixels: i itself on the page, else the
+// edge pixel (replicate), its mirror image about the edge pixel (reflect: a pad is < n, so one reflection lands on the page), or
+// -1 for the fill value (constant)
+__device__ __forceinline__ long long pad_index(long long i, uint32_t n, uint32_t mode) {
+    if (i >= 0 && i < n) return i;
+    if (mode == kPadReplicate) return i < 0 ? 0 : (long long)n - 1;
+    if (mode == kPadReflect) return i < 0 ? -i : 2 * ((long long)n - 1) - i;
+    return -1;
+}
+
+// load_band for a band that reaches into the border: band row y is page row rows[y] (its element offset in the stack, -1 for the
+// fill value) and band column x page column pad_index(cx + x), cols columns of pixels and zeros past them (past the padded width,
+// never read by a window).  Only page pixels are read; the fill value goes into the band as it is
+template <HalfFormat kFmt = kHalfFloat16, class T>
+__device__ __forceinline__ void load_band_padded(float *band, const T *__restrict__ image, const long long *rows, long long cx,
+                                                 uint32_t width, uint32_t mode, float value, uint32_t box_w, uint32_t cols) {
+    for (uint32_t x = threadIdx.x; x < box_w; x += blockDim.x) {
+        const long long c = x < cols ? pad_index(cx + x, width, mode) : -1;
+        const float fill = x < cols ? value : 0.0f;
+#pragma unroll 4
+        for (int y = 0; y < 16; y++) {
+            const long long o = rows[y];
+            band[y * box_w + x] = c < 0 || o < 0 ? fill : band_elem<kFmt>(__ldg(image + o + c));
+        }
+    }
+}
+
 __global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a) {
     extern __shared__ __align__(16) uint8_t smem[];
     float *band = reinterpret_cast<float *>(smem);        // [16][box_w]
@@ -367,14 +401,29 @@ __global__ void __launch_bounds__(kWinCta) k_quantize_windows(const WindowRun a)
     const size_t first = row * a.out_w + c0;   // the CTA's windows first .. first + per_cta - 1, clipped to the row and the pass
     const size_t lo = max(first, a.w0), hi = min(first + min(a.per_cta, a.out_w - c0), a.w0 + a.n);
     if (lo >= hi) return;
-    // the band: rows r * stride_y .. + 15 of plane p, columns x0 .. x0 + box_w - 1 (zeros past the plane's width, never read by a
-    // window); the plane's offset is 64-bit, past 2^31 elements in a stack of large pages.  16-bit planes are widened to float32
-    // here, so everything after the band load is the float32 kernel's
-    const uint32_t x0 = c0 * a.stride_x, cols = min(a.box_w, a.width - x0);
-    const size_t at = p * a.plane_pitch + (size_t)r * a.stride_y * a.pitch + x0;   // elements
-    if (a.half == kHalfFloat16) load_band<kHalfFloat16>(band, static_cast<const uint16_t *>(a.image) + at, a.pitch, a.box_w, cols);
-    else if (a.half == kHalfBFloat16) load_band<kHalfBFloat16>(band, static_cast<const uint16_t *>(a.image) + at, a.pitch, a.box_w, cols);
-    else load_band(band, static_cast<const float *>(a.image) + at, a.pitch, a.box_w, cols);
+    // the band: padded rows r * stride_y .. + 15 of plane p, padded columns x0 .. x0 + box_w - 1 (zeros past the padded width,
+    // never read by a window); the plane's offset is 64-bit, past 2^31 elements in a stack of large pages.  16-bit planes are
+    // widened to float32 here, so everything after the band load is the float32 kernel's
+    const uint32_t x0 = c0 * a.stride_x, cols = min(a.box_w, a.pad_w - x0);
+    const long long y0 = (long long)r * a.stride_y - a.top, cx = (long long)x0 - a.left;   // the band's first pixel on the page
+    if (y0 >= 0 && y0 + 16 <= a.height && cx >= 0 && cx + cols <= a.width) {   // wholly on the page: every unpadded CTA
+        const size_t at = p * a.plane_pitch + (size_t)y0 * a.pitch + (size_t)cx;   // elements
+        if (a.half == kHalfFloat16) load_band<kHalfFloat16>(band, static_cast<const uint16_t *>(a.image) + at, a.pitch, a.box_w, cols);
+        else if (a.half == kHalfBFloat16) load_band<kHalfBFloat16>(band, static_cast<const uint16_t *>(a.image) + at, a.pitch, a.box_w, cols);
+        else load_band(band, static_cast<const float *>(a.image) + at, a.pitch, a.box_w, cols);
+    } else {   // a border CTA: its 16 rows mapped once, into colmax's space (not written before the band is complete)
+        long long *rows = reinterpret_cast<long long *>(colmax);
+        if (threadIdx.x < 16) {
+            const long long y = pad_index(y0 + threadIdx.x, a.height, a.pad_mode);
+            rows[threadIdx.x] = y < 0 ? -1 : (long long)(p * a.plane_pitch + (size_t)y * a.pitch);
+        }
+        __syncthreads();
+        if (a.half == kHalfFloat16)
+            load_band_padded<kHalfFloat16>(band, static_cast<const uint16_t *>(a.image), rows, cx, a.width, a.pad_mode, a.pad_value, a.box_w, cols);
+        else if (a.half == kHalfBFloat16)
+            load_band_padded<kHalfBFloat16>(band, static_cast<const uint16_t *>(a.image), rows, cx, a.width, a.pad_mode, a.pad_value, a.box_w, cols);
+        else load_band_padded(band, static_cast<const float *>(a.image), rows, cx, a.width, a.pad_mode, a.pad_value, a.box_w, cols);
+    }
     __syncthreads();
     for (uint32_t x = threadIdx.x; x < a.box_w; x += blockDim.x) {
         float m = 0.0f;
@@ -415,7 +464,13 @@ bool launch_quantize_windows(const WindowGrid &g, size_t w0, size_t n, int8_t *o
     a.half = g.half;
     a.pitch = g.pitch;
     a.plane_pitch = g.plane_pitch;
+    a.height = g.height;
     a.width = g.width;
+    a.top = g.top;
+    a.left = g.left;
+    a.pad_w = g.width + g.left + g.right;
+    a.pad_mode = g.pad_mode;
+    a.pad_value = g.pad_value;
     a.stride_y = g.stride_y;
     a.stride_x = g.stride_x;
     a.out_h = g.out_h;

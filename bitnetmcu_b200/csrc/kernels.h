@@ -102,19 +102,27 @@ void launch_quantize_images(const float *in, uint32_t elems, int8_t *out, size_t
 // the same on 16-bit elements of format fmt [n][elems]: what the float32 kernel gives on them widened to float32
 void launch_quantize_images(const uint16_t *in, HalfFormat fmt, uint32_t elems, int8_t *out, size_t n, cudaStream_t st);
 
-// The 16x16 windows of a stack of planes (sections 9, 10 and 12 of the header) of float32 elements (half == 0) or 16-bit ones of
-// format half: plane p is image + p * plane_pitch elements, [height][pitch] on the device (16-byte aligned, pitch and plane_pitch
-// multiples of 16 bytes), its windows on an (stride_y, stride_x) grid of out_h x out_w without padding.  Windows are numbered
-// plane by plane, row-major within a plane: w = (p * out_h + r) * out_w + c.
+// how a padded page's border pixels are made (section 13 of the header; the values of BNM_PAD_*): the fill value, the nearest
+// edge pixel, or the mirror image about the edge pixel (which is not repeated)
+enum PadMode : uint32_t { kPadConstant = 0, kPadReplicate = 1, kPadReflect = 2 };
+
+// The 16x16 windows of a stack of planes (sections 9, 10, 12 and 13 of the header) of float32 elements (half == 0) or 16-bit ones
+// of format half: plane p is image + p * plane_pitch elements, [height][pitch] on the device (16-byte aligned, pitch and plane_pitch
+// multiples of 16 bytes), padded by top / left / right pixels (bottom ones only count in out_h) in pad_mode, its windows on an
+// (stride_y, stride_x) grid of out_h x out_w over the padded plane.  Windows are numbered plane by plane, row-major within a
+// plane: w = (p * out_h + r) * out_w + c.  Without padding every pad is 0.  Padded height and width fit in 32 bits.
 struct WindowGrid {
     const void *image;
     uint32_t half;   // 0: float32 elements; kHalfFloat16 / kHalfBFloat16: 16-bit elements of that format
     uint32_t planes, height, width;
     size_t pitch, plane_pitch;
     uint32_t stride_y, stride_x, out_h, out_w;
+    uint32_t top = 0, left = 0, right = 0, pad_mode = kPadConstant;   // pixels added above, left, right; a PadMode
+    float pad_value = 0.0f;                                           // kPadConstant: the border's pixel value
 };
 // windows w0 .. w0 + n - 1 of g, each flattened row-major and scaled as launch_quantize_images scales an image (16-bit elements:
-// widened to float32 first) -> int8 [n][256] (16-byte aligned).  false when the kernel cannot get its shared memory.
+// widened to float32 first; border pixels made as pad_mode says) -> int8 [n][256] (16-byte aligned).  false when the kernel
+// cannot get its shared memory.
 bool launch_quantize_windows(const WindowGrid &g, size_t w0, size_t n, int8_t *out, cudaStream_t st);
 
 // ---- scoring both engines (bnm_compare_engines_device): counts = uint64 {images, correct_c, correct_py, mismatches}, the layout of

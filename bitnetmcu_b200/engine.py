@@ -34,12 +34,32 @@ def _half_format(dtype) -> Optional[int]:
     return {torch.float32: None, torch.float16: _lib.FLOAT16, torch.bfloat16: _lib.BFLOAT16}[dtype]
 
 
-def window_grid(height: int, width: int, stride) -> Tuple[int, int]:
-    """(out_h, out_w) of the 16x16 windows of a height x width image on a stride grid without padding (include/bitnetmcu_b200.h
-    section 9); stride is an int or (stride_y, stride_x), each >= 1.  (0, 0)-sized when the image is under 16 pixels either way."""
+def _pad_sides(padding) -> Tuple[int, int, int, int]:
+    """(left, right, top, bottom) of a window scan's padding: an int for all four sides, or a 4-sequence in F.pad's order"""
+    if isinstance(padding, int):
+        return (padding,) * 4
+    sides = tuple(int(v) for v in padding)
+    if len(sides) != 4:
+        raise ValueError(f"padding: an int or (left, right, top, bottom), got {padding!r}")
+    return sides
+
+
+_PAD_MODES = {"constant": _lib.PAD_CONSTANT, "replicate": _lib.PAD_REPLICATE, "reflect": _lib.PAD_REFLECT}
+
+
+def window_grid(height: int, width: int, stride, padding=None) -> Tuple[int, int]:
+    """(out_h, out_w) of the 16x16 windows of a height x width image on a stride grid (include/bitnetmcu_b200.h section 9);
+    stride is an int or (stride_y, stride_x), each >= 1.  (0, 0)-sized when the image is under 16 pixels either way.  padding:
+    None, or an int / (left, right, top, bottom) as F.pad takes it (section 13): the grid over the padded image, and (0, 0) for
+    an image of no pixels."""
     sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
     if sy < 1 or sx < 1:
         raise ValueError(f"window_grid: strides must be >= 1, got {(sy, sx)}")
+    if padding is not None:
+        if height == 0 or width == 0:
+            return 0, 0
+        left, right, top, bottom = _pad_sides(padding)
+        height, width = height + top + bottom, width + left + right
     if height < 16 or width < 16:
         return 0, 0
     return (height - 16) // sy + 1, (width - 16) // sx + 1
@@ -192,8 +212,7 @@ class Engine:
         assert image.dim() == 2 and image.stride(1) == 1
         if _half_format(image.dtype) is not None:
             one = [None if t is None else t.unsqueeze(0) for t in (logits, labels)]
-            self._windows_call(None, self.lib.bnm_scan_windows_device_f16, image, stride,
-                               [(one[0], torch.int32, (self.n_classes,)), (one[1], 4, ())], stream)
+            self._windows_call("bnm_scan_windows", image, stride, [(one[0], torch.int32, (self.n_classes,)), (one[1], 4, ())], stream)
             return
         sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
         h, w = image.shape
@@ -202,55 +221,68 @@ class Engine:
         self._device_call(self.lib.bnm_infer_windows_device_f32, image, torch.float32,
                           [(logits, torch.int32, (out_h, out_w, self.n_classes)), (labels, 4, (out_h, out_w))], stream, lead=lead)
 
-    # ---- window scan of a stack of pages (include/bitnetmcu_b200.h section 10) -------------------------------------------------
+    # ---- window scan of a stack of pages (include/bitnetmcu_b200.h sections 10, 12 and 13) ---------------------------------------
     # pages: a torch.float32 [P, H, W] stack on this GPU ([H, W]: one page) with unit column stride; its row stride is the pitch
     # and its plane stride the plane pitch (multiples of 4).  stride: an int or (sy, sx).  Every output is [P, out_h, out_w, ...]
-    # with (out_h, out_w) = window_grid(H, W, stride); window (p, r, c) covers pages[p, r*sy : r*sy+16, c*sx : c*sx+16], and its
-    # results are those of the matching entry on that window flattened.  torch.float16 / torch.bfloat16 pages (section 12;
-    # pitches multiples of 8): what float32 gives on ``pages.float()``, reading 2 bytes per pixel.  Asynchronous on ``stream``
-    # (default: torch's current stream).
-    def _windows_call(self, fn, fn16, pages, stride, args, stream) -> None:
-        """fn(handle, the stack's bnm_windows, *args, stream) on float32 pages, or fn16(handle, the stack's bnm_windows_f16, format,
-        *args, stream) on 16-bit ones, as _device_call passes args, a tensor argument's shape given past the window grid
-        [P, out_h, out_w]"""
+    # with (out_h, out_w) = window_grid(H, W, stride, padding); window (p, r, c) covers pages[p, r*sy : r*sy+16, c*sx : c*sx+16],
+    # and its results are those of the matching entry on that window flattened.  torch.float16 / torch.bfloat16 pages (section 12;
+    # pitches multiples of 8): what float32 gives on ``pages.float()``, reading 2 bytes per pixel.  padding (section 13): None
+    # (the unpadded entry), or an int / (left, right, top, bottom) of at most 15 each, with pad_mode "constant", "replicate" or
+    # "reflect" and pad_value the constant mode's float32 fill: what the unpadded call gives on
+    # ``F.pad(pages.float(), padding, pad_mode, pad_value)``, without that copy.  Asynchronous on ``stream`` (default: torch's
+    # current stream).
+    def _windows_call(self, stem, pages, stride, args, stream, padding=None, pad_mode="constant", pad_value=0.0) -> None:
+        """The window entry named stem + ("_padded" with a padding) + "_device" (+ "_f16" on 16-bit pages): fn(handle, the stack's
+        bnm_windows[, format][, its bnm_window_padding], *args, stream), as _device_call passes args, a tensor argument's shape
+        given past the window grid [P, out_h, out_w]"""
         p = pages if pages.dim() == 3 else pages.unsqueeze(0)
         assert p.dim() == 3 and p.stride(2) == 1
         fmt = _half_format(p.dtype)
         sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
         n_p, h, w = p.shape
         desc = _lib.BnmWindows(p.data_ptr(), n_p, h, w, p.stride(1), p.stride(0), sy, sx)
-        grid = (n_p,) + window_grid(h, w, (sy, sx))
+        grid = (n_p,) + window_grid(h, w, (sy, sx), padding)
         args = [(a[0], a[1], grid + a[2]) if isinstance(a, tuple) else a for a in args]
-        lead = (C.byref(desc),) if fmt is None else (C.byref(desc), fmt)
-        self._device_call(fn if fmt is None else fn16, p, p.dtype, args, stream, lead=lead)
+        lead = [C.byref(desc)] if fmt is None else [C.byref(desc), fmt]
+        if padding is not None:
+            if pad_mode not in _PAD_MODES:
+                raise ValueError(f"pad_mode must be one of {sorted(_PAD_MODES)}, got {pad_mode!r}")
+            pad = _lib.BnmWindowPadding(*_pad_sides(padding), _PAD_MODES[pad_mode], float(pad_value))
+            lead.append(C.byref(pad))
+        name = stem + ("_padded" if padding is not None else "") + "_device" + ("_f16" if fmt is not None else "")
+        self._device_call(getattr(self.lib, name), p, p.dtype, args, stream, lead=tuple(lead))
 
-    def scan_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
+    def scan_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None, *, padding=None,
+                            pad_mode: str = "constant", pad_value: float = 0.0) -> None:
         """The C engine on every window of a stack of pages: logits torch.int32 [P, out_h, out_w, n_classes] or None, labels
         [P, out_h, out_w] (4-byte elements) or None (not both None); ``infer_device_f32`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_scan_windows_device, self.lib.bnm_scan_windows_device_f16, pages, stride,
-                           [(logits, torch.int32, (self.n_classes,)), (labels, 4, ())], stream)
+        self._windows_call("bnm_scan_windows", pages, stride, [(logits, torch.int32, (self.n_classes,)), (labels, 4, ())], stream,
+                           padding, pad_mode, pad_value)
 
-    def scan_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
+    def scan_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None, *, padding=None,
+                                 pad_mode: str = "constant", pad_value: float = 0.0) -> None:
         """The C engine's top-k of every window: classes [P, out_h, out_w, k] (4-byte elements), scores torch.int32
         [P, out_h, out_w, k] or None; ``topk_device_f32`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_scan_windows_topk_device, self.lib.bnm_scan_windows_topk_device_f16, pages, stride,
-                           [int(k), (classes, 4, (k,)), (scores, torch.int32, (k,))], stream)
+        self._windows_call("bnm_scan_windows_topk", pages, stride, [int(k), (classes, 4, (k,)), (scores, torch.int32, (k,))], stream,
+                           padding, pad_mode, pad_value)
 
-    def emulate_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None) -> None:
+    def emulate_windows_device(self, pages, stride, logits=None, labels=None, stream: Optional[int] = None, *, padding=None,
+                               pad_mode: str = "constant", pad_value: float = 0.0) -> None:
         """The emulator on every window: logits torch.float64 [P, out_h, out_w, n_classes] or None, labels [P, out_h, out_w]
         or None (not both None); ``inference_quantized_device`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_emulate_windows_device, self.lib.bnm_emulate_windows_device_f16, pages, stride,
-                           [(logits, torch.float64, (self.n_classes,)), (labels, 4, ())], stream)
+        self._windows_call("bnm_emulate_windows", pages, stride, [(logits, torch.float64, (self.n_classes,)), (labels, 4, ())], stream,
+                           padding, pad_mode, pad_value)
 
-    def emulate_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None) -> None:
+    def emulate_windows_topk_device(self, pages, stride, k: int, classes, scores=None, stream: Optional[int] = None, *, padding=None,
+                                    pad_mode: str = "constant", pad_value: float = 0.0) -> None:
         """The emulator's top-k of every window: classes [P, out_h, out_w, k], scores torch.float64 [P, out_h, out_w, k] or
         None; ``emulate_topk_device`` on each window."""
         import torch
-        self._windows_call(self.lib.bnm_emulate_windows_topk_device, self.lib.bnm_emulate_windows_topk_device_f16, pages, stride,
-                           [int(k), (classes, 4, (k,)), (scores, torch.float64, (k,))], stream)
+        self._windows_call("bnm_emulate_windows_topk", pages, stride, [int(k), (classes, 4, (k,)), (scores, torch.float64, (k,))],
+                           stream, padding, pad_mode, pad_value)
 
     def compare_engines_device(self, images, truth=None, labels_c=None, labels_py=None, counts=None, stream: Optional[int] = None) -> None:
         """Both engines on the same float images in one call (test_inference.py:130-175): images torch.float32 [n, img_bytes] on

@@ -28,7 +28,7 @@
  * on different streams, and each call's results are exactly those of the same call made alone.  The exceptions are
  * bnm_model_set_option and bnm_model_destroy: like any handle's, they must not overlap other calls on that model.  A call's
  * device scratch (CNN features, the layer-by-layer path's buffers, scaled images and windows, the emulator's planes) is its own,
- * the window entries' of sections 9 and 10 included, allocated
+ * the window entries' of sections 9, 10, 12 and 13 included, allocated
  * stream-ordered on the call's stream from a memory pool of the model that keeps what it has: concurrency costs memory, as each
  * call in flight holds its own chunk's scratch -- for example 256 MB of CNN features per 2^20-image chunk -- and the pool holds
  * the most that was ever in flight at once until the model is destroyed.  No call synchronises the host with another.
@@ -46,7 +46,9 @@
  * 16-bit entries of section 11: bnm_infer_batch_device_f16, bnm_emulate_batch_device_f16, bnm_compare_engines_device_f16,
  * bnm_infer_topk_device_f16, bnm_emulate_topk_device_f16 and bnm_quantize_images_device_f16, and the four 16-bit window entries of
  * section 12: bnm_scan_windows_device_f16, bnm_scan_windows_topk_device_f16, bnm_emulate_windows_device_f16 and
- * bnm_emulate_windows_topk_device_f16) may be captured into a CUDA graph on
+ * bnm_emulate_windows_topk_device_f16, and the eight padded window entries of section 13: bnm_scan_windows_padded_device,
+ * bnm_scan_windows_topk_padded_device, bnm_emulate_windows_padded_device, bnm_emulate_windows_topk_padded_device and their
+ * _f16 forms) may be captured into a CUDA graph on
  * its stream, in any capture mode, in any combination and from any thread.  Each replay gives exactly the results of the same call made eagerly on the buffers'
  * contents at replay time; bnm_compare_engines_device adds to `counts` on every replay.  A graph keeps what its capture decided:
  * the route, the routing options (BNM_OPT_PATH, BNM_OPT_CHUNK_IMAGES, BNM_OPT_CNN_FRONTEND, BNM_OPT_LAUNCH_OVERLAP) and the
@@ -491,6 +493,60 @@ BNM_API int bnm_emulate_windows_device_f16(bnm_model *m, const bnm_windows_f16 *
                                            void *stream);
 BNM_API int bnm_emulate_windows_topk_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format, uint32_t k, uint32_t *classes,
                                                 double *scores, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 13. Padded pages: the window scan of sections 10 and 12 over pages with a border of up to 15 pixels on each side, made as
+ *     torch.nn.functional.pad makes it, without a padded copy of the stack.  With 7 pixels before and 8 after, at stride 1, a
+ *     page of H x W pixels has H x W windows, one centred on every pixel.
+ * ------------------------------------------------------------------------------------------- */
+enum { BNM_PAD_CONSTANT = 0, BNM_PAD_REPLICATE = 1, BNM_PAD_REFLECT = 2 };
+typedef struct bnm_window_padding {
+    uint32_t left, right, top, bottom;  /* pixels added on each side of every plane: 0..15 (torch.nn.functional.pad's order) */
+    uint32_t mode;                       /* BNM_PAD_*                                                                        */
+    float value;                         /* BNM_PAD_CONSTANT: the border's pixel value, float32 (for 16-bit planes too)       */
+} bnm_window_padding;
+/* Each entry below is the sibling named beside it with `const bnm_window_padding *padding` after the descriptor (after `format`
+ * for the 16-bit ones):
+ *   bnm_scan_windows_padded_device             bnm_scan_windows_device
+ *   bnm_scan_windows_topk_padded_device        bnm_scan_windows_topk_device
+ *   bnm_emulate_windows_padded_device          bnm_emulate_windows_device
+ *   bnm_emulate_windows_topk_padded_device     bnm_emulate_windows_topk_device
+ *   bnm_scan_windows_padded_device_f16         bnm_scan_windows_device_f16
+ *   bnm_scan_windows_topk_padded_device_f16    bnm_scan_windows_topk_device_f16
+ *   bnm_emulate_windows_padded_device_f16      bnm_emulate_windows_device_f16
+ *   bnm_emulate_windows_topk_padded_device_f16 bnm_emulate_windows_topk_device_f16
+ * Every output is bit for bit the sibling's output on F.pad(pages.float(), (left, right, top, bottom), mode, value), the modes
+ * named as torch names them: BNM_PAD_CONSTANT fills the border with `value` (used as float32, for 16-bit planes too),
+ * BNM_PAD_REPLICATE repeats the edge pixel, BNM_PAD_REFLECT mirrors the page about the edge pixel, which is not repeated.  The
+ * grid is out_h = (height + top + bottom - 16) / stride_y + 1 when height + top + bottom >= 16, else 0 (out_w likewise, computed
+ * in 64 bits); window (p, r, c) covers padded rows r * stride_y .. + 15 and padded columns c * stride_x .. + 15 of plane p, in
+ * section 10's order and layout.  Only pixels inside [0, height) x [0, width) of each plane are read: pitch padding, rows below a
+ * page and gaps between planes never are.  So a NaN or infinite pixel that the border repeats or mirrors makes every window
+ * covering a copy of it the all-zero row, and a NaN or infinite `value` does so to every window touching the border (sections 5
+ * and 9).  Argument checks are the sibling's, and BNM_E_ARG for a NULL padding, a side over 15, a mode outside BNM_PAD_*,
+ * reflect padding with top or bottom >= height or left or right >= width (torch's rule), or a padded page over 2^32 - 1 pixels
+ * either way.  planes == 0, height == 0 or width == 0: returns 0 and writes nothing.  Routes are the sibling's, with the same
+ * scaling kernel: "windows route: <padded entry>: k_quantize_windows + ..." under BNM_VERBOSE.  Threads, per-call scratch,
+ * graphs ("Graphs") and BNM_OPT_LAUNCH_OVERLAP mode 2 (a launch of another kind: its fused launch and the int8 launch after it
+ * keep their wait) follow the sibling.  Asynchronous on `stream`, no host synchronisation. */
+BNM_API int bnm_scan_windows_padded_device(bnm_model *m, const bnm_windows *windows, const bnm_window_padding *padding, int32_t *logits,
+                                           uint32_t *labels, void *stream);
+BNM_API int bnm_scan_windows_topk_padded_device(bnm_model *m, const bnm_windows *windows, const bnm_window_padding *padding, uint32_t k,
+                                                uint32_t *classes, int32_t *scores, void *stream);
+BNM_API int bnm_emulate_windows_padded_device(bnm_model *m, const bnm_windows *windows, const bnm_window_padding *padding, double *logits,
+                                              uint32_t *labels, void *stream);
+BNM_API int bnm_emulate_windows_topk_padded_device(bnm_model *m, const bnm_windows *windows, const bnm_window_padding *padding, uint32_t k,
+                                                   uint32_t *classes, double *scores, void *stream);
+BNM_API int bnm_scan_windows_padded_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format, const bnm_window_padding *padding,
+                                               int32_t *logits, uint32_t *labels, void *stream);
+BNM_API int bnm_scan_windows_topk_padded_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format,
+                                                    const bnm_window_padding *padding, uint32_t k, uint32_t *classes, int32_t *scores,
+                                                    void *stream);
+BNM_API int bnm_emulate_windows_padded_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format,
+                                                  const bnm_window_padding *padding, double *logits, uint32_t *labels, void *stream);
+BNM_API int bnm_emulate_windows_topk_padded_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format,
+                                                       const bnm_window_padding *padding, uint32_t k, uint32_t *classes, double *scores,
+                                                       void *stream);
 
 #ifdef __cplusplus
 }
