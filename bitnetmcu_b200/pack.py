@@ -170,15 +170,23 @@ def random_fc_model(enc: int, widths: Sequence[int] = (256, 64, 64, 64, 10), see
     return m
 
 
+def max_n_activations(model: M.Model) -> int:
+    """MAX_N_ACTIVATIONS of a header: the size of BitMnistInference's stack buffers (BitNetMCU_MNIST_dll.c:49-50,96-97).
+    The exporter writes the widest layer input (exportquant.py:64), but the driver also keeps each layer's outputs there and,
+    for CNN models, uses the int32 buffer as 16x16 scratch and the int8 one as the channels x 4 int32 features: fewer than
+    256 would overflow the stack of a 16-channel model."""
+    fc = model.fc_layers
+    return max([256, model.channels * 4] + [l.n_in for l in fc] + [l.n_out for l in fc])
+
+
 def write_header(model: M.Model, path: str, runname: str = "bitnetmcu_b200") -> None:
     """Emit a reference-compatible ``BitNetMCU_model.h`` (exportquant.py:68-84,164-259)."""
-    fc = [l for l in model.layers if l.kind == M.LAYER_FC]
     cls = "CNNMNIST" if model.model_class == M.MODEL_CNNMNIST else "FCMNIST"
     out = ["// Automatically generated header file", f"// Quantized model exported from {runname}",
            "// Generated by bitnetmcu_b200.pack.write_header (layout of exportquant.py)", "", "#include <stdint.h>", "",
            "#ifndef BITNETMCU_MODEL_H", "#define BITNETMCU_MODEL_H", "", f"#define MODEL_{cls}", "",
            f"#define NUM_LAYERS {len(model.layers)}", "",
-           f"#define MAX_N_ACTIVATIONS {max([l.n_in for l in fc] + [model.channels * 4])}", ""]
+           f"#define MAX_N_ACTIVATIONS {max_n_activations(model)}", ""]
     for l in model.layers:
         n = l.name
         if l.kind == M.LAYER_FC:
