@@ -270,7 +270,7 @@ static int build_fc_dev(bnm_model *m) {
     // fused plan (may legitimately be unavailable for exotic shapes: the layered path then serves the model)
     char err[256] = {0};
     uint32_t in_bytes = m->model_class == BNM_MODEL_CNNMNIST ? m->feat_stride : m->img_bytes;
-    m->plan = fc_chain_plan_create(m->fc.data(), (int)m->fc.size(), in_bytes, m->device, m->sm_count, err, sizeof(err));
+    m->plan = fc_chain_plan_create(m->fc.data(), (int)m->fc.size(), in_bytes, m->device, m->sm_count, m->verbose, err, sizeof(err));
     m->plan_err = err;
     fc_chain_plan_set_overlap(m->plan, effective_overlap(m));
     return 0;
@@ -500,6 +500,8 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         if (cudaMemPoolCreate(&m->pool, &props) != cudaSuccess || cudaMemPoolSetAttribute(m->pool, cudaMemPoolAttrReleaseThreshold, &keep) != cudaSuccess)
             rc = fail(BNM_E_CUDA, "scratch memory pool: %s", cudaGetErrorString(cudaGetLastError()));
     }
+    // before the plan: a rebuild (BNM_OPT_NF4_EXTENSION) keeps the diagnostics of the model's creation, whatever the environment then
+    m->verbose = getenv("BNM_VERBOSE") != nullptr;
     if (rc == 0) rc = build_fc_dev(m);
     if (rc == 0 && m->d_err.grow(sizeof(int), true) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaMalloc failed");
     if (rc == 0) {
@@ -508,7 +510,6 @@ extern "C" int bnm_model_create(int model_class, const bnm_layer *layers, uint32
         if (rc == 0 && cudaStreamCreateWithFlags(&m->small.stream, cudaStreamNonBlocking) != cudaSuccess) rc = fail(BNM_E_CUDA, "cudaStreamCreate failed");
     }
     if (rc != 0) { std::string keep = g_err; bnm_model_destroy(m); g_err = keep; return rc; }
-    m->verbose = getenv("BNM_VERBOSE") != nullptr;
     if (m->verbose) {   // diagnostics: the routes of bnm_emulate_batch_device and bnm_compare_engines_device on the default path
         print_route(m, "emulator route", choose_route(m, kEngineEmul, kInF32, false));
         print_route(m, "engines route", choose_route(m, kEngineBoth, kInF32, false));

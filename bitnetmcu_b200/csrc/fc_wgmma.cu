@@ -161,7 +161,7 @@ struct FcChainPlan {
         bool valid = false;
     };
     LaunchRecord eager, captured;
-    bool verbose = false;             // BNM_VERBOSE at plan creation: every int8-form launch names its wait decision
+    bool verbose = false;             // every int8-form launch names its wait decision (fc_chain_plan_create)
     // guards the tensor-map cache and the bookkeeping above together with the launch they describe: launches from several host
     // threads enqueue in the order the bookkeeping records
     std::mutex mu;
@@ -1158,7 +1158,7 @@ static const ChainKernel kTwoPipeRows[3] = {
     row<64, 2, false, 2>("fc_chain_kernel<64,2,2,16,fixed>", fc_chain_kernel<64, 2, false, 2, 16, true>, kFixedOutBytes),
 };
 
-FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
+FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count, bool verbose,
                                   char *err, size_t err_len) {
     auto fail = [&](const char *msg) -> FcChainPlan * { if (err) snprintf(err, err_len, "%s", msg); return nullptr; };
     if (n_layers < 1 || n_layers > kMaxFcLayers) return fail("fused path: 1..8 FC layers");
@@ -1231,7 +1231,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
         forms[f] = layout(s, k, np);
     }
     if (fixed) plan->int8_general = layout(kForms[kFormInt8], &kTwoPipeRows[1], pipes);
-    if (getenv("BNM_VERBOSE")) {   // diagnostics: the shapes this plan launches
+    if (verbose) {   // diagnostics: the shapes this plan launches
         const bool has_float = forms[kFormFloat].kernel;
         auto args = [&](FcForm f) { return has_float ? strchr(forms[f].kernel->name, '<') : ""; };   // the template arguments
         char f_stages[32] = "";
@@ -1245,7 +1245,7 @@ FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32
                 forms[kFormTopK].kernel->name, forms[kFormTopK].n_stages, forms[kFormEmulTopK].kernel->name, forms[kFormEmulTopK].n_stages,
                 forms[kFormTopK].smem_bytes);
     }
-    plan->verbose = getenv("BNM_VERBOSE") != nullptr;
+    plan->verbose = verbose;
     plan->in_bytes = in_bytes;
     plan->sm_count = sm_count;
     plan->device = device;

@@ -150,7 +150,8 @@ void launch_engine_counts(const uint32_t *labels_c, const uint32_t *labels_py, c
 
 // ---- fused wgmma FC chain (fc_wgmma.cu)
 struct FcChainPlan;  // opaque, owned by the model
-FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count,
+// verbose: print the plan's shapes now and every int8-form launch's wait decision (the model's BNM_VERBOSE at its creation)
+FcChainPlan *fc_chain_plan_create(const FcLayerDev *layers, int n_layers, uint32_t in_bytes, int device, int sm_count, bool verbose,
                                   char *err, size_t err_len);
 void fc_chain_plan_destroy(FcChainPlan *p);
 // kFormInt8 launches: 0 plain launches, 1 programmatic dependent launch (inputs read after the previous kernel completed), 2 launches

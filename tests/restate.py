@@ -26,15 +26,16 @@ def scale_images(x):
     return np.where(np.isnan(y), np.float32(0), y).astype(np.int8)
 
 
-def bitlinear(model, act):
+def bitlinear(model, act, nf4_extension=False):
     """the BitLinear layers (BitNetMCU.py:452-457, 527-530) on activations [n, k] -> float64 logits: per layer a float64
     product with the weight levels, a power-of-two rescale of every row to a maximum of at most 127 with round-half-even and
-    ReLU, and no rescale after the last layer"""
+    ReLU, and no rescale after the last layer.  The levels are the engine's integer weights over the level scale: 4bit layers
+    take their integers (the reference's +0.01 offset is not), NF4 layers zeros, or the extension's LUT with nf4_extension."""
     fc = [l for l in model.layers if l.kind == M.LAYER_FC]
     act = act.astype(np.float64)
     for i, l in enumerate(fc):
         # weight levels over the columns the previous layer delivers (Ternary pads n_in with zero trits)
-        w = P.decode_int_weights(l).astype(np.float64)[:, :act.shape[1]] / 2.0 ** LEVEL_SHIFT.get(l.bitperweight, 0)
+        w = P.decode_int_weights(l, nf4_extension).astype(np.float64)[:, :act.shape[1]] / 2.0 ** LEVEL_SHIFT.get(l.bitperweight, 0)
         conv = act @ w.T
         if i + 1 == len(fc):
             return conv
@@ -42,9 +43,9 @@ def bitlinear(model, act):
         act = np.round(conv * np.exp2(np.floor(np.log2(127.0 / top)))).clip(0, 127)
 
 
-def emulate_fc(model, x):
+def emulate_fc(model, x, nf4_extension=False):
     """float32 images [n, img_bytes] of an FC model -> the emulator's float64 logits [n, n_classes]"""
-    return bitlinear(model, scale_images(x))
+    return bitlinear(model, scale_images(x), nf4_extension)
 
 
 def _conv_relu(a, w):
@@ -91,11 +92,11 @@ def cnn_features(model, x):
     return cnn_stages(model, x)[3]
 
 
-def emulate(model, x, block=512):
-    """float32 images -> the emulator's float64 logits, FC and CNN models"""
+def emulate(model, x, block=512, nf4_extension=False):
+    """float32 images -> the emulator's float64 logits, FC and CNN models; NF4 layers decoded as BNM_OPT_NF4_EXTENSION says"""
     if model.model_class == 0:
-        return emulate_fc(model, x)
-    return np.concatenate([bitlinear(model, cnn_features(model, x[i:i + block])) for i in range(0, len(x), block)])
+        return emulate_fc(model, x, nf4_extension)
+    return np.concatenate([bitlinear(model, cnn_features(model, x[i:i + block]), nf4_extension) for i in range(0, len(x), block)])
 
 
 # ---- the C engine's CNN front-end (dll.c:64-80) ------------------------------------------------------------------------------

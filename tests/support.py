@@ -263,6 +263,29 @@ def scattered_edge_images(n, elems, seed):
     return x
 
 
+def quantized_model_list(m, nf4_extension=False):
+    """the reference emulator's layer list for model m (tests/golden/make_emulator_golden.py): weight levels = the integer
+    weights over the encoding's level scale (NF4: zeros, or the extension's LUT with nf4_extension), Ternary's zero pad columns
+    dropped"""
+    from bitnetmcu_b200 import model as M, pack as P
+    from restate import LEVEL_SHIFT
+    out, width = [], m.img_bytes if m.model_class == 0 else m.channels * 4
+    for l in m.layers:
+        if l.kind == M.LAYER_FC:
+            w = P.decode_int_weights(l, nf4_extension).astype(np.float64)[:, :width] / 2.0 ** LEVEL_SHIFT.get(l.bitperweight, 0)
+            width = l.n_out
+            out.append({"layer_type": "BitLinear", "incoming_weights": l.n_in, "outgoing_weights": l.n_out,
+                        "quantized_weights": w.tolist(), "WScale": "PerTensor", "bpw": 0, "quantization_type": M.ENC_NAMES[l.bitperweight]})
+        elif l.kind == M.LAYER_CONV33:
+            first = l.n_in == 16
+            out.append({"layer_type": "BitConv2d", "in_channels": 1 if first else l.n_out, "out_channels": l.n_out, "kernel_size": (3, 3),
+                        "stride": 1, "padding": 0, "groups": 1 if first else l.n_out, "quantized_weights": l.weights.astype(np.float64).tolist(),
+                        "incoming_x": 0, "incoming_y": 0, "outgoing_x": 0, "outgoing_y": 0, "bpw": 8, "quantization_type": "8bit"})
+        else:
+            out.append({"layer_type": "MaxPool2d", "kernel_size": 2, "stride": 2})
+    return out
+
+
 def crafted_cnn_case():
     """images: all zero, and one negative pixel among zeros, then normal rows; models: a random CNN and two whose conv2 or
     conv3 taps are all <= 0 (no positive output on non-negative inputs).  -> (images, [(model, what)])"""

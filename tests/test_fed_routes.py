@@ -29,7 +29,7 @@ import pytest
 from bitnetmcu_b200 import model as M, pack as P
 from restate import TILE, LEVEL_SHIFT, cnn_stages, emulate, scale_images
 from support import CHAIN_ROWS, Sweep, cnn_model, engine, frontends, gather_call, kernel_clone, kernel_copies_are_kernels, \
-    kernel_copy, lib, plan_line, plan_ring, scattered_edge_images, verbose_engine  # noqa: F401  (lib, kernel_copies_are_kernels: fixtures)
+    kernel_copy, lib, plan_line, plan_ring, quantized_model_list, scattered_edge_images, verbose_engine  # noqa: F401  (lib, kernel_copies_are_kernels: fixtures)
 
 REF_PY = "/root/reference"
 N_UNIQUE = 389                        # distinct images per model; batches repeat them (row i is image i % N_UNIQUE)
@@ -205,26 +205,6 @@ def test_float_models_oracle_matches_reference(oracle, reference, row):
     want_lo, want_la = reference.infer(m, imgs)
     lo, la = oracle.infer(m, imgs)
     assert np.array_equal(lo, want_lo) and np.array_equal(la, want_la), row
-
-
-def quantized_model_list(m):
-    """the reference emulator's layer list for model m (tests/golden/make_emulator_golden.py): weight levels = the integer
-    weights over the encoding's level scale, Ternary's zero pad columns dropped"""
-    out, width = [], m.img_bytes if m.model_class == 0 else m.channels * 4
-    for l in m.layers:
-        if l.kind == M.LAYER_FC:
-            w = P.decode_int_weights(l).astype(np.float64)[:, :width] / 2.0 ** LEVEL_SHIFT.get(l.bitperweight, 0)
-            width = l.n_out
-            out.append({"layer_type": "BitLinear", "incoming_weights": l.n_in, "outgoing_weights": l.n_out,
-                        "quantized_weights": w.tolist(), "WScale": "PerTensor", "bpw": 0, "quantization_type": M.ENC_NAMES[l.bitperweight]})
-        elif l.kind == M.LAYER_CONV33:
-            first = l.n_in == 16
-            out.append({"layer_type": "BitConv2d", "in_channels": 1 if first else l.n_out, "out_channels": l.n_out, "kernel_size": (3, 3),
-                        "stride": 1, "padding": 0, "groups": 1 if first else l.n_out, "quantized_weights": l.weights.astype(np.float64).tolist(),
-                        "incoming_x": 0, "incoming_y": 0, "outgoing_x": 0, "outgoing_y": 0, "bpw": 8, "quantization_type": "8bit"})
-        else:
-            out.append({"layer_type": "MaxPool2d", "kernel_size": 2, "stride": 2})
-    return out
 
 
 @pytest.mark.skipif(not os.path.isfile(os.path.join(REF_PY, "BitNetMCU.py")), reason="needs the reference's BitNetMCU.py")

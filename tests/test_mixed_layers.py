@@ -30,7 +30,8 @@ from bitnetmcu_b200 import model as M, pack as P
 from conftest import load_model
 from restate import LEVEL_SHIFT, Plan, emulate, plan_of, scale_images
 from support import (Sweep, both_engines, c_float, chain, emulator, fp130_codes, int8_images, lib, out, plan_line, plan_ring,  # noqa: F401
-                     scattered_edge_images, to_device as t, top_k, verbose_engine, with_plus128)                     # (lib: fixture)
+                     quantized_model_list, scattered_edge_images, to_device as t, top_k, verbose_engine,             # (lib: fixture)
+                     with_plus128)
 
 REF_PY = "/root/reference"
 N_UNIQUE = 389          # distinct images per model; batches repeat them (row i is image i % N_UNIQUE)
@@ -122,11 +123,6 @@ def layout(name):
     return plan_of(model(name), BY_NAME[name].nf4_ext)
 
 
-def exact(m):
-    """restate.emulate is the emulator bit for bit: no 4bit or NF4 layer (their levels are approximated by design)"""
-    return not any(l.bitperweight in (U4, NF4) for l in m.fc_layers)
-
-
 # ---- CPU: the layout and the cases -----------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize("name", NAMES)
@@ -185,11 +181,11 @@ def test_cases_cover_every_layout():
     seen = {(l.bitperweight, "first" if i == 0 else "last" if i + 1 == len(model(n).fc_layers) else "hidden")
             for n in mixed for i, l in enumerate(model(n).fc_layers)}
     assert seen == {(e, p) for e in P.QUANT_IDS.values() for p in ("first", "hidden", "last")}, seen
-    # both emulator logit scales after a first layer of the other scale, on chains the emulator is checked on exactly: on the
-    # one-kernel float forms, and scale 1 after 0.5 on the int8 emulator form too
+    # both emulator logit scales after a first layer of the other scale: on the one-kernel float forms, and scale 1 after 0.5
+    # on the int8 emulator form too
     def scales(float_forms):
         return {(2.0 ** -LEVEL_SHIFT.get(model(n).fc_layers[0].bitperweight, 0), lays[n].logit_scale) for n in mixed
-                if exact(model(n)) and lays[n].float_forms == float_forms}
+                if lays[n].float_forms == float_forms}
     assert {(1.0, 0.5), (0.5, 1.0)} <= scales(True), scales(True)
     assert (0.5, 1.0) in scales(False), scales(False)
     # mixed chains past the float forms' limits: wider than 64, more than 16 classes
@@ -198,18 +194,6 @@ def test_cases_cover_every_layout():
 
 
 # ---- CPU: the models against the unmodified reference -------------------------------------------------------------------------
-
-def quantized_model_list(m):
-    """the reference emulator's layer list for FC model m (tests/golden/make_emulator_golden.py): weight levels = the integer
-    weights over the encoding's level scale, Ternary's zero pad columns dropped"""
-    out, width = [], m.img_bytes
-    for l in m.fc_layers:
-        w = P.decode_int_weights(l).astype(np.float64)[:, :width] / 2.0 ** LEVEL_SHIFT.get(l.bitperweight, 0)
-        width = l.n_out
-        out.append({"layer_type": "BitLinear", "incoming_weights": l.n_in, "outgoing_weights": l.n_out,
-                    "quantized_weights": w.tolist(), "WScale": "PerTensor", "bpw": 0, "quantization_type": M.ENC_NAMES[l.bitperweight]})
-    return out
-
 
 REFERENCE_SAMPLE = [n for n in NAMES if BY_NAME[n].kind != "subset" or n[-4:] in ("1111", "2222", "2111", "1112", "1212")]
 
@@ -226,17 +210,18 @@ def test_oracle_matches_reference(oracle, reference, name):
 
 
 @pytest.mark.skipif(not os.path.isfile(os.path.join(REF_PY, "BitNetMCU.py")), reason="needs the reference's BitNetMCU.py")
-@pytest.mark.parametrize("name", [n for n in REFERENCE_SAMPLE if exact(model(n))])
+@pytest.mark.parametrize("name", REFERENCE_SAMPLE)
 def test_emulate_matches_reference_emulator(name):
-    """restate.emulate equals the reference's QuantizedModel.inference_quantized"""
+    """restate.emulate equals the reference's QuantizedModel.inference_quantized on the engine's integer levels (4bit and NF4
+    layers too, NF4 with the extension where the case has it)"""
     if REF_PY not in sys.path:
         sys.path.append(REF_PY)
     from BitNetMCU import QuantizedModel
-    m = model(name)
+    m, ext = model(name), BY_NAME[name].nf4_ext
     x = scattered_edge_images(N_UNIQUE, m.img_bytes, 9)
     qm = QuantizedModel()
-    qm.quantized_model = quantized_model_list(m)
-    assert np.array_equal(emulate(m, x), np.asarray(qm.inference_quantized(x), dtype=np.float64)), name
+    qm.quantized_model = quantized_model_list(m, ext)
+    assert np.array_equal(emulate(m, x, nf4_extension=ext), np.asarray(qm.inference_quantized(x), dtype=np.float64)), name
 
 
 # ---- GPU helpers --------------------------------------------------------------------------------------------------------------
@@ -246,7 +231,7 @@ class Data:
 
     def __init__(self, name, oracle):
         self.name, self.m, self.ext, self.oracle = name, model(name), BY_NAME[name].nf4_ext, oracle
-        self.exact, self.C = exact(self.m), self.m.n_classes
+        self.C = self.m.n_classes
         seed = NAMES.index(name)
         self.q_np = int8_images(N_UNIQUE, self.m.img_bytes, seed)
         self.x_np = scattered_edge_images(N_UNIQUE, self.m.img_bytes, seed + 1000)
@@ -256,10 +241,9 @@ class Data:
         self.q, self.x, self.lo, self.la, self.xlo, self.xla = map(t, (self.q_np, self.x_np, self.lo_np, self.la_np, xlo, xla.astype(np.int32)))
         self.ks = sorted({1, 5, min(self.C, MAX_TOPK)})
         self.topk_c = {k: tuple(map(t, top_k(self.lo_np, k))) for k in self.ks}
-        if self.exact:
-            emu = emulate(self.m, self.x_np)
-            self.emu, self.emu_la = t(emu), t(np.argmax(emu, axis=1).astype(np.int32))
-            self.topk_py = {k: tuple(map(t, top_k(emu, k))) for k in self.ks}
+        emu = emulate(self.m, self.x_np, nf4_extension=self.ext)
+        self.emu, self.emu_la = t(emu), t(np.argmax(emu, axis=1).astype(np.int32))
+        self.topk_py = {k: tuple(map(t, top_k(emu, k))) for k in self.ks}
         self.half = {}   # format -> the float32 entries' results on the widened rows (half_results)
 
     def idx(self, n):
@@ -315,9 +299,8 @@ def half_results(e, d, fmt):
         xw = d.x.to(getattr(torch, fmt)).float()
         r = {"lo": torch.empty((N_UNIQUE, d.C), dtype=torch.int32, device="cuda"), "la": torch.empty(N_UNIQUE, dtype=torch.int32, device="cuda")}
         e.infer_device_f32(xw, r["lo"], r["la"])
-        if d.exact:
-            r["emu"], r["emu_la"] = torch.empty((N_UNIQUE, d.C), dtype=torch.float64, device="cuda"), torch.empty_like(r["la"])
-            e.inference_quantized_device(xw, r["emu"], r["emu_la"])
+        r["emu"], r["emu_la"] = torch.empty((N_UNIQUE, d.C), dtype=torch.float64, device="cuda"), torch.empty_like(r["la"])
+        e.inference_quantized_device(xw, r["emu"], r["emu_la"])
         torch.cuda.synchronize()
         xw_np = xw.cpu().numpy()
         fin = np.isfinite(xw_np).all(axis=1)
@@ -325,20 +308,18 @@ def half_results(e, d, fmt):
         wlo, wla = d.oracle.infer(d.m, scale_images(xw_np[fin]), nf4_extension=d.ext)
         assert np.array_equal(r["lo"].cpu().numpy()[fin], wlo), (d.name, fmt, "float32 logits on the widened rows")
         assert np.array_equal(r["la"].cpu().numpy()[fin], wla.astype(np.int32)), (d.name, fmt, "float32 labels on the widened rows")
-        if d.exact:
-            assert np.array_equal(r["emu"].cpu().numpy()[fin], emulate(d.m, xw_np[fin])), (d.name, fmt, "emulator on the widened rows")
+        assert np.array_equal(r["emu"].cpu().numpy()[fin], emulate(d.m, xw_np[fin], nf4_extension=d.ext)), \
+            (d.name, fmt, "emulator on the widened rows")
         d.half[fmt] = r
     return d.half[fmt]
 
 
 def top_k_entries(e, d, n, q, x):
-    """the C engine's top-k on the int8 rows, and the emulator's on the float rows where it is exact: classes and scores"""
+    """the C engine's top-k on the int8 rows, and the emulator's on the float rows: classes and scores"""
     import torch
     for k in d.ks:
-        calls = [("C engine", e.topk_device, q, torch.int32, d.topk_c[k])]
-        if d.exact:
-            calls.append(("emulator", e.emulate_topk_device, x, torch.float64, d.topk_py[k]))
-        for what, fn, imgs, dtype, (want_cls, want_sc) in calls:
+        for what, fn, imgs, dtype, (want_cls, want_sc) in (("C engine", e.topk_device, q, torch.int32, d.topk_c[k]),
+                                                           ("emulator", e.emulate_topk_device, x, torch.float64, d.topk_py[k])):
             cls, sc = out((n, k), torch.int32, -1), out((n, k), dtype, -7)
             fn(imgs, k, cls[:n], sc[:n])
             torch.cuda.synchronize()
@@ -381,15 +362,13 @@ def test_entries(lib, oracle, capfd, monkeypatch, name):
             hlo, hla = e.infer(d.q_np[hi])
             assert np.array_equal(hlo, d.lo_np[hi]) and np.array_equal(hla.astype(np.int32), d.la_np[hi]), (name, n, "host pipeline")
             c_float(e, d, n, x, d.xlo, d.xla, "float32")
-            if d.exact:
-                emulator(e, d, n, x, d.emu, d.emu_la, "float32")
-            both_engines(e, d, n, x, d.xla, d.emu_la if d.exact else None, "float32")
+            emulator(e, d, n, x, d.emu, d.emu_la, "float32")
+            both_engines(e, d, n, x, d.xla, d.emu_la, "float32")
             for fmt in ("float16", "bfloat16"):
                 h, xh = half_results(e, d, fmt), x.to(getattr(torch, fmt))
                 c_float(e, d, n, xh, h["lo"], h["la"], fmt)
-                if d.exact:
-                    emulator(e, d, n, xh, h["emu"], h["emu_la"], fmt)
-                both_engines(e, d, n, xh, h["la"], h.get("emu_la"), fmt)
+                emulator(e, d, n, xh, h["emu"], h["emu_la"], fmt)
+                both_engines(e, d, n, xh, h["la"], h["emu_la"], fmt)
                 del xh
             top_k_entries(e, d, n, q, x)
             del q, x
@@ -417,7 +396,6 @@ def test_layered_path(lib, oracle, name):
             d.check(n, lo, d.lo, -5, "layered int8 logits")
             d.check(n, la, d.la, -7, "layered int8 labels")
             c_float(e, d, n, d.x[i], d.xlo, d.xla, "layered float32")
-            if d.exact:
-                emulator(e, d, n, d.x[i], d.emu, d.emu_la, "layered")
+            emulator(e, d, n, d.x[i], d.emu, d.emu_la, "layered")
     finally:
         e.close()

@@ -35,7 +35,7 @@ from bitnetmcu_b200 import model as M, pack as P
 from restate import (REFUSE_SMEM, SMEM_LIMIT, Plan, batch_size, emulate, plan_lines, plan_of, scale_images,
                      tile_schedule)
 from support import (both_engines, c_float, chain, emulator, int8_images, lib, out, plan_line,  # noqa: F401  (lib: fixture)
-                     run_emulator_layered, scattered_edge_images, to_device, top_k, verbose_engine)
+                     scattered_edge_images, to_device, top_k, verbose_engine)
 
 N_UNIQUE = 389          # distinct images per model; batches repeat them (row i is image i % N_UNIQUE)
 N_DRAWS = 48
@@ -164,11 +164,6 @@ def plan(name):
     return plan_of(model(name), BY_NAME[name].nf4_ext)
 
 
-def exact(m):
-    """restate.emulate is the emulator bit for bit: no 4bit or NF4 layer (their levels are approximated by design)"""
-    return not any(l.bitperweight in (U4, NF4) for l in m.fc_layers)
-
-
 def describe(name):
     m, c = model(name), BY_NAME[name]
     layers = " -> ".join(f"{M.ENC_NAMES[l.bitperweight]}{'+' if len(s) > 2 else ''} {l.n_out}" for l, s in zip(m.fc_layers, c.layers))
@@ -201,10 +196,8 @@ def coverage_gaps():
         if 64 < max(p.n_pad) <= 80 and sorted(p.n_pad)[-2:][0] <= 32:
             seen.add("widest layer 65..80 beside narrow ones")
         if m.img_bytes % 128:
-            seen.add("rows inside an atom: int8")
+            seen |= {"rows inside an atom: int8", "rows inside an atom: emulator"}
             seen |= {"rows inside an atom: float forms"} if p.float_forms else set()
-        if exact(m) and m.img_bytes % 128:
-            seen.add("rows inside an atom: exact emulator")
         if 1 in p.planes and 2 in p.planes:
             seen.add("+128 planes in some layers only")
         if len({l.bitperweight for l in fc}) >= 3:
@@ -233,7 +226,7 @@ def coverage_gaps():
         {"hidden n_out < n_pad", "K-steps rounded past the previous n_pad", "K-steps dropped past the previous n_pad: 1 pipes",
          "K-steps dropped past the previous n_pad: 2 pipes", "K-steps dropped past the previous n_pad: float forms",
          "widest layer 65..80 beside narrow ones", "rows inside an atom: int8", "rows inside an atom: float forms",
-         "rows inside an atom: exact emulator", "+128 planes in some layers only", "three or more encodings",
+         "rows inside an atom: emulator", "+128 planes in some layers only", "three or more encodings",
          "NF4 with the extension", "float forms", "no float forms", "refused: weights do not fit"} | \
         {f"hidden width off 16 into {e}" for e in ("8bit", "4bit", "4bitsym", "FP130", "NF4", "Ternary")} | \
         {"one-pipe-512 boundary", "one-pipe-752 boundary", "two-pipes-384 boundary", "two-pipes-272 boundary",
@@ -312,7 +305,7 @@ class Data:
 
     def __init__(self, name, judge, oracle):
         self.name, self.m, self.ext = name, model(name), BY_NAME[name].nf4_ext
-        self.exact, self.C = exact(self.m), self.m.n_classes
+        self.C = self.m.n_classes
         infer = oracle.infer if self.ext or judge is None else judge.infer
         kw = {"nf4_extension": True} if self.ext else {}
         seed = NAMES.index(name)
@@ -329,19 +322,19 @@ class Data:
         self.topk_c = {k: tuple(map(to_device, top_k(self.lo_np, k))) for k in self.ks}
         self.infer, self.kw = infer, kw
 
-    def emulator_reference(self, e):
-        """the emulator's float64 logits on x_np: restate.emulate where it is exact, else the layer-by-layer emulator"""
-        emu = emulate(self.m, self.x_np) if self.exact else run_emulator_layered(e, self.x_np)[0]
+    def emulator_reference(self):
+        """the emulator's float64 logits on x_np: restate.emulate, NF4 layers decoded as the engine's option says"""
+        emu = emulate(self.m, self.x_np, nf4_extension=self.ext)
         self.emu, self.emu_la = to_device(emu), to_device(np.argmax(emu, axis=1).astype(np.int32))
         self.topk_py = {k: tuple(map(to_device, top_k(emu, k))) for k in self.ks}
 
-    def half(self, e, fmt):
+    def half(self, fmt):
         """the 16-bit rows of fmt on the device and their expectations: (rows, C logits, C labels, emulator logits, labels)"""
         import torch
         xh = to_device(self.xh_np).to(getattr(torch, fmt))
         xw = xh.float().cpu().numpy()
         lo, la = self.infer(self.m, scale_images(xw), **self.kw)
-        emu = emulate(self.m, xw) if self.exact else run_emulator_layered(e, xw)[0]
+        emu = emulate(self.m, xw, nf4_extension=self.ext)
         return xh, to_device(lo), to_device(la.astype(np.int32)), to_device(emu), to_device(np.argmax(emu, axis=1).astype(np.int32))
 
     def idx(self, n):
@@ -408,8 +401,8 @@ def test_entries(lib, judge, oracle, name):
     try:
         p = plan(name)
         big = past_first_trip(p, torch.cuda.get_device_properties(0).multi_processor_count) if isinstance(p, Plan) else 5 * 128 + 37
-        d.emulator_reference(e)
-        halves = [(fmt, d.half(e, fmt)) for fmt in ("float16", "bfloat16")] if NAMES.index(name) % 4 == 0 else []
+        d.emulator_reference()
+        halves = [(fmt, d.half(fmt)) for fmt in ("float16", "bfloat16")] if NAMES.index(name) % 4 == 0 else []
         for n in (1, 129, big):
             i = d.idx(n)
             q, x = d.q[i], d.x[i]
