@@ -1257,7 +1257,9 @@ static int run_call(bnm_model *m, const Call &c) {
         return infer_small(m, static_cast<const int8_t *>(c.images), c.n, static_cast<int32_t *>(o.logits), o.labels);
     CU_TRY(cudaSetDevice(m->device));
     const Route r = choose_route(m, c.engine, c.in, c.topk, c.windows);
-    if ((c.topk || c.windows) && m->verbose) print_route(m, (std::string(c.windows ? "windows route: " : "topk route: ") + c.name).c_str(), r);
+    // the lines of the model's creation name the float32 routes only: a 16-bit call names its own (a 16-bit form or scaling kernel)
+    if ((c.topk || c.windows || half_in(c.in)) && m->verbose)
+        print_route(m, (std::string(c.windows ? "windows route: " : c.topk ? "topk route: " : "16-bit route: ") + c.name).c_str(), r);
     if (o.gather && !r.fused)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     cudaStream_t st = static_cast<cudaStream_t>(c.stream);

@@ -445,7 +445,8 @@ BNM_API int bnm_emulate_windows_topk_device(bnm_model *m, const bnm_windows *win
  * Routes: a 16-bit call takes its sibling's route.  Where that is one kernel with the input scaling fused (FC models on the fused
  * path with rows of up to 256 elements, up to 64 wide and at most 16 classes), that kernel's 16-bit form reads the 16-bit rows;
  * every other route scales each pass of 16-bit images into the call's scratch (k_quantize_images<float16> or <bfloat16>), then
- * runs its int8 route on them.  Asynchronous on `stream`, no host synchronisation. */
+ * runs its int8 route on them.  With BNM_VERBOSE set at model creation every call names its kernels: "16-bit route: <entry>: ..."
+ * ("topk route: <entry>: ..." for the top-k entries).  Asynchronous on `stream`, no host synchronisation. */
 BNM_API int bnm_infer_batch_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, int32_t *logits, uint32_t *labels,
                                        void *stream);
 BNM_API int bnm_emulate_batch_device_f16(bnm_model *m, const uint16_t *images, int format, size_t n, double *logits, uint32_t *labels,

@@ -3,9 +3,12 @@ dumped once, the ring sweep on this GPU, and the models, inputs and device calls
 
 Test modules import the fixture by name (`from support import lib`): pytest finds fixtures in a module's globals."""
 import functools
+import gc
 import os
 import re
 import subprocess
+import time
+from typing import Callable, NamedTuple, Optional, Tuple
 
 import numpy as np
 import pytest
@@ -473,3 +476,199 @@ def build_c_shim(tmp, name):
     subprocess.run(["gcc", "-o", exe, os.path.join(ROOT, "host", "bitnetmcu_b200_test.c"), os.path.join(ROOT, "host", "bitnetmcu_b200_dll.c")] + common,
                    check=True)
     return dll, exe, d
+
+
+# ---- batches past 2^31 and 2^32 bytes ------------------------------------------------------------------------------------------
+# A large batch is periodic: U unique rows (an odd prime), row i of the batch unique row i mod U, built on the device by
+# index_select, so nothing of GB size crosses the host.  Its expected result is the same entry on the U unique rows, pinned to the
+# oracle or to restate, then tiled and compared on the device, in slices.  A 32-bit product anywhere in an offset would displace a
+# read or a write by 2^31 or 2^32 bytes, which with U odd lands on another unique row: check_wrapped_offsets shows, on the CPU, that
+# the expected result there differs for most rows.  Every output buffer holds a sentinel, checked past row n.
+
+U = 8191                        # unique rows of a batch, an odd prime
+P = 89                          # period of a window-scan page in both directions, an odd prime
+SPARE = 128                     # sentinel rows past n in every output buffer
+SLICE_BYTES = 256 << 20         # bytes of a row slice the device builds or compares at a time
+GiB = 1 << 30
+SENTINEL_I32, SENTINEL_F64, SENTINEL_I8 = -0x3C3C3C3D, -7.25e300, -0x3D   # fill of every output buffer
+WRAPS = (1 << 31, 1 << 32)      # the byte displacements of a wrapped 32-bit offset
+
+
+def row_uid(rows):
+    """the unique row of batch rows (NumPy or torch integers)"""
+    return rows % U
+
+
+class Spec(NamedTuple):
+    kind: str                     # the entry's key in its module's expected()
+    name: str                     # the model
+    n: int                        # images or windows
+    in_bytes: Optional[int]       # bytes per input row (None: the window scan, whose pages stay small)
+    outputs: Tuple[str, ...]      # what the call writes
+    uid: Callable = row_uid
+    planes: int = 1               # window scan: pages in the stack
+
+
+def _differ(a, b):
+    return (a != b).reshape(len(a), -1).any(axis=1)
+
+
+def check_wrapped_offsets(case, s, res):
+    """for every read and write of case s whose offsets pass a wrap W (2^31 or 2^32 bytes), the result a read or write displaced
+    by W would give differs from the expected one (res: {output: NumPy [unique, ...]}) for most rows: reads of input row
+    a - W / in_bytes, and the bytes a wrapped write of row a would put over the rows there, on every output of the call"""
+    checked = 0
+    for w in WRAPS:
+        if s.in_bytes and s.n * s.in_bytes > w:
+            assert w % s.in_bytes == 0
+            d = w // s.in_bytes
+            a = np.arange(d, min(s.n, d + U))
+            diff = np.zeros(a.size, dtype=bool)
+            for o in s.outputs:
+                diff |= _differ(res[o][s.uid(a)], res[o][s.uid(a - d)])
+            assert diff.mean() > 0.5, (case, "input", w, d, diff.mean())
+            checked += 1
+        for o in s.outputs:
+            e = np.ascontiguousarray(res[o])
+            rb = e[0].nbytes
+            if s.n * rb <= w:
+                continue
+            b = e.view(np.uint8).reshape(e.shape[0], rb)
+            a = np.arange(-(-w // rb), min(s.n, -(-w // rb) + U))
+            pos = (a * rb - w)[:, None] + np.arange(rb)
+            under = b[s.uid(pos // rb), pos % rb]          # what the rows there hold
+            diff = _differ(b[s.uid(a)], under)
+            assert diff.mean() > 0.5, (case, o, w, diff.mean())
+            checked += 1
+    assert checked, (case, "no offset of this case passes 2^31 bytes")
+    assert s.in_bytes is None or (s.n - 77) & (s.n - 78) == 0, (case, "n is not 77 past a power of two")
+
+
+def _free():
+    import torch
+    gc.collect()
+    torch.cuda.empty_cache()
+    return torch.cuda.mem_get_info()[0]
+
+
+class Case:
+    """one case: its need checked against the free device memory (skip with the figure); on exit its engines closed and its
+    peak device memory (torch's tensors, and what the library held, as the device sees it) and wall time printed"""
+
+    def __init__(self, what, n, need):
+        self.what, self.n, self.need = what, n, need
+        self.engines = []
+
+    def engine(self, make):
+        self.engines.append(make())
+        return self.engines[-1]
+
+    def __enter__(self):
+        import torch
+        free = _free()
+        if free < self.need:
+            pytest.skip(f"{self.what}: needs {self.need / GiB:.1f} GiB of device memory, {free / GiB:.1f} GiB free")
+        torch.cuda.reset_peak_memory_stats()
+        self.free0, self.reserved0 = free, torch.cuda.memory_reserved()
+        self.t0 = time.perf_counter()
+        return self
+
+    def __exit__(self, *exc):
+        import torch
+        torch.cuda.synchronize()
+        # the library's scratch pools keep their high-water mark until the engine closes
+        held = (self.free0 - torch.cuda.mem_get_info()[0]) - (torch.cuda.memory_reserved() - self.reserved0)
+        for e in self.engines:
+            e.close()
+        if exc[0] is None:
+            peak = torch.cuda.max_memory_reserved() - self.reserved0 + held
+            print(f"large batch: {self.what}: n = {self.n}, peak device memory {peak / GiB:.2f} GiB, "
+                  f"wall {time.perf_counter() - self.t0:.2f} s")
+        _free()
+        return False
+
+
+def _dtype(a):
+    import torch
+    return {np.dtype(np.float64): torch.float64, np.dtype(np.int8): torch.int8}.get(a.dtype, torch.int32)
+
+
+def slices(t, n):
+    """(start, end) of row slices of about SLICE_BYTES of tensor t, up to row n"""
+    step = max(1, SLICE_BYTES // (t[0].numel() * t.element_size()))
+    return [(s, min(n, s + step)) for s in range(0, n, step)]
+
+
+def _on_device(unique):
+    """unique rows (NumPy, or a torch tensor for the 16-bit formats NumPy lacks) on the device"""
+    import torch
+    u = unique if isinstance(unique, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(unique))
+    return u.cuda()
+
+
+def periodic(unique, n):
+    """the CUDA batch [n, ...] whose row i is unique row i mod U, built slice by slice with index_select"""
+    import torch
+    u = _on_device(unique)
+    out = torch.empty((n,) + tuple(u.shape[1:]), dtype=u.dtype, device="cuda")
+    for s, e in slices(out, n):
+        torch.index_select(u, 0, row_uid(torch.arange(s, e, device="cuda")), out=out[s:e])
+    return out
+
+
+def _sentinel(dtype):
+    import torch
+    return {torch.float64: SENTINEL_F64, torch.int8: SENTINEL_I8}.get(dtype, SENTINEL_I32)
+
+
+def outputs(res, names, n):
+    """{output: CUDA tensor [n + SPARE, ...] filled with the sentinel}, shaped like the expected rows"""
+    import torch
+    return {o: torch.full((n + SPARE,) + res[o].shape[1:], _sentinel(_dtype(res[o])), dtype=_dtype(res[o]), device="cuda")
+            for o in names}
+
+
+def views(outs, n, lead=None):
+    """rows :n of every output buffer (reshaped to lead + row shape when given)"""
+    return {o: (t[:n] if lead is None else t[:n].reshape(lead + tuple(t.shape[1:]))) for o, t in outs.items()}
+
+
+def want_on_device(got, res, what):
+    """the small call's outputs (CUDA, rows :U') equal the expected NumPy rows: -> them as CUDA tensors"""
+    out = {}
+    for o, t in got.items():
+        w = res[o]
+        g = t[:w.shape[0]].cpu().numpy()
+        bad = np.flatnonzero(_differ(g.astype(w.dtype) if w.dtype == np.uint32 else g, w))
+        assert bad.size == 0, (what, o, "small call", f"{bad.size} unique rows differ from the reference, first {bad[:6].tolist()}")
+        out[o] = t[:w.shape[0]].clone()
+    return out
+
+
+def check_tiled(got, want, n, uid, what):
+    """rows :n of got equal want[uid(row)], compared on the device in slices; rows n: still hold the sentinel"""
+    import torch
+    for o, t in got.items():
+        w = want[o]
+        for s, e in slices(t, n):
+            bad = (t[s:e] != w.index_select(0, uid(torch.arange(s, e, device="cuda")))).reshape(e - s, -1).any(dim=1)
+            if bool(bad.any()):
+                rows = (torch.nonzero(bad)[:6, 0] + s).tolist()
+                raise AssertionError((what, o, f"{int(bad.sum())} rows of {s}..{e} wrong, first {rows}",
+                                      f"byte offsets {[r * t[0].numel() * t.element_size() for r in rows]}"))
+        assert bool((t[n:] == _sentinel(t.dtype)).all()), (what, o, "written past row n")
+
+
+def check_input(x, unique, what):
+    """the periodic batch x still holds its rows"""
+    import torch
+    u = _on_device(unique)
+    for s, e in slices(x, x.shape[0]):
+        assert torch.equal(x[s:e], u.index_select(0, row_uid(torch.arange(s, e, device="cuda")))), (what, "input changed", s)
+
+
+def need(s, res, extra=0):
+    """device bytes of a case: the batch, the outputs with their sentinel rows, and 1 GiB for a comparison slice, the unique rows'
+    results and the library's scratch and planes"""
+    per_row = sum(res[o][0].nbytes for o in s.outputs)
+    return s.n * (s.in_bytes or 0) + (s.n + SPARE) * per_row + GiB + extra

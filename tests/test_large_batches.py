@@ -14,28 +14,21 @@ differs for most rows.  Every output buffer holds a sentinel, checked past row n
 Each case closes its engine (a model's scratch pool keeps what it took), frees its tensors, states the device memory it needs,
 skips with that figure when the GPU has less free, and prints its n, peak device memory and wall time."""
 import functools
-import gc
-import time
-from typing import Callable, NamedTuple, Optional, Tuple
 
 import numpy as np
 import pytest
 
 from conftest import load_model
 from restate import emulate, scale_images
-from support import lib, normal_images, random_fc, verbose_engine  # noqa: F401  (lib: a fixture)
+from support import (WRAPS, GiB, P, SENTINEL_I32, SPARE, U, Case, Spec, check_input, check_tiled,  # noqa: F401
+                     check_wrapped_offsets, lib, need, normal_images, outputs, periodic, random_fc, row_uid, verbose_engine, views,
+                     want_on_device)
+# (lib: a fixture)
 
-U = 8191                        # unique rows of a batch, an odd prime
-P = 89                          # period of a window-scan page in both directions, an odd prime
 PAGE = 4096                     # a window-scan page is PAGE x PAGE floats
 N22, N23, N24, N25 = ((1 << b) + 77 for b in (22, 23, 24, 25))
 K_FUSED_PASS = 1 << 28          # images per fused FC launch (kFusedPass, capi.cu)
 N_GATHER = 2 * 148 * 128 + 77
-SPARE = 128                     # sentinel rows past n in every output buffer
-SLICE_BYTES = 256 << 20         # bytes of a row slice the device builds or compares at a time
-GiB = 1 << 30
-SENTINEL_I32, SENTINEL_F64 = -0x3C3C3C3D, -7.25e300   # fill of every output buffer
-WRAPS = (1 << 31, 1 << 32)      # the byte displacements of a wrapped 32-bit offset
 
 MODELS = {
     "fc": lambda: load_model("fc"),                                 # 4bitsym-64, the fixed-shape row
@@ -120,26 +113,11 @@ def expected(oracle, kind, name):
     return _EXPECTED[key]
 
 
-def row_uid(rows):
-    """the unique row of batch rows (NumPy or torch integers)"""
-    return rows % U
-
-
 def window_uid(rows):
     """the unique window of windows of a stack of pages at stride 1, plane p at phase (7 p, 3 p)"""
     per = (PAGE - 15) * (PAGE - 15)
     p, r = rows // per, rows % per
     return ((r // (PAGE - 15) + 7 * p) % P) * P + (r % (PAGE - 15) + 3 * p) % P
-
-
-class Spec(NamedTuple):
-    kind: str                     # the entry's key in expected()
-    name: str                     # the model
-    n: int                        # images or windows
-    in_bytes: Optional[int]       # bytes per input row (None: the window scan, whose pages stay small)
-    outputs: Tuple[str, ...]      # what the call writes
-    uid: Callable = row_uid
-    planes: int = 1               # window scan: pages in the stack
 
 
 SPECS = {
@@ -173,42 +151,13 @@ GATHERS = [("labels u8", 1, (1 << 32) - 1000, 1 << 32), ("labels", 4, (1 << 29) 
 
 # ---- CPU: a wrapped offset would show ----------------------------------------------------------------------------------------
 
-def _differ(a, b):
-    return (a != b).reshape(len(a), -1).any(axis=1)
-
-
 @pytest.mark.parametrize("case", list(SPECS))
 def test_a_wrapped_offset_shows(oracle, case):
     """for every read and write whose offsets pass a wrap W (2^31 or 2^32 bytes), the result a read or write displaced by W
     would give differs from the expected one for most rows: reads of input row a - W / in_bytes, and the bytes a wrapped write
     of row a would put over the rows there, on the labels of a labels-only call and on every output of the others"""
     s = SPECS[case]
-    res = expected(oracle, s.kind, s.name)
-    checked = 0
-    for w in WRAPS:
-        if s.in_bytes and s.n * s.in_bytes > w:
-            assert w % s.in_bytes == 0
-            d = w // s.in_bytes
-            a = np.arange(d, min(s.n, d + U))
-            diff = np.zeros(a.size, dtype=bool)
-            for o in s.outputs:
-                diff |= _differ(res[o][s.uid(a)], res[o][s.uid(a - d)])
-            assert diff.mean() > 0.5, (case, "input", w, d, diff.mean())
-            checked += 1
-        for o in s.outputs:
-            e = np.ascontiguousarray(res[o])
-            rb = e[0].nbytes
-            if s.n * rb <= w:
-                continue
-            b = e.view(np.uint8).reshape(e.shape[0], rb)
-            a = np.arange(-(-w // rb), min(s.n, -(-w // rb) + U))
-            pos = (a * rb - w)[:, None] + np.arange(rb)
-            under = b[s.uid(pos // rb), pos % rb]          # what the rows there hold
-            diff = _differ(b[s.uid(a)], under)
-            assert diff.mean() > 0.5, (case, o, w, diff.mean())
-            checked += 1
-    assert checked, (case, "no offset of this case passes 2^31 bytes")
-    assert s.in_bytes is None or (s.n - 77) & (s.n - 78) == 0, (case, "n is not 77 past a power of two")
+    check_wrapped_offsets(case, s, expected(oracle, s.kind, s.name))
 
 
 def test_wrapped_gather_rows_land_on_sentinels():
@@ -223,123 +172,6 @@ def test_wrapped_gather_rows_land_on_sentinels():
 
 
 # ---- GPU helpers ---------------------------------------------------------------------------------------------------------------
-
-def _free():
-    import torch
-    gc.collect()
-    torch.cuda.empty_cache()
-    return torch.cuda.mem_get_info()[0]
-
-
-class Case:
-    """one case: its need checked against the free device memory (skip with the figure); on exit its engines closed and its
-    peak device memory (torch's tensors, and what the library held, as the device sees it) and wall time printed"""
-
-    def __init__(self, what, n, need):
-        self.what, self.n, self.need = what, n, need
-        self.engines = []
-
-    def engine(self, make):
-        self.engines.append(make())
-        return self.engines[-1]
-
-    def __enter__(self):
-        import torch
-        free = _free()
-        if free < self.need:
-            pytest.skip(f"{self.what}: needs {self.need / GiB:.1f} GiB of device memory, {free / GiB:.1f} GiB free")
-        torch.cuda.reset_peak_memory_stats()
-        self.free0, self.reserved0 = free, torch.cuda.memory_reserved()
-        self.t0 = time.perf_counter()
-        return self
-
-    def __exit__(self, *exc):
-        import torch
-        torch.cuda.synchronize()
-        # the library's scratch pools keep their high-water mark until the engine closes
-        held = (self.free0 - torch.cuda.mem_get_info()[0]) - (torch.cuda.memory_reserved() - self.reserved0)
-        for e in self.engines:
-            e.close()
-        if exc[0] is None:
-            peak = torch.cuda.max_memory_reserved() - self.reserved0 + held
-            print(f"large batch: {self.what}: n = {self.n}, peak device memory {peak / GiB:.2f} GiB, "
-                  f"wall {time.perf_counter() - self.t0:.2f} s")
-        _free()
-        return False
-
-
-def _dtype(a):
-    import torch
-    return torch.float64 if a.dtype == np.float64 else torch.int32
-
-
-def slices(t, n):
-    """(start, end) of row slices of about SLICE_BYTES of tensor t, up to row n"""
-    step = max(1, SLICE_BYTES // (t[0].numel() * t.element_size()))
-    return [(s, min(n, s + step)) for s in range(0, n, step)]
-
-
-def periodic(unique, n):
-    """the CUDA batch [n, ...] whose row i is unique row i mod U, built slice by slice with index_select"""
-    import torch
-    u = torch.from_numpy(np.ascontiguousarray(unique)).cuda()
-    out = torch.empty((n,) + tuple(u.shape[1:]), dtype=u.dtype, device="cuda")
-    for s, e in slices(out, n):
-        torch.index_select(u, 0, row_uid(torch.arange(s, e, device="cuda")), out=out[s:e])
-    return out
-
-
-def _sentinel(dtype):
-    import torch
-    return SENTINEL_F64 if dtype == torch.float64 else SENTINEL_I32
-
-
-def outputs(res, names, n):
-    """{output: CUDA tensor [n + SPARE, ...] filled with the sentinel}, shaped like the expected rows"""
-    import torch
-    return {o: torch.full((n + SPARE,) + res[o].shape[1:], _sentinel(_dtype(res[o])), dtype=_dtype(res[o]), device="cuda")
-            for o in names}
-
-
-def views(outs, n, lead=None):
-    """rows :n of every output buffer (reshaped to lead + row shape when given)"""
-    return {o: (t[:n] if lead is None else t[:n].reshape(lead + tuple(t.shape[1:]))) for o, t in outs.items()}
-
-
-def want_on_device(got, res, what):
-    """the small call's outputs (CUDA, rows :U') equal the expected NumPy rows: -> them as CUDA tensors"""
-    import torch
-    out = {}
-    for o, t in got.items():
-        w = res[o]
-        g = t[:w.shape[0]].cpu().numpy()
-        bad = np.flatnonzero(_differ(g.astype(w.dtype) if w.dtype == np.uint32 else g, w))
-        assert bad.size == 0, (what, o, "small call", f"{bad.size} unique rows differ from the reference, first {bad[:6].tolist()}")
-        out[o] = t[:w.shape[0]].clone()
-    return out
-
-
-def check_tiled(got, want, n, uid, what):
-    """rows :n of got equal want[uid(row)], compared on the device in slices; rows n: still hold the sentinel"""
-    import torch
-    for o, t in got.items():
-        w = want[o]
-        for s, e in slices(t, n):
-            bad = (t[s:e] != w.index_select(0, uid(torch.arange(s, e, device="cuda")))).reshape(e - s, -1).any(dim=1)
-            if bool(bad.any()):
-                rows = (torch.nonzero(bad)[:6, 0] + s).tolist()
-                raise AssertionError((what, o, f"{int(bad.sum())} rows of {s}..{e} wrong, first {rows}",
-                                      f"byte offsets {[r * t[0].numel() * t.element_size() for r in rows]}"))
-        assert bool((t[n:] == _sentinel(t.dtype)).all()), (what, o, "written past row n")
-
-
-def check_input(x, unique, what):
-    """the periodic batch x still holds its rows"""
-    import torch
-    u = torch.from_numpy(np.ascontiguousarray(unique)).cuda()
-    for s, e in slices(x, x.shape[0]):
-        assert torch.equal(x[s:e], u.index_select(0, row_uid(torch.arange(s, e, device="cuda")))), (what, "input changed", s)
-
 
 def _engine(name, path=0, frontend=None):
     from bitnetmcu_b200 import _lib
@@ -366,13 +198,6 @@ def run(e, kind, x, o):
 
 def rows_of(s):
     return rows_f32(s.name) if s.kind in ("c_f32", "emul", "engines") else rows_i8(s.name)
-
-
-def need(s, res, extra=0):
-    """device bytes of a case: the batch, the outputs with their sentinel rows, and 1 GiB for a comparison slice, the unique rows'
-    results and the library's scratch and planes"""
-    per_row = sum(res[o][0].nbytes for o in s.outputs)
-    return s.n * (s.in_bytes or 0) + (s.n + SPARE) * per_row + GiB + extra
 
 
 def entry_case(oracle, case, e_factory, what=None):
