@@ -32,12 +32,14 @@ EXPORTED = [
     "bnm_scan_windows_padded_device", "bnm_scan_windows_topk_padded_device", "bnm_emulate_windows_padded_device",
     "bnm_emulate_windows_topk_padded_device", "bnm_scan_windows_padded_device_f16", "bnm_scan_windows_topk_padded_device_f16",
     "bnm_emulate_windows_padded_device_f16", "bnm_emulate_windows_topk_padded_device_f16",
+    "bnm_scan_windows", "bnm_scan_windows_topk", "bnm_emulate_windows", "bnm_emulate_windows_topk",
 ]
 
 PATH_AUTO, PATH_LAYERS, PATH_TCGEN05 = 0, 1, 2
 OPT_PATH, OPT_NF4_EXTENSION, OPT_CHUNK_IMAGES, OPT_LAUNCH_OVERLAP, OPT_CNN_FRONTEND = 1, 2, 3, 4, 5
 CNN_AUTO, CNN_CUDA_CORES, CNN_TENSOR_CORES = 0, 1, 2
 FLOAT16, BFLOAT16 = 1, 2   # BNM_FLOAT16, BNM_BFLOAT16 (section 11)
+FLOAT32 = 3                # BNM_FLOAT32 (section 14: host pages)
 PAD_CONSTANT, PAD_REPLICATE, PAD_REFLECT = 0, 1, 2   # BNM_PAD_* (section 13)
 
 
@@ -68,6 +70,13 @@ class BnmWindowPadding(C.Structure):
     torch.nn.functional.pad's order, its mode (PAD_*) and the constant mode's fill value."""
     _fields_ = [("left", C.c_uint32), ("right", C.c_uint32), ("top", C.c_uint32), ("bottom", C.c_uint32), ("mode", C.c_uint32),
                 ("value", C.c_float)]
+
+
+class BnmWindowsHost(C.Structure):
+    """bnm_windows_host (include/bitnetmcu_b200.h section 14): a stack of equally sized planes in host memory, their element
+    format (FLOAT32, FLOAT16 or BFLOAT16), pitches in elements and the window strides."""
+    _fields_ = [("image", C.c_void_p), ("format", C.c_int), ("planes", C.c_uint32), ("height", C.c_uint32), ("width", C.c_uint32),
+                ("pitch", C.c_size_t), ("plane_pitch", C.c_size_t), ("stride_y", C.c_uint32), ("stride_x", C.c_uint32)]
 
 
 _lib = None
@@ -139,6 +148,10 @@ def load() -> C.CDLL:
                                                             vp]),
         "bnm_emulate_windows_topk_padded_device_f16": (C.c_int, [vp, C.POINTER(BnmWindows), C.c_int, C.POINTER(BnmWindowPadding), u32,
                                                                  vp, vp, vp]),
+        "bnm_scan_windows": (C.c_int, [vp, C.POINTER(BnmWindowsHost), C.POINTER(BnmWindowPadding), vp, vp]),
+        "bnm_scan_windows_topk": (C.c_int, [vp, C.POINTER(BnmWindowsHost), C.POINTER(BnmWindowPadding), u32, vp, vp]),
+        "bnm_emulate_windows": (C.c_int, [vp, C.POINTER(BnmWindowsHost), C.POINTER(BnmWindowPadding), vp, vp]),
+        "bnm_emulate_windows_topk": (C.c_int, [vp, C.POINTER(BnmWindowsHost), C.POINTER(BnmWindowPadding), u32, vp, vp]),
         "ReLUNorm": (u32, [vp, vp, u32]),
         "processfclayer": (None, [vp, vp, i32, u32, u32, vp]),
         "processconv33ReLU": (vp, [vp, vp, u32, u32, vp]),

@@ -912,9 +912,65 @@ static int infer_small(bnm_model *m, const int8_t *images, size_t n, int32_t *lo
     return rc;
 }
 
-// Route r (not the two engines' one) on host buffers in chunks of chunk_images, each through one slot's buffers: images in,
-// run_route, out's arrays back.  Synchronous.
-static int infer_pipelined(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out) {
+// A band of a host window scan (section 14): window rows row .. row + rows - 1 of planes plane .. plane + planes - 1 (several
+// planes: whole ones, rows == out_h), its windows contiguous in window order.
+struct WindowBand {
+    size_t plane, planes;
+    uint32_t row, rows;
+};
+static const size_t kBandWindows = kPass;   // windows per band at most: the window route's pass
+
+// the page rows [*a, *e) that window rows r0 .. r1 - 1 of page grid g read (the first window row of a plane starts at page row
+// -top): the rows their windows cover and, with reflect, down to the mirror image of the topmost border row they read, which the
+// windows need not cover (out_h * stride_y small next to top).  The bottom border's mirror rows are covered by the band rule
+static void band_rows(const WindowGrid &g, uint32_t r0, uint32_t r1, long long *a, long long *e) {
+    const long long y0 = (long long)r0 * g.stride_y - g.top;   // the first window's first page row
+    *a = std::max(0ll, y0);
+    *e = std::min((long long)g.height, (long long)(r1 - 1) * g.stride_y - g.top + 16);
+    if (g.pad_mode == kPadReflect && y0 < 0) *e = std::max(*e, std::min((long long)g.height, 1 - y0));
+}
+
+// The bands of page grid g (of elem-byte pixels) at `budget` bytes of page pixels per band: the rule of the header's section 14.
+// Each band's rows contain every page row its windows read, the border rows that replicate or reflect padding maps onto included.
+static std::vector<WindowBand> window_bands(const WindowGrid &g, size_t elem, size_t budget) {
+    std::vector<WindowBand> bands;
+    const size_t row_bytes = (size_t)g.width * elem, plane_windows = (size_t)g.out_h * g.out_w;
+    long long a, e;
+    band_rows(g, 0, g.out_h, &a, &e);
+    const size_t plane_bytes = (size_t)(e - a) * row_bytes;
+    if (plane_bytes <= budget && plane_windows <= kBandWindows) {   // runs of whole planes
+        const size_t per = std::min(budget / plane_bytes, kBandWindows / plane_windows);
+        for (size_t p = 0; p < g.planes; p += per) bands.push_back({p, std::min(per, g.planes - p), 0, g.out_h});
+        return bands;
+    }
+    const long long sy = g.stride_y, top = g.top, H = g.height;
+    const long long by_bytes = ((long long)(budget / row_bytes) - 16) / sy + 1;   // may be < 1: one window row is the least
+    const size_t R = (size_t)std::max(1ll, std::min(by_bytes, (long long)(kBandWindows / g.out_w)));
+    // the first band: every window row that starts in the top border (band_rows adds the rows reflect mirrors them onto)
+    const size_t head = (size_t)((top + sy - 1) / sy);
+    // t: the band holding window row t runs to the plane's end (none when no window reaches below the page)
+    size_t t = g.out_h;
+    const long long over = (long long)(g.out_h - 1) * sy - top + 16 - H;   // rows the last window reaches below the page
+    if (over > 0) {
+        t = H + top >= 16 ? (size_t)((H + top - 16) / sy + 1) : 0;   // the first row reaching into the bottom border
+        if (g.pad_mode == kPadReflect) t = std::min(t, (size_t)((H - 1 - over + top) / sy));
+    }
+    for (size_t p = 0; p < g.planes; p++)
+        for (size_t s = 0, end; s < g.out_h; s = end) {
+            end = s ? s + R : std::max(R, head);
+            if (end > t || end >= g.out_h) end = g.out_h;
+            bands.push_back({p, 1, (uint32_t)s, (uint32_t)(end - s)});
+        }
+    return bands;
+}
+
+// Route r (not the two engines' one) on host buffers, each unit through one slot's buffers: its input in, run_route, out's arrays
+// back, those copies enqueued after the next unit's input and kernels so that a pageable destination, which blocks the thread
+// until its copy is done, does not hold up the next unit.  The units are chunks of chunk_images images, or with win the bands of
+// the window scan of the host pages of grid win (window_bands), each band's page rows copied into the slot's staging and scanned
+// there through a grid shifted to the band.  Synchronous.  name: the entry, for the band line under BNM_VERBOSE.
+static int infer_pipelined(bnm_model *m, const Route &r, const void *images, size_t n, const FcOutputs &out,
+                           const WindowGrid *win = nullptr, const char *name = nullptr) {
     RelaxedCaptureMode relaxed;
     std::lock_guard<std::mutex> turn(m->host_mu);   // large host calls take turns: each one keeps the copy engines busy alone
     const size_t chunk = std::min(n, m->chunk_images), k = out.topk.k;
@@ -922,34 +978,86 @@ static int infer_pipelined(bnm_model *m, const Route &r, const void *images, siz
     // int32; bnm_infer_batch sizes it and d_labels whether or not it takes them), d_labels the label, d_classes the top-k classes
     const size_t in_bytes = in_elem_bytes(r.in) * m->img_bytes, el = r.engine == kEngineEmul ? 8 : 4;
     const size_t logit_bytes = (k ? (out.topk.scores ? k : 0) : m->n_classes) * el, label_bytes = k ? 0 : 4, class_bytes = k * 4;
+    // a window scan's bands, and its staging rows: the page's, rounded up to 16 bytes
+    const size_t px = in_elem_bytes(r.in), dpitch = win ? round_up(win->width, 16 / (uint32_t)px) : 0;
+    std::vector<WindowBand> bands;
+    size_t units = (n + chunk - 1) / chunk, items = chunk, staged = chunk * in_bytes;   // per unit at most: images or windows, bytes
+    if (win) {
+        bands = window_bands(*win, px, m->chunk_images * 1024);
+        units = bands.size();
+        items = staged = 0;
+        for (const auto &b : bands) {
+            long long a, e;
+            band_rows(*win, b.row, b.row + b.rows, &a, &e);
+            items = std::max(items, b.planes * b.rows * win->out_w);
+            staged = std::max(staged, b.planes * (size_t)(e - a) * dpitch * px);
+        }
+        if (m->verbose) print_route(m, ("host windows: " + std::string(name) + ": " + std::to_string(units) + " bands").c_str(), r);
+    }
     bool small = false;
     for (auto &s : m->slots)
-        small = small || s.d_images.bytes < chunk * in_bytes || s.d_classes.bytes < chunk * class_bytes ||
-                s.d_logits.bytes < chunk * logit_bytes || s.d_labels.bytes < chunk * label_bytes;
+        small = small || s.d_images.bytes < staged || s.d_classes.bytes < items * class_bytes ||
+                s.d_logits.bytes < items * logit_bytes || s.d_labels.bytes < items * label_bytes;
     if (small) {
         for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));   // no chunk of an earlier call may still use a buffer that is reallocated
         for (auto &s : m->slots) {
-            CU_TRY(s.d_images.grow(chunk * in_bytes));
-            CU_TRY(s.d_classes.grow(chunk * class_bytes));
-            CU_TRY(s.d_logits.grow(chunk * logit_bytes));
-            CU_TRY(s.d_labels.grow(chunk * label_bytes));
+            CU_TRY(s.d_images.grow(staged));
+            CU_TRY(s.d_classes.grow(items * class_bytes));
+            CU_TRY(s.d_logits.grow(items * logit_bytes));
+            CU_TRY(s.d_labels.grow(items * label_bytes));
         }
     }
-    // every chunk's scratch is its own (run_route): the chunks of every path overlap in time on all three streams
+    // every unit's scratch is its own (run_route): the units of every path overlap in time on all three streams
     char *h_logits = static_cast<char *>(k ? out.topk.scores : out.logits);   // where d_logits goes
-    size_t c = 0;
-    for (size_t b = 0; b < n; b += chunk, c++) {
-        const size_t nb = std::min(chunk, n - b);
-        PipeSlot &s = m->slots[c % 3];
-        CU_TRY(cudaMemcpyAsync(s.d_images.p, static_cast<const char *>(images) + b * in_bytes, nb * in_bytes, cudaMemcpyHostToDevice, s.stream));
+    auto copy_out = [&](PipeSlot &s, size_t b, size_t nb) -> int {   // items b .. b + nb - 1 from slot s
+        if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, s.d_classes.p, nb * class_bytes, cudaMemcpyDeviceToHost, s.stream));
+        if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * logit_bytes, s.d_logits.p, nb * logit_bytes, cudaMemcpyDeviceToHost, s.stream));
+        if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, s.d_labels.p, nb * 4, cudaMemcpyDeviceToHost, s.stream));
+        return 0;
+    };
+    PipeSlot *prev = nullptr;
+    size_t prev_b = 0, prev_nb = 0;
+    for (size_t u = 0, b = 0; u < units; u++) {
+        PipeSlot &s = m->slots[u % 3];
+        size_t nb = std::min(chunk, n - b);
+        WindowGrid band;   // the window scan: the band's rows in the slot's staging
+        if (win) {
+            const WindowBand &B = bands[u];
+            long long a, e;
+            band_rows(*win, B.row, B.row + B.rows, &a, &e);
+            const size_t rows = (size_t)(e - a), spitch = win->pitch * px;
+            const char *src = static_cast<const char *>(win->image) + (B.plane * win->plane_pitch + (size_t)a * win->pitch) * px;
+            if (B.planes > 1 && rows == win->height && win->plane_pitch == win->height * win->pitch)   // one run of rows
+                CU_TRY(cudaMemcpy2DAsync(s.d_images.p, dpitch * px, src, spitch, win->width * px, B.planes * rows, cudaMemcpyHostToDevice, s.stream));
+            else
+                for (size_t p = 0; p < B.planes; p++)
+                    CU_TRY(cudaMemcpy2DAsync(s.d_images.p + p * rows * dpitch * px, dpitch * px, src + p * win->plane_pitch * px, spitch,
+                                             win->width * px, rows, cudaMemcpyHostToDevice, s.stream));
+            band = *win;
+            band.image = s.d_images.p;
+            band.planes = (uint32_t)B.planes;
+            band.height = (uint32_t)rows;
+            band.pitch = dpitch;
+            band.plane_pitch = B.planes > 1 ? rows * dpitch : 0;
+            band.out_h = B.rows;
+            band.top = (uint32_t)(a - ((long long)B.row * win->stride_y - win->top));   // > 0 in a plane's first band only
+            nb = B.planes * B.rows * win->out_w;
+        } else {
+            CU_TRY(cudaMemcpyAsync(s.d_images.p, static_cast<const char *>(images) + b * in_bytes, nb * in_bytes, cudaMemcpyHostToDevice, s.stream));
+        }
         uint32_t *d_labels = reinterpret_cast<uint32_t *>(s.d_labels.p), *d_classes = reinterpret_cast<uint32_t *>(s.d_classes.p);
         const FcOutputs d{out.logits ? s.d_logits.p : nullptr, out.labels ? d_labels : nullptr, nullptr,
                          {(uint32_t)k, d_classes, out.topk.scores ? s.d_logits.p : nullptr}};
-        if (int rc = run_route(m, r, s.d_images.p, nb, d, s.stream, StreamCapture{})) return rc;
-        if (k) CU_TRY(cudaMemcpyAsync(out.topk.classes + b * k, d_classes, nb * class_bytes, cudaMemcpyDeviceToHost, s.stream));
-        if (h_logits) CU_TRY(cudaMemcpyAsync(h_logits + b * logit_bytes, s.d_logits.p, nb * logit_bytes, cudaMemcpyDeviceToHost, s.stream));
-        if (out.labels) CU_TRY(cudaMemcpyAsync(out.labels + b, d_labels, nb * 4, cudaMemcpyDeviceToHost, s.stream));
+        if (int rc = run_route(m, r, s.d_images.p, nb, d, s.stream, StreamCapture{}, win ? &band : nullptr)) return rc;
+        if (prev)
+            if (int rc = copy_out(*prev, prev_b, prev_nb)) return rc;
+        prev = &s;
+        prev_b = b;
+        prev_nb = nb;
+        b += nb;
     }
+    if (prev)
+        if (int rc = copy_out(*prev, prev_b, prev_nb)) return rc;
     for (auto &s : m->slots) CU_TRY(cudaStreamSynchronize(s.stream));
     return 0;
 }
@@ -1253,17 +1361,18 @@ static int run_call(bnm_model *m, const Call &c) {
     if (int rc = check_call(m, c)) return rc;
     if (c.n == 0) return 0;
     const FcOutputs &o = c.out;
-    if (c.host && c.engine == kEngineC && !c.topk && c.n <= kSmallBatch && c.n <= m->chunk_images)   // sets the device where it launches
+    if (c.host && c.engine == kEngineC && !c.topk && !c.windows && c.n <= kSmallBatch && c.n <= m->chunk_images)   // sets the device where it launches
         return infer_small(m, static_cast<const int8_t *>(c.images), c.n, static_cast<int32_t *>(o.logits), o.labels);
     CU_TRY(cudaSetDevice(m->device));
     const Route r = choose_route(m, c.engine, c.in, c.topk, c.windows);
-    // the lines of the model's creation name the float32 routes only: a 16-bit call names its own (a 16-bit form or scaling kernel)
-    if ((c.topk || c.windows || half_in(c.in)) && m->verbose)
+    // the lines of the model's creation name the float32 routes only: a 16-bit call names its own (a 16-bit form or scaling kernel);
+    // a host window scan names its route with its bands (infer_pipelined)
+    if ((c.topk || c.windows || half_in(c.in)) && m->verbose && !(c.host && c.windows))
         print_route(m, (std::string(c.windows ? "windows route: " : c.topk ? "topk route: " : "16-bit route: ") + c.name).c_str(), r);
     if (o.gather && !r.fused)
         return fail(BNM_E_UNSUPPORTED, "the fused result exchange needs the fused tensor-core path (model: %s)", m->plan_err.c_str());
     cudaStream_t st = static_cast<cudaStream_t>(c.stream);
-    if (c.host) return infer_pipelined(m, r, c.images, c.n, o);
+    if (c.host) return infer_pipelined(m, r, c.images, c.n, o, c.windows, c.name);
     const StreamCapture cap = capture_of(st);
     if (c.engine == kEngineBoth && !r.fused) return run_engines(m, r, c.images, c.n, o, st, cap);
     return run_route(m, r, c.images, c.n, o, st, cap, c.windows);
@@ -1331,12 +1440,14 @@ extern "C" int bnm_emulate_topk_device(bnm_model *m, const float *images, size_t
 // from the planes into the call's scratch, then that entry's route runs on the scaled rows; a fused FC launch after it keeps its
 // wait and counts as a launch of another kind.  w's checks and pad's (NULL: no padding, the grid of sections 9 to 12), then call c
 // (name, engine, the planes' element kind, top-k, outputs, alignment, stream) on its windows.  Windows: bnm_windows or
-// bnm_windows_f16, whose fields differ in the image's element type only.
+// bnm_windows_f16, whose fields differ in the image's element type only, or (a host call, section 14) bnm_windows_host, whose
+// rows and planes may be any number of elements apart.
 template <class Windows> static int run_windows(bnm_model *m, const Windows *w, Call c, const bnm_window_padding *pad = nullptr) {
     if (int rc = require_device()) return rc;
     if (!w) return fail(BNM_E_ARG, "%s: null window descriptor", c.name);
     if (!w->stride_y || !w->stride_x) return fail(BNM_E_ARG, "%s: zero stride (%u, %u)", c.name, w->stride_y, w->stride_x);
-    const size_t row_elems = 16 / in_elem_bytes(c.in);   // elements in 16 bytes
+    const size_t row_elems = c.host ? 1 : 16 / in_elem_bytes(c.in);   // elements in 16 bytes: a device page's row and plane alignment
+    if (c.host && w->pitch < w->width) return fail(BNM_E_ARG, "%s: pitch %zu must be >= width %u", c.name, w->pitch, w->width);
     if (w->pitch < w->width || w->pitch % row_elems)
         return fail(BNM_E_ARG, "%s: pitch %zu must be >= width %u and a multiple of %zu elements (16-byte rows)", c.name, w->pitch,
                     w->width, row_elems);
@@ -1542,6 +1653,40 @@ extern "C" int bnm_emulate_windows_topk_padded_device_f16(bnm_model *m, const bn
                                                           void *stream) {
     return run_windows_padded_half(m, w, format, padding, {"bnm_emulate_windows_topk_padded_device_f16", kEngineEmul, kInF16, true, nullptr,
                                                            0, {nullptr, nullptr, nullptr, {k, classes, scores}}, {16, 1, 4, 8}, stream});
+}
+
+// Host pages (section 14): the stacked window entries on a stack in host memory, padded or not (pad NULL), in the element kind of
+// its format; call c of the device sibling with host buffers, run by infer_pipelined band by band
+static int run_windows_host(bnm_model *m, const bnm_windows_host *w, const bnm_window_padding *pad, Call c) {
+    if (int rc = require_device()) return rc;
+    if (!w) return fail(BNM_E_ARG, "%s: null window descriptor", c.name);
+    if (w->format != BNM_FLOAT32 && w->format != BNM_FLOAT16 && w->format != BNM_BFLOAT16)
+        return fail(BNM_E_ARG, "%s: format %d, must be BNM_FLOAT32 (3), BNM_FLOAT16 (1) or BNM_BFLOAT16 (2)", c.name, w->format);
+    c.in = w->format == BNM_FLOAT32 ? kInF32 : w->format == BNM_BFLOAT16 ? kInBF16 : kInF16;
+    return run_windows(m, w, c, pad);
+}
+
+extern "C" int bnm_scan_windows(bnm_model *m, const bnm_windows_host *w, const bnm_window_padding *padding, int32_t *logits,
+                                uint32_t *labels) {
+    return run_windows_host(m, w, padding, {"bnm_scan_windows", kEngineC, kInF32, false, nullptr, 0, {logits, labels}, {}, nullptr, true});
+}
+
+extern "C" int bnm_scan_windows_topk(bnm_model *m, const bnm_windows_host *w, const bnm_window_padding *padding, uint32_t k,
+                                     uint32_t *classes, int32_t *scores) {
+    return run_windows_host(m, w, padding, {"bnm_scan_windows_topk", kEngineC, kInF32, true, nullptr, 0,
+                                            {nullptr, nullptr, nullptr, {k, classes, scores}}, {}, nullptr, true});
+}
+
+extern "C" int bnm_emulate_windows(bnm_model *m, const bnm_windows_host *w, const bnm_window_padding *padding, double *logits,
+                                   uint32_t *labels) {
+    return run_windows_host(m, w, padding, {"bnm_emulate_windows", kEngineEmul, kInF32, false, nullptr, 0, {logits, labels}, {}, nullptr,
+                                            true});
+}
+
+extern "C" int bnm_emulate_windows_topk(bnm_model *m, const bnm_windows_host *w, const bnm_window_padding *padding, uint32_t k,
+                                        uint32_t *classes, double *scores) {
+    return run_windows_host(m, w, padding, {"bnm_emulate_windows_topk", kEngineEmul, kInF32, true, nullptr, 0,
+                                            {nullptr, nullptr, nullptr, {k, classes, scores}}, {}, nullptr, true});
 }
 
 // host buffers: n <= kSmallBatch images share a launch with concurrent small calls, larger batches run the chunked pipeline

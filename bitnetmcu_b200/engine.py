@@ -13,6 +13,7 @@ torch is used only as plumbing for device memory / streams in ``infer_device``.
 from __future__ import annotations
 
 import ctypes as C
+import sys
 from typing import Optional, Tuple
 
 import numpy as np
@@ -45,6 +46,64 @@ def _pad_sides(padding) -> Tuple[int, int, int, int]:
 
 
 _PAD_MODES = {"constant": _lib.PAD_CONSTANT, "replicate": _lib.PAD_REPLICATE, "reflect": _lib.PAD_REFLECT}
+
+
+def _host_pages(pages):
+    """(format, pointer, the array that owns the pixels, (P, H, W), pitch, plane pitch) of host pages (section 14): a NumPy float32 /
+    float16 array or a CPU torch tensor of float32, float16 or bfloat16, [P, H, W] or [H, W].  A view whose column stride is not
+    one element, whose rows overlap (a row stride under the width, as a broadcast row has), or with a negative or partial-element
+    stride is copied to a contiguous array first."""
+    torch = sys.modules.get("torch")
+    if torch is not None and isinstance(pages, torch.Tensor):
+        if pages.device.type != "cpu":
+            raise ValueError(f"host pages must be a CPU tensor, got one on {pages.device}: use the *_device methods")
+        fmt = {torch.float32: _lib.FLOAT32, torch.float16: _lib.FLOAT16, torch.bfloat16: _lib.BFLOAT16}.get(pages.dtype)
+        if fmt is None:
+            raise TypeError(f"host pages: float32, float16 or bfloat16, got {pages.dtype}")
+        p = pages if pages.dim() == 3 else pages.unsqueeze(0)
+        if p.dim() != 3:
+            raise ValueError(f"host pages: [P, H, W] or [H, W], got shape {tuple(pages.shape)}")
+        if not _unit_columns(p.shape, p.stride(), 1):
+            p = p.contiguous()
+        return (fmt, p.data_ptr(), p, tuple(p.shape)) + _pitches(p.shape, p.stride())
+    a = np.asarray(pages)
+    fmt = {np.dtype(np.float32): _lib.FLOAT32, np.dtype(np.float16): _lib.FLOAT16}.get(a.dtype)
+    if fmt is None:
+        raise TypeError(f"host pages: float32 or float16, got {a.dtype}")
+    a = a[None] if a.ndim == 2 else a
+    if a.ndim != 3:
+        raise ValueError(f"host pages: [P, H, W] or [H, W], got shape {np.shape(pages)}")
+    if not _unit_columns(a.shape, a.strides, a.itemsize):
+        a = np.ascontiguousarray(a)
+    return (fmt, a.ctypes.data, a, a.shape) + _pitches(a.shape, [s // a.itemsize for s in a.strides])
+
+
+def _unit_columns(shape, strides, unit) -> bool:
+    """whether a [P, H, W] view's columns are one element (unit) apart, its rows at least a row apart (not a broadcast or
+    overlapping rows) and its planes a whole number of elements >= 0 apart; a stride of an axis of one element or less is never
+    used"""
+    return all(n <= 1 or (s >= 0 and s % unit == 0 and (i != 1 or s >= unit * shape[2]) and (i < 2 or s == unit))
+               for i, (n, s) in enumerate(zip(shape, strides)))
+
+
+def _pitches(shape, strides) -> Tuple[int, int]:
+    """(pitch, plane pitch) in elements of a [P, H, W] view (strides in elements), those of a compact stack on an axis of one
+    element or less and for a view of no elements"""
+    p, h, w = shape
+    if p * h * w == 0:
+        return w, h * w
+    pitch = strides[1] if h > 1 else w
+    return pitch, (strides[0] if p > 1 else h * pitch)
+
+
+def _host_out(out: Optional[np.ndarray], want: bool, shape, dtype) -> Optional[np.ndarray]:
+    """out (checked: C-contiguous, writeable, of dtype and shape), else a new array when wanted, else None"""
+    if out is None:
+        return np.empty(shape, dtype=dtype) if want else None
+    if out.dtype != dtype or tuple(out.shape) != tuple(shape) or not out.flags.c_contiguous or not out.flags.writeable:
+        raise ValueError(f"output array: a writeable C-contiguous {np.dtype(dtype)} array of shape {tuple(shape)}, got "
+                         f"{out.dtype} {out.shape}")
+    return out
 
 
 def window_grid(height: int, width: int, stride, padding=None) -> Tuple[int, int]:
@@ -283,6 +342,79 @@ class Engine:
         import torch
         self._windows_call("bnm_emulate_windows_topk", pages, stride, [int(k), (classes, 4, (k,)), (scores, torch.float64, (k,))],
                            stream, padding, pad_mode, pad_value)
+
+    # ---- window scan of host pages (include/bitnetmcu_b200.h section 14) ----------------------------------------------------------
+    # pages: a [P, H, W] stack ([H, W]: one page) in host memory, a NumPy float32 / float16 array or a CPU torch tensor of
+    # torch.float32, torch.float16 or torch.bfloat16 (pinned or not), any strided view with unit column stride (others are copied
+    # to a contiguous array first).  The library copies it to the GPU band by band, scanning one band while the next is copied,
+    # and returns NumPy arrays [P, out_h, out_w, ...] with (out_h, out_w) = window_grid(H, W, stride, padding): bit for bit what
+    # the matching ``*_device`` method returns on the same stack copied to the GPU.  stride, padding, pad_mode and pad_value are
+    # those of the device methods.  out_*: NumPy arrays of the output's dtype and shape, C-contiguous, to write into instead.
+    def _host_windows_call(self, stem, pages, stride, args, padding, pad_mode, pad_value) -> None:
+        """the host window entry stem(handle, the stack's bnm_windows_host, its bnm_window_padding or NULL, *args)"""
+        fmt, ptr, _keep, shape, pitch, plane_pitch = _host_pages(pages)
+        sy, sx = (stride, stride) if isinstance(stride, int) else (int(stride[0]), int(stride[1]))
+        desc = _lib.BnmWindowsHost(ptr, fmt, shape[0], shape[1], shape[2], pitch, plane_pitch, sy, sx)
+        pad = None
+        if padding is not None:
+            if pad_mode not in _PAD_MODES:
+                raise ValueError(f"pad_mode must be one of {sorted(_PAD_MODES)}, got {pad_mode!r}")
+            pad = C.byref(_lib.BnmWindowPadding(*_pad_sides(padding), _PAD_MODES[pad_mode], float(pad_value)))
+        _lib.check(getattr(self.lib, stem)(self.handle, C.byref(desc), pad, *args), stem)
+
+    def _host_grid(self, pages, stride, padding) -> Tuple[int, int, int]:
+        shape = tuple(np.shape(pages))
+        return (shape[0] if len(shape) == 3 else 1,) + window_grid(shape[-2], shape[-1], stride, padding)
+
+    def scan_windows(self, pages, stride, want_labels: bool = True, want_logits: bool = True, out_logits: Optional[np.ndarray] = None,
+                     out_labels: Optional[np.ndarray] = None, *, padding=None, pad_mode: str = "constant",
+                     pad_value: float = 0.0) -> Tuple[Optional[np.ndarray], Optional[np.ndarray]]:
+        """The C engine on every window of host pages -> (logits int32 [P, out_h, out_w, n_classes], labels uint32
+        [P, out_h, out_w]), either None when not asked for; ``scan_windows_device`` on the pages copied to the GPU."""
+        grid = self._host_grid(pages, stride, padding)
+        logits = _host_out(out_logits, want_logits, grid + (self.n_classes,), np.int32)
+        labels = _host_out(out_labels, want_labels, grid, np.uint32)
+        if logits is None and labels is None:
+            raise ValueError("Engine.scan_windows: ask for logits, labels or both")
+        self._host_windows_call("bnm_scan_windows", pages, stride, [_ptr(logits), _ptr(labels)], padding, pad_mode, pad_value)
+        return logits, labels
+
+    def scan_windows_topk(self, pages, stride, k: int, want_scores: bool = True, out_classes: Optional[np.ndarray] = None,
+                          out_scores: Optional[np.ndarray] = None, *, padding=None, pad_mode: str = "constant",
+                          pad_value: float = 0.0) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+        """The C engine's top-k of every window of host pages -> (classes uint32 [P, out_h, out_w, k], scores int32
+        [P, out_h, out_w, k] or None with ``want_scores=False``); ``scan_windows_topk_device`` on the pages copied to the GPU."""
+        grid = self._host_grid(pages, stride, padding)
+        classes = _host_out(out_classes, True, grid + (k,), np.uint32)
+        scores = _host_out(out_scores, want_scores, grid + (k,), np.int32)
+        self._host_windows_call("bnm_scan_windows_topk", pages, stride, [int(k), _ptr(classes), _ptr(scores)], padding, pad_mode,
+                                pad_value)
+        return classes, scores
+
+    def emulate_windows(self, pages, stride, want_labels: bool = True, want_logits: bool = True,
+                        out_logits: Optional[np.ndarray] = None, out_labels: Optional[np.ndarray] = None, *, padding=None,
+                        pad_mode: str = "constant", pad_value: float = 0.0) -> Tuple[Optional[np.ndarray], Optional[np.ndarray]]:
+        """The emulator on every window of host pages -> (logits float64 [P, out_h, out_w, n_classes], labels uint32
+        [P, out_h, out_w]), either None when not asked for; ``emulate_windows_device`` on the pages copied to the GPU."""
+        grid = self._host_grid(pages, stride, padding)
+        logits = _host_out(out_logits, want_logits, grid + (self.n_classes,), np.float64)
+        labels = _host_out(out_labels, want_labels, grid, np.uint32)
+        if logits is None and labels is None:
+            raise ValueError("Engine.emulate_windows: ask for logits, labels or both")
+        self._host_windows_call("bnm_emulate_windows", pages, stride, [_ptr(logits), _ptr(labels)], padding, pad_mode, pad_value)
+        return logits, labels
+
+    def emulate_windows_topk(self, pages, stride, k: int, want_scores: bool = True, out_classes: Optional[np.ndarray] = None,
+                             out_scores: Optional[np.ndarray] = None, *, padding=None, pad_mode: str = "constant",
+                             pad_value: float = 0.0) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+        """The emulator's top-k of every window of host pages -> (classes uint32 [P, out_h, out_w, k], scores float64
+        [P, out_h, out_w, k] or None with ``want_scores=False``); ``emulate_windows_topk_device`` on the pages copied to the GPU."""
+        grid = self._host_grid(pages, stride, padding)
+        classes = _host_out(out_classes, True, grid + (k,), np.uint32)
+        scores = _host_out(out_scores, want_scores, grid + (k,), np.float64)
+        self._host_windows_call("bnm_emulate_windows_topk", pages, stride, [int(k), _ptr(classes), _ptr(scores)], padding, pad_mode,
+                                pad_value)
+        return classes, scores
 
     def compare_engines_device(self, images, truth=None, labels_c=None, labels_py=None, counts=None, stream: Optional[int] = None) -> None:
         """Both engines on the same float images in one call (test_inference.py:130-175): images torch.float32 [n, img_bytes] on

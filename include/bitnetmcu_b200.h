@@ -20,6 +20,7 @@
  * Section 9 classifies every 16x16 window of a larger float image on a stride grid (window scan).
  * Section 10 scans a stack of such images in one call, on either engine, with labels, logits or top-k.
  * Section 11 takes float16 and bfloat16 images on the float device entries.
+ * Sections 12 and 13 scan 16-bit pages and pages with padded borders; section 14 scans page stacks that live in host memory.
  *
  * Pointers are plain host (or, where the name says _device, CUDA device) pointers; sizes are element
  * counts unless named *_bytes.  All-integer arithmetic: results are bit-exact with the reference.
@@ -548,6 +549,66 @@ BNM_API int bnm_emulate_windows_padded_device_f16(bnm_model *m, const bnm_window
 BNM_API int bnm_emulate_windows_topk_padded_device_f16(bnm_model *m, const bnm_windows_f16 *windows, int format,
                                                        const bnm_window_padding *padding, uint32_t k, uint32_t *classes, double *scores,
                                                        void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * 14. Host pages: the window scan of sections 10, 12 and 13 on a stack of pages in host memory (a NumPy array, a plain-C
+ *     buffer).  The library streams the stack to the GPU in bands and scans one band while the next is being copied, so device
+ *     memory never holds the whole stack and the copies run under the scan.
+ * ------------------------------------------------------------------------------------------- */
+#define BNM_FLOAT32 3    /* IEEE 754 binary32 (host pages only; the 16-bit entries of sections 11 to 13 reject it) */
+typedef struct bnm_windows_host {
+    const void *image;        /* plane p starts at image + p * plane_pitch elements; host memory, pinned or pageable, any alignment */
+    int format;               /* BNM_FLOAT32, BNM_FLOAT16 or BNM_BFLOAT16: the elements of every plane                           */
+    uint32_t planes;          /* >= 0; 0 = no windows                                                                            */
+    uint32_t height, width;   /* of every plane                                                                                  */
+    size_t pitch;             /* elements between rows: >= width                                                                 */
+    size_t plane_pitch;       /* elements between planes (ignored when planes <= 1)                                              */
+    uint32_t stride_y, stride_x;
+} bnm_windows_host;
+/* Each entry below is the section 10 sibling named beside it on host buffers, with `const bnm_windows_host *windows` and an
+ * optional `const bnm_window_padding *padding` (section 13; NULL: no border) in place of `const bnm_windows *windows`:
+ *   bnm_scan_windows           bnm_scan_windows_device
+ *   bnm_scan_windows_topk      bnm_scan_windows_topk_device
+ *   bnm_emulate_windows        bnm_emulate_windows_device
+ *   bnm_emulate_windows_topk   bnm_emulate_windows_topk_device
+ * Every output is a host buffer, with the sibling's types, window order and layout, NULL combinations and k rules; no buffer needs
+ * any alignment.  Results are bit for bit those of the matching device entry (bnm_scan_windows_device, its _padded_device form
+ * with a padding, the _f16 forms for 16-bit pages) on the same stack after it has been copied to the GPU.  Pixels outside
+ * [0, height) x [0, width) of each plane (pitch padding, rows below a page, gaps between planes) are never read and never change
+ * a result.  The call returns when the results are in the caller's buffers.
+ * Argument failures are the sibling's, with its texts: BNM_E_ARG for a NULL descriptor, a format other than BNM_FLOAT32,
+ * BNM_FLOAT16 or BNM_BFLOAT16, a zero stride, pitch < width, no output, a bad k, and the padding rules of section 13 (reflect
+ * checked against the page); BNM_E_UNSUPPORTED for a model whose images are not 256 elements.  No windows: returns 0 and writes
+ * nothing (a top-k call still checks k).
+ * Bands.  The grid of windows is cut into bands, each a run of whole planes or a run of window rows inside one plane, never part
+ * of two planes.  A band's page rows (the rows its windows cover, the 16 - stride_y halo rows it shares with its neighbours
+ * included, and in a plane's first band with reflect padding at least rows 0 .. top, the mirror images of the top border rows,
+ * which its windows need not cover) are copied with cudaMemcpy2DAsync into staging of one of the model's three pipeline slots (the buffers of
+ * BNM_OPT_CHUNK_IMAGES's pipeline), the window route of the sibling runs on them, and the band's outputs are copied back;
+ * bands go round-robin over the slots' streams, so one band's copies overlap another's scan.  With B = BNM_OPT_CHUNK_IMAGES x
+ * 1 KiB of page pixels (64 MiB at the default chunk) and a plane's page rows taking width x height' x element bytes (height':
+ * its first band's page rows from row 0 to its last window's last row, within the page):
+ *   - a plane of at most B and 2^20 windows is whole: consecutive whole planes share a band while it holds at most B of page
+ *     pixels and 2^20 windows;
+ *   - every other plane is cut into bands of R = max(1, min(floor((B / (width x element bytes) - 16) / stride_y) + 1,
+ *     floor(2^20 / out_w))) window rows, from its first window row, except that its first band holds at least every window row
+ *     whose window starts in the top border; and
+ *     when windows reach into the bottom border, the band that would hold window row t runs to the plane's last window row: t is
+ *     the first window row that reaches into the bottom border or, with reflect, the last window row that starts at or above
+ *     page row height - 1 - e if that is smaller (e: the rows the last window reaches below the page).
+ * So top and bottom padding belong to a plane's first and last band only, left and right padding to every band, and the edge
+ * bands hold every page row that replicate or reflect padding maps onto.  Results do not depend on the bands.
+ * Threads and graphs: these calls take turns with the other large host calls (section 3), and work while another thread
+ * captures a graph in any mode, leaving that capture valid ("Graphs").  With BNM_VERBOSE set at model creation every call prints
+ * "bitnetmcu_b200: host windows: <entry>: <bands> bands: k_quantize_windows + ...", the route of each band. */
+BNM_API int bnm_scan_windows(bnm_model *m, const bnm_windows_host *windows, const bnm_window_padding *padding, int32_t *logits,
+                             uint32_t *labels);
+BNM_API int bnm_scan_windows_topk(bnm_model *m, const bnm_windows_host *windows, const bnm_window_padding *padding, uint32_t k,
+                                  uint32_t *classes, int32_t *scores);
+BNM_API int bnm_emulate_windows(bnm_model *m, const bnm_windows_host *windows, const bnm_window_padding *padding, double *logits,
+                                uint32_t *labels);
+BNM_API int bnm_emulate_windows_topk(bnm_model *m, const bnm_windows_host *windows, const bnm_window_padding *padding, uint32_t k,
+                                     uint32_t *classes, double *scores);
 
 #ifdef __cplusplus
 }
